@@ -13,7 +13,7 @@
 // Phases of one LM trial (workers = all threads of the cluster):
 //   residual   thread/edge      EdgeSE3ProjectXYZ::computeError + Huber rho, edge factors   (HOT LOOP A)
 //   build      8 lanes/point: Hll, bl;  warp/chunk of a pose's edges: Hpp, bp               (HOT LOOP B)
-//   schur      thread/point: (Hll + lambda I)^-1;  warp/chunk of (e1, e2) pairs of one pose pair:
+//   schur      thread/point: (Hll + lambda I)^-1;  warp/chunk of the edge pairs of one pose pair:
 //              Hschur = Hpp - sum B1^T (w1 w2 A1 Hll^-1 A2^T) B2                            (HOT LOOP C)
 //   ldlt       CTA 0, matrix in shared memory: blocked LDL^T with look-ahead, rhs carried as an extra row
 //   backsub    8 lanes/point    x_l = Hll^-1 (b_l - W^T x_p)
@@ -64,20 +64,25 @@ struct Dev {
     const double* obs;                // nE x 2
     const float* invSigma2;           // nE
     const int* ptStart;               // nL + 1
-    const int* poseEdges;             // edge lists of the free poses (internal edge ids, ascending), back to back
-    const int2* pairs;                // (edge of pose i1, edge of pose i2) observing the same point
+    // POSE-MAJOR order: the edge lists of the free poses (ascending point) back to back; position k in them is the pose-major
+    // index of the edge.  The Schur phase reads the edge factors in this order, so neighbouring lanes share lines.
+    const int* poseEdges;             // internal edge id at pose-major index k
+    const int2* pairs;                // (pose-major index of the edge of pose i1, of the edge of pose i2) observing the same point
     const int* pairPt;                // that point
     // Schur work list: tasks 0..nF-1 = diagonal blocks (items = edges of the pose), nF.. = off-diagonal blocks (items = pairs);
     // every task is cut into chunks of SCH items so that all warps of the cluster get the same amount of work
     int nChunks; const int4* chunkHdr; const int* taskChunkStart;   // nChunks x (first item, items, pose A, pose B or -1), nTasks + 1
-    const int* poseEdgePt;            // nE: point of poseEdges[k]
+    const int* poseEdgePt;            // nE: point of the edge at pose-major index k
     double* Spart;                    // nChunks x 42 partial sums (36 block entries + 6 rhs entries for diagonal tasks)
     double* Ppart;                    // (chunks of the diagonal tasks) x 28: partial sums of Hpp (21) and bp (6)
     double* err;                      // nE x 2
     double *E4a, *E4b;                // nE x 4 edge factors (x/z, y/z, 1/z, w): linearisation point / trial state (swapped on accept)
+    double2* K;                       // 2 x nE: the factors at the linearisation point at pose-major index k, as two arrays
+                                      // (x/z, y/z) | (1/z, w); written by phase_build_poses_partial, read by the Schur phase
     double *Hpp, *bp;                 // nF x 36, nF x 6
     double *Hll, *bl;                 // nL x 6 (00 01 02 11 12 22), nL x 3
-    double* PT;                       // nL x 12 point records: upper triangle of (Hll + lambda I)^-1 (6), (Hll + lambda I)^-1 bl (3), 3 pad
+    double2* PT;                      // point records as arrays over the points: (d00 d01) | (d02 d11) | (d12 d22) | (db0 db1), nL each,
+                                      // then db2 (nL doubles); Dinv = (Hll + lambda I)^-1 (upper triangle), db = Dinv bl
     double *Hs, *bs;                  // n x n (only when it does not fit in shared memory), n
     double* x;                        // n + 3 nL
     double* partial;                  // 4 rotating slots x 16 doubles: per-CTA partial sums + broadcast words
@@ -287,14 +292,20 @@ __device__ double phase_errors(const Dev& D, const Ctx& c, double* __restrict__ 
 // EdgeSE3ProjectXYZ::linearizeOplus (-projectJac * R and -projectJac * [-[Xc]x | I], Pinhole.cpp:71-81) are
 //   A = -diag(fx iz, fy iz) t,   t = [R0 - xn R2 ; R1 - yn R2]                           (2x3)
 //   B =  diag(fx, fy) b,         b = [xn yn, -(1 + xn^2), yn, -iz, 0, xn iz ; 1 + yn^2, -xn yn, -xn, 0, -iz, yn iz]   (2x6)
-// A 32-byte record as two 128-bit global loads (LDG.E.128, the widest sm_90 has): the gathers of the Schur phase are bound
-// by look-ups per instruction, not by bytes, so each record is fetched with as few instructions as the ISA allows
+// A 32-byte record as two 128-bit global loads (LDG.E.128, the widest sm_90 has)
 __device__ __forceinline__ void ld256(const double* p, double& a, double& b, double& c, double& d) {
     asm volatile("ld.global.v2.f64 {%0, %1}, [%2];" : "=d"(a), "=d"(b) : "l"(p));
     asm volatile("ld.global.v2.f64 {%0, %1}, [%2];" : "=d"(c), "=d"(d) : "l"(p + 2));
 }
 __device__ __forceinline__ void load_e4(const double* __restrict__ E, int e, double& xn, double& yn, double& iz, double& w) {
     ld256(E + 4 * (size_t)e, xn, yn, iz, w);
+}
+// The same factors from the pose-major arrays (K = (x/z, y/z) of every edge, then (1/z, w)), at pose-major index k.  The Schur
+// phase is bound by L1 look-ups per load instruction, and here the lanes of a warp read neighbouring k: a diagonal chunk reads
+// 32 consecutive entries (4 lines per LDG.128 instead of 32)
+__device__ __forceinline__ void load_k4(const double2* __restrict__ K, int nE, int k, double& xn, double& yn, double& iz, double& w) {
+    const double2 a = K[k], b = K[nE + k];
+    xn = a.x; yn = a.y; iz = b.x; w = b.y;
 }
 __device__ __forceinline__ void edge_t(const double* R, double xn, double yn, double* t) {
 #pragma unroll
@@ -372,10 +383,11 @@ __device__ void phase_build_points(const Dev& D, const Ctx& c, const double* __r
 constexpr int SCH = LBA_SCH;       // items per chunk of the pose / pose-pair work lists
 constexpr int IPL = SCH / 32;      // items per lane
 constexpr int UNR = LBA_UNR;       // items in flight per lane in the Schur chunk loops
-constexpr int PTR = 12;            // doubles per point record: d00 d01 d02 d11 | d12 d22 db0 db1 | db2 - - -   (Dinv = (Hll + lambda I)^-1, db = Dinv bl)
 
 // ---- per free pose Hpp, bp.  partial: warp per chunk of the pose's edges (the chunks of the diagonal Schur tasks), lane per
-//      edge, 21 + 6 sums reduce-scattered to Spart; combine: thread per (pose, entry), chunks added in order ----
+//      edge, 21 + 6 sums reduce-scattered to Spart; combine: thread per (pose, entry), chunks added in order.
+//      The chunks cover every pose-major index once, so the partial step also writes the pose-major copy K of the factors
+//      that the Schur phase reads (coalesced stores; the factors stay fixed for all trials of an iteration) ----
 __device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const double* __restrict__ E) {
     const int lane = c.tid & 31;
     const int nDiag = D.taskChunkStart[D.nF];
@@ -387,9 +399,10 @@ __device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const doub
 #pragma unroll
         for (int i = 0; i < 27; ++i) acc[i] = 0;
         for (int i = lane; i < h.y; i += 32) {
-            const int e = D.poseEdges[h.x + i];
+            const int k = h.x + i, e = D.poseEdges[k];
             double xn, yn, iz, w, b0[6], b1[6];
             load_e4(E, e, xn, yn, iz, w);
+            D.K[k] = make_double2(xn, yn); D.K[D.nE + k] = make_double2(iz, w);
             edge_b(xn, yn, iz, b0, b1);
             const double2 er = *reinterpret_cast<const double2*>(D.err + 2 * (size_t)e);
             const double c0 = w * fx * fx, c1 = w * fy * fy;          // w B^T B = c0 b0^T b0 + c1 b1^T b1
@@ -447,10 +460,16 @@ __device__ __forceinline__ void point_record(const Dev& D, int p, const double* 
     const double o0 = c00 * id, o1 = c10 * id, o2 = c20 * id;
     const double o4 = (m0 * m8 - m2 * m2) * id, o5 = (m2 * m1 - m0 * m5) * id, o8 = (m0 * m4 - m1 * m1) * id;
     const double b0 = bl3[0], b1 = bl3[1], b2 = bl3[2];
-    double2* O = reinterpret_cast<double2*>(D.PT + PTR * (size_t)p);
-    O[0] = make_double2(o0, o1); O[1] = make_double2(o2, o4); O[2] = make_double2(o5, o8);
-    O[3] = make_double2(o0 * b0 + o1 * b1 + o2 * b2, o1 * b0 + o4 * b1 + o5 * b2);
-    O[4] = make_double2(o2 * b0 + o5 * b1 + o8 * b2, 0.0);
+    const size_t nL = D.nL;
+    double2* O = D.PT + p;
+    O[0] = make_double2(o0, o1); O[nL] = make_double2(o2, o4); O[2 * nL] = make_double2(o5, o8);
+    O[3 * nL] = make_double2(o0 * b0 + o1 * b1 + o2 * b2, o1 * b0 + o4 * b1 + o5 * b2);
+    reinterpret_cast<double*>(D.PT + 4 * nL)[p] = o2 * b0 + o5 * b1 + o8 * b2;
+}
+// Dinv of point p (00 01 02 11 12 22) from the point records
+__device__ __forceinline__ void load_dinv(const double2* __restrict__ PT, size_t nL, int p, double* dv) {
+    const double2 a = PT[p], b = PT[nL + p], c = PT[2 * nL + p];
+    dv[0] = a.x; dv[1] = a.y; dv[2] = b.x; dv[3] = b.y; dv[4] = c.x; dv[5] = c.y;
 }
 __device__ void phase_point_prep(const Dev& D, const Ctx& c, double lambda) {
     for (int p = c.wid; p < D.nL; p += c.nw) {
@@ -463,14 +482,15 @@ __device__ void phase_point_prep(const Dev& D, const Ctx& c, double lambda) {
 }
 
 // ---- Schur complement (block_solver.hpp:396-431), two steps.
-//   partial: the work list (diagonal block i: edges of pose i; off-diagonal block (i1 < i2): the precomputed (e1, e2) pairs)
+//   partial: the work list (diagonal block i: edges of pose i; off-diagonal block (i1 < i2): the precomputed (k1, k2) pairs)
 //            is cut into chunks of SCH items; one warp per chunk, one lane per item.  An item adds
 //                b1^T M b2,   M[k][l] = g1_k g2_l (t1_k Hll^-1 t2_l^T),   g_k = w f_k^2 / z
 //            (= W1 Hll^-1 W2^T with W = w B^T A) into the lane's 36 accumulators; diagonal items also add
-//            W Hll^-1 bl = -sum_k b_k g_k (t_k . db).  The item's three records (two edges, one point) are per-lane
-//            gathers -- the phase is bound by L1 look-ups (~39 clk per 32-lane LDG.256 of 32 distinct lines), so the
-//            chunk's indices sit in a warp-private shared-memory buffer and the gathers of item j + 1 are issued before
-//            the arithmetic of item j.  The lanes' sums are reduce-scattered into Spart.
+//            W Hll^-1 bl = -sum_k b_k g_k (t_k . db).  The item's operands (two edges, one point) are per-lane loads and
+//            the phase is bound by L1 look-ups, one per distinct line of a warp's load instruction (tools/microbench), so
+//            they are read from the pose-major edge arrays and the point arrays: the lanes of a chunk hold ascending points
+//            and neighbouring pose-major indices and share lines.  The chunk's indices are loaded into registers up front and
+//            UNR items are in flight per lane.  The lanes' sums are reduce-scattered into Spart.
 //   combine: thread per (task, entry): ordered sum of the task's chunks -> lower triangle of the reduced camera system
 //            (diagonal: Hpp_i + lambda I - sum, bs_i = bp_i - sum; off-diagonal: block (i2, i1) = -(sum)^T). ----
 __device__ __forceinline__ void schur_item(const double* t1, const double* t2, const double* dv, double g10, double g11, double g20, double g21,
@@ -500,8 +520,8 @@ __device__ __forceinline__ void schur_item(const double* t1, const double* t2, c
 }
 struct PairOps { double a[4], b[4], dv[6]; };          // edge 1, edge 2 (x/z, y/z, 1/z, w), Dinv
 struct DiagOps { double a[4], dv[6], db[3]; };
-__device__ __forceinline__ void schur_chunk_offdiag(const int2* __restrict__ pairs, const int* __restrict__ pairPt, const double* __restrict__ PT, const double* __restrict__ E,
-                                                  const double* pcache, double* out42, int4 h) {
+__device__ __forceinline__ void schur_chunk_offdiag(const int2* __restrict__ pairs, const int* __restrict__ pairPt, const double2* __restrict__ PT, size_t nL,
+                                                  const double2* __restrict__ K, int nE, const double* pcache, double* out42, int4 h) {
     const int lane = threadIdx.x & 31;
     const int cnt = h.y;
     int2 rpr[IPL]; int rpt[IPL];
@@ -518,13 +538,10 @@ __device__ __forceinline__ void schur_chunk_offdiag(const int2* __restrict__ pai
         const int i = lane + 32 * j;
         if (i < cnt) {
             PairOps o;
-            const int e1 = rpr[j].x, e2 = rpr[j].y, ip = rpt[j];
-            ld256(E + 4 * (size_t)e1, o.a[0], o.a[1], o.a[2], o.a[3]);
-            ld256(E + 4 * (size_t)e2, o.b[0], o.b[1], o.b[2], o.b[3]);
-            const double* pt = PT + PTR * (size_t)ip;
-            ld256(pt, o.dv[0], o.dv[1], o.dv[2], o.dv[3]);
-            const double2 t = *reinterpret_cast<const double2*>(pt + 4);
-            o.dv[4] = t.x; o.dv[5] = t.y;
+            const int k1 = rpr[j].x, k2 = rpr[j].y, ip = rpt[j];
+            load_k4(K, nE, k1, o.a[0], o.a[1], o.a[2], o.a[3]);
+            load_k4(K, nE, k2, o.b[0], o.b[1], o.b[2], o.b[3]);
+            load_dinv(PT, nL, ip, o.dv);
             double t1[6], t2[6], b10[6], b11[6], b20[6], b21[6];
             edge_t(P1 + 7, o.a[0], o.a[1], t1); edge_t(P2 + 7, o.b[0], o.b[1], t2);
             edge_b(o.a[0], o.a[1], o.a[2], b10, b11); edge_b(o.b[0], o.b[1], o.b[2], b20, b21);
@@ -538,15 +555,17 @@ __device__ __forceinline__ void schur_chunk_offdiag(const int2* __restrict__ pai
     if (n > 0) out[0] = acc[0];
     if (n > 1) out[1] = acc[1];
 }
-__device__ __forceinline__ void schur_chunk_diag(const int* __restrict__ poseEdges, const int* __restrict__ poseEdgePt, const double* __restrict__ PT, const double* __restrict__ E,
-                                               const double* pcache, double* out42, int4 h) {
+// the items of a diagonal chunk are the edges at pose-major indices h.x .. h.x + cnt - 1: the factors are read coalesced
+__device__ __forceinline__ void schur_chunk_diag(const int* __restrict__ poseEdgePt, const double2* __restrict__ PT, size_t nL,
+                                               const double2* __restrict__ K, int nE, const double* pcache, double* out42, int4 h) {
     const int lane = threadIdx.x & 31;
     const int cnt = h.y;
-    int red[IPL], rpt[IPL];
+    int rpt[IPL];
 #pragma unroll
-    for (int j = 0; j < IPL; ++j) { const int i = lane + 32 * j; if (i < cnt) { red[j] = poseEdges[h.x + i]; rpt[j] = poseEdgePt[h.x + i]; } else { red[j] = 0; rpt[j] = 0; } }
+    for (int j = 0; j < IPL; ++j) { const int i = lane + 32 * j; rpt[j] = i < cnt ? poseEdgePt[h.x + i] : 0; }
     const double* P1 = pcache + PC * h.z;
     const double f10 = P1[16] * P1[16], f11 = P1[17] * P1[17];
+    const double* db2 = reinterpret_cast<const double*>(PT + 4 * nL);
     double acc[42];
 #pragma unroll
     for (int i = 0; i < 42; ++i) acc[i] = 0;
@@ -555,12 +574,11 @@ __device__ __forceinline__ void schur_chunk_diag(const int* __restrict__ poseEdg
         const int i = lane + 32 * j;
         if (i < cnt) {
             DiagOps o;
-            const int e1 = red[j], ip = rpt[j];
-            ld256(E + 4 * (size_t)e1, o.a[0], o.a[1], o.a[2], o.a[3]);
-            const double* pt = PT + PTR * (size_t)ip;
-            ld256(pt, o.dv[0], o.dv[1], o.dv[2], o.dv[3]);
-            ld256(pt + 4, o.dv[4], o.dv[5], o.db[0], o.db[1]);
-            o.db[2] = pt[8];
+            const int ip = rpt[j];
+            load_k4(K, nE, h.x + i, o.a[0], o.a[1], o.a[2], o.a[3]);
+            load_dinv(PT, nL, ip, o.dv);
+            const double2 db = PT[3 * nL + ip];
+            o.db[0] = db.x; o.db[1] = db.y; o.db[2] = db2[ip];
             double t1[6], b10[6], b11[6];
             edge_t(P1 + 7, o.a[0], o.a[1], t1);
             edge_b(o.a[0], o.a[1], o.a[2], b10, b11);
@@ -577,14 +595,14 @@ __device__ __forceinline__ void schur_chunk_diag(const int* __restrict__ poseEdg
     if (n > 0) out[0] = acc[0];
     if (n > 1) out[1] = acc[1];
 }
-__device__ void phase_schur_partial(const Dev& D, const Ctx& c, const double* __restrict__ E) {
+__device__ void phase_schur_partial(const Dev& D, const Ctx& c, const double2* __restrict__ K) {
     // CTA barrier at entry: the previous phase (combine of the pose sums) leaves the warps of a CTA out of step, and warps that
     // enter this gather-bound phase out of step ran it 3x slower (measured); a barrier per round of chunks on top was slower again.
     __syncthreads();
     for (int ch = c.crank * NWARP + (c.tid >> 5); ch < D.nChunks; ch += c.csize * NWARP) {
         const int4 h = D.chunkHdr[ch];      // first item, items, pose A, pose B (-1: diagonal task)
-        if (h.w >= 0) schur_chunk_offdiag(D.pairs, D.pairPt, D.PT, E, c.pc, D.Spart + 42 * (size_t)ch, h);
-        else schur_chunk_diag(D.poseEdges, D.poseEdgePt, D.PT, E, c.pc, D.Spart + 42 * (size_t)ch, h);
+        if (h.w >= 0) schur_chunk_offdiag(D.pairs, D.pairPt, D.PT, D.nL, K, D.nE, c.pc, D.Spart + 42 * (size_t)ch, h);
+        else schur_chunk_diag(D.poseEdgePt, D.PT, D.nL, K, D.nE, c.pc, D.Spart + 42 * (size_t)ch, h);
     }
 }
 __device__ void phase_schur_combine(const Dev& D, const Ctx& c, double lambda, double* Hs, int ld) {
@@ -814,7 +832,8 @@ __device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* 
 #pragma unroll
             for (int i = 0; i < 3; ++i) cl[i] += __shfl_xor_sync(gmask, cl[i], o);
         }
-        const double* Di = D.PT + PTR * (size_t)p;      // 00 01 02 11 12 22
+        double Di[6];      // 00 01 02 11 12 22
+        load_dinv(D.PT, D.nL, p, Di);
         const double* b3 = D.bl + 3 * (size_t)p;
         const double bl0 = b3[0], bl1 = b3[1], bl2 = b3[2];
         const double c0 = cl[0] + bl0, c1 = cl[1] + bl1, c2 = cl[2] + bl2;
@@ -936,7 +955,7 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
             int ok2 = 1;
             if (D.nF) {
                 TICK();
-                phase_schur_partial(D, c, Elin);
+                phase_schur_partial(D, c, D.K);
                 csync();
                 TOCK(4); TICK();
                 phase_schur_combine(D, c, lambda, HsRemote, ld);   // every CTA writes entries into CTA 0's shared memory through DSMEM
@@ -998,8 +1017,8 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
 // =============================================================================================
 // BlockSolver::buildStructure (block_solver.hpp:143-295) on the device: one CTA per problem turns the caller's edge list
 // into the index structures of the LM kernel -- edges sorted by point (stable), the (free pose, point) -> edge table, the
-// per-pose edge lists, the (e1, e2) pair list of every off-diagonal Schur block, and the chunked work list.  Only the raw
-// graph (28 B per edge) crosses PCIe; the derived lists (~2.3 MB per 40k-edge problem) never exist on the host.
+// per-pose edge lists (the pose-major edge order), the pair list of every off-diagonal Schur block in pose-major indices, and
+// the chunked work list.  Only the raw graph (28 B per edge) crosses PCIe; the derived lists (~2.3 MB per 40k-edge problem) never exist on the host.
 // Every list is in a deterministic order (by point, ties by the caller's edge index).
 // status: 0 ok, 1 edge index out of range, 2 duplicate (point, keyframe) observation, 3 pair list larger than sized.
 // =============================================================================================
@@ -1137,23 +1156,27 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     }
     __syncthreads();
     if (s_err) { if (tid == 0) status[blockIdx.x] = s_err; return; }
-    // 6. the lists themselves (ascending point = ascending internal edge id) and the chunk headers
-    for (int t = warp; t < nTasks; t += BT / 32) {
-        const int *r1, *r2;
-        taskRows(t, r1, r2);
-        int pos = D.bItemStart[t];
-        for (int p0 = 0; p0 < nL; p0 += 32) {
-            const int p = p0 + lane;
-            const int e1 = p < nL ? r1[p] : -1, e2 = p < nL ? r2[p] : -1;
-            const bool f = e1 >= 0 && e2 >= 0;
-            const unsigned m = __ballot_sync(0xffffffffu, f);
-            if (f) {
-                const int k = pos + __popc(m & ((1u << lane) - 1));
-                if (t < nF) { poseEdges[k] = e1; poseEdgePt[k] = p; }
-                else { pairs[k] = make_int2(e1, e2); pairPt[k] = p; }
+    // 6. the lists themselves (ascending point = ascending internal edge id) and the chunk headers; the pose lists first: the
+    //    position of an edge in them is its pose-major index (kept in bTmp, free since step 3), and the pair lists hold those
+    for (int pass = 0; pass < 2; ++pass) {
+        for (int t = (pass ? nF : 0) + warp; t < (pass ? nTasks : nF); t += BT / 32) {
+            const int *r1, *r2;
+            taskRows(t, r1, r2);
+            int pos = D.bItemStart[t];
+            for (int p0 = 0; p0 < nL; p0 += 32) {
+                const int p = p0 + lane;
+                const int e1 = p < nL ? r1[p] : -1, e2 = p < nL ? r2[p] : -1;
+                const bool f = e1 >= 0 && e2 >= 0;
+                const unsigned m = __ballot_sync(0xffffffffu, f);
+                if (f) {
+                    const int k = pos + __popc(m & ((1u << lane) - 1));
+                    if (t < nF) { poseEdges[k] = e1; poseEdgePt[k] = p; D.bTmp[e1] = k; }
+                    else { pairs[k] = make_int2(D.bTmp[e1], D.bTmp[e2]); pairPt[k] = p; }
+                }
+                pos += __popc(m);
             }
-            pos += __popc(m);
         }
+        __syncthreads();
     }
     for (int t = tid; t < nTasks; t += BT) {
         int poseA, poseB = -1;
@@ -1216,8 +1239,8 @@ struct Solver {
         b += al(16 * cc) + al(4 * (tasks + 1));                                   // chunk headers, task chunk starts
         b += 2 * al(4 * (nL + 1)) + al(4 * nE) + al(4 * nP * nL) + 2 * al(4 * tasks);   // structure-build scratch
         b += al(56 * nP) + al(24 * nL);                                           // second state buffers
-        b += al(16 * nE) + 2 * al(32 * nE);                                       // err, edge factors x 2
-        b += al(288 * nP) + al(48 * nP) + al(48 * nL) + al(96 * nL) + al(24 * nL);   // Hpp, bp, Hll, PT, bl
+        b += al(16 * nE) + 3 * al(32 * nE);                                       // err, edge factors x 2, pose-major copy
+        b += al(288 * nP) + al(48 * nP) + al(48 * nL) + al(72 * nL) + al(24 * nL);   // Hpp, bp, Hll, PT, bl
         b += al(8 * 42 * cc) + al(8 * 28 * (nP + nE / SCH + 1));                  // Spart, Ppart
         b += al(8 * n * n) + al(8 * n) + al(8 * (n + 3 * nL)) + al(8 * (4 * PSLOT + 8));   // Hs, bs, x, partial
         return b;
@@ -1304,9 +1327,10 @@ struct Solver {
         D.ptsB = (double*)(d_arena + carve(24 * (size_t)nL));
         D.err = (double*)(d_arena + carve(16 * (size_t)nE));
         D.E4a = (double*)(d_arena + carve(32 * (size_t)nE)); D.E4b = (double*)(d_arena + carve(32 * (size_t)nE));
+        D.K = (double2*)(d_arena + carve(32 * (size_t)nE));
         D.Hpp = (double*)(d_arena + carve(288 * (size_t)std::max(nF, 1))); D.bp = (double*)(d_arena + carve(48 * (size_t)std::max(nF, 1)));
         D.Hll = (double*)(d_arena + carve(48 * (size_t)nL)); D.bl = (double*)(d_arena + carve(24 * (size_t)nL));
-        D.PT = (double*)(d_arena + carve(96 * (size_t)nL));
+        D.PT = (double2*)(d_arena + carve(72 * (size_t)nL));
         D.Spart = (double*)(d_arena + carve(8 * 42 * cc));
         D.Ppart = (double*)(d_arena + carve(8 * 28 * ((size_t)nP + (size_t)nE / SCH + 1)));
         D.Hs = (double*)(d_arena + carve(8 * (size_t)n * n)); D.bs = (double*)(d_arena + carve(8 * (size_t)std::max(n, 1)));

@@ -1,6 +1,7 @@
 // Microbenchmarks that size the LBA kernel: (1) DFMA issue rate per SM, (2) cost of per-lane gathers of 32-byte records
 // (32 distinct 128-byte lines per warp instruction) from an L2-resident array, loaded as lba.cu loads them (2 x LDG.128), next to
-// 16-byte records (1 x LDG.128: half the bytes and half the look-ups).  Times are SM cycles from clock64(), so they do not depend on
+// 16-byte records (1 x LDG.128: half the bytes and half the look-ups), (3) cost of one 8-byte field per lane (LDG.64) when a warp
+// instruction touches 32, 4 or 2 lines (random gather, half-density and dense structure-of-arrays reads).  Times are SM cycles from clock64(), so they do not depend on
 // the clock the card runs at.
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -40,6 +41,28 @@ __global__ void gather(const double* __restrict__ E, const int* __restrict__ idx
     if (threadIdx.x == 0) cyc[blockIdx.x] = clock64() - t0;
     o[t] = s;
 }
+// one 8-byte field per lane (LDG.64), the load of a structure-of-arrays operand; how many lines an instruction touches is set by
+// the index pattern the host writes
+__global__ void gather8(const double* __restrict__ A, const int* __restrict__ idx, double* o, long long* cyc, int nPerThread, int stride) {
+    double s = 0;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    __syncthreads();
+    const long long t0 = clock64();
+    for (int k = 0; k < nPerThread; k += 4) {
+        int e[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) e[u] = idx[(size_t)(k + u) * stride + t];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            double a;
+            asm volatile("ld.global.f64 %0, [%1];" : "=d"(a) : "l"(A + e[u]));
+            s += a;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) cyc[blockIdx.x] = clock64() - t0;
+    o[t] = s;
+}
 static double mean_cycles(const long long* d, int n) {
     long long h[1024]; cudaMemcpy(h, d, 8 * n, cudaMemcpyDeviceToHost);
     double s = 0; for (int i = 0; i < n; ++i) s += (double)h[i];
@@ -68,6 +91,29 @@ int main() {
         const double clk = mean_cycles(cyc, blocks);
         printf("gather %s, %3d SMs x 512 thr: %.1f clk per warp-record-gather per SM\n", mode ? "16 B records, 1 x LDG.128" : "32 B records, 2 x LDG.128",
                blocks, clk / ((nt / 32) * (double)per));
+    }
+    // 8-byte fields of the same 2 MB as a double array: every warp instruction reads 32 random lines (each lane its own), the 2 lines
+    // of 32 consecutive doubles (dense SoA: lane i reads base + i), or the 4 lines of every other double (half density: base + 2 i)
+    const int nDbl = 4 * nRec;
+    const char* pat[3] = {"random, 32 lines", "dense SoA, 2 lines", "half density, 4 lines"};
+    for (int mode = 0; mode < 3; ++mode) {
+        for (size_t k = 0; k < (size_t)per; ++k)
+            for (int w = 0; w < total / 32; ++w) {
+                r = r * 1664525u + 1013904223u;
+                const int base = (int)((r >> 8) % (unsigned)(nDbl / 64)) * 64;   // 512-byte aligned
+                for (int l = 0; l < 32; ++l) {
+                    int v = base + (mode == 2 ? 2 * l : l);
+                    if (mode == 0) { r = r * 1664525u + 1013904223u; v = (int)((r >> 8) % (unsigned)nDbl); }
+                    h[k * total + 32 * w + l] = v;
+                }
+            }
+        cudaMemcpy(idx, h, 4 * (size_t)per * total, cudaMemcpyHostToDevice);
+        for (int blocks : {8, nsm}) {
+            gather8<<<blocks, nt>>>(E, idx, o, cyc, per, total); gather8<<<blocks, nt>>>(E, idx, o, cyc, per, total); cudaDeviceSynchronize();
+            const double clk = mean_cycles(cyc, blocks);
+            printf("gather 8 B field, 1 x LDG.64, %-22s %3d SMs x 512 thr: %.1f clk per warp-instruction per SM\n", pat[mode], blocks,
+                   clk / ((nt / 32) * (double)per));
+        }
     }
     printf("%s\n", cudaGetErrorString(cudaGetLastError()));
     return 0;
