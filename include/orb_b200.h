@@ -314,6 +314,29 @@ typedef struct OrbmTriFrame {
 } OrbmTriFrame;
 int orbm_search_for_triangulation(orbm_handle* h, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
                                   int nlevels, const float* ep2, const float* F12, int bCoarse, int checkOrientation, int32_t* matches12, int32_t* nmatches);
+/* LocalMapping::CreateNewMapPoints (src/LocalMapping.cc, the vpNeighKFs loop from :296; monocular keyframes) for ONE new keyframe KF1 against
+ * its nKF2 neighbours, in vpNeighKFs order: per neighbour ORBmatcher(0.6f, false).SearchForTriangulation (no rotation histogram), then per
+ * match the ray parallax test (cos < 0.9998, or < 0.9996 when bInertial), GeometricTools::Triangulate (4x4 SVD), positive depth and the
+ * reprojection test in both keyframes, the far-point cut (thFarPoints > 0) and the scale-consistency test.  A feature of KF1 that received a
+ * point from neighbour j is skipped by the searches of every later neighbour, as in the reference (the point was added to KF1).
+ * Caller's job: picking the neighbours, the baseline / median-depth skip, CheckNewKeyFrames, and the pointer graph (see INTEGRATION.md).
+ * Tcw [1 + nKF2][12]: GetPose().matrix3x4() row-major, KF1 first; Ow [1 + nKF2][3]: GetCameraCenter(); cam [1 + nKF2][4]: fx, fy, cx, cy.
+ * ep2, F12, scaleFactors, levelSigma2, nlevels, bCoarse: as in orbm_search_for_triangulation.  scaleFactor: mfScaleFactor of KF1. */
+typedef struct OrbmNewPointsIn {
+    const OrbmTriFrame* KF1; int nKF2; const OrbmTriFrame* KF2;
+    const float* ep2; const float* F12;
+    const float* scaleFactors; const float* levelSigma2; int nlevels;
+    const float* Tcw; const float* Ow; const float* cam;
+    float scaleFactor; int bCoarse; int bInertial; float thFarPoints;
+} OrbmNewPointsIn;
+/* One new map point, observed by KF1 at idx1 and by neighbour kf2 at idx2; normal / minDistance / maxDistance as
+ * MapPoint::UpdateNormalAndDepth sets them (reference keyframe KF1). */
+typedef struct OrbmNewPoint {
+    int32_t kf2, idx1, idx2; float x3D[3]; float normal[3]; float minDistance, maxDistance;
+} OrbmNewPoint;
+/* out [KF1.N]: the new points in the order the reference creates them ((neighbour, idx1) ascending), *nNew of them.  nmatches [nKF2]: the
+ * reference's vMatchedIndices.size() per neighbour; ncreated [nKF2]: points created from each neighbour.  Host pointers; 3 launches. */
+int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNewPoint* out, int* nNew, int32_t* nmatches, int32_t* ncreated);
 /* void MapPoint::ComputeDistinctiveDescriptors() (src/MapPoint.cc:329-403) for nPoints map points at once (LocalMapping::ProcessNewKeyFrame /
  * CreateNewMapPoints call it per point): the observed descriptors of point p are rows obsStart[p] .. obsStart[p+1] of `descriptors`;
  * best[p] = row (relative to obsStart[p]) with the least median Hamming distance to the others, -1 for a point without observations. */

@@ -18,6 +18,24 @@ ORB_OK, ORB_ERR_EMPTY, ORB_ERR_ARG, ORB_ERR_CAPACITY, ORB_ERR_CUDA, ORB_ERR_ASPE
 #: numpy view of OrbKeyPoint / cv::KeyPoint (28 bytes)
 KP_DTYPE = np.dtype([('x', 'f4'), ('y', 'f4'), ('size', 'f4'), ('angle', 'f4'), ('response', 'f4'),
                      ('octave', 'i4'), ('class_id', 'i4')])
+#: numpy view of OrbmNewPoint (44 bytes): one map point made by LocalMapping::CreateNewMapPoints
+NEW_POINT_DTYPE = np.dtype([('kf2', 'i4'), ('idx1', 'i4'), ('idx2', 'i4'), ('x3D', 'f4', 3), ('normal', 'f4', 3), ('minDistance', 'f4'),
+                            ('maxDistance', 'f4')])
+assert NEW_POINT_DTYPE.itemsize == 44
+
+
+class OrbmTriFrame(C.Structure):
+    """A keyframe for the triangulation search (include/orb_b200.h)."""
+    _fields_ = [('N', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('hasMapPoint', C.c_void_p), ('nEntries', C.c_int),
+                ('fvNode', C.c_void_p), ('fvFeature', C.c_void_p)]
+
+
+class OrbmNewPointsIn(C.Structure):
+    """Input of orbm_create_new_map_points (include/orb_b200.h)."""
+    _fields_ = [('KF1', C.POINTER(OrbmTriFrame)), ('nKF2', C.c_int), ('KF2', C.POINTER(OrbmTriFrame)), ('ep2', C.c_void_p), ('F12', C.c_void_p),
+                ('scaleFactors', C.c_void_p), ('levelSigma2', C.c_void_p), ('nlevels', C.c_int), ('Tcw', C.c_void_p), ('Ow', C.c_void_p),
+                ('cam', C.c_void_p), ('scaleFactor', C.c_float), ('bCoarse', C.c_int), ('bInertial', C.c_int), ('thFarPoints', C.c_float)]
+
 
 _lib = None
 
@@ -587,6 +605,38 @@ class ORBmatcher:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_for_triangulation')
         return nm, m12
+
+    def CreateNewMapPoints(self, kf1, kf2_list, scale_factors, level_sigma2, ep, F12, Tcw, Ow, cam, scale_factor, coarse=False, inertial=False,
+                           th_far_points=0.0):
+        """``LocalMapping::CreateNewMapPoints`` (src/LocalMapping.cc, the vpNeighKFs loop from :296; monocular keyframes) after the neighbour
+        selection: the new map points of keyframe ``kf1`` triangulated against the neighbours ``kf2_list`` (in vpNeighKFs order), exactly as
+        the reference's loop creates them.  Keyframes as in :meth:`SearchForTriangulation`; ``Tcw`` [1 + n, 3, 4] (KF1 first), ``Ow`` [1 + n, 3],
+        ``cam`` [1 + n, 4]; ``th_far_points`` 0 = off.  Returns (records, nmatches [n], ncreated [n]): ``records`` is a ``NEW_POINT_DTYPE``
+        array in creation order.  The matcher's own settings are not used: the reference builds ``ORBmatcher(0.6f, false)`` here."""
+        keep = []
+
+        def mk(kf):
+            a = [_c(kf['kps'], KP_DTYPE), _c(kf['desc'], np.uint8), _c(kf['has_mp'], np.uint8), _c(kf['fv'][0], np.int32), _c(kf['fv'][1], np.int32)]
+            keep.append(a)
+            return OrbmTriFrame(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[3]), a[3].ctypes.data, a[4].ctypes.data)
+        f1 = mk(kf1)
+        n2 = len(kf2_list)
+        f2 = (OrbmTriFrame * max(n2, 1))(*[mk(k) for k in kf2_list])
+        arrs = [_c(scale_factors, np.float32), _c(level_sigma2, np.float32), _c(ep, np.float32).reshape(-1, 2), _c(F12, np.float32).reshape(-1, 9),
+                _c(Tcw, np.float32).reshape(-1, 12), _c(Ow, np.float32).reshape(-1, 3), _c(cam, np.float32).reshape(-1, 4)]
+        assert len(arrs[4]) == len(arrs[5]) == len(arrs[6]) == n2 + 1 and len(arrs[2]) == len(arrs[3]) == n2
+        inp = OrbmNewPointsIn(C.pointer(f1), n2, C.cast(f2, C.POINTER(OrbmTriFrame)), arrs[2].ctypes.data, arrs[3].ctypes.data, arrs[0].ctypes.data,
+                              arrs[1].ctypes.data, len(arrs[0]), arrs[4].ctypes.data, arrs[5].ctypes.data, arrs[6].ctypes.data, float(scale_factor),
+                              int(coarse), int(inertial), float(th_far_points))
+        out = np.zeros(max(f1.N, 1), NEW_POINT_DTYPE)
+        nm, nc = np.zeros(n2, np.int32), np.zeros(n2, np.int32)
+        n = C.c_int(0)
+        L = lib()
+        L.orbm_create_new_map_points.argtypes = [C.c_void_p] * 6
+        rc = L.orbm_create_new_map_points(self._h, C.byref(inp), _ptr(out), C.byref(n), _ptr(nm), _ptr(nc))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_create_new_map_points')
+        return out[:n.value].copy(), nm, nc
 
     def ComputeDistinctiveDescriptors(self, obs_list):
         """``MapPoint::ComputeDistinctiveDescriptors`` for a list of map points (each an [n, 32] u8 array of observed descriptors): index of the chosen row."""

@@ -14,6 +14,7 @@
 //           the current claim state.  Claims live in a shared-memory bitset.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
+#include <float.h>
 #include <math.h>
 #include <string.h>
 #include <string>
@@ -940,6 +941,259 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams Q) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// LocalMapping::CreateNewMapPoints (src/LocalMapping.cc, the vpNeighKFs loop from :296; monocular keyframes) after the search:
+// new_points_kernel checks one (neighbour k, idx1) match per thread -- ray parallax, GeometricTools::Triangulate (Eigen's two-sided
+// Jacobi SVD of the 4x4 in registers), depth, reprojection, far points, scale -- and fills the record MapPoint::UpdateNormalAndDepth gives.
+// new_points_commit_kernel applies the sequential rule (DESIGN.md section 4): the point of idx1 comes from the first k whose match
+// passes, and a match of a later neighbour at that idx1 is one the reference never sees.  Every rounding and contraction is the
+// oracle's (oracle/mapping_oracle.cpp), which documents the evaluation order.
+// ---------------------------------------------------------------------------------------------
+enum : uint8_t { NP_NO_MATCH = 0, NP_LOW_PARALLAX, NP_SVD_W0, NP_DEPTH1, NP_DEPTH2, NP_REPROJ1, NP_REPROJ2, NP_ZERO_DIST, NP_FAR, NP_SCALE, NP_CREATED };
+constexpr int NP_MAX_SWEEPS = 64;       // Eigen has no limit; a float 4x4 converges in a handful of sweeps (oracle)
+constexpr int NP_NT = 128, NPC_NT = 1024;
+
+struct NewPointsParams {
+    int N1, nKF2, nlevels, bInertial;
+    float ratioFactor, thFar;
+    const OrbKeyPoint* kps1; const TriPair* pairs; const int* matches12;     // [nKF2][N1]
+    const float *scaleFactors, *levelSigma2, *Tcw, *Ow, *cam;                // Tcw / Ow / cam: [1 + nKF2] keyframes, KF1 first
+    uint8_t* reason; OrbmNewPoint* recs; int* winner;                        // [nKF2][N1], [nKF2][N1], [N1]
+    int* counts; OrbmNewPoint* out;                                          // nNew, nmatches [nKF2], ncreated [nKF2]; out [N1]
+};
+
+struct NpRot { float c, s; };
+__device__ __forceinline__ float fmaxe(float a, float b) { return a < b ? b : a; }   // std::max
+__device__ __forceinline__ NpRot np_make_jacobi(float x, float y, float z) {           // Eigen JacobiRotation::makeJacobi (real)
+    const float deno = fmul(2.0f, fabsf(y));
+    if (deno < FLT_MIN) return {1.0f, 0.0f};
+    const float tau = fdiv(fsub(x, z), deno);
+    const float w = __fsqrt_rn(fadd(fmul(tau, tau), 1.0f));
+    const float t = tau > 0.0f ? fdiv(1.0f, fadd(tau, w)) : fdiv(1.0f, fsub(tau, w));
+    const float sign_t = t > 0.0f ? 1.0f : -1.0f;
+    const float n = fdiv(1.0f, __fsqrt_rn(fadd(fmul(t, t), 1.0f)));
+    return {n, fmul(fmul(fmul(-sign_t, fdiv(y, fabsf(y))), fabsf(t)), n)};
+}
+template <int P, int Q> __device__ __forceinline__ void np_rot_rows(float (&W)[4][4], NpRot j) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float x = W[P][i], y = W[Q][i];
+        W[P][i] = fadd(fmul(j.c, x), fmul(j.s, y)); W[Q][i] = fadd(fmul(-j.s, x), fmul(j.c, y));
+    }
+}
+template <int P, int Q> __device__ __forceinline__ void np_rot_cols(float (&W)[4][4], NpRot j) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float x = W[i][P], y = W[i][Q];
+        W[i][P] = fadd(fmul(j.c, x), fmul(j.s, y)); W[i][Q] = fadd(fmul(-j.s, x), fmul(j.c, y));
+    }
+}
+// One pair (p, q) of a Jacobi sweep (JacobiSVD::compute + real_2x2_jacobi_svd).
+template <int P, int Q> __device__ __forceinline__ void np_jacobi_pair(float (&W)[4][4], float (&V)[4][4], float& maxDiag, bool& finished) {
+    const float threshold = fmaxe(FLT_MIN, fmul(2.0f * FLT_EPSILON, maxDiag));
+    if (!(fabsf(W[P][Q]) > threshold || fabsf(W[Q][P]) > threshold)) return;
+    finished = false;
+    const float m00 = W[P][P], m01 = W[P][Q], m10 = W[Q][P], m11 = W[Q][Q];
+    NpRot r1;
+    const float t = fadd(m00, m11), d = fsub(m10, m01);
+    if (fabsf(d) < FLT_MIN) r1 = {1.0f, 0.0f};
+    else {
+        const float u = fdiv(t, d);
+        const float tmp = __fsqrt_rn(fadd(1.0f, fmul(u, u)));
+        r1 = {fdiv(u, tmp), fdiv(1.0f, tmp)};
+    }
+    const float n00 = fadd(fmul(r1.c, m00), fmul(r1.s, m10)), n01 = fadd(fmul(r1.c, m01), fmul(r1.s, m11));
+    const float n11 = fadd(fmul(-r1.s, m01), fmul(r1.c, m11));
+    const NpRot jr = np_make_jacobi(n00, n01, n11);
+    const NpRot jrt = {jr.c, -jr.s};
+    const NpRot jl = {fsub(fmul(r1.c, jrt.c), fmul(r1.s, jrt.s)), fadd(fmul(r1.c, jrt.s), fmul(r1.s, jrt.c))};
+    np_rot_rows<P, Q>(W, jl);
+    np_rot_cols<P, Q>(W, jrt);
+    np_rot_cols<P, Q>(V, jrt);
+    maxDiag = fmaxe(maxDiag, fmaxe(fabsf(W[P][P]), fabsf(W[Q][Q])));
+}
+// GeometricTools::Triangulate: false when V(3, 3) of the smallest singular value is 0.
+__device__ __forceinline__ bool np_triangulate(float x1, float y1, float x2, float y2, const float* T1, const float* T2, float* x3D) {
+    float W[4][4], V[4][4];
+    float scale = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        W[0][j] = fsub(fmul(x1, T1[8 + j]), T1[j]);
+        W[1][j] = fsub(fmul(y1, T1[8 + j]), T1[4 + j]);
+        W[2][j] = fsub(fmul(x2, T2[8 + j]), T2[j]);
+        W[3][j] = fsub(fmul(y2, T2[8 + j]), T2[4 + j]);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) scale = fmaxe(scale, fabsf(W[i][j]));
+    if (scale == 0.0f) scale = 1.0f;
+    float maxDiag = 0.0f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { W[i][j] = fdiv(W[i][j], scale); V[i][j] = i == j ? 1.0f : 0.0f; }
+        maxDiag = fmaxe(maxDiag, fabsf(W[i][i]));
+    }
+    bool finished = false;
+    for (int sweep = 0; !finished && sweep < NP_MAX_SWEEPS; ++sweep) {
+        finished = true;
+        np_jacobi_pair<1, 0>(W, V, maxDiag, finished);
+        np_jacobi_pair<2, 0>(W, V, maxDiag, finished);
+        np_jacobi_pair<2, 1>(W, V, maxDiag, finished);
+        np_jacobi_pair<3, 0>(W, V, maxDiag, finished);
+        np_jacobi_pair<3, 1>(W, V, maxDiag, finished);
+        np_jacobi_pair<3, 2>(W, V, maxDiag, finished);
+    }
+    // sort the singular values in decreasing order (first maximum wins); only the permutation of V's columns is kept
+    float s[4];
+    int perm[4] = {0, 1, 2, 3};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) s[i] = fabsf(W[i][i]);
+    bool stop = false;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        int pos = i;
+#pragma unroll
+        for (int k = i + 1; k < 4; ++k) {
+            float sp = s[i];
+#pragma unroll
+            for (int l = i + 1; l < 4; ++l) if (l == pos) sp = s[l];
+            if (s[k] > sp) pos = k;
+        }
+        float smax = s[i];
+#pragma unroll
+        for (int l = i + 1; l < 4; ++l) if (l == pos) smax = s[l];
+        stop = stop || smax == 0.0f;
+        if (!stop) {
+#pragma unroll
+            for (int l = i + 1; l < 4; ++l)
+                if (l == pos) { const float ts = s[i]; s[i] = s[l]; s[l] = ts; const int tp = perm[i]; perm[i] = perm[l]; perm[l] = tp; }
+        }
+    }
+    float v[4] = {V[0][0], V[1][0], V[2][0], V[3][0]};
+#pragma unroll
+    for (int c = 1; c < 4; ++c)
+        if (perm[3] == c) { v[0] = V[0][c]; v[1] = V[1][c]; v[2] = V[2][c]; v[3] = V[3][c]; }
+    if (v[3] == 0.0f) return false;
+    x3D[0] = fdiv(v[0], v[3]); x3D[1] = fdiv(v[1], v[3]); x3D[2] = fdiv(v[2], v[3]);
+    return true;
+}
+
+__device__ __forceinline__ float np_row(const float* T, int r, const float* x) {
+    return fadd(fadd(fadd(fmul(T[4 * r], x[0]), fmul(T[4 * r + 1], x[1])), fmul(T[4 * r + 2], x[2])), T[4 * r + 3]);
+}
+__device__ __forceinline__ float np_norm(const float* a) { return __fsqrt_rn(fadd(fadd(fmul(a[0], a[0]), fmul(a[1], a[1])), fmul(a[2], a[2]))); }
+
+__global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
+    const int idx1 = blockIdx.x * NP_NT + threadIdx.x, k = blockIdx.y;
+    if (idx1 >= P.N1) return;
+    const size_t slot = (size_t)k * P.N1 + idx1;
+    const int idx2 = P.matches12[slot];
+    uint8_t why = NP_NO_MATCH;
+    if (idx2 >= 0) {
+        const OrbKeyPoint kp1 = P.kps1[idx1], kp2 = P.pairs[k].kps2[idx2];
+        float T1[12], T2[12], O1[3], O2[3], c1[4], c2[4];
+#pragma unroll
+        for (int i = 0; i < 12; ++i) { T1[i] = P.Tcw[i]; T2[i] = P.Tcw[12 * (k + 1) + i]; }
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { O1[i] = P.Ow[i]; O2[i] = P.Ow[3 * (k + 1) + i]; }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { c1[i] = P.cam[i]; c2[i] = P.cam[4 * (k + 1) + i]; }
+        const float xn1[3] = {fdiv(fsub(kp1.x, c1[2]), c1[0]), fdiv(fsub(kp1.y, c1[3]), c1[1]), 1.0f};
+        const float xn2[3] = {fdiv(fsub(kp2.x, c2[2]), c2[0]), fdiv(fsub(kp2.y, c2[3]), c2[1]), 1.0f};
+        float ray1[3], ray2[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            ray1[i] = fadd(fadd(fmul(T1[i], xn1[0]), fmul(T1[4 + i], xn1[1])), fmul(T1[8 + i], xn1[2]));
+            ray2[i] = fadd(fadd(fmul(T2[i], xn2[0]), fmul(T2[4 + i], xn2[1])), fmul(T2[8 + i], xn2[2]));
+        }
+        const float dot = fadd(fadd(fmul(ray1[0], ray2[0]), fmul(ray1[1], ray2[1])), fmul(ray1[2], ray2[2]));
+        const float cp = fdiv(dot, fmul(np_norm(ray1), np_norm(ray2)));
+        float x3D[3];
+        if (!(cp < fadd(cp, 1.0f) && cp > 0.0f && ((P.bInertial && (double)cp < 0.9996) || (!P.bInertial && (double)cp < 0.9998)))) why = NP_LOW_PARALLAX;
+        else if (!np_triangulate(xn1[0], xn1[1], xn2[0], xn2[1], T1, T2, x3D)) why = NP_SVD_W0;
+        else {
+            const float z1 = np_row(T1, 2, x3D), z2 = np_row(T2, 2, x3D);
+            const float u1 = fadd(fdiv(fmul(c1[0], np_row(T1, 0, x3D)), z1), c1[2]), v1 = fadd(fdiv(fmul(c1[1], np_row(T1, 1, x3D)), z1), c1[3]);
+            const float ex1 = fsub(u1, kp1.x), ey1 = fsub(v1, kp1.y);
+            const float u2 = fadd(fdiv(fmul(c2[0], np_row(T2, 0, x3D)), z2), c2[2]), v2 = fadd(fdiv(fmul(c2[1], np_row(T2, 1, x3D)), z2), c2[3]);
+            const float ex2 = fsub(u2, kp2.x), ey2 = fsub(v2, kp2.y);
+            const float nv1[3] = {fsub(x3D[0], O1[0]), fsub(x3D[1], O1[1]), fsub(x3D[2], O1[2])};
+            const float nv2[3] = {fsub(x3D[0], O2[0]), fsub(x3D[1], O2[1]), fsub(x3D[2], O2[2])};
+            const float dist1 = np_norm(nv1), dist2 = np_norm(nv2);
+            const float sf1 = P.scaleFactors[kp1.octave];
+            if (z1 <= 0.0f) why = NP_DEPTH1;
+            else if (z2 <= 0.0f) why = NP_DEPTH2;
+            else if ((double)__fmaf_rn(ex1, ex1, fmul(ey1, ey1)) > 5.991 * (double)P.levelSigma2[kp1.octave]) why = NP_REPROJ1;   // one FMA, see oracle
+            else if ((double)__fmaf_rn(ex2, ex2, fmul(ey2, ey2)) > 5.991 * (double)P.levelSigma2[kp2.octave]) why = NP_REPROJ2;
+            else if (dist1 == 0.0f || dist2 == 0.0f) why = NP_ZERO_DIST;
+            else if (P.thFar > 0.0f && (dist1 >= P.thFar || dist2 >= P.thFar)) why = NP_FAR;
+            else {
+                const float ratioDist = fdiv(dist2, dist1), ratioOctave = fdiv(sf1, P.scaleFactors[kp2.octave]);
+                if (fmul(ratioDist, P.ratioFactor) < ratioOctave || ratioDist > fmul(ratioOctave, P.ratioFactor)) why = NP_SCALE;
+                else {
+                    why = NP_CREATED;
+                    OrbmNewPoint r;
+                    r.kf2 = k; r.idx1 = idx1; r.idx2 = idx2;
+#pragma unroll
+                    for (int i = 0; i < 3; ++i) { r.x3D[i] = x3D[i]; r.normal[i] = fdiv(fadd(fadd(0.0f, fdiv(nv1[i], dist1)), fdiv(nv2[i], dist2)), 2.0f); }
+                    r.maxDistance = fmul(dist1, sf1);
+                    r.minDistance = fdiv(r.maxDistance, P.scaleFactors[P.nlevels - 1]);
+                    P.recs[slot] = r;
+                }
+            }
+        }
+    }
+    P.reason[slot] = why;
+}
+
+// One CTA: winner[idx1] = first neighbour that created idx1's point; then per neighbour, in order, the counts and the records compacted in
+// idx1 order (thread t owns a contiguous run of idx1, a block scan gives each run its place).
+__global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsParams P) {
+    __shared__ int s_scan[NPC_NT / 32], s_msum[NPC_NT / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, N1 = P.N1, K = P.nKF2;
+    for (int i = tid; i < N1; i += NPC_NT) {
+        int w = -1;
+        for (int k = 0; k < K && w < 0; ++k) if (P.reason[(size_t)k * N1 + i] == NP_CREATED) w = k;
+        P.winner[i] = w;
+    }
+    __syncthreads();
+    const int per = (N1 + NPC_NT - 1) / NPC_NT, i0 = min(N1, tid * per), i1 = min(N1, i0 + per);
+    int base = 0;
+    for (int k = 0; k < K; ++k) {
+        int c = 0, mt = 0;
+        for (int i = i0; i < i1; ++i) {
+            const int w = P.winner[i];
+            c += w == k;
+            mt += P.matches12[(size_t)k * N1 + i] >= 0 && (w < 0 || w >= k);     // the reference's search skips idx1 once an earlier k made its point
+        }
+        int incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+        const int msum = __reduce_add_sync(0xffffffffu, mt);
+        if (lane == 31) s_scan[wid] = incl;
+        if (lane == 0) s_msum[wid] = msum;
+        __syncthreads();
+        if (wid == 0) {
+            int v = s_scan[lane], m = s_msum[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+            m = __reduce_add_sync(0xffffffffu, m);
+            s_scan[lane] = v;                                   // inclusive over warps
+            if (lane == 0) s_msum[0] = m;
+        }
+        __syncthreads();
+        int pos = base + (wid ? s_scan[wid - 1] : 0) + incl - c;
+        for (int i = i0; i < i1; ++i) if (P.winner[i] == k) P.out[pos++] = P.recs[(size_t)k * N1 + i];
+        const int created = s_scan[NPC_NT / 32 - 1];
+        if (tid == 0) { P.counts[1 + k] = s_msum[0]; P.counts[1 + K + k] = created; }
+        base += created;
+        __syncthreads();
+    }
+    if (tid == 0) P.counts[0] = base;
+}
+
+// ---------------------------------------------------------------------------------------------
 // MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:329-403) for a batch of map points: warp per map point, lane per observation row;
 // the row's median distance (element (int)(0.5 (n - 1)) of the sorted row) by bisection on the distance value; first minimum wins.
 // ---------------------------------------------------------------------------------------------
@@ -1019,6 +1273,7 @@ struct Matcher {
     uint8_t* d_arena = nullptr; size_t arenaBytes = 0;
     uint8_t* h_arena = nullptr;
     uint8_t* d_batch = nullptr; size_t batchBytes = 0;   // device staging for the host-pointer batch entry point
+    uint8_t* h_tri = nullptr; size_t hTriBytes = 0;      // pinned host mirror of d_batch for the triangulation entry points
     int launches = 0;
 
     ~Matcher() {
@@ -1026,6 +1281,7 @@ struct Matcher {
         void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_arena, d_batch};
         for (void* p : ptrs) if (p) cudaFree(p);
         if (h_arena) cudaFreeHost(h_arena);
+        if (h_tri) cudaFreeHost(h_tri);
         if (evWait) cudaEventDestroy(evWait);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -1546,6 +1802,80 @@ static bool tri_frame_ok(const OrbmTriFrame* f) {
     for (int e = 0; e < f->nEntries; ++e) if (f->fvFeature[e] < 0 || f->fvFeature[e] >= f->N || (e && f->fvNode[e] < f->fvNode[e - 1])) return false;
     return true;
 }
+// Staging of one SearchForTriangulation call (KF1 against nKF2 neighbours), shared by orbm_search_for_triangulation and
+// orbm_create_new_map_points.  Device (and pinned host mirror) layout, 256-byte aligned pieces:
+//   inputs: level tables | KF1 | per pair: KF2 arrays | the caller's extra inputs | pair table
+//   outputs: nmatches [nKF2] | matches12 [nKF2][N1] | evBin [nKF2][N1] | the caller's extra outputs
+// The inputs go up in ONE copy, then tri_match_kernel runs on the handle's stream.
+struct TriExtra { const void* src; size_t bytes; };
+struct TriStage {
+    uint8_t *d, *h;                     // device base, pinned host mirror
+    size_t oCnt, oM12, oOut;            // nmatches, matches12, the caller's outputs
+    size_t extraIn[4];                  // offsets of the caller's extra inputs
+    TriParams Q;
+};
+static int tri_search_launch(Matcher& m, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
+                             int nlevels, const float* ep2, const float* F12, int bCoarse, int checkOrientation, int nExtra, const TriExtra* extra,
+                             size_t outBytes, TriStage* S) {
+    const size_t N1 = (size_t)KF1->N, E1 = (size_t)KF1->nEntries;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
+    const size_t oSf = take(4 * (size_t)nlevels), oSg = take(4 * (size_t)nlevels);
+    const size_t oK1 = take(N1 * sizeof(OrbKeyPoint)), oD1 = take(N1 * 32), oM1 = take(N1), oN1 = take(4 * E1), oF1 = take(4 * E1);
+    struct Off { size_t kp, de, mp, fn, ff; };
+    std::vector<Off> po(nKF2);
+    for (int k = 0; k < nKF2; ++k) {
+        const size_t N2 = (size_t)KF2[k].N, E2 = (size_t)KF2[k].nEntries;
+        po[k] = {take(N2 * sizeof(OrbKeyPoint)), take(N2 * 32), take(N2), take(4 * E2), take(4 * E2)};
+    }
+    for (int e = 0; e < nExtra; ++e) S->extraIn[e] = take(extra[e].bytes);
+    const size_t oTab = take(sizeof(TriPair) * (size_t)nKF2);
+    const size_t inBytes = off;
+    S->oCnt = take(4 * (size_t)nKF2); S->oM12 = take(4 * N1 * nKF2);
+    const size_t oEv = take(N1 * nKF2);
+    S->oOut = take(outBytes);
+    if (off > m.batchBytes) {                                   // grow the device staging
+        if (m.d_batch) cudaFree(m.d_batch);
+        m.d_batch = nullptr; m.batchBytes = 0;
+        CK(cudaMalloc(&m.d_batch, off));
+        m.batchBytes = off;
+    }
+    if (off > m.hTriBytes) {                                    // every call ends with a stream synchronise, so the old buffer is idle
+        if (m.h_tri) cudaFreeHost(m.h_tri);
+        m.h_tri = nullptr; m.hTriBytes = 0;
+        CK(cudaMallocHost(&m.h_tri, off));
+        m.hTriBytes = off;
+    }
+    uint8_t *d = m.d_batch, *hb = m.h_tri;
+    S->d = d; S->h = hb;
+    auto put = [&](size_t o, const void* src, size_t bytes) { if (bytes) memcpy(hb + o, src, bytes); };
+    put(oSf, scaleFactors, 4 * (size_t)nlevels); put(oSg, levelSigma2, 4 * (size_t)nlevels);
+    put(oK1, KF1->keypoints, N1 * sizeof(OrbKeyPoint)); put(oD1, KF1->descriptors, N1 * 32); put(oM1, KF1->hasMapPoint, N1);
+    put(oN1, KF1->fvNode, 4 * E1); put(oF1, KF1->fvFeature, 4 * E1);
+    TriPair* tab = (TriPair*)(hb + oTab);
+    for (int k = 0; k < nKF2; ++k) {
+        const size_t N2 = (size_t)KF2[k].N, E2 = (size_t)KF2[k].nEntries;
+        put(po[k].kp, KF2[k].keypoints, N2 * sizeof(OrbKeyPoint)); put(po[k].de, KF2[k].descriptors, N2 * 32); put(po[k].mp, KF2[k].hasMapPoint, N2);
+        put(po[k].fn, KF2[k].fvNode, 4 * E2); put(po[k].ff, KF2[k].fvFeature, 4 * E2);
+        TriPair T; memset(&T, 0, sizeof(T));
+        T.N2 = (int)N2; T.E2 = (int)E2;
+        T.kps2 = (const OrbKeyPoint*)(d + po[k].kp); T.desc2 = d + po[k].de; T.hasMP2 = d + po[k].mp; T.fvNode2 = (const int*)(d + po[k].fn); T.fvFeat2 = (const int*)(d + po[k].ff);
+        memcpy(T.ep, ep2 + 2 * (size_t)k, 8); memcpy(T.F12, F12 + 9 * (size_t)k, 36);
+        T.matches12 = (int*)(d + S->oM12) + (size_t)k * N1; T.nmatches = (int*)(d + S->oCnt) + k; T.evBin = d + oEv + (size_t)k * N1;
+        memcpy(tab + k, &T, sizeof(T));
+    }
+    for (int e = 0; e < nExtra; ++e) put(S->extraIn[e], extra[e].src, extra[e].bytes);
+    cudaStream_t st = m.stream;
+    CK(cudaMemcpyAsync(d, hb, inBytes, cudaMemcpyHostToDevice, st));
+    TriParams& Q = S->Q; memset(&Q, 0, sizeof(Q));
+    Q.N1 = (int)N1; Q.E1 = (int)E1; Q.coarse = bCoarse; Q.checkOri = checkOrientation;
+    Q.kps1 = (const OrbKeyPoint*)(d + oK1); Q.desc1 = d + oD1; Q.hasMP1 = d + oM1; Q.fvNode1 = (const int*)(d + oN1); Q.fvFeat1 = (const int*)(d + oF1);
+    Q.scaleFactors = (const float*)(d + oSf); Q.levelSigma2 = (const float*)(d + oSg); Q.pairs = (const TriPair*)(d + oTab);
+    tri_match_kernel<<<nKF2, TM_NT, 0, st>>>(Q);
+    CK(cudaGetLastError());
+    return ORB_OK;
+}
+
 int orbm_search_for_triangulation(orbm_handle* h, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
                                   int nlevels, const float* ep2, const float* F12, int bCoarse, int checkOrientation, int32_t* matches12, int32_t* nmatches) {
     if (!h || nKF2 < 0 || !tri_frame_ok(KF1) || (nKF2 && (!KF2 || !ep2 || !F12 || !matches12 || !nmatches)) || !scaleFactors || !levelSigma2 || nlevels < 1 || nlevels > 256) {
@@ -1558,57 +1888,70 @@ int orbm_search_for_triangulation(orbm_handle* h, const OrbmTriFrame* KF1, int n
     if (nKF2 == 0) return ORB_OK;
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
-    const size_t N1 = (size_t)KF1->N, E1 = (size_t)KF1->nEntries;
+    const size_t N1 = (size_t)KF1->N;
     for (size_t i = 0; i < (size_t)nKF2 * N1; ++i) matches12[i] = -1;
     for (int k = 0; k < nKF2; ++k) nmatches[k] = 0;
     if (N1 == 0) return ORB_OK;
-    // one staging buffer: tables | KF1 | per pair: KF2 arrays, outputs | pair table
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-    const size_t oSf = take(4 * (size_t)nlevels), oSg = take(4 * (size_t)nlevels);
-    const size_t oK1 = take(N1 * sizeof(OrbKeyPoint)), oD1 = take(N1 * 32), oM1 = take(N1), oN1 = take(4 * E1), oF1 = take(4 * E1);
-    struct Off { size_t kp, de, mp, fn, ff, out, ev; };
-    std::vector<Off> po(nKF2);
-    for (int k = 0; k < nKF2; ++k) {
-        const size_t N2 = (size_t)KF2[k].N, E2 = (size_t)KF2[k].nEntries;
-        po[k] = {take(N2 * sizeof(OrbKeyPoint)), take(N2 * 32), take(N2), take(4 * E2), take(4 * E2), take(4 * N1), take(N1)};
-    }
-    const size_t oCnt = take(4 * (size_t)nKF2), oTab = take(sizeof(TriPair) * (size_t)nKF2);
-    if (off > m.batchBytes) {                                   // grow the device staging (mapping-side call: pageable copies are fine)
-        if (m.d_batch) cudaFree(m.d_batch);
-        m.d_batch = nullptr; m.batchBytes = 0;
-        CK(cudaMalloc(&m.d_batch, off));
-        m.batchBytes = off;
-    }
-    uint8_t* d = m.d_batch;
-    cudaStream_t st = m.stream;
-    auto up = [&](size_t o, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess; };
-    CK(up(oSf, scaleFactors, 4 * (size_t)nlevels)); CK(up(oSg, levelSigma2, 4 * (size_t)nlevels));
-    CK(up(oK1, KF1->keypoints, N1 * sizeof(OrbKeyPoint))); CK(up(oD1, KF1->descriptors, N1 * 32)); CK(up(oM1, KF1->hasMapPoint, N1));
-    CK(up(oN1, KF1->fvNode, 4 * E1)); CK(up(oF1, KF1->fvFeature, 4 * E1));
-    std::vector<TriPair> tab(nKF2);
-    for (int k = 0; k < nKF2; ++k) {
-        const size_t N2 = (size_t)KF2[k].N, E2 = (size_t)KF2[k].nEntries;
-        CK(up(po[k].kp, KF2[k].keypoints, N2 * sizeof(OrbKeyPoint))); CK(up(po[k].de, KF2[k].descriptors, N2 * 32)); CK(up(po[k].mp, KF2[k].hasMapPoint, N2));
-        CK(up(po[k].fn, KF2[k].fvNode, 4 * E2)); CK(up(po[k].ff, KF2[k].fvFeature, 4 * E2));
-        TriPair& T = tab[k];
-        T.N2 = (int)N2; T.E2 = (int)E2;
-        T.kps2 = (const OrbKeyPoint*)(d + po[k].kp); T.desc2 = d + po[k].de; T.hasMP2 = d + po[k].mp; T.fvNode2 = (const int*)(d + po[k].fn); T.fvFeat2 = (const int*)(d + po[k].ff);
-        memcpy(T.ep, ep2 + 2 * (size_t)k, 8); memcpy(T.F12, F12 + 9 * (size_t)k, 36);
-        T.matches12 = (int*)(d + po[k].out); T.nmatches = (int*)(d + oCnt) + k; T.evBin = d + po[k].ev;
-    }
-    CK(cudaMemcpyAsync(d + oTab, tab.data(), sizeof(TriPair) * (size_t)nKF2, cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));                              // `tab` is pageable host memory: the copy must be done before it goes out of scope
-    TriParams Q; memset(&Q, 0, sizeof(Q));
-    Q.N1 = (int)N1; Q.E1 = (int)E1; Q.coarse = bCoarse; Q.checkOri = checkOrientation;
-    Q.kps1 = (const OrbKeyPoint*)(d + oK1); Q.desc1 = d + oD1; Q.hasMP1 = d + oM1; Q.fvNode1 = (const int*)(d + oN1); Q.fvFeat1 = (const int*)(d + oF1);
-    Q.scaleFactors = (const float*)(d + oSf); Q.levelSigma2 = (const float*)(d + oSg); Q.pairs = (const TriPair*)(d + oTab);
-    tri_match_kernel<<<nKF2, TM_NT, 0, st>>>(Q);
+    TriStage S;
+    const int rc = tri_search_launch(m, KF1, nKF2, KF2, scaleFactors, levelSigma2, nlevels, ep2, F12, bCoarse, checkOrientation, 0, nullptr, 0, &S);
+    if (rc) return rc;
     m.launches = 1;
-    CK(cudaGetLastError());
-    for (int k = 0; k < nKF2; ++k) CK(cudaMemcpyAsync(matches12 + (size_t)k * N1, d + po[k].out, 4 * N1, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(nmatches, d + oCnt, 4 * (size_t)nKF2, cudaMemcpyDeviceToHost, st));
+    cudaStream_t st = m.stream;
+    CK(cudaMemcpyAsync(S.h + S.oCnt, S.d + S.oCnt, S.oM12 - S.oCnt + 4 * N1 * nKF2, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    memcpy(nmatches, S.h + S.oCnt, 4 * (size_t)nKF2);
+    memcpy(matches12, S.h + S.oM12, 4 * N1 * nKF2);
+    return ORB_OK;
+}
+
+int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNewPoint* out, int* nNew, int32_t* nmatches, int32_t* ncreated) {
+    if (!h || !in || !nNew || in->nKF2 < 0 || !tri_frame_ok(in->KF1) || (in->KF1->N && !out) ||
+        (in->nKF2 && (!in->KF2 || !in->ep2 || !in->F12 || !nmatches || !ncreated)) || !in->scaleFactors || !in->levelSigma2 || in->nlevels < 1 ||
+        in->nlevels > 256 || !in->Tcw || !in->Ow || !in->cam || !(in->scaleFactor > 0.0f) || !(in->thFarPoints >= 0.0f)) {
+        set_error("orbm_create_new_map_points: bad argument (feature vectors must be sorted by node id, indices in range; Tcw / Ow / cam for 1 + nKF2 keyframes)");
+        return ORB_ERR_ARG;
+    }
+    const OrbmTriFrame* KF1 = in->KF1;
+    const int nKF2 = in->nKF2, nl = in->nlevels;
+    for (int i = 0; i < KF1->N; ++i) if (KF1->keypoints[i].octave < 0 || KF1->keypoints[i].octave >= nl) { set_error("orbm_create_new_map_points: keypoint octave out of range"); return ORB_ERR_ARG; }
+    for (int k = 0; k < nKF2; ++k) {
+        if (!tri_frame_ok(in->KF2 + k)) { set_error("orbm_create_new_map_points: bad KF2 entry"); return ORB_ERR_ARG; }
+        for (int i = 0; i < in->KF2[k].N; ++i) if (in->KF2[k].keypoints[i].octave < 0 || in->KF2[k].keypoints[i].octave >= nl) { set_error("orbm_create_new_map_points: keypoint octave out of range"); return ORB_ERR_ARG; }
+    }
+    *nNew = 0;
+    for (int k = 0; k < nKF2; ++k) { nmatches[k] = 0; ncreated[k] = 0; }
+    const size_t N1 = (size_t)KF1->N, K = (size_t)nKF2;
+    if (K == 0 || N1 == 0) return ORB_OK;
+    Matcher& m = h->m;
+    CK(cudaSetDevice(m.device));
+    const TriExtra extra[3] = {{in->Tcw, 48 * (K + 1)}, {in->Ow, 12 * (K + 1)}, {in->cam, 16 * (K + 1)}};
+    // outputs after the search's: reason [K][N1] | recs [K][N1] | winner [N1] | counts (1 + 2K) | out [N1]   (counts .. out are downloaded)
+    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+    const size_t oReason = 0, oRecs = al(K * N1), oWin = oRecs + al(sizeof(OrbmNewPoint) * K * N1), oCounts = oWin + al(4 * N1),
+                 oRec = oCounts + al(4 * (1 + 2 * K)), outBytes = oRec + sizeof(OrbmNewPoint) * N1;
+    TriStage S;
+    const int rc = tri_search_launch(m, KF1, nKF2, in->KF2, in->scaleFactors, in->levelSigma2, nl, in->ep2, in->F12, in->bCoarse, 0, 3, extra, outBytes, &S);
+    if (rc) return rc;
+    uint8_t* d = S.d + S.oOut;
+    NewPointsParams P; memset(&P, 0, sizeof(P));
+    P.N1 = (int)N1; P.nKF2 = nKF2; P.nlevels = nl; P.bInertial = in->bInertial ? 1 : 0;
+    P.ratioFactor = 1.5f * in->scaleFactor; P.thFar = in->thFarPoints;
+    P.kps1 = S.Q.kps1; P.pairs = S.Q.pairs; P.matches12 = (const int*)(S.d + S.oM12);
+    P.scaleFactors = S.Q.scaleFactors; P.levelSigma2 = S.Q.levelSigma2;
+    P.Tcw = (const float*)(S.d + S.extraIn[0]); P.Ow = (const float*)(S.d + S.extraIn[1]); P.cam = (const float*)(S.d + S.extraIn[2]);
+    P.reason = d + oReason; P.recs = (OrbmNewPoint*)(d + oRecs); P.winner = (int*)(d + oWin); P.counts = (int*)(d + oCounts); P.out = (OrbmNewPoint*)(d + oRec);
+    cudaStream_t st = m.stream;
+    new_points_kernel<<<dim3((unsigned)((N1 + NP_NT - 1) / NP_NT), (unsigned)K), NP_NT, 0, st>>>(P);
+    new_points_commit_kernel<<<1, NPC_NT, 0, st>>>(P);
+    m.launches = 3;
+    CK(cudaGetLastError());
+    uint8_t* hb = S.h + S.oOut;
+    CK(cudaMemcpyAsync(hb + oCounts, d + oCounts, outBytes - oCounts, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const int* cnt = (const int*)(hb + oCounts);
+    *nNew = cnt[0];
+    memcpy(nmatches, cnt + 1, 4 * K); memcpy(ncreated, cnt + 1 + K, 4 * K);
+    memcpy(out, hb + oRec, sizeof(OrbmNewPoint) * (size_t)cnt[0]);
     return ORB_OK;
 }
 
