@@ -213,7 +213,7 @@ typedef struct OrbmFrustumIn {
 /* Outputs, one per map point: inView = mbTrackInView (the return value); projX / projY = mTrackProjX / Y (-1 when the
  * point is behind the camera or outside the image; set as soon as the bounds test passes, like the reference);
  * projXR, depth (= |Pc|), level (mnTrackScaleLevel), viewCos are written only for points in view (0 / -1 otherwise: the
- * reference leaves those fields untouched). */
+ * reference leaves those fields untouched).  M <= max_mappoints of the handle (ORB_ERR_CAPACITY otherwise). */
 int orbm_frustum_project(orbm_handle* h, const OrbmFrustumIn* in, uint8_t* inView, float* projX, float* projY, float* projXR,
                          float* depth, int32_t* level, float* viewCos);
 
@@ -343,9 +343,9 @@ int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNe
 int orbm_distinctive_descriptors(orbm_handle* h, int nPoints, const int32_t* obsStart, const uint8_t* descriptors, int32_t* best);
 
 /* cv::BFMatcher(NORM_HAMMING).knnMatch(query, train, k=2) as used at src/Frame.cc:1144: idx/dist are Q x 2,
- * ordered by (distance, lower train index); missing neighbours are -1.  Host pointers. */
+ * ordered by (distance, lower train index); missing neighbours are -1.  Q and T are unbounded.  Host pointers. */
 int orbm_bf_knn2(orbm_handle* h, const uint8_t* query, int Q, const uint8_t* train, int T, int32_t* idx, int32_t* dist);
-/* ORBmatcher::DescriptorDistance (src/ORBmatcher.cc:2058-2074) for n descriptor pairs a[i], b[i].  Host pointers. */
+/* ORBmatcher::DescriptorDistance (src/ORBmatcher.cc:2058-2074) for n descriptor pairs a[i], b[i]; n is unbounded.  Host pointers. */
 int orbm_descriptor_distance(orbm_handle* h, const uint8_t* a, const uint8_t* b, int n, int32_t* out);
 int orbm_last_launch_count(const orbm_handle* h);
 

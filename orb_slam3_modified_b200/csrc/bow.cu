@@ -16,17 +16,9 @@
 
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
+#include "staging.h"
 
 using orbx::set_error;
-
-#define CK(call)                                                                   \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));         \
-            return ORB_ERR_CUDA;                                                   \
-        }                                                                          \
-    } while (0)
 
 namespace bow {
 
@@ -153,9 +145,8 @@ struct Vocabulary {
     Voc V{};
     uint8_t* d_arena = nullptr;
     cudaStream_t st = nullptr;
-    // scratch for the host entry point
-    uint8_t* d_work = nullptr; size_t workBytes = 0;
-    ~Vocabulary() { cudaSetDevice(device); if (d_arena) cudaFree(d_arena); if (d_work) cudaFree(d_work); if (st) cudaStreamDestroy(st); }
+    orbx::Staging staging;       // the host entry point's operands
+    ~Vocabulary() { cudaSetDevice(device); if (d_arena) cudaFree(d_arena); if (st) cudaStreamDestroy(st); }
 };
 
 }  // namespace bow
@@ -174,13 +165,11 @@ int orbv_create(orbv_handle** out, const OrbVocabulary* voc, int device) {
     const int nChildren = voc->childStart[n];
     for (int i = 0; i < n; ++i) if (voc->childStart[i + 1] < voc->childStart[i]) { set_error("orbv_create: childStart must be non-decreasing"); return ORB_ERR_ARG; }
     for (int c = 0; c < nChildren; ++c) if (voc->children[c] <= 0 || voc->children[c] >= n) { set_error("orbv_create: child index out of range"); return ORB_ERR_ARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("orbv_create: bad device index"); return ORB_ERR_ARG; }
+    if (int rc = orbx::check_device(device)) return rc;
     CK(cudaSetDevice(device));
     orbv_handle* h = new orbv_handle();
     Vocabulary& v = h->v;
-    v.device = device;
+    v.device = v.staging.device = device;
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t oCS = 0, oCh = oCS + al(4 * (size_t)(n + 1)), oW = oCh + al(4 * (size_t)nChildren), oD = oW + al(4 * (size_t)n), oWt = oD + al(32 * (size_t)n),
                  total = oWt + al(8 * (size_t)n);
@@ -224,28 +213,18 @@ int orbv_transform_batch(orbv_handle* h, int batch, const uint8_t* desc, const i
     Vocabulary& v = h->v;
     CK(cudaSetDevice(v.device));
     const size_t B = batch, K = cap;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t oD = 0, oN = oD + al(32 * B * K), oSW = oN + al(4 * B), oSWt = oSW + al(4 * B * K), oSN = oSWt + al(8 * B * K), oW = oSN + al(4 * B * K), oV = oW + al(4 * B * K),
-                 oNW = oV + al(8 * B * K), oFN = oNW + al(4 * B), oFF = oFN + al(4 * B * K), oNE = oFF + al(4 * B * K), total = oNE + al(4 * B);
-    if (total > v.workBytes) {
-        if (v.d_work) cudaFree(v.d_work);
-        v.d_work = nullptr; v.workBytes = 0;
-        CK(cudaMalloc(&v.d_work, total));
-        v.workBytes = total;
-    }
-    uint8_t* d = v.d_work; cudaStream_t st = v.st;
-    CK(cudaMemcpyAsync(d + oD, desc, 32 * B * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oN, n, 4 * B, cudaMemcpyHostToDevice, st));
-    int rc = orbv_transform_batch_device(h, batch, d + oD, (const int*)(d + oN), cap, levelsup, (int*)(d + oSW), (double*)(d + oSWt), (int*)(d + oSN), (int*)(d + oW),
-                                         (double*)(d + oV), (int*)(d + oNW), (int*)(d + oFN), (int*)(d + oFF), (int*)(d + oNE), st);
+    orbx::Staging& S = v.staging;
+    S.begin();
+    const int pD = S.in(desc, 32 * B * K), pN = S.in(n, 4 * B), pSW = S.scratch(4 * B * K), pSWt = S.scratch(8 * B * K), pSN = S.scratch(4 * B * K),
+              pW = S.out(wordId, 4 * B * K), pV = S.out(wordValue, 8 * B * K), pNW = S.out(nWords, 4 * B), pFN = S.out(fvNode, 4 * B * K),
+              pFF = S.out(fvFeature, 4 * B * K), pNE = S.out(nEntries, 4 * B);
+    int rc = S.reserve();
     if (rc) return rc;
-    CK(cudaMemcpyAsync(wordId, d + oW, 4 * B * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(wordValue, d + oV, 8 * B * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(nWords, d + oNW, 4 * B, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(fvNode, d + oFN, 4 * B * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(fvFeature, d + oFF, 4 * B * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(nEntries, d + oNE, 4 * B, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S.upload(v.st));
+    rc = orbv_transform_batch_device(h, batch, S.dev(pD), S.dev<int>(pN), cap, levelsup, S.dev<int>(pSW), S.dev<double>(pSWt), S.dev<int>(pSN), S.dev<int>(pW),
+                                     S.dev<double>(pV), S.dev<int>(pNW), S.dev<int>(pFN), S.dev<int>(pFF), S.dev<int>(pNE), v.st);
+    if (rc) return rc;
+    CK(S.download(v.st));
     return ORB_OK;
 }
 

@@ -1,4 +1,4 @@
-// Small device-side helpers shared by the kernels of this library.
+// Small device-side helpers shared by the kernels of this library, and the host-side error plumbing of its entry points.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,15 +8,34 @@
 #include <string>
 #include <utility>
 
+#include "../../include/orb_b200.h"
+
 namespace orbx {
 
 void set_error(const std::string& s);
+
+#define CK(call)                                                                   \
+    do {                                                                           \
+        cudaError_t e_ = (call);                                                   \
+        if (e_ != cudaSuccess) {                                                   \
+            orbx::set_error(std::string(#call) + ": " + cudaGetErrorString(e_));   \
+            return ORB_ERR_CUDA;                                                   \
+        }                                                                          \
+    } while (0)
+
+// The device check of every entry point that takes a device index: ORB_ERR_CUDA without a device, ORB_ERR_ARG for an index out of range.
+inline int check_device(int device) {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
+    if (device < 0 || device >= n) { set_error("bad device index " + std::to_string(device) + " (" + std::to_string(n) + " CUDA devices)"); return ORB_ERR_ARG; }
+    return ORB_OK;
+}
 
 // The library is compiled for sm_90a alone (__graft_entry__.py): its cubins load on compute capability 9.0 and on no other device.
 inline int require_sm90(int major, int minor) {
     if (major == 9 && minor == 0) return 0;
     set_error("device is not sm_90 (Hopper); this library is built for sm_90a only and has no other code path");
-    return -4;
+    return ORB_ERR_CUDA;
 }
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of the (function, device) pair, not of a handle: several handles of
@@ -30,7 +49,7 @@ inline int ensure_dynamic_smem(Kernel* kernel, size_t bytes, int device) {
     size_t& cur = current[std::make_pair((const void*)kernel, device)];
     if (bytes <= cur || bytes <= 48 * 1024) return 0;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute(MaxDynamicSharedMemorySize): ") + cudaGetErrorString(e)); return -4; }
+    if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute(MaxDynamicSharedMemorySize): ") + cudaGetErrorString(e)); return ORB_ERR_CUDA; }
     cur = bytes;
     return 0;
 }

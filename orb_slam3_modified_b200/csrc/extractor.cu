@@ -18,15 +18,6 @@ namespace orbx {
 static thread_local std::string g_err;
 void set_error(const std::string& s) { g_err = s; }
 
-#define CK(call)                                                                              \
-    do {                                                                                      \
-        cudaError_t e_ = (call);                                                              \
-        if (e_ != cudaSuccess) {                                                              \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));                    \
-            return ORB_ERR_CUDA;                                                              \
-        }                                                                                     \
-    } while (0)
-
 static const int8_t h_pattern[1024] = {
 #include "brief_pattern.inc"
 };
@@ -464,9 +455,7 @@ int orbx_create(orbx_handle** out, int nfeatures, float scaleFactor, int nlevels
         set_error("orbx_create: bad argument");
         return ORB_ERR_ARG;
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("orbx_create: bad device index"); return ORB_ERR_ARG; }
+    if (int rc = check_device(device)) return rc;
     orbx_handle* h = new orbx_handle();
     Extractor& e = h->e;
     e.nfeatures = nfeatures; e.nlevels = nlevels; e.iniTh = iniThFAST; e.minTh = minThFAST; e.scaleFactor = scaleFactor;

@@ -18,17 +18,9 @@
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
 #include "inertial_dev.cuh"
+#include "staging.h"
 
 using orbx::set_error;
-
-#define CK(call)                                                                   \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));         \
-            return ORB_ERR_CUDA;                                                   \
-        }                                                                          \
-    } while (0)
 
 namespace imu {
 
@@ -573,37 +565,10 @@ __global__ void __launch_bounds__(PI_NT) pose_inertial_opt_kernel(PoseInertialPa
     if (tid < 21) { Q.state[21 * (size_t)f + tid] = s_st[tid]; if (LF) Q.prevState[21 * (size_t)f + tid] = s_sp[tid]; }
 }
 
-// host plumbing: one device arena per host thread and device, grown on demand (these are static functions in the reference)
-struct Scratch {
-    int device = -1; uint8_t* d = nullptr; size_t cap = 0; cudaStream_t st = nullptr;
-    ~Scratch() { if (d) { cudaSetDevice(device); cudaFree(d); } if (st) cudaStreamDestroy(st); }
-};
-static int scratch_for(int device, size_t bytes, Scratch** out) {
-    thread_local Scratch S;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("bad device index"); return ORB_ERR_ARG; }
-    CK(cudaSetDevice(device));
-    if (S.device != device || bytes > S.cap) {
-        if (S.d) { cudaSetDevice(S.device); cudaFree(S.d); S.d = nullptr; S.cap = 0; CK(cudaSetDevice(device)); }
-        if (S.st && S.device != device) { cudaStreamDestroy(S.st); S.st = nullptr; }
-        S.device = device;
-        CK(cudaMalloc(&S.d, bytes + bytes / 2 + 256));
-        S.cap = bytes + bytes / 2 + 256;
-    }
-    if (!S.st) CK(cudaStreamCreateWithFlags(&S.st, cudaStreamNonBlocking));
-    *out = &S;
-    return ORB_OK;
-}
-struct Bump {
-    uint8_t* base; size_t off = 0;
-    explicit Bump(uint8_t* b) : base(b) {}
-    size_t take(size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; }
-};
-
 }  // namespace imu
 
 using namespace imu;
+using orbx::ThreadStaging;
 
 extern "C" {
 
@@ -611,43 +576,38 @@ int imu_preintegrate_batch(int count, const int32_t* nMeas, int maxMeas, const f
                            const float* noise4, float* preint, int device) {
     if (count < 1 || maxMeas < 1 || !nMeas || !acc || !gyr || !dt || !bias6 || !noise4 || !preint) { set_error("imu_preintegrate_batch: bad argument"); return ORB_ERR_ARG; }
     const size_t C = count, M = maxMeas;
-    Bump B(nullptr);
-    const size_t oN = B.take(4 * C), oA = B.take(12 * C * M), oG = B.take(12 * C * M), oT = B.take(4 * C * M), oB = B.take(24 * C), oP = B.take(4 * P_SIZE * C);
-    Scratch* S;
-    int rc = scratch_for(device, B.off, &S);
+    ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
-    uint8_t* d = S->d; cudaStream_t st = S->st;
-    CK(cudaMemcpyAsync(d + oN, nMeas, 4 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oA, acc, 12 * C * M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oG, gyr, 12 * C * M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oT, dt, 4 * C * M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oB, bias6, 24 * C, cudaMemcpyHostToDevice, st));
+    S->begin();
+    const int pN = S->in(nMeas, 4 * C), pA = S->in(acc, 12 * C * M), pG = S->in(gyr, 12 * C * M), pT = S->in(dt, 4 * C * M), pB = S->in(bias6, 24 * C),
+              pP = S->out(preint, 4 * P_SIZE * C);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
     // IMU::Calib::Set (src/ImuTypes.cc:395-407): squares in float
     const float ng2 = noise4[0] * noise4[0], na2 = noise4[1] * noise4[1], ngw2 = noise4[2] * noise4[2], naw2 = noise4[3] * noise4[3];
-    imu_preintegrate_kernel<<<(count + 63) / 64, 64, 0, st>>>(count, (const int*)(d + oN), maxMeas, (const float*)(d + oA), (const float*)(d + oG),
-                                                              (const float*)(d + oT), (const float*)(d + oB), ng2, na2, ngw2, naw2, (float*)(d + oP));
+    imu_preintegrate_kernel<<<(count + 63) / 64, 64, 0, st>>>(count, S->dev<int>(pN), maxMeas, S->dev<float>(pA), S->dev<float>(pG), S->dev<float>(pT),
+                                                              S->dev<float>(pB), ng2, na2, ngw2, naw2, S->dev<float>(pP));
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(preint, d + oP, 4 * P_SIZE * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S->download(st));
     return ORB_OK;
 }
 
 int imu_information_batch(int count, const float* preint, double* info9, double* infoG, double* infoA, int device) {
     if (count < 1 || !preint || !info9 || !infoG || !infoA) { set_error("imu_information_batch: bad argument"); return ORB_ERR_ARG; }
     const size_t C = count;
-    Bump B(nullptr);
-    const size_t oP = B.take(4 * P_SIZE * C), oI = B.take(648 * C), oG = B.take(72 * C), oA = B.take(72 * C);
-    Scratch* S;
-    int rc = scratch_for(device, B.off, &S);
+    ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
-    uint8_t* d = S->d; cudaStream_t st = S->st;
-    CK(cudaMemcpyAsync(d + oP, preint, 4 * P_SIZE * C, cudaMemcpyHostToDevice, st));
-    imu_information_kernel<<<(count + 31) / 32, 32, 0, st>>>(count, (const float*)(d + oP), (double*)(d + oI), (double*)(d + oG), (double*)(d + oA));
+    S->begin();
+    const int pP = S->in(preint, 4 * P_SIZE * C), pI = S->out(info9, 648 * C), pG = S->out(infoG, 72 * C), pA = S->out(infoA, 72 * C);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
+    imu_information_kernel<<<(count + 31) / 32, 32, 0, st>>>(count, S->dev<float>(pP), S->dev<double>(pI), S->dev<double>(pG), S->dev<double>(pA));
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(info9, d + oI, 648 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(infoG, d + oG, 72 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(infoA, d + oA, 72 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S->download(st));
     return ORB_OK;
 }
 
@@ -655,23 +615,20 @@ int imu_inertial_edges(int count, const float* preint, const double* states36, c
                        double* chi2, double* rho, int device) {
     if (count < 1 || !preint || !states36 || !err9 || (info9 && !chi2)) { set_error("imu_inertial_edges: bad argument"); return ORB_ERR_ARG; }
     const size_t C = count;
-    Bump B(nullptr);
-    const size_t oP = B.take(4 * P_SIZE * C), oS = B.take(288 * C), oI = B.take(648 * C), oE = B.take(72 * C), oJ = B.take(1728 * C), oC = B.take(8 * C), oR = B.take(8 * C);
-    Scratch* S;
-    int rc = scratch_for(device, B.off, &S);
+    ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
-    uint8_t* d = S->d; cudaStream_t st = S->st;
-    CK(cudaMemcpyAsync(d + oP, preint, 4 * P_SIZE * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oS, states36, 288 * C, cudaMemcpyHostToDevice, st));
-    if (info9) CK(cudaMemcpyAsync(d + oI, info9, 648 * C, cudaMemcpyHostToDevice, st));
-    inertial_edges_kernel<<<(count + 31) / 32, 32, 0, st>>>(count, (const float*)(d + oP), nullptr, (const double*)(d + oS), info9 ? (const double*)(d + oI) : nullptr,
-                                                            huberDelta, (double*)(d + oE), J9x24 ? (double*)(d + oJ) : nullptr, (double*)(d + oC), rho ? (double*)(d + oR) : nullptr);
+    S->begin();
+    // chi2 is written whether or not the caller asked for it
+    const int pP = S->in(preint, 4 * P_SIZE * C), pS = S->in(states36, 288 * C), pI = S->in(info9, info9 ? 648 * C : 0), pE = S->out(err9, 72 * C),
+              pJ = S->out(J9x24, J9x24 ? 1728 * C : 0), pC = info9 ? S->out(chi2, 8 * C) : S->scratch(8 * C), pR = S->out(info9 ? rho : nullptr, rho ? 8 * C : 0);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
+    inertial_edges_kernel<<<(count + 31) / 32, 32, 0, st>>>(count, S->dev<float>(pP), nullptr, S->dev<double>(pS), info9 ? S->dev<double>(pI) : nullptr, huberDelta,
+                                                            S->dev<double>(pE), J9x24 ? S->dev<double>(pJ) : nullptr, S->dev<double>(pC), rho ? S->dev<double>(pR) : nullptr);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(err9, d + oE, 72 * C, cudaMemcpyDeviceToHost, st));
-    if (J9x24) CK(cudaMemcpyAsync(J9x24, d + oJ, 1728 * C, cudaMemcpyDeviceToHost, st));
-    if (info9) CK(cudaMemcpyAsync(chi2, d + oC, 8 * C, cudaMemcpyDeviceToHost, st));
-    if (info9 && rho) CK(cudaMemcpyAsync(rho, d + oR, 8 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S->download(st));
     return ORB_OK;
 }
 
@@ -682,36 +639,25 @@ int pose_inertial_optimization_last_kf_batch(int count, int cap, const int32_t* 
         set_error("pose_inertial_optimization_last_kf_batch: bad argument"); return ORB_ERR_ARG;
     }
     const size_t C = count, K = cap;
-    Bump B(nullptr);
-    const size_t oN = B.take(4 * C), oX = B.take(12 * C * K), oO = B.take(8 * C * K), oS = B.take(4 * C * K), oT = B.take(4 * C * K), oC = B.take(16 * C), oE = B.take(192),
-                 oP = B.take(4 * P_SIZE * C), oK = B.take(168 * C), oSt = B.take(168 * C), oEr = B.take(16 * C * K), oOut = B.take(C * K), oH = B.take(1800 * C), oR = B.take(4 * C);
-    Scratch* S;
-    int rc = scratch_for(device, B.off, &S);
+    ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
-    uint8_t* d = S->d; cudaStream_t st = S->st;
-    CK(cudaMemcpyAsync(d + oN, N, 4 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oX, Xw, 12 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oO, obs, 8 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oS, invSigma2, 4 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oT, trackDepth, 4 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oC, cam4, 16 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oE, extrinsics24, 192, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oP, preint, 4 * P_SIZE * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oK, kfState21, 168 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oSt, state21, 168 * C, cudaMemcpyHostToDevice, st));
+    S->begin();
+    const int pN = S->in(N, 4 * C), pX = S->in(Xw, 12 * C * K), pO = S->in(obs, 8 * C * K), pS = S->in(invSigma2, 4 * C * K), pT = S->in(trackDepth, 4 * C * K),
+              pC = S->in(cam4, 16 * C), pE = S->in(extrinsics24, 192), pP = S->in(preint, 4 * P_SIZE * C), pK = S->in(kfState21, 168 * C),
+              pSt = S->inout(state21, 168 * C), pOut = S->out(outlier, C * K), pH = S->out(H15, 1800 * C), pR = S->out(ret, 4 * C), pEr = S->scratch(16 * C * K);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
     PoseInertialParams Q;
     Q.count = count; Q.cap = cap; Q.recInit = bRecInit;
-    Q.N = (const int*)(d + oN); Q.Xw = (const float*)(d + oX); Q.obs = (const float*)(d + oO); Q.invSigma2 = (const float*)(d + oS); Q.trackDepth = (const float*)(d + oT);
-    Q.cam4 = (const float*)(d + oC); Q.extr = (const double*)(d + oE); Q.preint = (const float*)(d + oP); Q.kfState = (const double*)(d + oK); Q.state = (double*)(d + oSt);
-    Q.err = (double*)(d + oEr); Q.outlier = d + oOut; Q.H15 = (double*)(d + oH); Q.ret = (int*)(d + oR);
+    Q.N = S->dev<int>(pN); Q.Xw = S->dev<float>(pX); Q.obs = S->dev<float>(pO); Q.invSigma2 = S->dev<float>(pS); Q.trackDepth = S->dev<float>(pT);
+    Q.cam4 = S->dev<float>(pC); Q.extr = S->dev<double>(pE); Q.preint = S->dev<float>(pP); Q.kfState = S->dev<double>(pK); Q.state = S->dev<double>(pSt);
+    Q.err = S->dev<double>(pEr); Q.outlier = S->dev(pOut); Q.H15 = S->dev<double>(pH); Q.ret = S->dev<int>(pR);
     Q.preintKF = nullptr; Q.prior = nullptr; Q.priorH = nullptr; Q.prevState = nullptr;
     pose_inertial_opt_kernel<false><<<count, PI_NT, 0, st>>>(Q);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(state21, d + oSt, 168 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(outlier, d + oOut, C * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(H15, d + oH, 1800 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ret, d + oR, 4 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S->download(st));
     return ORB_OK;
 }
 
@@ -724,41 +670,26 @@ int pose_inertial_optimization_last_frame_batch(int count, int cap, const int32_
         set_error("pose_inertial_optimization_last_frame_batch: bad argument"); return ORB_ERR_ARG;
     }
     const size_t C = count, K = cap;
-    Bump B(nullptr);
-    const size_t oN = B.take(4 * C), oX = B.take(12 * C * K), oO = B.take(8 * C * K), oS = B.take(4 * C * K), oT = B.take(4 * C * K), oC = B.take(16 * C), oE = B.take(192),
-                 oP = B.take(4 * P_SIZE * C), oPk = B.take(4 * P_SIZE * C), oPr = B.take(168 * C), oPh = B.take(1800 * C), oPv = B.take(168 * C), oSt = B.take(168 * C),
-                 oEr = B.take(16 * C * K), oOut = B.take(C * K), oH = B.take(1800 * C), oR = B.take(4 * C);
-    Scratch* S;
-    int rc = scratch_for(device, B.off, &S);
+    ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
-    uint8_t* d = S->d; cudaStream_t st = S->st;
-    CK(cudaMemcpyAsync(d + oN, N, 4 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oX, Xw, 12 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oO, obs, 8 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oS, invSigma2, 4 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oT, trackDepth, 4 * C * K, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oC, cam4, 16 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oE, extrinsics24, 192, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oP, preintFrame, 4 * P_SIZE * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oPk, preintKF, 4 * P_SIZE * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oPr, prior21, 168 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oPh, priorH, 1800 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oPv, prevState21, 168 * C, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oSt, state21, 168 * C, cudaMemcpyHostToDevice, st));
+    S->begin();
+    const int pN = S->in(N, 4 * C), pX = S->in(Xw, 12 * C * K), pO = S->in(obs, 8 * C * K), pS = S->in(invSigma2, 4 * C * K), pT = S->in(trackDepth, 4 * C * K),
+              pC = S->in(cam4, 16 * C), pE = S->in(extrinsics24, 192), pP = S->in(preintFrame, 4 * P_SIZE * C), pPk = S->in(preintKF, 4 * P_SIZE * C),
+              pPr = S->in(prior21, 168 * C), pPh = S->in(priorH, 1800 * C), pPv = S->inout(prevState21, 168 * C), pSt = S->inout(state21, 168 * C),
+              pOut = S->out(outlier, C * K), pH = S->out(H15, 1800 * C), pR = S->out(ret, 4 * C), pEr = S->scratch(16 * C * K);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
     PoseInertialParams Q;
     Q.count = count; Q.cap = cap; Q.recInit = bRecInit;
-    Q.N = (const int*)(d + oN); Q.Xw = (const float*)(d + oX); Q.obs = (const float*)(d + oO); Q.invSigma2 = (const float*)(d + oS); Q.trackDepth = (const float*)(d + oT);
-    Q.cam4 = (const float*)(d + oC); Q.extr = (const double*)(d + oE); Q.preint = (const float*)(d + oP); Q.kfState = nullptr; Q.state = (double*)(d + oSt);
-    Q.err = (double*)(d + oEr); Q.outlier = d + oOut; Q.H15 = (double*)(d + oH); Q.ret = (int*)(d + oR);
-    Q.preintKF = (const float*)(d + oPk); Q.prior = (const double*)(d + oPr); Q.priorH = (const double*)(d + oPh); Q.prevState = (double*)(d + oPv);
+    Q.N = S->dev<int>(pN); Q.Xw = S->dev<float>(pX); Q.obs = S->dev<float>(pO); Q.invSigma2 = S->dev<float>(pS); Q.trackDepth = S->dev<float>(pT);
+    Q.cam4 = S->dev<float>(pC); Q.extr = S->dev<double>(pE); Q.preint = S->dev<float>(pP); Q.kfState = nullptr; Q.state = S->dev<double>(pSt);
+    Q.err = S->dev<double>(pEr); Q.outlier = S->dev(pOut); Q.H15 = S->dev<double>(pH); Q.ret = S->dev<int>(pR);
+    Q.preintKF = S->dev<float>(pPk); Q.prior = S->dev<double>(pPr); Q.priorH = S->dev<double>(pPh); Q.prevState = S->dev<double>(pPv);
     pose_inertial_opt_kernel<true><<<count, PI_NT, 0, st>>>(Q);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(state21, d + oSt, 168 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(prevState21, d + oPv, 168 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(outlier, d + oOut, C * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(H15, d + oH, 1800 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ret, d + oR, 4 * C, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S->download(st));
     return ORB_OK;
 }
 
@@ -770,34 +701,25 @@ int imu_mono_edges(const ImuMonoEdges* in, double* err2, double* Jpoint2x3, doub
     for (int e = 0; e < in->nEdges; ++e)
         if (in->edgePoint[e] < 0 || in->edgePoint[e] >= in->nPoints || in->edgePose[e] < 0 || in->edgePose[e] >= in->nPoses) { set_error("imu_mono_edges: edge index out of range"); return ORB_ERR_ARG; }
     const size_t E = in->nEdges, NP = in->nPoses, NL = in->nPoints;
-    Bump B(nullptr);
-    const size_t oPo = B.take(96 * NP), oX = B.take(192), oCm = B.take(16 * NP), oPt = B.take(24 * NL), oEp = B.take(4 * E), oEk = B.take(4 * E), oOb = B.take(16 * E),
-                 oIs = B.take(4 * E), oEr = B.take(16 * E), oJp = B.take(48 * E), oJx = B.take(96 * E), oC2 = B.take(8 * E), oRh = B.take(8 * E), oDp = B.take(E);
-    Scratch* S;
-    int rc = scratch_for(device, B.off, &S);
+    ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
-    uint8_t* d = S->d; cudaStream_t st = S->st;
-    CK(cudaMemcpyAsync(d + oPo, in->poses, 96 * NP, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oX, in->extrinsics, 192, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oCm, in->cam, 16 * NP, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oPt, in->points, 24 * NL, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oEp, in->edgePoint, 4 * E, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oEk, in->edgePose, 4 * E, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oOb, in->obs, 16 * E, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oIs, in->invSigma2, 4 * E, cudaMemcpyHostToDevice, st));
+    S->begin();
+    const int pPo = S->in(in->poses, 96 * NP), pX = S->in(in->extrinsics, 192), pCm = S->in(in->cam, 16 * NP), pPt = S->in(in->points, 24 * NL),
+              pEp = S->in(in->edgePoint, 4 * E), pEk = S->in(in->edgePose, 4 * E), pOb = S->in(in->obs, 16 * E), pIs = S->in(in->invSigma2, 4 * E),
+              pEr = S->out(err2, 16 * E), pJp = S->out(Jpoint2x3, Jpoint2x3 ? 48 * E : 0), pJx = S->out(Jpose2x6, Jpose2x6 ? 96 * E : 0), pC2 = S->out(chi2, 8 * E),
+              pRh = S->out(rho, rho ? 8 * E : 0), pDp = S->out(depthPositive, E);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
     MonoParams Q;
-    Q.nEdges = in->nEdges; Q.poses = (const double*)(d + oPo); Q.extr = (const double*)(d + oX); Q.cam = (const float*)(d + oCm); Q.points = (const double*)(d + oPt);
-    Q.edgePoint = (const int*)(d + oEp); Q.edgePose = (const int*)(d + oEk); Q.obs = (const double*)(d + oOb); Q.invSigma2 = (const float*)(d + oIs);
-    Q.huberDelta = in->huberDelta; Q.err = (double*)(d + oEr); Q.Jpoint = Jpoint2x3 ? (double*)(d + oJp) : nullptr; Q.Jpose = Jpose2x6 ? (double*)(d + oJx) : nullptr;
-    Q.chi2 = (double*)(d + oC2); Q.rho = rho ? (double*)(d + oRh) : nullptr; Q.depthPositive = d + oDp;
+    Q.nEdges = in->nEdges; Q.poses = S->dev<double>(pPo); Q.extr = S->dev<double>(pX); Q.cam = S->dev<float>(pCm); Q.points = S->dev<double>(pPt);
+    Q.edgePoint = S->dev<int>(pEp); Q.edgePose = S->dev<int>(pEk); Q.obs = S->dev<double>(pOb); Q.invSigma2 = S->dev<float>(pIs);
+    Q.huberDelta = in->huberDelta; Q.err = S->dev<double>(pEr); Q.Jpoint = Jpoint2x3 ? S->dev<double>(pJp) : nullptr; Q.Jpose = Jpose2x6 ? S->dev<double>(pJx) : nullptr;
+    Q.chi2 = S->dev<double>(pC2); Q.rho = rho ? S->dev<double>(pRh) : nullptr; Q.depthPositive = S->dev(pDp);
     mono_imu_edges_kernel<<<(in->nEdges + 127) / 128, 128, 0, st>>>(Q);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(err2, d + oEr, 16 * E, cudaMemcpyDeviceToHost, st));
-    if (Jpoint2x3) { CK(cudaMemcpyAsync(Jpoint2x3, d + oJp, 48 * E, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(Jpose2x6, d + oJx, 96 * E, cudaMemcpyDeviceToHost, st)); }
-    CK(cudaMemcpyAsync(chi2, d + oC2, 8 * E, cudaMemcpyDeviceToHost, st));
-    if (rho) CK(cudaMemcpyAsync(rho, d + oRh, 8 * E, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(depthPositive, d + oDp, E, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S->download(st));
     return ORB_OK;
 }
 

@@ -36,15 +36,6 @@
 
 using orbx::set_error;
 
-#define CK(call)                                                                   \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));         \
-            return ORB_ERR_CUDA;                                                   \
-        }                                                                          \
-    } while (0)
-
 namespace lba {
 
 struct Dev {
@@ -1470,9 +1461,7 @@ extern "C" {
 
 int lba_create_batch(lba_handle** out, int max_poses, int max_points, int max_edges, int max_batch, int device) {
     if (!out || max_poses < 1 || max_points < 1 || max_edges < 1 || max_batch < 1) { set_error("lba_create: bad argument"); return ORB_ERR_ARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("lba_create: bad device index"); return ORB_ERR_ARG; }
+    if (int rc = orbx::check_device(device)) return rc;
     lba_handle* h = new lba_handle();
     h->s.device = device; h->s.maxP = max_poses; h->s.maxL = max_points; h->s.maxE = max_edges; h->s.maxBatch = max_batch;
     int rc = h->s.init();

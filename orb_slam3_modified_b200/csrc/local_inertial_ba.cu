@@ -20,17 +20,9 @@
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
 #include "liba_pack.h"
+#include "staging.h"
 
 using orbx::set_error;
-
-#define CK(call)                                                                   \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));         \
-            return ORB_ERR_CUDA;                                                   \
-        }                                                                          \
-    } while (0)
 
 namespace liba {
 
@@ -97,28 +89,12 @@ __global__ void __launch_bounds__(NT) local_inertial_ba_kernel(const Dev* __rest
     }
 }
 
-// host plumbing: one arena per host thread and device, grown on demand; pinned staging for the packed input / output buffers
-struct Arena {
-    int device = -1;
-    uint8_t* d = nullptr; size_t dcap = 0;
-    uint8_t* h = nullptr; size_t hcap = 0;
-    cudaStream_t st = nullptr;
-    ~Arena() {
-        if (device >= 0) cudaSetDevice(device);
-        if (d) cudaFree(d);
-        if (h) cudaFreeHost(h);
-        if (st) cudaStreamDestroy(st);
-    }
-};
-
 }  // namespace liba
 
 extern "C" int local_inertial_ba_batch(int count, const LocalInertialBAProblem* problems, const LocalInertialBAResult* results, int32_t* iterationsOut, int device) {
     using namespace liba;
     if (count < 1 || !problems || !results) { set_error("local_inertial_ba_batch: bad argument"); return ORB_ERR_ARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("bad device index"); return ORB_ERR_ARG; }
+    if (int rc = orbx::check_device(device)) return rc;
     CK(cudaSetDevice(device));
     {   // the architecture check is made once per device (cudaGetDeviceProperties costs milliseconds)
         static int s_major[64], s_minor[64];
@@ -144,41 +120,31 @@ extern "C" int local_inertial_ba_batch(int count, const LocalInertialBAProblem* 
         inOff[i] = inTot; scOff[i] = scTot; outOff[i] = outTot;
         inTot += (lay[i].inBytes + 255) & ~(size_t)255; scTot += (lay[i].scBytes + 255) & ~(size_t)255; outTot += (lay[i].outBytes + 255) & ~(size_t)255;
     }
-    const size_t devOff = inTot;                                   // the Dev array rides at the end of the input region
-    const size_t inAll = inTot + (((size_t)count * sizeof(Dev) + 255) & ~(size_t)255);
-    const size_t dBytes = inAll + scTot + outTot, hBytes = inAll + outTot;
-
-    thread_local Arena A;
-    if (A.device != device) {
-        if (A.device >= 0) { cudaSetDevice(A.device); if (A.d) cudaFree(A.d); if (A.h) cudaFreeHost(A.h); if (A.st) cudaStreamDestroy(A.st); A.d = A.h = nullptr; A.st = nullptr; A.dcap = A.hcap = 0; }
-        CK(cudaSetDevice(device));
-        A.device = device;
-    }
-    if (!A.st) CK(cudaStreamCreateWithFlags(&A.st, cudaStreamNonBlocking));
-    if (dBytes > A.dcap) { if (A.d) { cudaFree(A.d); A.d = nullptr; A.dcap = 0; } CK(cudaMalloc(&A.d, dBytes + dBytes / 4)); A.dcap = dBytes + dBytes / 4; }
-    if (hBytes > A.hcap) { if (A.h) { cudaFreeHost(A.h); A.h = nullptr; A.hcap = 0; } CK(cudaMallocHost(&A.h, hBytes + hBytes / 4)); A.hcap = hBytes + hBytes / 4; }
-
-    uint8_t* hIn = A.h; uint8_t* hOut = A.h + inAll;
-    uint8_t* dIn = A.d; uint8_t* dSc = A.d + inAll; uint8_t* dOut = A.d + inAll + scTot;
-    Dev* hDev = (Dev*)(hIn + devOff);
+    orbx::ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
+    if (rc) return rc;
+    S->begin();
+    const int pIn = S->in(nullptr, inTot), pDev = S->in(nullptr, (size_t)count * sizeof(Dev)), pOut = S->out(nullptr, outTot), pSc = S->scratch(scTot);
+    if ((rc = S->reserve())) return rc;
+    uint8_t* hIn = S->host(pIn); uint8_t* hOut = S->host(pOut);
+    Dev* hDev = S->host<Dev>(pDev);
     {
         const std::string err = pack_batch(count, problems, lay.data(), inOff.data(), hIn);
         if (!err.empty()) { set_error(err); return ORB_ERR_ARG; }
     }
-    for (int i = 0; i < count; ++i) bind(hDev[i], problems[i], lay[i], dIn + inOff[i], dSc + scOff[i], dOut + outOff[i]);      // device addresses
+    for (int i = 0; i < count; ++i) bind(hDev[i], problems[i], lay[i], S->dev(pIn) + inOff[i], S->dev(pSc) + scOff[i], S->dev(pOut) + outOff[i]);      // device addresses
     const double msPack = ms_since(tStart);
     const auto tGpu = std::chrono::steady_clock::now();
-    CK(cudaMemcpyAsync(dIn, hIn, inAll, cudaMemcpyHostToDevice, A.st));
-    local_inertial_ba_kernel<<<count, NT, 0, A.st>>>((const Dev*)(dIn + devOff));
+    CK(S->upload(S->stream));
+    local_inertial_ba_kernel<<<count, NT, 0, S->stream>>>(S->dev<const Dev>(pDev));
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(hOut, dOut, outTot, cudaMemcpyDeviceToHost, A.st));
-    CK(cudaStreamSynchronize(A.st));
+    CK(S->download(S->stream));
     const double msGpu = ms_since(tGpu);
     for (int i = 0; i < count; ++i) {
         const int it = unpack_outputs(problems[i], results[i], lay[i], hOut + outOff[i]);
         if (iterationsOut) iterationsOut[i] = it;
     }
     if (trace) fprintf(stderr, "local_inertial_ba_batch: %d maps, check + layout + pack %.3f ms (%zu bytes in), copy in + kernel + copy out %.3f ms (%zu bytes out), total %.3f ms\n",
-                       count, msPack, inAll, msGpu, outTot, ms_since(tStart));
+                       count, msPack, inTot + (size_t)count * sizeof(Dev), msGpu, outTot, ms_since(tStart));
     return ORB_OK;
 }

@@ -21,23 +21,11 @@
 #include <vector>
 
 #include "../../include/orb_b200.h"
-#include "host_affinity.h"
 #include "device_utils.cuh"
 #include "exact_math.h"
+#include "staging.h"
 
-namespace orbx {
-void set_error(const std::string& s);
-}
 using orbx::set_error;
-
-#define CK(call)                                                                   \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));         \
-            return ORB_ERR_CUDA;                                                   \
-        }                                                                          \
-    } while (0)
 
 namespace orbm {
 
@@ -1269,19 +1257,14 @@ struct Matcher {
     float4* d_query = nullptr; int4 *d_resultIdx = nullptr, *d_resultDist = nullptr;
     int* d_status = nullptr;
     int numSMs = 132;
-    // staging for the host entry points (batch = 1) -- one arena
-    uint8_t* d_arena = nullptr; size_t arenaBytes = 0;
-    uint8_t* h_arena = nullptr;
-    uint8_t* d_batch = nullptr; size_t batchBytes = 0;   // device staging for the host-pointer batch entry point
-    uint8_t* h_tri = nullptr; size_t hTriBytes = 0;      // pinned host mirror of d_batch for the triangulation entry points
+    Staging staging;                                     // the single-call host entry points' operands
+    uint8_t* d_batch = nullptr; size_t batchBytes = 0;   // device staging of search_last_frame_batch_host (copied straight from the caller)
     int launches = 0;
 
     ~Matcher() {
         cudaSetDevice(device);
-        void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_arena, d_batch};
+        void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_batch};
         for (void* p : ptrs) if (p) cudaFree(p);
-        if (h_arena) cudaFreeHost(h_arena);
-        if (h_tri) cudaFreeHost(h_tri);
         if (evWait) cudaEventDestroy(evWait);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -1296,16 +1279,7 @@ struct Matcher {
         CK(cudaMalloc(&d_resultIdx, sizeof(int4) * mcap * B));
         CK(cudaMalloc(&d_resultDist, sizeof(int4) * mcap * B));
         CK(cudaMalloc(&d_status, sizeof(int) * B));
-        arenaBytes = (size_t)kcap * (28 + 32 + 4 + 1) + (size_t)mcap * (32 + 12 + 4 * 6 + 4) + 4096 + 64 * 64;
-        arenaBytes = (arenaBytes + 255) & ~(size_t)255;
-        const size_t bf = (size_t)(kcap + mcap) * 32 + (size_t)std::max(kcap, mcap) * 16 + 4096;
-        arenaBytes = std::max(arenaBytes, bf);
-        arenaBytes = std::max(arenaBytes, (size_t)(kcap + mcap) * (28 + 32 + 1 + 8 + 4 + 4 + 1) + 8192);   // SearchByBoW: keyframe + frame staged together
-        CK(cudaMalloc(&d_arena, arenaBytes));
-        {
-            orbx::ScopedGpuAffinity numaLocal(device);     // pinned pages on the GPU's NUMA node (host_affinity.h)
-            CK(cudaMallocHost(&h_arena, arenaBytes));
-        }
+        staging.device = device;
         batchBytes = B * ((size_t)kcap * (28 + 32 + 4 + 1) + (size_t)mcap * (1 + 12 + 4 + 4 + 1 + 32) + 28 + 16 + 13 * 256) + 4096;
         CK(cudaMalloc(&d_batch, batchBytes));
         CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -1368,7 +1342,6 @@ struct Matcher {
     }
 };
 
-// bump allocator over the paired host/device arenas
 // ---- Frame::isInFrustum + MapPoint::PredictScale, thread per map point (src/Frame.cc:512-574, src/MapPoint.cc:531-546).
 //      Every float operation is individually rounded in the order fixed by the oracle; std::log(float) is glibc's logf
 //      (exact_math.h: logf_glibc). ----
@@ -1411,20 +1384,6 @@ __global__ void frustum_project_kernel(FrustumParams Q) {
     Q.inView[i] = in; Q.projX[i] = px; Q.projY[i] = py; Q.projXR[i] = pxr; Q.depth[i] = dep; Q.level[i] = lvl; Q.viewCos[i] = vc;
 }
 
-struct Arena {
-    uint8_t *h, *d; size_t off = 0, cap;
-    Arena(uint8_t* h_, uint8_t* d_, size_t c) : h(h_), d(d_), cap(c) {}
-    template <class T> bool put(const T* src, size_t n, const T** dptr) {
-        off = (off + 63) & ~(size_t)63;
-        const size_t bytes = n * sizeof(T);
-        if (off + bytes > cap) return false;
-        if (src && bytes) memcpy(h + off, src, bytes);
-        *dptr = reinterpret_cast<const T*>(d + off);
-        off += bytes;
-        return true;
-    }
-};
-
 }  // namespace orbm
 
 using namespace orbm;
@@ -1435,9 +1394,7 @@ extern "C" {
 
 int orbm_create(orbm_handle** out, int max_batch, int max_keypoints, int max_mappoints, int device) {
     if (!out || max_batch < 1 || max_keypoints < 1 || max_mappoints < 1 || max_keypoints > 65535) { set_error("orbm_create: bad argument"); return ORB_ERR_ARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("orbm_create: bad device index"); return ORB_ERR_ARG; }
+    if (int rc = check_device(device)) return rc;
     orbm_handle* h = new orbm_handle();
     h->m.device = device; h->m.maxBatch = max_batch; h->m.kcap = max_keypoints; h->m.mcap = max_mappoints;
     int rc = h->m.init();
@@ -1449,40 +1406,37 @@ int orbm_create(orbm_handle** out, int max_batch, int max_keypoints, int max_map
 void orbm_destroy(orbm_handle* h) { delete h; }
 int orbm_last_launch_count(const orbm_handle* h) { return h ? h->m.launches : ORB_ERR_ARG; }
 
-static int stage_frame(Matcher& m, Arena& A, const OrbmFrame* fr, MatchParams& P, const int32_t* match, const uint8_t* claimed,
-                       int** dMatch, uint8_t** dClaimed, int** dN) {
+static bool frame_ok(const Matcher& m, const OrbmFrame* fr) {
     if (!fr || fr->K < 0 || fr->K > m.kcap || !fr->scaleFactors || fr->nlevels < 1 || !(fr->maxX > fr->minX) || !(fr->maxY > fr->minY)) {
-        set_error("bad OrbmFrame (K > max_keypoints?)"); return ORB_ERR_ARG;
+        set_error("bad OrbmFrame (K > max_keypoints?)"); return false;
     }
-    const int32_t* dm; const uint8_t* dc; const int* dn;
-    int counts[2] = {fr->K, 0};
-    bool ok = A.put(fr->keypoints, (size_t)fr->K, &P.kps) && A.put(fr->descriptors, (size_t)fr->K * 32, &P.desc) &&
-              A.put(fr->scaleFactors, (size_t)fr->nlevels, &P.scaleFactors) && A.put(match, (size_t)fr->K, &dm) &&
-              A.put(claimed, (size_t)fr->K, &dc) && A.put(counts, (size_t)2, &dn);
-    if (!ok) { set_error("matcher staging arena too small"); return ORB_ERR_CAPACITY; }
-    P.kcap = m.kcap; P.nlevels = fr->nlevels; P.batch = 1;
-    P.minX = fr->minX; P.minY = fr->minY; P.maxX = fr->maxX; P.maxY = fr->maxY;
-    *dMatch = const_cast<int*>(dm); *dClaimed = const_cast<uint8_t*>(dc); *dN = const_cast<int*>(dn);
-    P.nK = dn;
-    return ORB_OK;
+    return true;
 }
 
-static int finish_host(Matcher& m, Arena& A, MatchParams& P, int K, int mUse, int* dMatch, uint8_t* dClaimed, int* dN, int32_t* match,
-                       uint8_t* claimed, int* nmatches) {
-    cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(m.d_arena, m.h_arena, A.off, cudaMemcpyHostToDevice, st));
-    P.match = dMatch; P.claimed = dClaimed; P.nmatches = dN + 1;
-    int rc = m.run(P, K, mUse, st);
+// The current frame of the two single-frame searches: keypoints, descriptors and scale factors, match / claimed in and out, and
+// the counts {K, nmatches, M}.
+struct FramePieces { int kps, desc, sf, match, claimed, counts; };
+static FramePieces stage_frame(Staging& S, const OrbmFrame* fr, int32_t* match, uint8_t* claimed) {
+    const size_t K = fr->K;
+    return {S.in(fr->keypoints, sizeof(OrbKeyPoint) * K), S.in(fr->descriptors, 32 * K), S.in(fr->scaleFactors, 4 * (size_t)fr->nlevels),
+            S.inout(match, 4 * K), S.inout(claimed, K), S.inout(nullptr, 3 * sizeof(int))};
+}
+
+// Binds the frame to P, uploads, runs the fused matcher and brings match / claimed / nmatches back.  The staging is reserved.
+static int search_frame(Matcher& m, const FramePieces& f, const OrbmFrame* fr, int M, MatchParams& P, int* nmatches) {
+    Staging& S = m.staging;
+    int* counts = S.host<int>(f.counts);
+    counts[0] = fr->K; counts[1] = 0; counts[2] = M;
+    P.kps = S.dev<OrbKeyPoint>(f.kps); P.desc = S.dev(f.desc); P.scaleFactors = S.dev<float>(f.sf);
+    P.match = S.dev<int>(f.match); P.claimed = S.dev(f.claimed);
+    P.nK = S.dev<int>(f.counts); P.nmatches = S.dev<int>(f.counts) + 1; P.nM = P.nK + 2;
+    P.batch = 1; P.kcap = m.kcap; P.mcap = m.mcap; P.nlevels = fr->nlevels;
+    P.minX = fr->minX; P.minY = fr->minY; P.maxX = fr->maxX; P.maxY = fr->maxY;
+    CK(S.upload(m.stream));
+    int rc = m.run(P, fr->K, M, m.stream);
     if (rc) return rc;
-    // results come back through the same arena offsets
-    const size_t oM = (uint8_t*)dMatch - m.d_arena, oC = (uint8_t*)dClaimed - m.d_arena, oN = (uint8_t*)dN - m.d_arena;
-    CK(cudaMemcpyAsync(m.h_arena + oM, dMatch, sizeof(int) * K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(m.h_arena + oC, dClaimed, K, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(m.h_arena + oN, dN, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    memcpy(match, m.h_arena + oM, sizeof(int) * K);
-    memcpy(claimed, m.h_arena + oC, K);
-    *nmatches = ((int*)(m.h_arena + oN))[1];
+    CK(S.download(m.stream));
+    *nmatches = counts[1];
     return ORB_OK;
 }
 
@@ -1491,23 +1445,22 @@ int orbm_search_local_map(orbm_handle* h, const OrbmFrame* fr, const OrbmLocalPo
     if (!h || !pts || !match || !claimed || !nmatches || pts->M < 0 || pts->M > h->m.mcap) { set_error("orbm_search_local_map: bad argument"); return ORB_ERR_ARG; }
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
-    MatchParams P; memset(&P, 0, sizeof(P));
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
-    int *dMatch, *dN; uint8_t* dClaimed;
-    int rc = stage_frame(m, A, fr, P, match, claimed, &dMatch, &dClaimed, &dN);
-    if (rc) return rc;
-    ((int*)(m.h_arena + ((uint8_t*)dN - m.d_arena)))[1] = 0;
+    if (!frame_ok(m, fr)) return ORB_ERR_ARG;
     const size_t M = pts->M;
-    int mcount[1] = {pts->M};
-    bool ok = A.put(pts->inView, M, &P.inView) && A.put(pts->bad, M, &P.bad) && A.put(pts->depth, M, &P.depth) &&
-              A.put(pts->projX, M, &P.projX) && A.put(pts->projY, M, &P.projY) && A.put(pts->level, M, &P.level) &&
-              A.put(pts->viewCos, M, &P.viewCos) && A.put(pts->hasObs, M, &P.hasObs) && A.put(pts->descriptors, M * 32, &P.mpDesc) &&
-              A.put(mcount, (size_t)1, &P.nM);
-    if (!ok) { set_error("matcher staging arena too small"); return ORB_ERR_CAPACITY; }
     for (size_t i = 0; i < M; ++i)
         if (pts->inView[i] && !pts->bad[i] && (pts->level[i] < 0 || pts->level[i] >= fr->nlevels)) { set_error("map point level out of range"); return ORB_ERR_ARG; }
-    P.mcap = m.mcap; P.mode = 0; P.th = th; P.nnratio = nnratio; P.bFar = bFar; P.thFar = thFar;
-    return finish_host(m, A, P, fr->K, pts->M, dMatch, dClaimed, dN, match, claimed, nmatches);
+    Staging& S = m.staging;
+    S.begin();
+    const FramePieces f = stage_frame(S, fr, match, claimed);
+    const int pIn = S.in(pts->inView, M), pBad = S.in(pts->bad, M), pDepth = S.in(pts->depth, 4 * M), pX = S.in(pts->projX, 4 * M), pY = S.in(pts->projY, 4 * M),
+              pLevel = S.in(pts->level, 4 * M), pCos = S.in(pts->viewCos, 4 * M), pObs = S.in(pts->hasObs, M), pDesc = S.in(pts->descriptors, 32 * M);
+    int rc = S.reserve();
+    if (rc) return rc;
+    MatchParams P; memset(&P, 0, sizeof(P));
+    P.inView = S.dev(pIn); P.bad = S.dev(pBad); P.depth = S.dev<float>(pDepth); P.projX = S.dev<float>(pX); P.projY = S.dev<float>(pY);
+    P.level = S.dev<int>(pLevel); P.viewCos = S.dev<float>(pCos); P.hasObs = S.dev(pObs); P.mpDesc = S.dev(pDesc);
+    P.mode = 0; P.th = th; P.nnratio = nnratio; P.bFar = bFar; P.thFar = thFar;
+    return search_frame(m, f, fr, pts->M, P, nmatches);
 }
 
 int orbm_search_last_frame(orbm_handle* h, const OrbmFrame* fr, const OrbmLastFrame* last, const float* Tcw7, const float* cam4,
@@ -1515,22 +1468,23 @@ int orbm_search_last_frame(orbm_handle* h, const OrbmFrame* fr, const OrbmLastFr
     if (!h || !last || !Tcw7 || !cam4 || !match || !claimed || !nmatches || last->M < 0 || last->M > h->m.mcap) { set_error("orbm_search_last_frame: bad argument"); return ORB_ERR_ARG; }
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
-    MatchParams P; memset(&P, 0, sizeof(P));
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
-    int *dMatch, *dN; uint8_t* dClaimed;
-    int rc = stage_frame(m, A, fr, P, match, claimed, &dMatch, &dClaimed, &dN);
-    if (rc) return rc;
+    if (!frame_ok(m, fr)) return ORB_ERR_ARG;
     const size_t M = last->M;
-    int mcount[1] = {last->M};
-    bool ok = A.put(last->valid, M, &P.valid) && A.put(last->xyz, M * 3, &P.xyz) && A.put(last->octave, M, &P.octave) &&
-              A.put(last->angle, M, &P.angle) && A.put(last->hasObs, M, &P.hasObs) && A.put(last->descriptors, M * 32, &P.mpDesc) &&
-              A.put(Tcw7, (size_t)7, &P.Tcw7) && A.put(mcount, (size_t)1, &P.nM);
-    if (!ok) { set_error("matcher staging arena too small"); return ORB_ERR_CAPACITY; }
     for (size_t i = 0; i < M; ++i)
         if (last->valid[i] && (last->octave[i] < 0 || last->octave[i] >= fr->nlevels)) { set_error("last-frame octave out of range"); return ORB_ERR_ARG; }
+    Staging& S = m.staging;
+    S.begin();
+    const FramePieces f = stage_frame(S, fr, match, claimed);
+    const int pValid = S.in(last->valid, M), pXyz = S.in(last->xyz, 12 * M), pOct = S.in(last->octave, 4 * M), pAng = S.in(last->angle, 4 * M),
+              pObs = S.in(last->hasObs, M), pDesc = S.in(last->descriptors, 32 * M), pT = S.in(Tcw7, 28);
+    int rc = S.reserve();
+    if (rc) return rc;
+    MatchParams P; memset(&P, 0, sizeof(P));
+    P.valid = S.dev(pValid); P.xyz = S.dev<float>(pXyz); P.octave = S.dev<int>(pOct); P.angle = S.dev<float>(pAng); P.hasObs = S.dev(pObs);
+    P.mpDesc = S.dev(pDesc); P.Tcw7 = S.dev<float>(pT);
     memcpy(P.cam, cam4, sizeof(float) * 4);
-    P.mcap = m.mcap; P.mode = 1; P.th = th; P.checkOri = checkOri;
-    return finish_host(m, A, P, fr->K, last->M, dMatch, dClaimed, dN, match, claimed, nmatches);
+    P.mode = 1; P.th = th; P.checkOri = checkOri;
+    return search_frame(m, f, fr, last->M, P, nmatches);
 }
 
 int orbm_search_last_frame_batch_device(orbm_handle* h, const OrbmBatchDevice* in, float th, int checkOri, int32_t* d_match,
@@ -1602,32 +1556,32 @@ int orbm_search_for_initialization(orbm_handle* h, const OrbmFrame* F1, const Or
     *nmatches = 0;
     for (size_t i = 0; i < K1; ++i) matches12[i] = -1;              // vnMatches12 = vector<int>(F1.mvKeysUn.size(),-1), :651
     if (K1 == 0) return ORB_OK;
-    MatchParams P; memset(&P, 0, sizeof(P));
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
-    std::vector<float> px(K1), py(K1), ang(K1); std::vector<int> lvl(K1);
+    Staging& S = m.staging;
+    S.begin();
+    const int pKps = S.in(F2->keypoints, sizeof(OrbKeyPoint) * K2), pDesc = S.in(F2->descriptors, 32 * K2), pMpDesc = S.in(F1->descriptors, 32 * K1),
+              pX = S.in(nullptr, 4 * K1), pY = S.in(nullptr, 4 * K1), pAng = S.in(nullptr, 4 * K1), pLvl = S.in(nullptr, 4 * K1), pCounts = S.in(nullptr, 8),
+              pMatch = S.out(matches12, 4 * K1), pN = S.out(nmatches, 4), pQ = S.out(nullptr, sizeof(float4) * K1);
+    int rc = S.reserve();
+    if (rc) return rc;
+    float *px = S.host<float>(pX), *py = S.host<float>(pY), *ang = S.host<float>(pAng);
+    int* lvl = S.host<int>(pLvl);
     for (size_t i = 0; i < K1; ++i) { px[i] = prevMatched[2 * i]; py[i] = prevMatched[2 * i + 1]; ang[i] = F1->keypoints[i].angle; lvl[i] = F1->keypoints[i].octave; }
-    int counts[2] = {F2->K, F1->K};
-    const int* dCounts; const int32_t* dMatch; const int* dN;
-    bool ok = A.put(F2->keypoints, K2, &P.kps) && A.put(F2->descriptors, K2 * 32, &P.desc) && A.put(F1->descriptors, K1 * 32, &P.mpDesc) &&
-              A.put(px.data(), K1, &P.projX) && A.put(py.data(), K1, &P.projY) && A.put(ang.data(), K1, &P.angle) && A.put(lvl.data(), K1, &P.level) &&
-              A.put(counts, (size_t)2, &dCounts);
-    const size_t inBytes = A.off;
-    ok = ok && A.put((const int32_t*)nullptr, K1, &dMatch) && A.put((const int*)nullptr, (size_t)1, &dN);
-    if (!ok) { set_error("matcher staging arena too small"); return ORB_ERR_CAPACITY; }
-    P.nK = dCounts; P.nM = dCounts + 1;
+    S.host<int>(pCounts)[0] = F2->K; S.host<int>(pCounts)[1] = F1->K;
+    MatchParams P; memset(&P, 0, sizeof(P));
+    P.kps = S.dev<OrbKeyPoint>(pKps); P.desc = S.dev(pDesc); P.mpDesc = S.dev(pMpDesc);
+    P.projX = S.dev<float>(pX); P.projY = S.dev<float>(pY); P.angle = S.dev<float>(pAng); P.level = S.dev<int>(pLvl);
+    P.nK = S.dev<int>(pCounts); P.nM = P.nK + 1;
     P.batch = 1; P.kcap = m.kcap; P.mcap = m.mcap; P.nlevels = F2->nlevels; P.mode = 2;
     P.minX = F2->minX; P.minY = F2->minY; P.maxX = F2->maxX; P.maxY = F2->maxY;
     P.th = (float)windowSize; P.nnratio = nnratio; P.checkOri = checkOrientation;
-    P.match = const_cast<int32_t*>(dMatch); P.nmatches = const_cast<int*>(dN);
+    P.match = S.dev<int>(pMatch); P.nmatches = S.dev<int>(pN);
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(m.d_arena, m.h_arena, inBytes, cudaMemcpyHostToDevice, st));
-    int rc = m.run_init(P, F2->K, F1->K, st);
+    CK(S.upload(st));
+    rc = m.run_init(P, F2->K, F1->K, st);
     if (rc) return rc;
-    std::vector<float4> q(K1);
-    CK(cudaMemcpyAsync(matches12, dMatch, 4 * K1, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(nmatches, dN, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(q.data(), m.d_query, sizeof(float4) * K1, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(S.dev(pQ), m.d_query, sizeof(float4) * K1, cudaMemcpyDeviceToDevice, st));      // the updated window centres
+    CK(S.download(st));
+    const float4* q = S.host<float4>(pQ);
     for (size_t i = 0; i < K1; ++i) { prevMatched[2 * i] = q[i].x; prevMatched[2 * i + 1] = q[i].y; }
     return ORB_OK;
 }
@@ -1655,31 +1609,29 @@ static int search_by_bow_impl(orbm_handle* h, const OrbmBowFrame* KF, const uint
     if (match) for (int i = 0; i < F->N; ++i) match[i] = -1;
     if (match12) for (int i = 0; i < KF->N; ++i) match12[i] = -1;
     if (F->N == 0 || KF->N == 0) return ORB_OK;
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
+    const size_t nKF = KF->N, nF = F->N, eKF = KF->nEntries, eF = F->nEntries;
+    Staging& S = m.staging;
+    S.begin();
+    const int pKpsKF = S.in(KF->keypoints, sizeof(OrbKeyPoint) * nKF), pDescKF = S.in(KF->descriptors, 32 * nKF), pPtKF = S.in(kfPoint, nKF),
+              pNodeKF = S.in(KF->fvNode, 4 * eKF), pFeatKF = S.in(KF->fvFeature, 4 * eKF), pKpsF = S.in(F->keypoints, sizeof(OrbKeyPoint) * nF),
+              pDescF = S.in(F->descriptors, 32 * nF), pNodeF = S.in(F->fvNode, 4 * eF), pFeatF = S.in(F->fvFeature, 4 * eF), pPtF = S.in(fPoint, fPoint ? nF : 0),
+              pMatch = match ? S.out(match, 4 * nF) : S.scratch(4 * nF), pM12 = S.out(match12, match12 ? 4 * nKF : 0), pN = S.out(nmatches, 4),
+              pGs = S.scratch(4 * (eKF + 1)), pEv = S.scratch(nF);
+    int rc = S.reserve();
+    if (rc) return rc;
     BowMatchParams Q; memset(&Q, 0, sizeof(Q));
     Q.nKF = KF->N; Q.nF = F->N; Q.eKF = KF->nEntries; Q.eF = F->nEntries; Q.nnratio = nnratio; Q.checkOri = checkOrientation;
-    bool ok = A.put(KF->keypoints, (size_t)KF->N, &Q.kpsKF) && A.put(KF->descriptors, (size_t)KF->N * 32, &Q.descKF) && A.put(kfPoint, (size_t)KF->N, &Q.kfPoint) &&
-              A.put(KF->fvNode, (size_t)KF->nEntries, &Q.fvNodeKF) && A.put(KF->fvFeature, (size_t)KF->nEntries, &Q.fvFeatKF) &&
-              A.put(F->keypoints, (size_t)F->N, &Q.kpsF) && A.put(F->descriptors, (size_t)F->N * 32, &Q.descF) &&
-              A.put(F->fvNode, (size_t)F->nEntries, &Q.fvNodeF) && A.put(F->fvFeature, (size_t)F->nEntries, &Q.fvFeatF);
-    if (fPoint) ok = ok && A.put(fPoint, (size_t)F->N, &Q.fPoint);
-    const size_t inBytes = A.off;
-    const int *dMatch, *dN, *dGs, *dM12 = nullptr; const uint8_t* dEv;
-    ok = ok && A.put((const int*)nullptr, (size_t)F->N, &dMatch) && A.put((const int*)nullptr, (size_t)1, &dN) && A.put((const int*)nullptr, (size_t)KF->nEntries + 1, &dGs) &&
-         A.put((const uint8_t*)nullptr, (size_t)F->N, &dEv);
-    if (match12) ok = ok && A.put((const int*)nullptr, (size_t)KF->N, &dM12);
-    if (!ok) { set_error("matcher staging arena too small"); return ORB_ERR_CAPACITY; }
-    Q.match12 = const_cast<int*>(dM12); Q.strictLow = fPoint ? 1 : 0;
-    Q.match = const_cast<int*>(dMatch); Q.nmatches = const_cast<int*>(dN); Q.groupStart = const_cast<int*>(dGs); Q.evBin = const_cast<uint8_t*>(dEv);
+    Q.kpsKF = S.dev<OrbKeyPoint>(pKpsKF); Q.descKF = S.dev(pDescKF); Q.kfPoint = S.dev(pPtKF); Q.fvNodeKF = S.dev<int>(pNodeKF); Q.fvFeatKF = S.dev<int>(pFeatKF);
+    Q.kpsF = S.dev<OrbKeyPoint>(pKpsF); Q.descF = S.dev(pDescF); Q.fvNodeF = S.dev<int>(pNodeF); Q.fvFeatF = S.dev<int>(pFeatF);
+    if (fPoint) Q.fPoint = S.dev(pPtF);
+    Q.match12 = match12 ? S.dev<int>(pM12) : nullptr; Q.strictLow = fPoint ? 1 : 0;
+    Q.match = S.dev<int>(pMatch); Q.nmatches = S.dev<int>(pN); Q.groupStart = S.dev<int>(pGs); Q.evBin = S.dev(pEv);
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(m.d_arena, m.h_arena, inBytes, cudaMemcpyHostToDevice, st));
+    CK(S.upload(st));
     bow_match_kernel<<<1, BM_NT, 0, st>>>(Q);
     m.launches = 1;
     CK(cudaGetLastError());
-    if (match) CK(cudaMemcpyAsync(match, dMatch, 4 * (size_t)F->N, cudaMemcpyDeviceToHost, st));
-    if (match12) CK(cudaMemcpyAsync(match12, dM12, 4 * (size_t)KF->N, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(nmatches, dN, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S.download(st));
     return ORB_OK;
 }
 
@@ -1705,31 +1657,19 @@ static int project_search_impl(orbm_handle* h, const OrbmFrame* KF, const float*
     for (size_t i = 0; i < M; ++i) { bestIdx[i] = -1; bestDist[i] = 256; }
     if (M == 0 || K == 0) return ORB_OK;
     for (size_t k = 0; k < K; ++k) if (KF->keypoints[k].octave < 0 || KF->keypoints[k].octave >= KF->nlevels) { set_error("orbm_fuse_search: keypoint octave out of range"); return ORB_ERR_ARG; }
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-    const size_t oKp = take(K * sizeof(OrbKeyPoint)), oDe = take(K * 32), oSf = take(4 * (size_t)KF->nlevels), oIs = take(4 * (size_t)KF->nlevels), oSt = take(M),
-                 oXy = take(12 * M), oNo = take(12 * M), oMi = take(4 * M), oMa = take(4 * M), oMd = take(32 * M), oBi = take(4 * M), oBd = take(4 * M);
-    if (off > m.batchBytes) {                                   // grow the device staging (mapping-side call: pageable copies are fine)
-        if (m.d_batch) cudaFree(m.d_batch);
-        m.d_batch = nullptr; m.batchBytes = 0;
-        CK(cudaMalloc(&m.d_batch, off));
-        m.batchBytes = off;
-    }
-    uint8_t* d = m.d_batch;
+    const size_t nl = KF->nlevels;
+    Staging& S = m.staging;
+    S.begin();
+    const int pKp = S.in(KF->keypoints, sizeof(OrbKeyPoint) * K), pDe = S.in(KF->descriptors, 32 * K), pSf = S.in(KF->scaleFactors, 4 * nl),
+              pIs = S.in(invLevelSigma2, invLevelSigma2 ? 4 * nl : 0), pSt = S.in(pts->state, M), pXy = S.in(pts->worldPos, 12 * M),
+              pNo = S.in(pts->normal, mode == 0 ? 12 * M : 0), pMi = S.in(pts->minDistance, 4 * M), pMa = S.in(pts->maxDistance, 4 * M),
+              pMd = S.in(pts->descriptors, 32 * M), pBi = S.out(bestIdx, 4 * M), pBd = S.out(bestDist, 4 * M);
+    int rc = S.reserve();
+    if (rc) return rc;
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(d + oKp, KF->keypoints, K * sizeof(OrbKeyPoint), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oDe, KF->descriptors, K * 32, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oSf, KF->scaleFactors, 4 * (size_t)KF->nlevels, cudaMemcpyHostToDevice, st));
-    if (invLevelSigma2) CK(cudaMemcpyAsync(d + oIs, invLevelSigma2, 4 * (size_t)KF->nlevels, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oSt, pts->state, M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oXy, pts->worldPos, 12 * M, cudaMemcpyHostToDevice, st));
-    if (mode == 0) CK(cudaMemcpyAsync(d + oNo, pts->normal, 12 * M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oMi, pts->minDistance, 4 * M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oMa, pts->maxDistance, 4 * M, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + oMd, pts->descriptors, 32 * M, cudaMemcpyHostToDevice, st));
     FuseParams Q; memset(&Q, 0, sizeof(Q));
     MatchParams& P = Q.P;
-    P.kps = (const OrbKeyPoint*)(d + oKp); P.desc = d + oDe; P.scaleFactors = (const float*)(d + oSf); P.kcap = m.kcap; P.nlevels = KF->nlevels; P.batch = 1;
+    P.kps = S.dev<OrbKeyPoint>(pKp); P.desc = S.dev(pDe); P.scaleFactors = S.dev<float>(pSf); P.kcap = m.kcap; P.nlevels = KF->nlevels; P.batch = 1;
     P.minX = KF->minX; P.minY = KF->minY; P.maxX = KF->maxX; P.maxY = KF->maxY;
     P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX); P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
     P.th = th; memcpy(P.cam, cam4, 16);
@@ -1738,20 +1678,18 @@ static int project_search_impl(orbm_handle* h, const OrbmFrame* KF, const float*
     P.descInSmem = frame_smem_bytes(P.ks, 1, true) <= limit ? 1 : 0;
     const size_t sm = frame_smem_bytes(P.ks, 1, P.descInSmem != 0);
     if (sm > limit) { set_error("keyframe too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
-    int rc = ensure_dynamic_smem(fuse_search_kernel, sm, m.device);
-    if (rc) return rc;
-    Q.K = (int)K; Q.M = (int)M; Q.state = d + oSt; Q.mpDesc = d + oMd; Q.xyz = (const float*)(d + oXy); Q.normal = (const float*)(d + oNo);
-    Q.minD = (const float*)(d + oMi); Q.maxD = (const float*)(d + oMa); Q.invSigma2 = (const float*)(d + oIs);
+    if ((rc = ensure_dynamic_smem(fuse_search_kernel, sm, m.device))) return rc;
+    Q.K = (int)K; Q.M = (int)M; Q.state = S.dev(pSt); Q.mpDesc = S.dev(pMd); Q.xyz = S.dev<float>(pXy); Q.normal = S.dev<float>(pNo);
+    Q.minD = S.dev<float>(pMi); Q.maxD = S.dev<float>(pMa); Q.invSigma2 = S.dev<float>(pIs);
     if (mode == 0) { memcpy(Q.Tcw, Tcw7, 28); memcpy(Q.Ow, Ow3, 12); }
     Q.logSF = logScaleFactor; Q.mode = mode; Q.gate = invLevelSigma2 ? 1 : 0;
-    Q.bestIdx = (int*)(d + oBi); Q.bestDist = (int*)(d + oBd);
+    Q.bestIdx = S.dev<int>(pBi); Q.bestDist = S.dev<int>(pBd);
+    CK(S.upload(st));
     const int grid = (int)std::min<size_t>(16, (M + 127) / 128);          // every CTA rebuilds the grid: a few CTAs, ~8 map points per warp
     fuse_search_kernel<<<grid, MF_NT, sm, st>>>(Q);
     m.launches = 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(bestIdx, d + oBi, 4 * M, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(bestDist, d + oBd, 4 * M, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S.download(st));
     return ORB_OK;
 }
 
@@ -1802,76 +1740,55 @@ static bool tri_frame_ok(const OrbmTriFrame* f) {
     for (int e = 0; e < f->nEntries; ++e) if (f->fvFeature[e] < 0 || f->fvFeature[e] >= f->N || (e && f->fvNode[e] < f->fvNode[e - 1])) return false;
     return true;
 }
-// Staging of one SearchForTriangulation call (KF1 against nKF2 neighbours), shared by orbm_search_for_triangulation and
-// orbm_create_new_map_points.  Device (and pinned host mirror) layout, 256-byte aligned pieces:
-//   inputs: level tables | KF1 | per pair: KF2 arrays | the caller's extra inputs | pair table
-//   outputs: nmatches [nKF2] | matches12 [nKF2][N1] | evBin [nKF2][N1] | the caller's extra outputs
-// The inputs go up in ONE copy, then tri_match_kernel runs on the handle's stream.
-struct TriExtra { const void* src; size_t bytes; };
-struct TriStage {
-    uint8_t *d, *h;                     // device base, pinned host mirror
-    size_t oCnt, oM12, oOut;            // nmatches, matches12, the caller's outputs
-    size_t extraIn[4];                  // offsets of the caller's extra inputs
-    TriParams Q;
+// The SearchForTriangulation part (KF1 against nKF2 neighbours) shared by orbm_search_for_triangulation and
+// orbm_create_new_map_points.  tri_stage declares its pieces on the matcher's staging: the level tables, KF1, every neighbour's
+// arrays and the pair table in, nmatches [nKF2] and matches12 [nKF2][N1] out to the given destinations (device only when null).
+// After the caller has declared its own pieces and reserved, tri_launch fills the pair table, uploads everything in ONE copy
+// and runs tri_match_kernel on the handle's stream.
+struct TriPieces {
+    int sf, sg, kp1, de1, mp1, fn1, ff1, tab, cnt, m12, ev;
+    struct Neighbour { int kp, de, mp, fn, ff; };
+    std::vector<Neighbour> kf2;
 };
-static int tri_search_launch(Matcher& m, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
-                             int nlevels, const float* ep2, const float* F12, int bCoarse, int checkOrientation, int nExtra, const TriExtra* extra,
-                             size_t outBytes, TriStage* S) {
-    const size_t N1 = (size_t)KF1->N, E1 = (size_t)KF1->nEntries;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-    const size_t oSf = take(4 * (size_t)nlevels), oSg = take(4 * (size_t)nlevels);
-    const size_t oK1 = take(N1 * sizeof(OrbKeyPoint)), oD1 = take(N1 * 32), oM1 = take(N1), oN1 = take(4 * E1), oF1 = take(4 * E1);
-    struct Off { size_t kp, de, mp, fn, ff; };
-    std::vector<Off> po(nKF2);
+static TriPieces tri_stage(Staging& S, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
+                           int nlevels, int32_t* nmatches, int32_t* matches12) {
+    const size_t N1 = (size_t)KF1->N, E1 = (size_t)KF1->nEntries, K = (size_t)nKF2;
+    TriPieces t;
+    t.sf = S.in(scaleFactors, 4 * (size_t)nlevels); t.sg = S.in(levelSigma2, 4 * (size_t)nlevels);
+    t.kp1 = S.in(KF1->keypoints, sizeof(OrbKeyPoint) * N1); t.de1 = S.in(KF1->descriptors, 32 * N1); t.mp1 = S.in(KF1->hasMapPoint, N1);
+    t.fn1 = S.in(KF1->fvNode, 4 * E1); t.ff1 = S.in(KF1->fvFeature, 4 * E1);
     for (int k = 0; k < nKF2; ++k) {
         const size_t N2 = (size_t)KF2[k].N, E2 = (size_t)KF2[k].nEntries;
-        po[k] = {take(N2 * sizeof(OrbKeyPoint)), take(N2 * 32), take(N2), take(4 * E2), take(4 * E2)};
+        t.kf2.push_back({S.in(KF2[k].keypoints, sizeof(OrbKeyPoint) * N2), S.in(KF2[k].descriptors, 32 * N2), S.in(KF2[k].hasMapPoint, N2),
+                         S.in(KF2[k].fvNode, 4 * E2), S.in(KF2[k].fvFeature, 4 * E2)});
     }
-    for (int e = 0; e < nExtra; ++e) S->extraIn[e] = take(extra[e].bytes);
-    const size_t oTab = take(sizeof(TriPair) * (size_t)nKF2);
-    const size_t inBytes = off;
-    S->oCnt = take(4 * (size_t)nKF2); S->oM12 = take(4 * N1 * nKF2);
-    const size_t oEv = take(N1 * nKF2);
-    S->oOut = take(outBytes);
-    if (off > m.batchBytes) {                                   // grow the device staging
-        if (m.d_batch) cudaFree(m.d_batch);
-        m.d_batch = nullptr; m.batchBytes = 0;
-        CK(cudaMalloc(&m.d_batch, off));
-        m.batchBytes = off;
-    }
-    if (off > m.hTriBytes) {                                    // every call ends with a stream synchronise, so the old buffer is idle
-        if (m.h_tri) cudaFreeHost(m.h_tri);
-        m.h_tri = nullptr; m.hTriBytes = 0;
-        CK(cudaMallocHost(&m.h_tri, off));
-        m.hTriBytes = off;
-    }
-    uint8_t *d = m.d_batch, *hb = m.h_tri;
-    S->d = d; S->h = hb;
-    auto put = [&](size_t o, const void* src, size_t bytes) { if (bytes) memcpy(hb + o, src, bytes); };
-    put(oSf, scaleFactors, 4 * (size_t)nlevels); put(oSg, levelSigma2, 4 * (size_t)nlevels);
-    put(oK1, KF1->keypoints, N1 * sizeof(OrbKeyPoint)); put(oD1, KF1->descriptors, N1 * 32); put(oM1, KF1->hasMapPoint, N1);
-    put(oN1, KF1->fvNode, 4 * E1); put(oF1, KF1->fvFeature, 4 * E1);
-    TriPair* tab = (TriPair*)(hb + oTab);
+    t.tab = S.in(nullptr, sizeof(TriPair) * K);
+    t.cnt = nmatches ? S.out(nmatches, 4 * K) : S.scratch(4 * K);
+    t.m12 = matches12 ? S.out(matches12, 4 * N1 * K) : S.scratch(4 * N1 * K);
+    t.ev = S.scratch(N1 * K);
+    return t;
+}
+static int tri_launch(Matcher& m, const TriPieces& t, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* ep2, const float* F12,
+                      int bCoarse, int checkOrientation, TriParams* Q) {
+    Staging& S = m.staging;
+    const size_t N1 = (size_t)KF1->N;
+    TriPair* tab = S.host<TriPair>(t.tab);
     for (int k = 0; k < nKF2; ++k) {
-        const size_t N2 = (size_t)KF2[k].N, E2 = (size_t)KF2[k].nEntries;
-        put(po[k].kp, KF2[k].keypoints, N2 * sizeof(OrbKeyPoint)); put(po[k].de, KF2[k].descriptors, N2 * 32); put(po[k].mp, KF2[k].hasMapPoint, N2);
-        put(po[k].fn, KF2[k].fvNode, 4 * E2); put(po[k].ff, KF2[k].fvFeature, 4 * E2);
+        const TriPieces::Neighbour& p = t.kf2[k];
         TriPair T; memset(&T, 0, sizeof(T));
-        T.N2 = (int)N2; T.E2 = (int)E2;
-        T.kps2 = (const OrbKeyPoint*)(d + po[k].kp); T.desc2 = d + po[k].de; T.hasMP2 = d + po[k].mp; T.fvNode2 = (const int*)(d + po[k].fn); T.fvFeat2 = (const int*)(d + po[k].ff);
+        T.N2 = KF2[k].N; T.E2 = KF2[k].nEntries;
+        T.kps2 = S.dev<OrbKeyPoint>(p.kp); T.desc2 = S.dev(p.de); T.hasMP2 = S.dev(p.mp); T.fvNode2 = S.dev<int>(p.fn); T.fvFeat2 = S.dev<int>(p.ff);
         memcpy(T.ep, ep2 + 2 * (size_t)k, 8); memcpy(T.F12, F12 + 9 * (size_t)k, 36);
-        T.matches12 = (int*)(d + S->oM12) + (size_t)k * N1; T.nmatches = (int*)(d + S->oCnt) + k; T.evBin = d + oEv + (size_t)k * N1;
+        T.matches12 = S.dev<int>(t.m12) + (size_t)k * N1; T.nmatches = S.dev<int>(t.cnt) + k; T.evBin = S.dev(t.ev) + (size_t)k * N1;
         memcpy(tab + k, &T, sizeof(T));
     }
-    for (int e = 0; e < nExtra; ++e) put(S->extraIn[e], extra[e].src, extra[e].bytes);
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(d, hb, inBytes, cudaMemcpyHostToDevice, st));
-    TriParams& Q = S->Q; memset(&Q, 0, sizeof(Q));
-    Q.N1 = (int)N1; Q.E1 = (int)E1; Q.coarse = bCoarse; Q.checkOri = checkOrientation;
-    Q.kps1 = (const OrbKeyPoint*)(d + oK1); Q.desc1 = d + oD1; Q.hasMP1 = d + oM1; Q.fvNode1 = (const int*)(d + oN1); Q.fvFeat1 = (const int*)(d + oF1);
-    Q.scaleFactors = (const float*)(d + oSf); Q.levelSigma2 = (const float*)(d + oSg); Q.pairs = (const TriPair*)(d + oTab);
-    tri_match_kernel<<<nKF2, TM_NT, 0, st>>>(Q);
+    CK(S.upload(st));
+    memset(Q, 0, sizeof(*Q));
+    Q->N1 = (int)N1; Q->E1 = KF1->nEntries; Q->coarse = bCoarse; Q->checkOri = checkOrientation;
+    Q->kps1 = S.dev<OrbKeyPoint>(t.kp1); Q->desc1 = S.dev(t.de1); Q->hasMP1 = S.dev(t.mp1); Q->fvNode1 = S.dev<int>(t.fn1); Q->fvFeat1 = S.dev<int>(t.ff1);
+    Q->scaleFactors = S.dev<float>(t.sf); Q->levelSigma2 = S.dev<float>(t.sg); Q->pairs = S.dev<TriPair>(t.tab);
+    tri_match_kernel<<<nKF2, TM_NT, 0, st>>>(*Q);
     CK(cudaGetLastError());
     return ORB_OK;
 }
@@ -1892,15 +1809,14 @@ int orbm_search_for_triangulation(orbm_handle* h, const OrbmTriFrame* KF1, int n
     for (size_t i = 0; i < (size_t)nKF2 * N1; ++i) matches12[i] = -1;
     for (int k = 0; k < nKF2; ++k) nmatches[k] = 0;
     if (N1 == 0) return ORB_OK;
-    TriStage S;
-    const int rc = tri_search_launch(m, KF1, nKF2, KF2, scaleFactors, levelSigma2, nlevels, ep2, F12, bCoarse, checkOrientation, 0, nullptr, 0, &S);
+    m.staging.begin();
+    const TriPieces t = tri_stage(m.staging, KF1, nKF2, KF2, scaleFactors, levelSigma2, nlevels, nmatches, matches12);
+    int rc = m.staging.reserve();
     if (rc) return rc;
+    TriParams Q;
+    if ((rc = tri_launch(m, t, KF1, nKF2, KF2, ep2, F12, bCoarse, checkOrientation, &Q))) return rc;
     m.launches = 1;
-    cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(S.h + S.oCnt, S.d + S.oCnt, S.oM12 - S.oCnt + 4 * N1 * nKF2, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    memcpy(nmatches, S.h + S.oCnt, 4 * (size_t)nKF2);
-    memcpy(matches12, S.h + S.oM12, 4 * N1 * nKF2);
+    CK(m.staging.download(m.stream));
     return ORB_OK;
 }
 
@@ -1924,34 +1840,34 @@ int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNe
     if (K == 0 || N1 == 0) return ORB_OK;
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
-    const TriExtra extra[3] = {{in->Tcw, 48 * (K + 1)}, {in->Ow, 12 * (K + 1)}, {in->cam, 16 * (K + 1)}};
-    // outputs after the search's: reason [K][N1] | recs [K][N1] | winner [N1] | counts (1 + 2K) | out [N1]   (counts .. out are downloaded)
-    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t oReason = 0, oRecs = al(K * N1), oWin = oRecs + al(sizeof(OrbmNewPoint) * K * N1), oCounts = oWin + al(4 * N1),
-                 oRec = oCounts + al(4 * (1 + 2 * K)), outBytes = oRec + sizeof(OrbmNewPoint) * N1;
-    TriStage S;
-    const int rc = tri_search_launch(m, KF1, nKF2, in->KF2, in->scaleFactors, in->levelSigma2, nl, in->ep2, in->F12, in->bCoarse, 0, 3, extra, outBytes, &S);
+    Staging& S = m.staging;
+    S.begin();
+    const TriPieces t = tri_stage(S, KF1, nKF2, in->KF2, in->scaleFactors, in->levelSigma2, nl, nullptr, nullptr);
+    // counts = {nNew, nmatches [K], ncreated [K]}; only the first nNew records go to `out`
+    const int pTcw = S.in(in->Tcw, 48 * (K + 1)), pOw = S.in(in->Ow, 12 * (K + 1)), pCam = S.in(in->cam, 16 * (K + 1)), pReason = S.scratch(K * N1),
+              pRecs = S.scratch(sizeof(OrbmNewPoint) * K * N1), pWin = S.scratch(4 * N1), pCounts = S.out(nullptr, 4 * (1 + 2 * K)),
+              pOut = S.out(nullptr, sizeof(OrbmNewPoint) * N1);
+    int rc = S.reserve();
     if (rc) return rc;
-    uint8_t* d = S.d + S.oOut;
+    TriParams Q;
+    if ((rc = tri_launch(m, t, KF1, nKF2, in->KF2, in->ep2, in->F12, in->bCoarse, 0, &Q))) return rc;
     NewPointsParams P; memset(&P, 0, sizeof(P));
     P.N1 = (int)N1; P.nKF2 = nKF2; P.nlevels = nl; P.bInertial = in->bInertial ? 1 : 0;
     P.ratioFactor = 1.5f * in->scaleFactor; P.thFar = in->thFarPoints;
-    P.kps1 = S.Q.kps1; P.pairs = S.Q.pairs; P.matches12 = (const int*)(S.d + S.oM12);
-    P.scaleFactors = S.Q.scaleFactors; P.levelSigma2 = S.Q.levelSigma2;
-    P.Tcw = (const float*)(S.d + S.extraIn[0]); P.Ow = (const float*)(S.d + S.extraIn[1]); P.cam = (const float*)(S.d + S.extraIn[2]);
-    P.reason = d + oReason; P.recs = (OrbmNewPoint*)(d + oRecs); P.winner = (int*)(d + oWin); P.counts = (int*)(d + oCounts); P.out = (OrbmNewPoint*)(d + oRec);
+    P.kps1 = Q.kps1; P.pairs = Q.pairs; P.matches12 = S.dev<int>(t.m12);
+    P.scaleFactors = Q.scaleFactors; P.levelSigma2 = Q.levelSigma2;
+    P.Tcw = S.dev<float>(pTcw); P.Ow = S.dev<float>(pOw); P.cam = S.dev<float>(pCam);
+    P.reason = S.dev(pReason); P.recs = S.dev<OrbmNewPoint>(pRecs); P.winner = S.dev<int>(pWin); P.counts = S.dev<int>(pCounts); P.out = S.dev<OrbmNewPoint>(pOut);
     cudaStream_t st = m.stream;
     new_points_kernel<<<dim3((unsigned)((N1 + NP_NT - 1) / NP_NT), (unsigned)K), NP_NT, 0, st>>>(P);
     new_points_commit_kernel<<<1, NPC_NT, 0, st>>>(P);
     m.launches = 3;
     CK(cudaGetLastError());
-    uint8_t* hb = S.h + S.oOut;
-    CK(cudaMemcpyAsync(hb + oCounts, d + oCounts, outBytes - oCounts, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const int* cnt = (const int*)(hb + oCounts);
+    CK(S.download(st));
+    const int* cnt = S.host<int>(pCounts);
     *nNew = cnt[0];
     memcpy(nmatches, cnt + 1, 4 * K); memcpy(ncreated, cnt + 1 + K, 4 * K);
-    memcpy(out, hb + oRec, sizeof(OrbmNewPoint) * (size_t)cnt[0]);
+    memcpy(out, S.host(pOut), sizeof(OrbmNewPoint) * (size_t)cnt[0]);
     return ORB_OK;
 }
 
@@ -1962,23 +1878,17 @@ int orbm_distinctive_descriptors(orbm_handle* h, int nPoints, const int32_t* obs
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
     const size_t total = (size_t)obsStart[nPoints];
-    const size_t need = 4 * ((size_t)nPoints + 1) + 32 * total + 4 * (size_t)nPoints + 1024;
-    if (need > m.batchBytes) {                                  // grow the device staging (cudaMemcpy from pageable host memory: rare, mapping-side call)
-        if (m.d_batch) cudaFree(m.d_batch);
-        m.d_batch = nullptr; m.batchBytes = 0;
-        CK(cudaMalloc(&m.d_batch, need));
-        m.batchBytes = need;
-    }
-    uint8_t* d = m.d_batch;
-    const size_t oS = 0, oD = (4 * ((size_t)nPoints + 1) + 255) & ~(size_t)255, oB = (oD + 32 * total + 255) & ~(size_t)255;
+    Staging& S = m.staging;
+    S.begin();
+    const int pS = S.in(obsStart, 4 * ((size_t)nPoints + 1)), pD = S.in(descriptors, 32 * total), pB = S.out(best, 4 * (size_t)nPoints);
+    int rc = S.reserve();
+    if (rc) return rc;
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(d + oS, obsStart, 4 * ((size_t)nPoints + 1), cudaMemcpyHostToDevice, st));
-    if (total) CK(cudaMemcpyAsync(d + oD, descriptors, 32 * total, cudaMemcpyHostToDevice, st));
-    distinctive_kernel<<<(nPoints + 7) / 8, 256, 0, st>>>(nPoints, (const int*)(d + oS), d + oD, (int*)(d + oB));
+    CK(S.upload(st));
+    distinctive_kernel<<<(nPoints + 7) / 8, 256, 0, st>>>(nPoints, S.dev<int>(pS), S.dev(pD), S.dev<int>(pB));
     m.launches = 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(best, d + oB, 4 * (size_t)nPoints, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S.download(st));
     return ORB_OK;
 }
 
@@ -1989,36 +1899,31 @@ int orbm_frustum_project(orbm_handle* h, const OrbmFrustumIn* in, uint8_t* inVie
         set_error("orbm_frustum_project: bad argument"); return ORB_ERR_ARG;
     }
     Matcher& m = h->m;
+    if (in->M > m.mcap) { set_error("orbm_frustum_project: more map points than max_mappoints"); return ORB_ERR_CAPACITY; }
     CK(cudaSetDevice(m.device));
     const size_t M = in->M;
     if (M == 0) return ORB_OK;
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
+    Staging& S = m.staging;
+    S.begin();
+    const int pP = S.in(in->worldPos, 12 * M), pN = S.in(in->normal, 12 * M), pMin = S.in(in->minDistInv, 4 * M), pMax = S.in(in->maxDistInv, 4 * M),
+              pRaw = S.in(in->maxDistance, 4 * M), pX = S.out(projX, 4 * M), pY = S.out(projY, 4 * M), pXR = S.out(projXR, 4 * M),
+              pD = S.out(depth, 4 * M), pC = S.out(viewCos, 4 * M), pL = S.out(level, 4 * M), pIn = S.out(inView, M);
+    int rc = S.reserve();
+    if (rc) return rc;
     FrustumParams Q; memset(&Q, 0, sizeof(Q));
     Q.M = in->M;
-    bool ok = A.put(in->worldPos, M * 3, &Q.P) && A.put(in->normal, M * 3, &Q.N) && A.put(in->minDistInv, M, &Q.minD) &&
-              A.put(in->maxDistInv, M, &Q.maxD) && A.put(in->maxDistance, M, &Q.maxRaw);
-    const size_t inBytes = A.off;
-    const uint8_t* dIn; const float *dX, *dY, *dXR, *dD, *dC; const int* dL;
-    ok = ok && A.put((const float*)nullptr, M, &dX) && A.put((const float*)nullptr, M, &dY) && A.put((const float*)nullptr, M, &dXR) &&
-         A.put((const float*)nullptr, M, &dD) && A.put((const float*)nullptr, M, &dC) && A.put((const int*)nullptr, M, &dL) &&
-         A.put((const uint8_t*)nullptr, M, &dIn);
-    if (!ok) { set_error("orbm_frustum_project: more map points than the staging arena holds (max_mappoints)"); return ORB_ERR_CAPACITY; }
+    Q.P = S.dev<float>(pP); Q.N = S.dev<float>(pN); Q.minD = S.dev<float>(pMin); Q.maxD = S.dev<float>(pMax); Q.maxRaw = S.dev<float>(pRaw);
     memcpy(Q.R, in->Rcw, sizeof(Q.R)); memcpy(Q.t, in->tcw, sizeof(Q.t)); memcpy(Q.Ow, in->Ow, sizeof(Q.Ow)); memcpy(Q.cam, in->cam, sizeof(Q.cam));
     Q.minX = in->minX; Q.minY = in->minY; Q.maxX = in->maxX; Q.maxY = in->maxY; Q.mbf = in->mbf; Q.logSF = in->logScaleFactor;
     Q.cosLimit = in->viewingCosLimit; Q.nLevels = in->nScaleLevels;
-    Q.inView = const_cast<uint8_t*>(dIn); Q.projX = const_cast<float*>(dX); Q.projY = const_cast<float*>(dY); Q.projXR = const_cast<float*>(dXR);
-    Q.depth = const_cast<float*>(dD); Q.viewCos = const_cast<float*>(dC); Q.level = const_cast<int*>(dL);
+    Q.inView = S.dev(pIn); Q.projX = S.dev<float>(pX); Q.projY = S.dev<float>(pY); Q.projXR = S.dev<float>(pXR);
+    Q.depth = S.dev<float>(pD); Q.viewCos = S.dev<float>(pC); Q.level = S.dev<int>(pL);
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(m.d_arena, m.h_arena, inBytes, cudaMemcpyHostToDevice, st));
+    CK(S.upload(st));
     frustum_project_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(Q);
     m.launches = 1;
     CK(cudaGetLastError());
-    const size_t outOff = (const uint8_t*)dX - m.d_arena, outBytes = A.off - outOff;
-    CK(cudaMemcpyAsync(m.h_arena + outOff, m.d_arena + outOff, outBytes, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    auto hp = [&](const void* d) { return m.h_arena + ((const uint8_t*)d - m.d_arena); };
-    memcpy(projX, hp(dX), 4 * M); memcpy(projY, hp(dY), 4 * M); memcpy(projXR, hp(dXR), 4 * M); memcpy(depth, hp(dD), 4 * M);
-    memcpy(viewCos, hp(dC), 4 * M); memcpy(level, hp(dL), 4 * M); memcpy(inView, hp(dIn), M);
+    CK(S.download(st));
     return ORB_OK;
 }
 
@@ -2027,19 +1932,17 @@ int orbm_bf_knn2(orbm_handle* h, const uint8_t* query, int Q, const uint8_t* tra
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
     if (Q == 0) return ORB_OK;
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
-    const uint8_t *dq, *dt; const int *di, *dd;
-    if (!(A.put(query, (size_t)Q * 32, &dq) && A.put(train, (size_t)T * 32, &dt))) { set_error("orbm_bf_knn2: more descriptors than max_keypoints + max_mappoints"); return ORB_ERR_CAPACITY; }
-    const size_t inBytes = A.off;
-    if (!(A.put((const int*)nullptr, (size_t)Q * 2, &di) && A.put((const int*)nullptr, (size_t)Q * 2, &dd))) { set_error("orbm_bf_knn2: staging arena too small"); return ORB_ERR_CAPACITY; }
+    Staging& S = m.staging;
+    S.begin();
+    const int pQ = S.in(query, 32 * (size_t)Q), pT = S.in(train, 32 * (size_t)T), pI = S.out(idx, 8 * (size_t)Q), pD = S.out(dist, 8 * (size_t)Q);
+    int rc = S.reserve();
+    if (rc) return rc;
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(m.d_arena, m.h_arena, inBytes, cudaMemcpyHostToDevice, st));
-    bf_knn2_kernel<<<(Q + BF_NT / 32 - 1) / (BF_NT / 32), BF_NT, 0, st>>>(dq, Q, dt, T, const_cast<int*>(di), const_cast<int*>(dd));
+    CK(S.upload(st));
+    bf_knn2_kernel<<<(Q + BF_NT / 32 - 1) / (BF_NT / 32), BF_NT, 0, st>>>(S.dev(pQ), Q, S.dev(pT), T, S.dev<int>(pI), S.dev<int>(pD));
     m.launches = 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(idx, di, sizeof(int) * 2 * Q, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(dist, dd, sizeof(int) * 2 * Q, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S.download(st));
     return ORB_OK;
 }
 
@@ -2048,18 +1951,17 @@ int orbm_descriptor_distance(orbm_handle* h, const uint8_t* a, const uint8_t* b,
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
     if (n == 0) return ORB_OK;
-    Arena A(m.h_arena, m.d_arena, m.arenaBytes);
-    const uint8_t *da, *db; const int* dout;
-    if (!(A.put(a, (size_t)n * 32, &da) && A.put(b, (size_t)n * 32, &db))) { set_error("orbm_descriptor_distance: too many pairs for the staging arena"); return ORB_ERR_CAPACITY; }
-    const size_t inBytes = A.off;
-    if (!A.put((const int*)nullptr, (size_t)n, &dout)) { set_error("orbm_descriptor_distance: staging arena too small"); return ORB_ERR_CAPACITY; }
+    Staging& S = m.staging;
+    S.begin();
+    const int pA = S.in(a, 32 * (size_t)n), pB = S.in(b, 32 * (size_t)n), pO = S.out(out, 4 * (size_t)n);
+    int rc = S.reserve();
+    if (rc) return rc;
     cudaStream_t st = m.stream;
-    CK(cudaMemcpyAsync(m.d_arena, m.h_arena, inBytes, cudaMemcpyHostToDevice, st));
-    hamming_pairs_kernel<<<(n + 255) / 256, 256, 0, st>>>(da, db, n, const_cast<int*>(dout));
+    CK(S.upload(st));
+    hamming_pairs_kernel<<<(n + 255) / 256, 256, 0, st>>>(S.dev(pA), S.dev(pB), n, S.dev<int>(pO));
     m.launches = 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, dout, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(S.download(st));
     return ORB_OK;
 }
 

@@ -10,20 +10,9 @@
 #include <string>
 
 #include "../../include/orb_b200.h"
+#include "staging.h"
 
-namespace orbx {
-void set_error(const std::string& s);
-}
 using orbx::set_error;
-
-#define CK(call)                                                                   \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));         \
-            return ORB_ERR_CUDA;                                                   \
-        }                                                                          \
-    } while (0)
 
 namespace poseopt {
 
@@ -302,52 +291,25 @@ int pose_optimization_batch(int count, int cap, const int32_t* N, const double* 
     if (count < 1 || cap < 1 || !N || !pose7 || !cam4 || !Xw || !obs || !invSigma2 || !poseOut || !outlier || !nInliers) {
         set_error("pose_optimization_batch: bad argument"); return ORB_ERR_ARG;
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device (this library has no CPU path)"); return ORB_ERR_CUDA; }
-    if (device < 0 || device >= ndev) { set_error("pose_optimization_batch: bad device index"); return ORB_ERR_ARG; }
-    CK(cudaSetDevice(device));
     const size_t C = count, K = cap;
-    // device scratch + stream are kept per host thread and device (PoseOptimization is a static function in the reference: no object
-    // to own them) and grow on demand: a call costs copies + one launch, not a cudaMalloc / cudaFree pair
-    struct Scratch { int device = -1; uint8_t* d = nullptr; size_t cap = 0; cudaStream_t st = nullptr;
-                     ~Scratch() { if (d) { cudaSetDevice(device); cudaFree(d); } if (st) cudaStreamDestroy(st); } };
-    thread_local Scratch S;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t oN = take(4 * C), oP = take(56 * C), oC = take(16 * C), oX = take(24 * C * K), oO = take(16 * C * K), oS = take(4 * C * K),
-                 oE = take(16 * C * K), oPo = take(56 * C), oOut = take(C * K), oNi = take(4 * C);
-    if (S.device != device || off > S.cap) {
-        if (S.d) { cudaSetDevice(S.device); cudaFree(S.d); S.d = nullptr; S.cap = 0; CK(cudaSetDevice(device)); }
-        if (S.st && S.device != device) { cudaStreamDestroy(S.st); S.st = nullptr; }
-        S.device = device;
-        CK(cudaMalloc(&S.d, off + off / 2));
-        S.cap = off + off / 2;
-    }
-    if (!S.st) CK(cudaStreamCreateWithFlags(&S.st, cudaStreamNonBlocking));
-    uint8_t* d = S.d;
-    cudaStream_t st = S.st;
-    int rc = ORB_OK;
-    do {
-#define TRY(call) { cudaError_t e_ = (call); if (e_ != cudaSuccess) { set_error(cudaGetErrorString(e_)); rc = ORB_ERR_CUDA; break; } }
-        TRY(cudaMemcpyAsync(d + oN, N, 4 * C, cudaMemcpyHostToDevice, st));
-        TRY(cudaMemcpyAsync(d + oP, pose7, 56 * C, cudaMemcpyHostToDevice, st));
-        TRY(cudaMemcpyAsync(d + oC, cam4, 16 * C, cudaMemcpyHostToDevice, st));
-        TRY(cudaMemcpyAsync(d + oX, Xw, 24 * C * K, cudaMemcpyHostToDevice, st));
-        TRY(cudaMemcpyAsync(d + oO, obs, 16 * C * K, cudaMemcpyHostToDevice, st));
-        TRY(cudaMemcpyAsync(d + oS, invSigma2, 4 * C * K, cudaMemcpyHostToDevice, st));
-        Params P;
-        P.count = count; P.cap = cap; P.N = (const int*)(d + oN); P.pose7 = (const double*)(d + oP); P.cam4 = (const float*)(d + oC);
-        P.Xw = (const double*)(d + oX); P.obs = (const double*)(d + oO); P.invSigma2 = (const float*)(d + oS); P.delta = huberDelta;
-        P.err = (double*)(d + oE); P.poseOut = (double*)(d + oPo); P.outlier = d + oOut; P.nInliers = (int*)(d + oNi);
-        pose_opt_kernel<<<count, NT, 0, st>>>(P);
-        TRY(cudaGetLastError());
-        TRY(cudaMemcpyAsync(poseOut, d + oPo, 56 * C, cudaMemcpyDeviceToHost, st));
-        TRY(cudaMemcpyAsync(outlier, d + oOut, C * K, cudaMemcpyDeviceToHost, st));
-        TRY(cudaMemcpyAsync(nInliers, d + oNi, 4 * C, cudaMemcpyDeviceToHost, st));
-        TRY(cudaStreamSynchronize(st));
-#undef TRY
-    } while (0);
-    return rc;
+    orbx::ThreadStaging* S;
+    int rc = orbx::thread_staging(device, &S);
+    if (rc) return rc;
+    S->begin();
+    const int pN = S->in(N, 4 * C), pP = S->in(pose7, 56 * C), pC = S->in(cam4, 16 * C), pX = S->in(Xw, 24 * C * K), pO = S->in(obs, 16 * C * K),
+              pS = S->in(invSigma2, 4 * C * K), pPo = S->out(poseOut, 56 * C), pOut = S->out(outlier, C * K), pNi = S->out(nInliers, 4 * C),
+              pE = S->scratch(16 * C * K);
+    if ((rc = S->reserve())) return rc;
+    cudaStream_t st = S->stream;
+    CK(S->upload(st));
+    Params P;
+    P.count = count; P.cap = cap; P.N = S->dev<int>(pN); P.pose7 = S->dev<double>(pP); P.cam4 = S->dev<float>(pC);
+    P.Xw = S->dev<double>(pX); P.obs = S->dev<double>(pO); P.invSigma2 = S->dev<float>(pS); P.delta = huberDelta;
+    P.err = S->dev<double>(pE); P.poseOut = S->dev<double>(pPo); P.outlier = S->dev(pOut); P.nInliers = S->dev<int>(pNi);
+    pose_opt_kernel<<<count, NT, 0, st>>>(P);
+    CK(cudaGetLastError());
+    CK(S->download(st));
+    return ORB_OK;
 }
 
 }  // extern "C"
