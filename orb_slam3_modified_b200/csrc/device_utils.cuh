@@ -90,7 +90,19 @@ __device__ __forceinline__ int block_excl_scan(int* data, int m, int* warpTmp) {
     }
     return carry;
 }
-
+// Ordered sum of one double per thread over a CTA of NT threads: an xor butterfly in each warp, then the warp sums in warp order, so the
+// result is run-to-run reproducible and every thread gets the same value.  `sm` needs NT / 32 doubles.  All threads of the block must call.
+template <int NT> __device__ __forceinline__ double block_sum(double v, double* sm) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double r = 0;
+#pragma unroll
+    for (int w = 0; w < NT / 32; ++w) r += sm[w];
+    __syncthreads();
+    return r;
+}
 
 // 256-bit Hamming distance of two 32-byte descriptors held as 8 words (ORBmatcher::DescriptorDistance,
 // reference src/ORBmatcher.cc:2058-2074; the SWAR popcount there == __popc).

@@ -24,6 +24,9 @@ using orbx::set_error;
 
 namespace imu {
 
+using g2o::huber;
+using orbx::block_sum;
+
 
 // ---- Preintegrated::Initialize + IntegrateNewMeasurement over the measurements of one interval; thread per interval ----
 __global__ void imu_preintegrate_kernel(int count, const int* __restrict__ nMeas, int maxMeas, const float* __restrict__ acc, const float* __restrict__ gyr,
@@ -127,7 +130,11 @@ __global__ void inertial_edges_kernel(int count, const float* __restrict__ prein
         double c2 = 0;
         for (int i = 0; i < 9; ++i) { double s = 0; for (int j = 0; j < 9; ++j) s += Om[i * 9 + j] * err[j]; c2 += err[i] * s; }
         chi2Out[e] = c2;
-        if (rhoOut) { const double dsq = huberDelta * huberDelta; rhoOut[e] = (huberDelta <= 0 || c2 <= dsq) ? 1.0 : huberDelta / sqrt(c2); }
+        if (rhoOut) {
+            double r0, r1 = 1.0;                              // huberDelta <= 0: no robust kernel
+            if (!(huberDelta <= 0)) huber(c2, huberDelta, huberDelta * huberDelta, r0, r1);
+            rhoOut[e] = r1;
+        }
     }
 }
 
@@ -158,28 +165,18 @@ __global__ void mono_imu_edges_kernel(MonoParams Q) {
     m3mul(Rcb, Rbw, Rcw);
     m3vec(Rcb, tbw, tcw);
     for (int i = 0; i < 3; ++i) tcw[i] += tcb[i];
-    m3vec(Rcw, Xw, Xc);
-    for (int i = 0; i < 3; ++i) Xc[i] += tcw[i];
-    const double fx = cm[0], fy = cm[1], cx = cm[2], cy = cm[3];
-    const double e0 = Q.obs[2 * (size_t)e] - (fx * Xc[0] / Xc[2] + cx), e1 = Q.obs[2 * (size_t)e + 1] - (fy * Xc[1] / Xc[2] + cy);
+    double e0, e1;
+    const bool depthPos = mono_residual(Rcw, tcw, Xw, cm, Q.obs[2 * (size_t)e], Q.obs[2 * (size_t)e + 1], Xc, e0, e1);
     Q.err[2 * (size_t)e] = e0; Q.err[2 * (size_t)e + 1] = e1;
     const double c2 = (double)Q.invSigma2[e] * (e0 * e0 + e1 * e1);
     Q.chi2[e] = c2;
-    if (Q.rho) { const double dsq = Q.huberDelta * Q.huberDelta; Q.rho[e] = (Q.huberDelta <= 0 || c2 <= dsq) ? 1.0 : Q.huberDelta / sqrt(c2); }
-    Q.depthPositive[e] = (Rcw[6] * Xw[0] + Rcw[7] * Xw[1] + Rcw[8] * Xw[2] + tcw[2]) > 0.0;
-    if (!Q.Jpoint) return;
-    const double pj[6] = {fx / Xc[2], 0, -fx * Xc[0] / (Xc[2] * Xc[2]), 0, fy / Xc[2], -fy * Xc[1] / (Xc[2] * Xc[2])};
-    double* Jp = Q.Jpoint + 6 * (size_t)e;
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) Jp[i * 3 + j] = -(pj[i * 3] * Rcw[j] + pj[i * 3 + 1] * Rcw[3 + j] + pj[i * 3 + 2] * Rcw[6 + j]);
-    double Xb[3];
-    m3vec(Rbc, Xc, Xb);
-    for (int i = 0; i < 3; ++i) Xb[i] += tbc[i];
-    const double x = Xb[0], y = Xb[1], z = Xb[2];
-    const double Sd[18] = {0.0, z, -y, 1.0, 0.0, 0.0, -z, 0.0, x, 0.0, 1.0, 0.0, y, -x, 0.0, 0.0, 0.0, 1.0};
-    double PR[6];
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) PR[i * 3 + j] = pj[i * 3] * Rcb[j] + pj[i * 3 + 1] * Rcb[3 + j] + pj[i * 3 + 2] * Rcb[6 + j];
-    double* Jx = Q.Jpose + 12 * (size_t)e;
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 6; ++j) Jx[i * 6 + j] = PR[i * 3] * Sd[j] + PR[i * 3 + 1] * Sd[6 + j] + PR[i * 3 + 2] * Sd[12 + j];
+    if (Q.rho) {
+        double r0, r1 = 1.0;
+        if (!(Q.huberDelta <= 0)) huber(c2, Q.huberDelta, Q.huberDelta * Q.huberDelta, r0, r1);
+        Q.rho[e] = r1;
+    }
+    Q.depthPositive[e] = depthPos;
+    if (Q.Jpoint) mono_jacobians(Rcw, Rcb, Rbc, tbc, cm, Xc, Q.Jpoint + 6 * (size_t)e, Q.Jpose + 12 * (size_t)e);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -210,38 +207,13 @@ struct PoseInertialParams {
     const double *prior, *priorH;       // [count][21], [count][225]: ConstraintPoseImu of the previous frame
     double* prevState;                  // [count][21] in / out
 };
-__device__ __forceinline__ double pi_block_sum(double v, double* sm) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double r = 0;
-#pragma unroll
-    for (int w = 0; w < PI_NT / 32; ++w) r += sm[w];
-    __syncthreads();
-    return r;
-}
 // EdgeMonoOnlyPose at the cached camera pose: residual, depth sign and (optionally) the 2 x 6 Jacobian (src/G2oTypes.cc:375-395)
 __device__ __forceinline__ void mono_only_pose(const double* Rcw, const double* tcw, const double* Rcb, const double* Rbc, const double* tbc, const float* cm,
                                                const float* Xwf, const float* of, double& e0, double& e1, bool& depthPos, double* Jp) {
     const double X[3] = {(double)Xwf[0], (double)Xwf[1], (double)Xwf[2]};
     double Xc[3];
-    m3vec(Rcw, X, Xc);
-    for (int i = 0; i < 3; ++i) Xc[i] += tcw[i];
-    const double fx = cm[0], fy = cm[1], cx = cm[2], cy = cm[3];
-    e0 = (double)of[0] - (fx * Xc[0] / Xc[2] + cx);
-    e1 = (double)of[1] - (fy * Xc[1] / Xc[2] + cy);
-    depthPos = (Rcw[6] * X[0] + Rcw[7] * X[1] + Rcw[8] * X[2] + tcw[2]) > 0.0;
-    if (!Jp) return;
-    const double pj[6] = {fx / Xc[2], 0, -fx * Xc[0] / (Xc[2] * Xc[2]), 0, fy / Xc[2], -fy * Xc[1] / (Xc[2] * Xc[2])};
-    double Xb[3];
-    m3vec(Rbc, Xc, Xb);
-    for (int i = 0; i < 3; ++i) Xb[i] += tbc[i];
-    const double x = Xb[0], y = Xb[1], z = Xb[2];
-    const double Sd[18] = {0.0, z, -y, 1.0, 0.0, 0.0, -z, 0.0, x, 0.0, 1.0, 0.0, y, -x, 0.0, 0.0, 0.0, 1.0};
-    double PR[6];
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) PR[i * 3 + j] = pj[i * 3] * Rcb[j] + pj[i * 3 + 1] * Rcb[3 + j] + pj[i * 3 + 2] * Rcb[6 + j];
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 6; ++j) Jp[i * 6 + j] = PR[i * 3] * Sd[j] + PR[i * 3 + 1] * Sd[6 + j] + PR[i * 3 + 2] * Sd[12 + j];
+    depthPos = mono_residual(Rcw, tcw, X, cm, (double)of[0], (double)of[1], Xc, e0, e1);
+    if (Jp) mono_jacobians(Rcw, Rcb, Rbc, tbc, cm, Xc, nullptr, Jp);
 }
 // vertex updates of one frame: ImuCamPose::Update (twb += Rwb ut; Rwb = Rwb ExpSO3(ur)), v / bg / ba += dx
 __device__ void apply_update15(double* st, const double* dx, int& its) {
@@ -353,7 +325,8 @@ __global__ void __launch_bounds__(PI_NT) pose_inertial_opt_kernel(PoseInertialPa
                 mono_only_pose(Rcw, tcw, Rcb, Rbc, tbc, cm, Xw + 3 * i, ob + 2 * i, e0, e1, dp, Jp);
                 err[2 * i] = e0; err[2 * i + 1] = e1;
                 const double om = (double)is2[i], c2 = om * (e0 * e0 + e1 * e1);
-                const double w = (robust && c2 > dsqr) ? delta / sqrt(c2) : 1.0;
+                double r0, w = 1.0;
+                if (robust && c2 > dsqr) huber(c2, delta, dsqr, r0, w);       // c2 > dsqr, not huber's e2 <= dsqr: a NaN chi2 weighs 1 here
                 const double wo = w * om;
                 int t = 0;
 #pragma unroll
@@ -366,7 +339,7 @@ __global__ void __launch_bounds__(PI_NT) pose_inertial_opt_kernel(PoseInertialPa
             }
             double tot[27];
 #pragma unroll
-            for (int k = 0; k < 27; ++k) tot[k] = pi_block_sum(acc[k], s_red);
+            for (int k = 0; k < 27; ++k) tot[k] = block_sum<PI_NT>(acc[k], s_red);
             // (a) the two multi-vertex edges are linearised by two threads of different warps at the same time
             if (tid == 0) {
                 double S36[36];
@@ -386,7 +359,11 @@ __global__ void __launch_bounds__(PI_NT) pose_inertial_opt_kernel(PoseInertialPa
             // (c) the normal equations, one entry per thread.  x index -> column of the EdgeInertial Jacobian: current pose / velocity -> 15..23,
             //     current biases -> none, previous 15 -> 0..14
             double wPrior = 1.0;
-            if (LF) { double c2 = 0; for (int k = 0; k < 15; ++k) c2 += s_e15[k] * s_Oe15[k]; wPrior = c2 > 25.0 ? 5.0 / sqrt(c2) : 1.0; }   // RobustKernelHuber delta 5 (:5084-5092)
+            if (LF) {                                           // RobustKernelHuber delta 5 (:5084-5092); a NaN chi2 weighs 1, as at the mono edges
+                double c2 = 0, r0;
+                for (int k = 0; k < 15; ++k) c2 += s_e15[k] * s_Oe15[k];
+                if (c2 > 25.0) huber(c2, 5.0, 25.0, r0, wPrior);
+            }
             auto ecol = [](int i) { return i < 9 ? 15 + i : (i < 15 ? -1 : i - 15); };
             for (int idx = tid; idx < NX * NX; idx += PI_NT) {
                 const int i = idx / NX, j = idx - i * NX;
@@ -487,7 +464,7 @@ __global__ void __launch_bounds__(PI_NT) pose_inertial_opt_kernel(PoseInertialPa
     }
     double tot[21];
 #pragma unroll
-    for (int k = 0; k < 21; ++k) tot[k] = pi_block_sum(acc[k], s_red);
+    for (int k = 0; k < 21; ++k) tot[k] = block_sum<PI_NT>(acc[k], s_red);
     if (tid == 0) {
         double* Hout = Q.H15 + 225 * (size_t)f;
         double S36[36], e9[9], J[216];

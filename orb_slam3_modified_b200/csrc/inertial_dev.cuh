@@ -1,8 +1,11 @@
-// Device / host math shared by the inertial kernels (inertial.cu, local_inertial_ba.cu) and by the host-side emulation of the
-// LocalInertialBA kernel (tests/liba_emulate.cpp compiles the same phase functions with g++): SO3 helpers (reference src/G2oTypes.cc:777-861),
+// Device / host math shared by the optimiser kernels (lba.cu, pose_opt.cu, inertial.cu, local_inertial_ba.cu) and by the host-side emulation
+// of the LocalInertialBA kernel (tests/liba_emulate.cpp compiles the same phase functions with g++): SO3 helpers (reference src/G2oTypes.cc:777-861),
 // NormalizeRotation (src/ImuTypes.cc:34-37), the information matrices of EdgeInertial / EdgeGyroRW / EdgeAccRW (src/G2oTypes.cc:499-507,
-// src/Optimizer.cc:2645-2654), EdgeInertial::computeError / linearizeOplus (src/G2oTypes.cc:514-594).
+// src/Optimizer.cc:2645-2654), EdgeInertial::computeError / linearizeOplus (src/G2oTypes.cc:514-594), EdgeMono / EdgeMonoOnlyPose with ImuCamPose
+// (src/G2oTypes.cc:349-395), and in namespace g2o the g2o pieces every optimiser kernel uses: SE3Quat and VertexSE3Expmap::oplusImpl,
+// RobustKernelHuber::robustify and OptimizationAlgorithmLevenberg::solve's damping policy with ORB-SLAM3's nBad stop rule.
 #pragma once
+#include <float.h>
 #include <math.h>
 #if defined(__CUDACC__)
 #define IMU_HD __host__ __device__
@@ -252,6 +255,34 @@ IMU_HD inline void edge_inertial_dev(const float* __restrict__ P, const double* 
     m3mul(Rbw1, Rwb2, A); put(6, 18, A, 1.0);
     put(3, 21, Rbw1, 1.0);
 }
+// ---- EdgeMono / EdgeMonoOnlyPose with ImuCamPose (src/G2oTypes.cc:349-395), at the camera pose Rcw, tcw that ImuCamPose caches ----
+// computeError: the camera point Xc = Rcw X + tcw and the residual obs - Pinhole::project(Xc) (cam = fx fy cx cy); returns isDepthPositive
+IMU_HD inline bool mono_residual(const double* Rcw, const double* tcw, const double* X, const float* cam, double obs0, double obs1, double* Xc,
+                                 double& e0, double& e1) {
+    m3vec(Rcw, X, Xc);
+    for (int i = 0; i < 3; ++i) Xc[i] += tcw[i];
+    const double fx = cam[0], fy = cam[1], cx = cam[2], cy = cam[3];
+    e0 = obs0 - (fx * Xc[0] / Xc[2] + cx);
+    e1 = obs1 - (fy * Xc[1] / Xc[2] + cy);
+    return (Rcw[6] * X[0] + Rcw[7] * X[1] + Rcw[8] * X[2] + tcw[2]) > 0.0;
+}
+// linearizeOplus at the camera point Xc: Jpoint (2 x 3; null for EdgeMonoOnlyPose) = -proj_jac Rcw, Jpose (2 x 6) = proj_jac Rcb [[Xb]x | I]
+// with Xb = Rbc Xc + tbc the point in the body frame
+IMU_HD inline void mono_jacobians(const double* Rcw, const double* Rcb, const double* Rbc, const double* tbc, const float* cam, const double* Xc,
+                                  double* Jpoint, double* Jpose) {
+    const double fx = cam[0], fy = cam[1];
+    const double pj[6] = {fx / Xc[2], 0, -fx * Xc[0] / (Xc[2] * Xc[2]), 0, fy / Xc[2], -fy * Xc[1] / (Xc[2] * Xc[2])};
+    if (Jpoint)
+        for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) Jpoint[i * 3 + j] = -(pj[i * 3] * Rcw[j] + pj[i * 3 + 1] * Rcw[3 + j] + pj[i * 3 + 2] * Rcw[6 + j]);
+    double Xb[3];
+    m3vec(Rbc, Xc, Xb);
+    for (int i = 0; i < 3; ++i) Xb[i] += tbc[i];
+    const double x = Xb[0], y = Xb[1], z = Xb[2];
+    const double Sd[18] = {0.0, z, -y, 1.0, 0.0, 0.0, -z, 0.0, x, 0.0, 1.0, 0.0, y, -x, 0.0, 0.0, 0.0, 1.0};
+    double PR[6];
+    for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) PR[i * 3 + j] = pj[i * 3] * Rcb[j] + pj[i * 3 + 1] * Rcb[3 + j] + pj[i * 3 + 2] * Rcb[6 + j];
+    for (int i = 0; i < 2; ++i) for (int j = 0; j < 6; ++j) Jpose[i * 6 + j] = PR[i * 3] * Sd[j] + PR[i * 3 + 1] * Sd[6 + j] + PR[i * 3 + 2] * Sd[12 + j];
+}
 IMU_HD inline void exp_so3_d(const double* w, double* R) {      // ExpSO3(double) with its NormalizeRotation (src/G2oTypes.cc:782-798)
     const double d2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2], d = sqrt(d2);
     double W[9], W2[9], res[9];
@@ -264,3 +295,128 @@ IMU_HD inline void exp_so3_d(const double* w, double* R) {      // ExpSO3(double
 }
 
 }  // namespace imu
+
+// ---- the g2o pieces of every optimiser kernel: lba.cu and pose_opt.cu use the SE3Quat part, all five kernels the Huber kernel, and
+//      lba.cu, pose_opt.cu and liba_core.cuh the Levenberg-Marquardt policy ----
+namespace g2o {
+
+// ---- SE3Quat (g2o/types/se3quat.h), quaternion q = (w, x, y, z), pose T = q 4 | t 3 ----
+IMU_HD inline void qrot(const double* q, const double* v, double* o) {   // Eigen::Quaternion * Vector3
+    double ux = q[2] * v[2] - q[3] * v[1], uy = q[3] * v[0] - q[1] * v[2], uz = q[1] * v[1] - q[2] * v[0];
+    ux += ux; uy += uy; uz += uz;
+    o[0] = v[0] + q[0] * ux + (q[2] * uz - q[3] * uy);
+    o[1] = v[1] + q[0] * uy + (q[3] * ux - q[1] * uz);
+    o[2] = v[2] + q[0] * uz + (q[1] * uy - q[2] * ux);
+}
+IMU_HD inline void qnormalize(double* q) {
+    if (q[0] < 0) { q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3]; }
+    const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    q[0] /= n; q[1] /= n; q[2] /= n; q[3] /= n;
+}
+IMU_HD inline void qtoR(const double* q, double* R) {
+    const double tx = 2 * q[1], ty = 2 * q[2], tz = 2 * q[3];
+    const double twx = tx * q[0], twy = ty * q[0], twz = tz * q[0], txx = tx * q[1], txy = ty * q[1], txz = tz * q[1];
+    const double tyy = ty * q[2], tyz = tz * q[2], tzz = tz * q[3];
+    R[0] = 1 - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
+    R[3] = txy + twz; R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
+    R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1 - (txx + tyy);
+}
+IMU_HD inline void qfromR(const double* m, double* q) {
+    double t = m[0] + m[4] + m[8];
+    if (t > 0) {
+        t = sqrt(t + 1.0);
+        q[0] = 0.5 * t; t = 0.5 / t;
+        q[1] = (m[7] - m[5]) * t; q[2] = (m[2] - m[6]) * t; q[3] = (m[3] - m[1]) * t;
+    } else {
+        int i = 0;
+        if (m[4] > m[0]) i = 1;
+        if (m[8] > m[i * 3 + i]) i = 2;
+        const int j = (i + 1) % 3, k = (j + 1) % 3;
+        t = sqrt(m[i * 3 + i] - m[j * 3 + j] - m[k * 3 + k] + 1.0);
+        double v[3];
+        v[i] = 0.5 * t; t = 0.5 / t;
+        q[0] = (m[k * 3 + j] - m[j * 3 + k]) * t;
+        v[j] = (m[j * 3 + i] + m[i * 3 + j]) * t;
+        v[k] = (m[k * 3 + i] + m[i * 3 + k]) * t;
+        q[1] = v[0]; q[2] = v[1]; q[3] = v[2];
+    }
+}
+// VertexSE3Expmap::oplusImpl: T <- SE3Quat::exp(upd) * T   (g2o/types/se3quat.h:223-256, :101-110)
+IMU_HD inline void pose_oplus(double* T, const double* upd) {
+    const double om0 = upd[0], om1 = upd[1], om2 = upd[2];
+    const double theta = sqrt(om0 * om0 + om1 * om1 + om2 * om2);
+    const double O[9] = {0, -om2, om1, om2, 0, -om0, -om1, om0, 0};
+    double O2[9];
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) O2[i * 3 + j] = O[i * 3] * O[j] + O[i * 3 + 1] * O[3 + j] + O[i * 3 + 2] * O[6 + j];
+    double a, b, c, d;
+    if (theta < 0.00001) { a = 1.0; b = 1 / 2.0; c = 1 / 2.0; d = 1 / 6.0; }
+    else {
+        a = sin(theta) / theta; b = (1 - cos(theta)) / (theta * theta);
+        c = b; d = (theta - sin(theta)) / pow(theta, 3.0);
+    }
+    double R[9], V[9];
+    for (int i = 0; i < 9; ++i) {
+        const double I = (i % 4 == 0) ? 1.0 : 0.0;
+        R[i] = I + a * O[i] + b * O2[i];
+        V[i] = I + c * O[i] + d * O2[i];
+    }
+    double qe[4]; qfromR(R, qe);
+    const double te[3] = {V[0] * upd[3] + V[1] * upd[4] + V[2] * upd[5], V[3] * upd[3] + V[4] * upd[4] + V[5] * upd[5],
+                          V[6] * upd[3] + V[7] * upd[4] + V[8] * upd[5]};
+    qnormalize(qe);
+    double rt[3]; qrot(qe, T + 4, rt);
+    const double* q2 = T;
+    double qn[4] = {qe[0] * q2[0] - qe[1] * q2[1] - qe[2] * q2[2] - qe[3] * q2[3], qe[0] * q2[1] + qe[1] * q2[0] + qe[2] * q2[3] - qe[3] * q2[2],
+                    qe[0] * q2[2] + qe[2] * q2[0] + qe[3] * q2[1] - qe[1] * q2[3], qe[0] * q2[3] + qe[3] * q2[0] + qe[1] * q2[2] - qe[2] * q2[1]};
+    qnormalize(qn);
+    T[0] = qn[0]; T[1] = qn[1]; T[2] = qn[2]; T[3] = qn[3];
+    T[4] = te[0] + rt[0]; T[5] = te[1] + rt[1]; T[6] = te[2] + rt[2];
+}
+
+// RobustKernelHuber::robustify (robust_kernel_impl.cpp:78-91) with dsqr = delta * delta: rho0 = rho(e2), rho1 = rho'(e2).  A NaN e2 takes
+// the second branch, as in g2o.  dsqr is an argument so that a caller can keep it out of its per-edge loop.
+IMU_HD inline void huber(double e2, double delta, double dsqr, double& rho0, double& rho1) {
+    if (e2 <= dsqr) { rho0 = e2; rho1 = 1.0; }
+    else { const double s = sqrt(e2); rho0 = 2 * s * delta - dsqr; rho1 = delta / s; }
+}
+
+// OptimizationAlgorithmLevenberg::solve's damping (optimization_algorithm_levenberg.cpp:61-194) and the stop rule ORB-SLAM3 adds to it
+// (nBad: three iterations in a row that lower chi2 by less than a 1e-3 fraction).  Only the scalar policy: the caller builds and solves the
+// system, applies and undoes the step, and evaluates chi2.
+struct Levenberg {
+    static constexpr int maxTrials = 10;
+    double lambda = -1, ni = 2;
+    int nBad = 0;
+    // first iteration: the user's lambda when it is set, else computeLambdaInit = tau * the largest diagonal entry of H
+    IMU_HD void start(double userLambda, double maxDiag) {
+        lambda = userLambda > 0 ? userLambda : 1e-5 * maxDiag;
+        ni = 2; nBad = 0;
+    }
+    // one trial: rho = (currentChi - tempChi) / (x^T (lambda x + b) + 1e-3), a failed solve counting as tempChi = DBL_MAX.  On a good step
+    // lambda shrinks and currentChi takes tempChi (returns true); otherwise lambda grows and the caller undoes the step.
+    IMU_HD bool trial(double& currentChi, double tempChi, double xLxb, bool solved, double& rho) {
+        if (!solved) tempChi = DBL_MAX;
+        rho = currentChi - tempChi;
+        const double scale = xLxb + 1e-3;
+        rho /= scale;
+        if (rho > 0 && tempChi <= DBL_MAX && tempChi >= -DBL_MAX) {      // tempChi finite (NaN and +-inf fail)
+            double alpha = 1. - pow((2 * rho - 1), 3.0);
+            alpha = fmin(alpha, 2. / 3.);
+            lambda *= fmax(1. / 3., alpha);
+            ni = 2;
+            currentChi = tempChi;
+            return true;
+        }
+        lambda *= ni;
+        ni *= 2;
+        return false;
+    }
+    // end of an iteration of qmax trials: false when the optimisation stops
+    IMU_HD bool iteration_done(int qmax, double rho, double iniChi, double currentChi) {
+        if (qmax == maxTrials || rho == 0) return false;
+        if ((iniChi - currentChi) * 1e3 < iniChi) ++nBad; else nBad = 0;
+        return nBad < 3;
+    }
+};
+
+}  // namespace g2o

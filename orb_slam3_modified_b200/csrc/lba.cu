@@ -21,7 +21,6 @@
 // Every reduction is ordered (no floating-point atomics), so results are reproducible run to run.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
-#include <float.h>
 #include <math.h>
 #include <string.h>
 #include <algorithm>
@@ -33,10 +32,14 @@
 #include "../../include/orb_b200.h"
 #include "host_affinity.h"
 #include "device_utils.cuh"
+#include "inertial_dev.cuh"
 
 using orbx::set_error;
 
 namespace lba {
+
+using namespace g2o;
+using orbx::block_sum;
 
 struct Dev {
     int nP, nL, nE, nF, n;            // n = 6 nF
@@ -83,84 +86,6 @@ struct Dev {
     int iterations;
 };
 
-__device__ __forceinline__ void qrot(const double* q, const double* v, double* o) {   // q = (w,x,y,z)
-    double ux = q[2] * v[2] - q[3] * v[1], uy = q[3] * v[0] - q[1] * v[2], uz = q[1] * v[1] - q[2] * v[0];
-    ux += ux; uy += uy; uz += uz;
-    o[0] = v[0] + q[0] * ux + (q[2] * uz - q[3] * uy);
-    o[1] = v[1] + q[0] * uy + (q[3] * ux - q[1] * uz);
-    o[2] = v[2] + q[0] * uz + (q[1] * uy - q[2] * ux);
-}
-__device__ __forceinline__ void qnormalize(double* q) {
-    if (q[0] < 0) { q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3]; }
-    const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    q[0] /= n; q[1] /= n; q[2] /= n; q[3] /= n;
-}
-__device__ __forceinline__ void qtoR(const double* q, double* R) {
-    const double tx = 2 * q[1], ty = 2 * q[2], tz = 2 * q[3];
-    const double twx = tx * q[0], twy = ty * q[0], twz = tz * q[0], txx = tx * q[1], txy = ty * q[1], txz = tz * q[1];
-    const double tyy = ty * q[2], tyz = tz * q[2], tzz = tz * q[3];
-    R[0] = 1 - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
-    R[3] = txy + twz; R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
-    R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1 - (txx + tyy);
-}
-__device__ __forceinline__ void qfromR(const double* m, double* q) {
-    double t = m[0] + m[4] + m[8];
-    if (t > 0) {
-        t = sqrt(t + 1.0);
-        q[0] = 0.5 * t; t = 0.5 / t;
-        q[1] = (m[7] - m[5]) * t; q[2] = (m[2] - m[6]) * t; q[3] = (m[3] - m[1]) * t;
-    } else {
-        int i = 0;
-        if (m[4] > m[0]) i = 1;
-        if (m[8] > m[i * 3 + i]) i = 2;
-        const int j = (i + 1) % 3, k = (j + 1) % 3;
-        t = sqrt(m[i * 3 + i] - m[j * 3 + j] - m[k * 3 + k] + 1.0);
-        double v[3];
-        v[i] = 0.5 * t; t = 0.5 / t;
-        q[0] = (m[k * 3 + j] - m[j * 3 + k]) * t;
-        v[j] = (m[j * 3 + i] + m[i * 3 + j]) * t;
-        v[k] = (m[k * 3 + i] + m[i * 3 + k]) * t;
-        q[1] = v[0]; q[2] = v[1]; q[3] = v[2];
-    }
-}
-// VertexSE3Expmap::oplusImpl: T <- SE3Quat::exp(upd) * T   (g2o/types/se3quat.h:223-256, :101-110)
-__device__ void pose_oplus(double* T, const double* upd) {
-    const double om0 = upd[0], om1 = upd[1], om2 = upd[2];
-    const double theta = sqrt(om0 * om0 + om1 * om1 + om2 * om2);
-    const double O[9] = {0, -om2, om1, om2, 0, -om0, -om1, om0, 0};
-    double O2[9];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) O2[i * 3 + j] = O[i * 3] * O[j] + O[i * 3 + 1] * O[3 + j] + O[i * 3 + 2] * O[6 + j];
-    double a, b, c, d;
-    if (theta < 0.00001) { a = 1.0; b = 1 / 2.0; c = 1 / 2.0; d = 1 / 6.0; }
-    else {
-        a = sin(theta) / theta; b = (1 - cos(theta)) / (theta * theta);
-        c = b; d = (theta - sin(theta)) / pow(theta, 3.0);
-    }
-    double R[9], V[9];
-    for (int i = 0; i < 9; ++i) {
-        const double I = (i % 4 == 0) ? 1.0 : 0.0;
-        R[i] = I + a * O[i] + b * O2[i];
-        V[i] = I + c * O[i] + d * O2[i];
-    }
-    double qe[4]; qfromR(R, qe);
-    const double te[3] = {V[0] * upd[3] + V[1] * upd[4] + V[2] * upd[5], V[3] * upd[3] + V[4] * upd[4] + V[5] * upd[5],
-                          V[6] * upd[3] + V[7] * upd[4] + V[8] * upd[5]};
-    qnormalize(qe);
-    double rt[3]; qrot(qe, T + 4, rt);
-    const double* q2 = T;
-    double qn[4] = {qe[0] * q2[0] - qe[1] * q2[1] - qe[2] * q2[2] - qe[3] * q2[3], qe[0] * q2[1] + qe[1] * q2[0] + qe[2] * q2[3] - qe[3] * q2[2],
-                    qe[0] * q2[2] + qe[2] * q2[0] + qe[3] * q2[1] - qe[1] * q2[3], qe[0] * q2[3] + qe[3] * q2[0] + qe[1] * q2[2] - qe[2] * q2[1]};
-    qnormalize(qn);
-    T[0] = qn[0]; T[1] = qn[1]; T[2] = qn[2]; T[3] = qn[3];
-    T[4] = te[0] + rt[0]; T[5] = te[1] + rt[1]; T[6] = te[2] + rt[2];
-}
-
-__device__ __forceinline__ void robustify(const Dev& D, double e2, double& rho0, double& rho1) {   // RobustKernelHuber
-    if (e2 <= D.dsqr) { rho0 = e2; rho1 = 1.; }
-    else { const double s = sqrt(e2); rho0 = 2 * s * D.delta - D.dsqr; rho1 = D.delta / s; }
-}
-
-
 namespace cg = cooperative_groups;
 __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #ifndef LBA_NT
@@ -190,23 +115,10 @@ struct Ctx {
     const double* pts;     // point estimates of that state
 };
 
-// ordered block reduction of one double per thread; every thread returns the sum
-__device__ __forceinline__ double block_sum(double v, double* sm) {
-    const int tid = threadIdx.x;
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((tid & 31) == 0) sm[tid >> 5] = v;
-    __syncthreads();
-    double r = 0;
-#pragma unroll
-    for (int w = 0; w < NWARP; ++w) r += sm[w];
-    __syncthreads();
-    return r;
-}
 // cluster-wide ordered sum (per-CTA partials -> global slot -> cluster barrier -> added in rank order by every thread);
 // `flagIn` of CTA 0 / thread 0 is broadcast alongside.
 __device__ __forceinline__ double cluster_sum(const Dev& D, Ctx& c, double local, int flagIn, int& flagOut) {
-    const double s = block_sum(local, c.sm);
+    const double s = block_sum<NT>(local, c.sm);
     double* slot = D.partial + (size_t)(c.slot & 3) * PSLOT;
     if (c.tid == 0) {
         slot[c.crank] = s;
@@ -264,7 +176,7 @@ __device__ __forceinline__ double edge_error(const Dev& D, const double* P, cons
     *reinterpret_cast<double2*>(D.err + 2 * (size_t)e) = make_double2(e0, e1);
     const double is2 = (double)D.invSigma2[e];
     double r0, r1;
-    robustify(D, is2 * (e0 * e0 + e1 * e1), r0, r1);
+    huber(is2 * (e0 * e0 + e1 * e1), D.delta, D.dsqr, r0, r1);
     const double iz = 1.0 / zc;
     double2* o = reinterpret_cast<double2*>(Eout + 4 * (size_t)e);
     o[0] = make_double2(xc * iz, yc * iz);
@@ -899,10 +811,9 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
     cluster_sum(D, c, 0.0, (poller && stop && stop[stopIdx]) ? 1 : 0, term);   // initial terminate() poll + publishes the poses
     load_pose_cache(D, Pcur, s_pc);
 
-    double lambda = -1, ni = 2, currentChi = 0, firstChi = 0;
-    int nBad = 0, cj = 0, trials = 0;
-    const int maxTrials = 10;
-    const double goodUpper = 2. / 3., goodLower = 1. / 3., tau = 1e-5;
+    Levenberg lm;
+    double currentChi = 0, firstChi = 0;
+    int cj = 0, trials = 0;
     bool ok = true;
     __shared__ unsigned long long s_tph[11];     // per-phase ns of CTA 0 (thread 0), [10] = tick
     if (c.tid < 11) s_tph[c.tid] = 0;
@@ -917,29 +828,26 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
             currentChi = cluster_sum(D, c, phase_errors(D, c, Elin), 0, dummy);
             TOCK(0);
         }
-        double tempChi = currentChi;
         const double iniChi = currentChi;
         if (it == 0) firstChi = iniChi;
+        // the first iteration starts the LM policy: with the user's lambda before the build, else with H's largest diagonal entry after it
         const bool lambdaKnown = it > 0 || D.userLambdaInit > 0;
-        if (it == 0 && lambdaKnown) lambda = D.userLambdaInit;
+        if (it == 0 && lambdaKnown) lm.start(D.userLambdaInit, 0.0);
         TICK();
-        phase_build_points(D, c, Elin, lambdaKnown ? lambda : -1.0);
+        phase_build_points(D, c, Elin, lambdaKnown ? lm.lambda : -1.0);
         TOCK(1); TICK();
         phase_build_poses_partial(D, c, Elin);
         csync();
         phase_build_poses_combine(D, c);
         TOCK(2);
-        if (it == 0) {
-            if (!lambdaKnown) { csync(); lambda = tau * phase_maxdiag(D, c); }
-            ni = 2; nBad = 0;
-        }
+        if (!lambdaKnown) { csync(); lm.start(0.0, phase_maxdiag(D, c)); }
         bool needPrep = !lambdaKnown;
         double rho = 0;
         int qmax = 0;
         do {
             if (needPrep) {
                 TICK();
-                phase_point_prep(D, c, lambda);
+                phase_point_prep(D, c, lm.lambda);
                 csync();
                 TOCK(3);
             }
@@ -949,7 +857,7 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
                 phase_schur_partial(D, c, D.K);
                 csync();
                 TOCK(4); TICK();
-                phase_schur_combine(D, c, lambda, HsRemote, ld);   // every CTA writes entries into CTA 0's shared memory through DSMEM
+                phase_schur_combine(D, c, lm.lambda, HsRemote, ld);   // every CTA writes entries into CTA 0's shared memory through DSMEM
                 csync();
                 TOCK(6); TICK();
                 if (c.crank == 0) {
@@ -961,23 +869,13 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
                 TOCK(5);
             }
             TICK();
-            const double sP = phase_pose_trial(D, c, Pcur, Ptr, s_pcT, lambda);
+            const double sP = phase_pose_trial(D, c, Pcur, Ptr, s_pcT, lm.lambda);
             TOCK(7); TICK();
-            const double2 sc = phase_points_trial(D, c, Elin, Etrial, Xtr, s_pcT, lambda);
-            double scale0;
+            const double2 sc = phase_points_trial(D, c, Elin, Etrial, Xtr, s_pcT, lm.lambda);
+            double scale0, tempChi;
             cluster_sum2(D, c, sP + sc.x, sc.y, (poller && stop && stop[stopIdx]) ? 1 : 0, term, scale0, tempChi);
             TOCK(8);
-            if (!ok2) tempChi = DBL_MAX;
-            rho = currentChi - tempChi;
-            const double scale = scale0 + 1e-3;
-            rho /= scale;
-            if (rho > 0 && isfinite(tempChi)) {
-                double alpha = 1. - pow((2 * rho - 1), 3.0);
-                alpha = fmin(alpha, goodUpper);
-                const double scaleFactor = fmax(goodLower, alpha);
-                lambda *= scaleFactor;
-                ni = 2;
-                currentChi = tempChi;
+            if (lm.trial(currentChi, tempChi, scale0, ok2, rho)) {
                 double* sw;
                 sw = Elin; Elin = Etrial; Etrial = sw;
                 sw = Pcur; Pcur = Ptr; Ptr = sw;
@@ -985,24 +883,17 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
                 c.pts = Xcur;
                 for (int i = c.tid; i < PC * D.nP; i += NT) s_pc[i] = s_pcT[i];
                 __syncthreads();
-            } else {
-                lambda *= ni;                                   // the trial buffers are simply abandoned (pop)
-                ni *= 2;
-            }
+            }                                                   // a rejected trial's buffers are simply abandoned (pop)
             needPrep = true;
             ++qmax; ++trials;
-        } while (rho < 0 && qmax < maxTrials && !term);
+        } while (rho < 0 && qmax < Levenberg::maxTrials && !term);
         ++cj;
-        if (qmax == maxTrials || rho == 0) ok = false;
-        else {
-            if ((iniChi - currentChi) * 1e3 < iniChi) ++nBad; else nBad = 0;
-            if (nBad >= 3) ok = false;
-        }
+        ok = lm.iteration_done(qmax, rho, iniChi, currentChi);
     }
     phase_finalize(D, c);
     if (Pcur != D.poses) for (int i = c.wid; i < 7 * D.nP; i += c.nw) D.poses[i] = Pcur[i];
     if (c.wid == 0) for (int i = 0; i < 10; ++i) D.stats[8 + i] = (double)s_tph[i];
-    if (c.wid == 0) { D.stats[0] = cj; D.stats[1] = trials; D.stats[2] = lambda; D.stats[3] = currentChi; D.stats[4] = firstChi; }
+    if (c.wid == 0) { D.stats[0] = cj; D.stats[1] = trials; D.stats[2] = lm.lambda; D.stats[3] = currentChi; D.stats[4] = firstChi; }
 }
 
 // =============================================================================================

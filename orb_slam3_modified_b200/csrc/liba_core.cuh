@@ -17,7 +17,6 @@
 // VertexPose (rotation 3, translation 3: tangent of ImuCamPose::Update) | VertexVelocity | VertexGyroBias | VertexAccBias.
 // Sums run in fixed orders (edges of a point / of a keyframe in edge-index order), so a solve is run-to-run reproducible.
 #pragma once
-#include <float.h>
 #include <stdint.h>
 
 #include "inertial_dev.cuh"
@@ -25,6 +24,8 @@
 namespace liba {
 
 using namespace imu;
+using g2o::huber;
+using g2o::Levenberg;
 
 #ifndef LIBA_NT
 #define LIBA_NT 512
@@ -94,11 +95,6 @@ template <int N32> IMU_HD inline void stvec(double* p, const double* r) {
 #else
     for (int k = 0; k < 4 * N32; ++k) p[k] = r[k];
 #endif
-}
-IMU_HD inline void huber(double e2, double delta, double& rho0, double& rho1) {      // RobustKernelHuber::robustify
-    const double dsqr = delta * delta;
-    if (e2 <= dsqr) { rho0 = e2; rho1 = 1.0; }
-    else { const double s = sqrt(e2); rho0 = 2 * s * delta - dsqr; rho1 = delta / s; }
 }
 template <int N> IMU_HD inline double quad(const double* M, const double* e) {
     double s = 0;
@@ -170,7 +166,7 @@ template <class Exec> IMU_HD inline double compute_errors(const Dev& D, Exec& ex
             const double e1 = D.obs[2 * (size_t)e + 1] - ((double)c[1] * Xc[1] / Xc[2] + (double)c[3]);
             D.errM[2 * (size_t)e] = e0; D.errM[2 * (size_t)e + 1] = e1;
             double r0, r1;
-            huber((double)D.invSigma2[e] * (e0 * e0 + e1 * e1), deltaMono, r0, r1);
+            huber((double)D.invSigma2[e] * (e0 * e0 + e1 * e1), deltaMono, deltaMono * deltaMono, r0, r1);
             v += r0;
         }
         for (int i = tid; i < D.nI; i += NT) {
@@ -183,7 +179,7 @@ template <class Exec> IMU_HD inline double compute_errors(const Dev& D, Exec& ex
             const double* k2 = D.kfState + 21 * (size_t)D.ieKf2[i];
             for (int k = 0; k < 3; ++k) { eg[k] = k2[15 + k] - k1[15 + k]; ea[k] = k2[18 + k] - k1[18 + k]; }
             const double c = quad<9>(D.info9 + 81 * (size_t)i, e9);
-            if (D.ieRobust[i]) { double r0, r1; huber(c, deltaInertial, r0, r1); v += r0; } else v += c;
+            if (D.ieRobust[i]) { double r0, r1; huber(c, deltaInertial, deltaInertial * deltaInertial, r0, r1); v += r0; } else v += c;
             v += quad<3>(D.infoG + 9 * (size_t)i, eg) + quad<3>(D.infoA + 9 * (size_t)i, ea);
         }
         return v;
@@ -203,22 +199,12 @@ template <class Exec> IMU_HD inline void build_system(const Dev& D, Exec& ex, do
             const double* T = D.kfTcw + 12 * (size_t)D.eKf[e];
             double Xc[3];
             mono_camera_point(D, e, Xc);
-            const float* c = D.cam + 4 * (size_t)D.eKf[e];
-            const double fx = c[0], fy = c[1];
-            const double pj[6] = {fx / Xc[2], 0, -fx * Xc[0] / (Xc[2] * Xc[2]), 0, fy / Xc[2], -fy * Xc[1] / (Xc[2] * Xc[2])};
             double J[EJ];
             double* A = J; double* B = J + 6;
-            for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) A[i * 3 + j] = -(pj[i * 3] * T[j] + pj[i * 3 + 1] * T[3 + j] + pj[i * 3 + 2] * T[6 + j]);
-            double Xb[3];
-            for (int i = 0; i < 3; ++i) Xb[i] = Rbc[i * 3] * Xc[0] + Rbc[i * 3 + 1] * Xc[1] + Rbc[i * 3 + 2] * Xc[2] + tbc[i];
-            const double x = Xb[0], y = Xb[1], z = Xb[2];
-            const double Sd[18] = {0.0, z, -y, 1.0, 0.0, 0.0, -z, 0.0, x, 0.0, 1.0, 0.0, y, -x, 0.0, 0.0, 0.0, 1.0};
-            double PR[6];
-            for (int i = 0; i < 2; ++i) for (int j = 0; j < 3; ++j) PR[i * 3 + j] = pj[i * 3] * Rcb[j] + pj[i * 3 + 1] * Rcb[3 + j] + pj[i * 3 + 2] * Rcb[6 + j];
-            for (int i = 0; i < 2; ++i) for (int j = 0; j < 6; ++j) B[i * 6 + j] = PR[i * 3] * Sd[j] + PR[i * 3 + 1] * Sd[6 + j] + PR[i * 3 + 2] * Sd[12 + j];
+            mono_jacobians(T, Rcb, Rbc, tbc, D.cam + 4 * (size_t)D.eKf[e], Xc, A, B);
             const double e0 = D.errM[2 * (size_t)e], e1 = D.errM[2 * (size_t)e + 1], om = (double)D.invSigma2[e];
             double r0, r1;
-            huber(om * (e0 * e0 + e1 * e1), deltaMono, r0, r1);
+            huber(om * (e0 * e0 + e1 * e1), deltaMono, deltaMono * deltaMono, r0, r1);
             const double w = r1 * om;
             J[18] = w; J[19] = -om * e0 * r1; J[20] = -om * e1 * r1; J[21] = 0.0; J[22] = 0.0; J[23] = 0.0;
             stvec<6>(D.ejac + (size_t)EJ * e, J);
@@ -235,7 +221,7 @@ template <class Exec> IMU_HD inline void build_system(const Dev& D, Exec& ex, do
             edge_states(D, i, S);
             edge_inertial_dev(D.preint + (size_t)P_SIZE * i, S, e9, D.Jin + 216 * (size_t)i);
             double w = 1.0;
-            if (D.ieRobust[i]) { double r0; huber(quad<9>(D.info9 + 81 * (size_t)i, D.errI + 9 * (size_t)i), deltaInertial, r0, w); }
+            if (D.ieRobust[i]) { double r0; huber(quad<9>(D.info9 + 81 * (size_t)i, D.errI + 9 * (size_t)i), deltaInertial, deltaInertial * deltaInertial, r0, w); }
             D.win[i] = w;
         }
     });
@@ -625,67 +611,45 @@ template <class Exec> IMU_HD inline void run(const Dev& D, Exec& ex) {
     double chiNow = compute_errors(D, ex, deltaMono, deltaInertial);      // the robust chi2 of the errors the edges hold for the current estimate
     const float err = (float)chiNow;
 
-    double lambda = -1, ni = 2;
-    int nBad = 0, cj = 0, trials = 0;
-    const int maxTrials = 10;
+    Levenberg lm;
+    int cj = 0, trials = 0;
     bool ok = true;
     for (int it = 0; it < D.iterations && ok; ++it) {
         // solve() starts with computeActiveErrors(): the estimate has not changed since the last evaluation (the optimize() call itself, or the
         // accepted trial that ended the previous iteration), so the edges already hold exactly these errors
         double currentChi = chiNow;
-        double tempChi = currentChi;
         const double iniChi = currentChi;
         build_system(D, ex, deltaMono, deltaInertial);
         if (it == 0) {
-            if (D.lambdaInit > 0) lambda = D.lambdaInit;
-            else {
-                const double md = ex.max([&](int tid) {
+            double maxDiag = 0;
+            if (!(D.lambdaInit > 0))
+                maxDiag = ex.max([&](int tid) {
                     double m = 0;
                     for (int i = tid; i < n; i += NT) m = fmax(m, fabs(D.H[(size_t)i * n + i]));
                     for (int i = tid; i < 3 * D.nL; i += NT) m = fmax(m, fabs(D.Hll[9 * (size_t)(i / 3) + 4 * (i % 3)]));
                     return m;
                 });
-                lambda = 1e-5 * md;
-            }
-            ni = 2; nBad = 0;
+            lm.start(D.lambdaInit, maxDiag);
         }
         double rho = 0;
         int qmax = 0;
         do {
-            const bool ok2 = solve_system(D, ex, lambda);
+            const bool ok2 = solve_system(D, ex, lm.lambda);
             push_and_update(D, ex);
-            tempChi = compute_errors(D, ex, deltaMono, deltaInertial);
-            if (!ok2) tempChi = DBL_MAX;
-            rho = currentChi - tempChi;
+            const double tempChi = compute_errors(D, ex, deltaMono, deltaInertial);
             ex.tag(7);
-            double scale = ex.sum([&](int tid) {
+            const double scale = ex.sum([&](int tid) {
                 double s = 0;
-                for (int j = tid; j < n; j += NT) s += D.x[j] * (lambda * D.x[j] + D.b[j]);
-                for (int j = tid; j < 3 * D.nL; j += NT) s += D.x[n + j] * (lambda * D.x[n + j] + D.bl[j]);
+                for (int j = tid; j < n; j += NT) s += D.x[j] * (lm.lambda * D.x[j] + D.b[j]);
+                for (int j = tid; j < 3 * D.nL; j += NT) s += D.x[n + j] * (lm.lambda * D.x[n + j] + D.bl[j]);
                 return s;
             });
-            scale += 1e-3;
-            rho /= scale;
-            if (rho > 0 && tempChi <= DBL_MAX && tempChi >= -DBL_MAX) {
-                double alpha = 1. - pow((2 * rho - 1), 3.0);
-                alpha = fmin(alpha, 2. / 3.);
-                lambda *= fmax(1. / 3., alpha);
-                ni = 2;
-                currentChi = tempChi;
-                chiNow = tempChi;
-            } else {
-                lambda *= ni;
-                ni *= 2;
-                pop(D, ex);
-            }
+            if (lm.trial(currentChi, tempChi, scale, ok2, rho)) chiNow = currentChi;
+            else pop(D, ex);
             ++qmax; ++trials;
-        } while (rho < 0 && qmax < maxTrials);
+        } while (rho < 0 && qmax < Levenberg::maxTrials);
         ++cj;
-        if (qmax == maxTrials || rho == 0) ok = false;
-        else {
-            if ((iniChi - currentChi) * 1e3 < iniChi) ++nBad; else nBad = 0;
-            if (nBad >= 3) ok = false;
-        }
+        ok = lm.iteration_done(qmax, rho, iniChi, currentChi);
     }
     ex.tag(7);
     // err_end = activeRobustChi2() of the errors the edges hold (those of a rejected last trial included)
@@ -694,12 +658,12 @@ template <class Exec> IMU_HD inline void run(const Dev& D, Exec& ex) {
         for (int e = tid; e < D.nE; e += NT) {
             const double e0 = D.errM[2 * (size_t)e], e1 = D.errM[2 * (size_t)e + 1];
             double r0, r1;
-            huber((double)D.invSigma2[e] * (e0 * e0 + e1 * e1), deltaMono, r0, r1);
+            huber((double)D.invSigma2[e] * (e0 * e0 + e1 * e1), deltaMono, deltaMono * deltaMono, r0, r1);
             v += r0;
         }
         for (int i = tid; i < D.nI; i += NT) {
             const double c = quad<9>(D.info9 + 81 * (size_t)i, D.errI + 9 * (size_t)i);
-            if (D.ieRobust[i]) { double r0, r1; huber(c, deltaInertial, r0, r1); v += r0; } else v += c;
+            if (D.ieRobust[i]) { double r0, r1; huber(c, deltaInertial, deltaInertial * deltaInertial, r0, r1); v += r0; } else v += c;
             v += quad<3>(D.infoG + 9 * (size_t)i, D.errG + 3 * (size_t)i) + quad<3>(D.infoA + 9 * (size_t)i, D.errA + 3 * (size_t)i);
         }
         return v;
@@ -721,7 +685,7 @@ template <class Exec> IMU_HD inline void run(const Dev& D, Exec& ex) {
         for (int i = tid; i < 12 * D.nKF; i += NT) D.outTcw[i] = D.kfTcw[i];
         for (size_t i = tid; i < (size_t)3 * D.nL; i += NT) D.outPts[i] = D.pts[i];
         if (tid == 0) {
-            D.stats[0] = err; D.stats[1] = errEnd; D.stats[2] = failed ? 1.0 : 0.0; D.stats[3] = lambda; D.stats[4] = trials; D.stats[5] = cj;
+            D.stats[0] = err; D.stats[1] = errEnd; D.stats[2] = failed ? 1.0 : 0.0; D.stats[3] = lm.lambda; D.stats[4] = trials; D.stats[5] = cj;
             D.stats[6] = 0; D.stats[7] = 0;
         }
     });
