@@ -240,6 +240,69 @@ int orbm_search_last_frame_batch_device(orbm_handle* h, const OrbmBatchDevice* i
 int orbm_search_last_frame_batch(orbm_handle* h, const OrbmBatchDevice* in, float th, int checkOrientation,
                                  int32_t* match, uint8_t* claimed, int32_t* nmatches);
 
+/* Tracking::TrackWithMotionModel (reference src/Tracking.cc) from Optimizer::PoseOptimization(&mCurrentFrame) (:2912) through the "discard
+ * outliers" loop, for `batch` streams in three launches; monocular, IMU not initialised.  The caller keeps the nmatches < 20 retry and the
+ * success thresholds (it passes only the streams it wants optimised in `active`, [batch] or NULL = all).
+ * in: the slabs orbm_search_last_frame_batch* took (kps / nK of the current frame, xyz / hasObs of the last frame, cam, nlevels; in->Tcw7 =
+ * the pose the search used); invLevelSigma2 [nlevels] = mvInvLevelSigma2.  match / claimed [batch][kcap] and nmatches [batch] are what the
+ * search wrote and are updated in place.  PoseOptimization's edges are the keypoints i with match[i] >= 0 in ascending i, with
+ * Xw = (double)xyz[match[i]], obs = (double)kps[i].(x, y), invSigma2 = invLevelSigma2[kps[i].octave] (src/Optimizer.cc:877-884), the
+ * initial pose (double) of in->Tcw7, exactly pose_optimization_batch's algorithm.
+ * Out: pose7 [batch][7] (double, what pose_optimization_batch returns), Tcw7 [batch][7] the float pose after SetPose (may alias in->Tcw7;
+ * unchanged with fewer than 3 edges, where the reference returns before SetPose), discarded [batch][mcap] = 1 for the last-frame points of
+ * the outliers (their mnLastFrameSeen = current frame; 0 elsewhere), and for every outlier match = -1, claimed = 0, nmatches - 1;
+ * nmatchesMap [batch] = inliers whose point has observations.  Streams not in `active` are left untouched. */
+int orbm_motion_model_pose_batch_device(orbm_handle* h, const OrbmBatchDevice* in, const float* d_invLevelSigma2, const uint8_t* d_active,
+                                        int32_t* d_match, uint8_t* d_claimed, int32_t* d_nmatches, double* d_pose7, float* d_Tcw7,
+                                        uint8_t* d_discarded, int32_t* d_nmatchesMap, void* stream);
+/* Same with HOST pointers everywhere (one upload, three launches, one download); octaves and match indices out of range are rejected. */
+int orbm_motion_model_pose_batch(orbm_handle* h, const OrbmBatchDevice* in, const float* invLevelSigma2, const uint8_t* active, int32_t* match,
+                                 uint8_t* claimed, int32_t* nmatches, double* pose7, float* Tcw7, uint8_t* discarded, int32_t* nmatchesMap);
+
+/* Tracking::TrackLocalMap (reference src/Tracking.cc:2952) from SearchLocalPoints (:3346) through the statistics loop that sets
+ * mnMatchesInliers, for `batch` streams; monocular, IMU not initialised (so PoseOptimization runs), not only-tracking.  The caller keeps
+ * UpdateLocalMap (it provides the local map and lastToLocal), the thresholds, and the IncreaseVisible / IncreaseFound calls (visible /
+ * found say how many).  Precondition: every non-bad point the frame holds is in its local map (true on this path: UpdateLocalKeyFrames votes
+ * with the frame's matches), so a match without a local index is one the reference dropped.  On the device, per stream:
+ *   1. SearchLocalPoints' first loop: match[i] is remapped to its local index (lastToLocal[match[i]]; -1 or a bad point: match = -1);
+ *      a kept point gets visible += 1 and is "seen"; a point TrackWithMotionModel discarded is seen too (no visible count).
+ *   2. UpdatePoseMatrices from Tcw7; 3. isInFrustum + PredictScale (viewingCosLimit) for points neither seen nor bad: in view -> visible += 1;
+ *      nToMatch = the number in view.  4. SearchByProjection (local map; th[stream], nnratio, bFarPoints / thFarPoints): a keypoint is
+ *      claimed at entry when its point has observations; nmatches = its return value (0 when nToMatch == 0).
+ *   5. PoseOptimization over all matches (Xw = local worldPos) and SetPose; 6. found += 1 per inlier, mnMatchesInliers = inliers whose
+ *      point has observations.
+ * Five launches whatever the batch size. */
+typedef struct OrbmLocalMapBatch {
+    int batch, kcap, mcap, mcapLast, nlevels;
+    const OrbKeyPoint* kps; const uint8_t* desc; const int32_t* nK;   /* current frame [batch][kcap], [batch][kcap][32], [batch] */
+    float minX, minY, maxX, maxY;
+    const float* scaleFactors; const float* invLevelSigma2;          /* mvScaleFactors, mvInvLevelSigma2 [nlevels] */
+    float cam[4]; float mbf; float logScaleFactor;                    /* fx fy cx cy; mbf; mfLogScaleFactor */
+    const float* Tcw7;                                                /* [batch][7] the frame's pose (after the motion-model step) */
+    const int32_t* lastToLocal;   /* [batch][mcapLast]: local index of each last-frame point, -1 = bad; NULL: match is in local indices */
+    const uint8_t* discarded;     /* [batch][mcapLast] from the motion-model step ([batch][mcap] local indices without lastToLocal); may be NULL */
+    const int32_t* nM;            /* [batch] local points (mvpLocalMapPoints.size()) */
+    const float *worldPos, *normal;                                   /* [batch][mcap][3] */
+    const float *minDistInv, *maxDistInv, *maxDistance;               /* [batch][mcap]: GetMin/MaxDistanceInvariance(), mfMaxDistance */
+    const uint8_t *mpDesc, *hasObs, *bad;                             /* [batch][mcap][32], Observations() > 0, isBad() */
+    const float* th;              /* [batch]: 1 on the plain monocular path, 5 right after relocalisation, 15 when lost */
+    float nnratio; int bFarPoints; float thFarPoints; float viewingCosLimit;   /* 0.8, mbFarPoints, mThFarPoints, 0.5 */
+    const uint8_t* active;        /* [batch] or NULL = all; inactive streams are left untouched */
+} OrbmLocalMapBatch;
+typedef struct OrbmLocalMapResult {
+    int32_t* match;                /* [batch][kcap] in: as the motion-model step left it (last-frame or local indices); out: local indices */
+    uint8_t* claimed; uint8_t* outlier;                               /* [batch][kcap]: Observations() > 0 of the match, mvbOutlier */
+    int32_t* visible; int32_t* found;                                 /* [batch][mcap]: IncreaseVisible / IncreaseFound counts */
+    int32_t *nToMatch, *nmatches, *nInliers, *nMatchesInliers;        /* [batch] */
+    double* pose7; float* Tcw7;                                       /* [batch][7]: optimised pose (double) and SetPose's float pose */
+} OrbmLocalMapResult;
+int orbm_track_local_map_batch_device(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, void* stream);
+/* HOST pointers in `in` and `out` (one upload, five launches, one download); out-of-range octaves, match and lastToLocal indices are
+ * rejected; a slab wider than max_mappoints is ORB_ERR_CAPACITY. */
+int orbm_track_local_map_batch(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out);
+/* Same with the current frame on the device (in->kps, in->desc, in->nK from orbx_resident_slabs, stride in->kcap). */
+int orbm_track_local_map_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out);
+
 /* int ORBmatcher::SearchForInitialization(Frame &F1, Frame &F2, vector<cv::Point2f> &vbPrevMatched, vector<int> &vnMatches12,
  * int windowSize) (include/ORBmatcher.h:74, src/ORBmatcher.cc:648-763): the windowed brute-force search of the monocular
  * initialiser (Tracking::MonocularInitialization, src/Tracking.cc:2494-2495, nnratio 0.9, window 100).  F1.K <= max_mappoints and

@@ -217,6 +217,32 @@ protected:
     int device_;
 };
 
+// Tracking's per-frame steps after the last-frame search for a batch of streams (monocular, IMU not initialised; INTEGRATION.md §2):
+// TrackWithMotionModel's PoseOptimization + "discard outliers" loop, and TrackLocalMap from SearchLocalPoints through the statistics
+// loop.  Unlike ORBmatcher above it owns its matcher handle, sized for the batch; host pointers throughout.
+class BatchTracker {
+public:
+    BatchTracker(int max_batch, int max_keypoints, int max_mappoints, int device = 0) {
+        orb_check(orbm_create(&h_, max_batch, max_keypoints, max_mappoints, device), "orbm_create");
+    }
+    ~BatchTracker() { if (h_) orbm_destroy(h_); }
+    BatchTracker(const BatchTracker&) = delete;
+    BatchTracker& operator=(const BatchTracker&) = delete;
+    // in: the slabs of orbm_search_last_frame_batch; match / claimed / nmatches: what that search wrote (updated in place)
+    void MotionModelPose(const OrbmBatchDevice& in, const float* invLevelSigma2, const uint8_t* active, int32_t* match, uint8_t* claimed,
+                         int32_t* nmatches, double* pose7, float* Tcw7, uint8_t* discarded, int32_t* nmatchesMap) {
+        orb_check(orbm_motion_model_pose_batch(h_, &in, invLevelSigma2, active, match, claimed, nmatches, pose7, Tcw7, discarded, nmatchesMap),
+                  "orbm_motion_model_pose_batch");
+    }
+    void TrackLocalMap(const OrbmLocalMapBatch& in, const OrbmLocalMapResult& out) {
+        orb_check(orbm_track_local_map_batch(h_, &in, &out), "orbm_track_local_map_batch");
+    }
+    int LastLaunchCount() const { return orbm_last_launch_count(h_); }
+
+private:
+    orbm_handle* h_ = nullptr;
+};
+
 class Optimizer {
 public:
     // void static LocalBundleAdjustment(KeyFrame* pKF, bool* pbStopFlag, Map* pMap, int& num_fixedKF, int& num_OptKF, int& num_MPs, int& num_edges)

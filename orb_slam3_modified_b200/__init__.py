@@ -301,6 +301,22 @@ class _OrbmBatchDevice(C.Structure):
                 ('mpDesc', C.c_void_p), ('Tcw7', C.c_void_p), ('cam', C.c_float * 4), ('resetState', C.c_int)]
 
 
+class _OrbmLocalMapBatch(C.Structure):
+    _fields_ = ([(n, C.c_int) for n in ('batch', 'kcap', 'mcap', 'mcapLast', 'nlevels')] + [(n, C.c_void_p) for n in ('kps', 'desc', 'nK')] +
+                [(n, C.c_float) for n in ('minX', 'minY', 'maxX', 'maxY')] + [('scaleFactors', C.c_void_p), ('invLevelSigma2', C.c_void_p),
+                 ('cam', C.c_float * 4), ('mbf', C.c_float), ('logScaleFactor', C.c_float)] +
+                [(n, C.c_void_p) for n in ('Tcw7', 'lastToLocal', 'discarded', 'nM', 'worldPos', 'normal', 'minDistInv', 'maxDistInv', 'maxDistance',
+                                           'mpDesc', 'hasObs', 'bad', 'th')] +
+                [('nnratio', C.c_float), ('bFarPoints', C.c_int), ('thFarPoints', C.c_float), ('viewingCosLimit', C.c_float), ('active', C.c_void_p)])
+
+
+_LOCAL_MAP_OUT = ('match', 'claimed', 'outlier', 'visible', 'found', 'nToMatch', 'nmatches', 'nInliers', 'nMatchesInliers', 'pose7', 'Tcw7')
+
+
+class _OrbmLocalMapResult(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in _LOCAL_MAP_OUT]
+
+
 def _c(a, dt):
     return np.ascontiguousarray(a, dt)
 
@@ -462,6 +478,103 @@ class ORBmatcher:
         rc = fn(self._h, C.byref(s), th, int(self.mbCheckOrientation), _ptr(match), _ptr(claimed), _ptr(nmatches))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_last_frame_batch')
+
+    # --- Tracking's per-frame steps after the last-frame search, batched over streams (include/orb_b200.h) ---
+    def motion_model_pose_batch(self, d, inv_level_sigma2, match, claimed, nmatches, active=None):
+        """TrackWithMotionModel from PoseOptimization through the "discard outliers" loop for ``d['batch']`` streams (host numpy).
+        ``d``: the dict ``search_last_frame_batch`` took (kps, nK, xyz, hasObs, Tcw7, cam, kcap, mcap, nlevels are read); ``match`` /
+        ``claimed`` [B, kcap] and ``nmatches`` [B] are what the search wrote and are updated in place; ``active`` [B] u8 or None.
+        Returns dict(pose7 [B,7] f64, Tcw7 [B,7] f32, discarded [B,mcap] u8, nmatchesMap [B] i32); rows of inactive streams are zero."""
+        B, K, M = d['batch'], d['kcap'], d['mcap']
+        s = _OrbmBatchDevice()
+        s.batch, s.kcap, s.mcap, s.nlevels = B, K, M, d['nlevels']
+        keep = dict(kps=_c(d['kps'], KP_DTYPE), nK=_c(d['nK'], np.int32), xyz=_c(d['xyz'], np.float32), hasObs=_c(d['hasObs'], np.uint8),
+                    Tcw7=_c(d['Tcw7'], np.float32))
+        for k, a in keep.items():
+            setattr(s, k, a.ctypes.data)
+        s.cam = (C.c_float * 4)(*d['cam'])
+        isg = _c(inv_level_sigma2, np.float32)
+        act = None if active is None else _c(active, np.uint8)
+        out = dict(pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32), discarded=np.zeros((B, M), np.uint8), nmatchesMap=np.zeros(B, np.int32))
+        for a, dt in ((match, np.int32), (claimed, np.uint8), (nmatches, np.int32)):
+            assert a.dtype == dt and a.flags.c_contiguous
+        L = lib()
+        L.orbm_motion_model_pose_batch.argtypes = [C.c_void_p] * 11
+        rc = L.orbm_motion_model_pose_batch(self._h, C.byref(s), _ptr(isg), _ptr(act), _ptr(match), _ptr(claimed), _ptr(nmatches),
+                                            *[_ptr(out[k]) for k in ('pose7', 'Tcw7', 'discarded', 'nmatchesMap')])
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_motion_model_pose_batch')
+        return out
+
+    def motion_model_pose_batch_device(self, d, inv_level_sigma2, match, claimed, nmatches, pose7, Tcw7, discarded, nmatchesMap, active=None,
+                                       stream=0):
+        """Device form of :meth:`motion_model_pose_batch`: torch CUDA tensors in ``d`` and as arguments; enqueues on ``stream``."""
+        s = _OrbmBatchDevice()
+        s.batch, s.kcap, s.mcap, s.nlevels = d['batch'], d['kcap'], d['mcap'], d['nlevels']
+        for k in ('kps', 'nK', 'xyz', 'hasObs', 'Tcw7'):
+            setattr(s, k, d[k].data_ptr())
+        s.cam = (C.c_float * 4)(*d['cam'])
+        L = lib()
+        L.orbm_motion_model_pose_batch_device.argtypes = [C.c_void_p] * 12
+        rc = L.orbm_motion_model_pose_batch_device(self._h, C.byref(s), _ptr(inv_level_sigma2), _ptr(active), _ptr(match), _ptr(claimed),
+                                                   _ptr(nmatches), _ptr(pose7), _ptr(Tcw7), _ptr(discarded), _ptr(nmatchesMap), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_motion_model_pose_batch_device')
+
+    @staticmethod
+    def _local_map_struct(d, get):
+        s = _OrbmLocalMapBatch()
+        s.batch, s.kcap, s.mcap, s.nlevels = d['batch'], d['kcap'], d['mcap'], d['nlevels']
+        s.mcapLast = d.get('mcapLast', 0)
+        s.minX, s.minY, s.maxX, s.maxY = d['bounds']
+        s.cam = (C.c_float * 4)(*d['cam'])
+        s.mbf, s.logScaleFactor = float(d.get('mbf', 0.0)), float(np.float32(d['logScaleFactor']))
+        s.nnratio, s.bFarPoints, s.thFarPoints = float(d.get('nnratio', 0.8)), int(d.get('bFarPoints', 0)), float(d.get('thFarPoints', 0.0))
+        s.viewingCosLimit = float(d.get('viewingCosLimit', 0.5))
+        for k in ('kps', 'desc', 'nK', 'scaleFactors', 'invLevelSigma2', 'Tcw7', 'lastToLocal', 'discarded', 'nM', 'worldPos', 'normal', 'minDistInv',
+                  'maxDistInv', 'maxDistance', 'mpDesc', 'hasObs', 'bad', 'th', 'active'):
+            setattr(s, k, get(k))
+        return s
+
+    _LOCAL_MAP_DT = dict(kps=KP_DTYPE, desc=np.uint8, nK=np.int32, scaleFactors=np.float32, invLevelSigma2=np.float32, Tcw7=np.float32,
+                         lastToLocal=np.int32, discarded=np.uint8, nM=np.int32, worldPos=np.float32, normal=np.float32, minDistInv=np.float32,
+                         maxDistInv=np.float32, maxDistance=np.float32, mpDesc=np.uint8, hasObs=np.uint8, bad=np.uint8, th=np.float32, active=np.uint8)
+
+    def track_local_map_batch(self, d, match, resident=None):
+        """TrackLocalMap from SearchLocalPoints through the statistics loop for ``d['batch']`` streams (host numpy; see OrbmLocalMapBatch in
+        include/orb_b200.h for the keys; 'lastToLocal', 'discarded' and 'active' may be None or absent).  ``match`` [B, kcap] i32 is updated
+        in place (local indices afterwards).  ``resident`` = ``ORBextractor.resident_slabs()``: the current frame is read from the device.
+        Returns dict(claimed, outlier [B,kcap] u8, visible, found [B,mcap] i32, nToMatch, nmatches, nInliers, nMatchesInliers [B] i32,
+        pose7 [B,7] f64, Tcw7 [B,7] f32); rows of inactive streams are zero."""
+        B, K, M = d['batch'], d['kcap'], d['mcap']
+        keep = {k: _c(d[k], dt) for k, dt in self._LOCAL_MAP_DT.items() if d.get(k) is not None}
+        if resident is not None:
+            assert resident[3] == K
+            keep.update(kps=resident[0], desc=resident[1], nK=resident[2])
+        s = self._local_map_struct(d, lambda k: (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None)
+        assert match.dtype == np.int32 and match.flags.c_contiguous and match.shape == (B, K)
+        out = dict(match=match, claimed=np.zeros((B, K), np.uint8), outlier=np.zeros((B, K), np.uint8), visible=np.zeros((B, M), np.int32),
+                   found=np.zeros((B, M), np.int32), nToMatch=np.zeros(B, np.int32), nmatches=np.zeros(B, np.int32), nInliers=np.zeros(B, np.int32),
+                   nMatchesInliers=np.zeros(B, np.int32), pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32))
+        r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
+        fn = lib().orbm_track_local_map_batch_resident if resident is not None else lib().orbm_track_local_map_batch
+        fn.argtypes = [C.c_void_p] * 3
+        rc = fn(self._h, C.byref(s), C.byref(r))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_track_local_map_batch')
+        del out['match']
+        return out
+
+    def track_local_map_batch_device(self, d, out, stream=0):
+        """Device form of :meth:`track_local_map_batch`: torch CUDA tensors in ``d`` and ``out`` (keys of OrbmLocalMapResult; out['match']
+        is in / out); enqueues on ``stream``."""
+        s = self._local_map_struct(d, lambda k: d[k].data_ptr() if d.get(k) is not None else None)
+        r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
+        L = lib()
+        L.orbm_track_local_map_batch_device.argtypes = [C.c_void_p] * 4
+        rc = L.orbm_track_local_map_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_track_local_map_batch_device')
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """``int ORBmatcher::SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize)`` (src/ORBmatcher.cc:648-763).

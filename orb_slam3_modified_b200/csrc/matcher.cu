@@ -23,6 +23,8 @@
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
 #include "exact_math.h"
+#include "frame_pose.cuh"
+#include "pose_opt.h"
 #include "staging.h"
 
 using orbx::set_error;
@@ -48,6 +50,8 @@ struct MatchParams {
     float cam[4];
     float th, nnratio, thFar;
     int bFar, checkOri, resetState;
+    const float* thBatch;      // mode 0: per-stream th [batch] instead of th (orbm_track_local_map_batch*); null otherwise
+    const uint8_t* active;     // [batch] streams to run, or null (all)
     int ks, ms, descInSmem;   // shared-memory capacities of match_frame_kernel (keypoints, map points) and where the descriptors live
     // scratch
     float4* query;       // [batch][mcap]  u, v, r, bits(minLevel+1 | (maxLevel+1) << 8 | valid << 16)
@@ -236,7 +240,8 @@ __device__ __forceinline__ bool make_query(const MatchParams& P, int f, int i, f
         if (P.bad[o]) return false;
         const int lvl = min(max(P.level[o], 0), P.nlevels - 1);   // the host entry points reject out-of-range levels; device callers are clamped
         float rr = ((double)P.viewCos[o] > 0.998) ? 2.5f : 4.0f;   // RadiusByViewingCos :215-221
-        if (P.th != 1.0f) rr = fmul(rr, P.th);
+        const float th = P.thBatch ? P.thBatch[f] : P.th;
+        if (th != 1.0f) rr = fmul(rr, th);
         u = P.projX[o]; v = P.projY[o];
         r = fmul(rr, P.scaleFactors[lvl]);
         minL = lvl - 1; maxL = lvl;
@@ -325,6 +330,7 @@ __global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
     cg::cluster_group cluster = cg::this_cluster();
     const int C = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
     const int f = blockIdx.x / C, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (P.active && !P.active[f]) return;          // the whole cluster of an inactive stream leaves before its first cluster barrier
     const int K = min(P.nK[f], P.kcap), M = min(P.nM[f], P.mcap);
     const FrameSmem S = carve_frame_smem(smem_raw, P.ks, P.ms, P.descInSmem != 0);
     const OrbKeyPoint* kps = P.kps + (size_t)f * P.kcap;
@@ -1257,13 +1263,14 @@ struct Matcher {
     float4* d_query = nullptr; int4 *d_resultIdx = nullptr, *d_resultDist = nullptr;
     int* d_status = nullptr;
     int numSMs = 132;
+    uint8_t* d_track = nullptr;                          // scratch of the batched tracking calls, allocated by their first call (track_scratch)
     Staging staging;                                     // the single-call host entry points' operands
     uint8_t* d_batch = nullptr; size_t batchBytes = 0;   // device staging of search_last_frame_batch_host (copied straight from the caller)
     int launches = 0;
 
     ~Matcher() {
         cudaSetDevice(device);
-        void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_batch};
+        void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_batch, d_track};
         for (void* p : ptrs) if (p) cudaFree(p);
         if (evWait) cudaEventDestroy(evWait);
         if (stream) cudaStreamDestroy(stream);
@@ -1315,6 +1322,33 @@ struct Matcher {
     }
     int lastCluster = 1;
 
+    // The batched tracking calls' scratch, sized for max_batch x max_keypoints / max_mappoints: PoseOptimization's gathered edges
+    // ([B][kcap]), the frustum stage's per-point fields and flags ([B][mcap]) and the motion-model step's nInliers ([B]).
+    struct TrackScratch {
+        double *Xw, *obs, *err; float* is2; uint8_t* outl; int* edgeKp;
+        uint8_t *seen, *inView; float *projX, *projY, *depth, *viewCos; int *level, *nInliers;
+        int* N; double *poseIn, *poseTmp; float* cam4; int* nInlTmp;
+    } ts;
+    int track_scratch() {
+        if (d_track) return ORB_OK;
+        const size_t BK = (size_t)maxBatch * kcap, BM = (size_t)maxBatch * mcap;
+        const size_t B = maxBatch;
+        const size_t sizes[] = {24 * BK, 16 * BK, 16 * BK, 4 * BK, BK, 4 * BK, BM, BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * B, 4 * B, 56 * B, 56 * B, 16 * B, 4 * B};
+        size_t total = 0;
+        for (size_t b : sizes) total += (b + 255) & ~(size_t)255;
+        CK(cudaMalloc(&d_track, total));
+        void** slots[] = {(void**)&ts.Xw, (void**)&ts.obs, (void**)&ts.err, (void**)&ts.is2, (void**)&ts.outl, (void**)&ts.edgeKp, (void**)&ts.seen,
+                          (void**)&ts.inView, (void**)&ts.projX, (void**)&ts.projY, (void**)&ts.depth, (void**)&ts.viewCos, (void**)&ts.level,
+                          (void**)&ts.nInliers, (void**)&ts.N, (void**)&ts.poseIn, (void**)&ts.poseTmp, (void**)&ts.cam4, (void**)&ts.nInlTmp};
+        size_t off = 0;
+        for (int k = 0; k < 19; ++k) { *slots[k] = d_track + off; off += (sizes[k] + 255) & ~(size_t)255; }
+        return ORB_OK;
+    }
+    void bind_gather(poseopt::GatherArgs& A) const {
+        A.Xw = ts.Xw; A.obs = ts.obs; A.err = ts.err; A.invSigma2 = ts.is2; A.outlier = ts.outl; A.edgeKp = ts.edgeKp;
+        A.N = ts.N; A.poseIn = ts.poseIn; A.poseTmp = ts.poseTmp; A.cam4 = ts.cam4; A.nInlTmp = ts.nInlTmp;
+    }
+
     // SearchForInitialization: F2 in shared memory (K2 keypoints), K1 keypoints of F1 as the queries
     int run_init(MatchParams& P, int K2, int K1, cudaStream_t st) {
         P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX);
@@ -1352,11 +1386,11 @@ struct FrustumParams {
     int nLevels;
     uint8_t* inView; float *projX, *projY, *projXR, *depth, *viewCos; int* level;
 };
-__global__ void frustum_project_kernel(FrustumParams Q) {
+// One map point: the body of frustum_project_kernel and of the batched frustum stage of orbm_track_local_map_batch* (tlm_frustum_kernel).
+// Q supplies the pose, camera and image bounds and the point arrays (P, N, minD, maxD, maxRaw); the results go to the references.
+__device__ __forceinline__ void frustum_point(const FrustumParams& Q, int i, uint8_t& in, float& px, float& py, float& pxr, float& dep, float& vc, int& lvl) {
     using namespace orbx;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= Q.M) return;
-    uint8_t in = 0; float px = -1.f, py = -1.f, pxr = 0.f, dep = 0.f, vc = 0.f; int lvl = -1;
+    in = 0; px = -1.f; py = -1.f; pxr = 0.f; dep = 0.f; vc = 0.f; lvl = -1;
     const float X = Q.P[3 * i], Y = Q.P[3 * i + 1], Z = Q.P[3 * i + 2];
     const float xc = fadd(fadd(fadd(fmul(Q.R[0], X), fmul(Q.R[1], Y)), fmul(Q.R[2], Z)), Q.t[0]);
     const float yc = fadd(fadd(fadd(fmul(Q.R[3], X), fmul(Q.R[4], Y)), fmul(Q.R[5], Z)), Q.t[1]);
@@ -1381,7 +1415,79 @@ __global__ void frustum_project_kernel(FrustumParams Q) {
             }
         }
     }
+}
+__global__ void frustum_project_kernel(FrustumParams Q) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Q.M) return;
+    uint8_t in; float px, py, pxr, dep, vc; int lvl;
+    frustum_point(Q, i, in, px, py, pxr, dep, vc, lvl);
     Q.inView[i] = in; Q.projX[i] = px; Q.projY[i] = py; Q.projXR[i] = pxr; Q.depth[i] = dep; Q.level[i] = lvl; Q.viewCos[i] = vc;
+}
+
+// ---- Tracking::SearchLocalPoints (src/Tracking.cc:3346) up to the search, one CTA per stream: the first loop over the frame's matches
+//      (a bad point is dropped; the others are counted visible and marked seen -- mnLastFrameSeen), the points TrackWithMotionModel
+//      discarded marked seen, Frame::UpdatePoseMatrices, then Frame::isInFrustum (frustum_point) for every local point neither seen
+//      nor bad; a point in view is counted visible and becomes a query of the search.  claimed = the kept point has observations. ----
+struct TrackLocalParams {
+    int batch, kcap, mcap, mcapLast;
+    const uint8_t* active; const int *nK, *nM;
+    int* match; uint8_t* claimed;                        // [batch][kcap]
+    const int* lastToLocal; const uint8_t* discarded;    // [batch][mcapLast] (discarded: [batch][mcap] without lastToLocal)
+    const float* Tcw7;                                   // [batch][7]
+    FrustumParams F;                                     // camera, bounds, limits; point arrays = the [batch][mcap] slabs
+    const uint8_t *bad, *hasObs;
+    uint8_t *seen, *inView; float *projX, *projY, *depth, *viewCos; int* level;   // scratch [batch][mcap]
+    int *visible, *found, *nToMatch;
+};
+constexpr int TL_NT = 512;
+__global__ void __launch_bounds__(TL_NT) tlm_frustum_kernel(TrackLocalParams T) {
+    __shared__ FrustumParams s_Q;
+    __shared__ int s_n;
+    const int f = blockIdx.x, tid = threadIdx.x;
+    if (T.active && !T.active[f]) return;
+    const int K = min(T.nK[f], T.kcap), M = min(T.nM[f], T.mcap);
+    const size_t kb = (size_t)f * T.kcap, pb = (size_t)f * T.mcap;
+    if (tid == 0) {
+        s_Q = T.F;
+        s_Q.M = M; s_Q.P = T.F.P + 3 * pb; s_Q.N = T.F.N + 3 * pb; s_Q.minD = T.F.minD + pb; s_Q.maxD = T.F.maxD + pb; s_Q.maxRaw = T.F.maxRaw + pb;
+        update_pose_matrices(T.Tcw7 + 7 * (size_t)f, s_Q.R, s_Q.t, s_Q.Ow);
+        s_n = 0;
+    }
+    for (int p = tid; p < T.mcap; p += TL_NT) { T.seen[pb + p] = 0; T.inView[pb + p] = 0; T.visible[pb + p] = 0; T.found[pb + p] = 0; }
+    for (int i = K + tid; i < T.kcap; i += TL_NT) T.claimed[kb + i] = 0;
+    __syncthreads();
+    for (int i = tid; i < K; i += TL_NT) {
+        const int m = T.match[kb + i];
+        if (m < 0) { T.claimed[kb + i] = 0; continue; }
+        const int p = T.lastToLocal ? (m < T.mcapLast ? T.lastToLocal[(size_t)f * T.mcapLast + m] : -1) : m;
+        if (p < 0 || p >= M || T.bad[pb + p]) { T.match[kb + i] = -1; T.claimed[kb + i] = 0; continue; }
+        T.match[kb + i] = p; T.claimed[kb + i] = T.hasObs[pb + p] ? 1 : 0;
+        atomicAdd(&T.visible[pb + p], 1);
+        T.seen[pb + p] = 1;
+    }
+    if (T.discarded) {
+        const int n = T.lastToLocal ? T.mcapLast : M;
+        const size_t db = (size_t)f * (T.lastToLocal ? T.mcapLast : T.mcap);
+        for (int j = tid; j < n; j += TL_NT) {
+            if (!T.discarded[db + j]) continue;
+            const int p = T.lastToLocal ? T.lastToLocal[db + j] : j;
+            if (p >= 0 && p < M) T.seen[pb + p] = 1;
+        }
+    }
+    __syncthreads();
+    int cnt = 0;
+    for (int p = tid; p < M; p += TL_NT) {
+        if (T.seen[pb + p] || T.bad[pb + p]) continue;
+        uint8_t in; float px, py, pxr, dep, vc; int lvl;
+        frustum_point(s_Q, p, in, px, py, pxr, dep, vc, lvl);
+        if (!in) continue;
+        T.inView[pb + p] = 1; T.projX[pb + p] = px; T.projY[pb + p] = py; T.depth[pb + p] = dep; T.viewCos[pb + p] = vc; T.level[pb + p] = lvl;
+        T.visible[pb + p] += 1;
+        ++cnt;
+    }
+    if (cnt) atomicAdd(&s_n, cnt);
+    __syncthreads();
+    if (tid == 0) T.nToMatch[f] = s_n;
 }
 
 }  // namespace orbm
@@ -1963,6 +2069,223 @@ int orbm_descriptor_distance(orbm_handle* h, const uint8_t* a, const uint8_t* b,
     CK(cudaGetLastError());
     CK(S.download(st));
     return ORB_OK;
+}
+
+
+// ---- TrackWithMotionModel's pose step and TrackLocalMap for a batch of streams (include/orb_b200.h) ----
+static bool batch_shape_ok(const Matcher& m, int batch, int kcap, int mcap, int nlevels) {
+    return batch >= 1 && batch <= m.maxBatch && kcap >= 1 && kcap <= m.kcap && mcap >= 1 && nlevels >= 1 && nlevels <= 256;
+}
+static int motion_model_pose_launch(Matcher& m, const OrbmBatchDevice* in, const float* invLevelSigma2, const uint8_t* active, int32_t* match,
+                                    uint8_t* claimed, int32_t* nmatches, double* pose7, float* Tcw7, uint8_t* discarded, int32_t* nmatchesMap,
+                                    cudaStream_t st) {
+    int rc = m.track_scratch();
+    if (rc) return rc;
+    poseopt::GatherArgs A; memset(&A, 0, sizeof(A));
+    A.batch = in->batch; A.kcap = in->kcap; A.pstride = in->mcap; A.nlevels = in->nlevels; A.mode = poseopt::MOTION_MODEL;
+    A.active = active; A.kps = in->kps; A.nK = in->nK; A.match = match; A.claimed = claimed; A.nmatches = nmatches;
+    A.xyz = in->xyz; A.hasObs = in->hasObs; A.invLevelSigma2 = invLevelSigma2; memcpy(A.cam, in->cam, 16);
+    A.TcwIn = in->Tcw7; A.TcwOut = Tcw7; A.poseOut = pose7; A.nInliers = m.ts.nInliers; A.discarded = discarded; A.nmatchesMap = nmatchesMap;
+    m.bind_gather(A);
+    CK(poseopt::launch_gathered(A, st));
+    m.launches = 3;
+    return ORB_OK;
+}
+
+int orbm_motion_model_pose_batch_device(orbm_handle* h, const OrbmBatchDevice* in, const float* d_invLevelSigma2, const uint8_t* d_active,
+                                        int32_t* d_match, uint8_t* d_claimed, int32_t* d_nmatches, double* d_pose7, float* d_Tcw7,
+                                        uint8_t* d_discarded, int32_t* d_nmatchesMap, void* stream) {
+    if (!h || !in || !batch_shape_ok(h->m, in->batch, in->kcap, in->mcap, in->nlevels) || !in->kps || !in->nK || !in->xyz || !in->hasObs ||
+        !in->Tcw7 || !d_invLevelSigma2 || !d_match || !d_claimed || !d_nmatches || !d_pose7 || !d_Tcw7 || !d_discarded || !d_nmatchesMap) {
+        set_error("orbm_motion_model_pose_batch_device: bad argument (sizes or null slabs)"); return ORB_ERR_ARG;
+    }
+    CK(cudaSetDevice(h->m.device));
+    return motion_model_pose_launch(h->m, in, d_invLevelSigma2, d_active, d_match, d_claimed, d_nmatches, d_pose7, d_Tcw7, d_discarded,
+                                    d_nmatchesMap, (cudaStream_t)stream);
+}
+
+// Copies row b of a downloaded piece to the caller for the active streams only (inactive streams are left untouched).
+static void copy_active_rows(const Staging& S, int piece, void* dst, size_t rowBytes, int batch, const uint8_t* active) {
+    if (!dst) return;
+    const uint8_t* src = S.host(piece);
+    for (int b = 0; b < batch; ++b)
+        if (!active || active[b]) memcpy((uint8_t*)dst + b * rowBytes, src + b * rowBytes, rowBytes);
+}
+
+int orbm_motion_model_pose_batch(orbm_handle* h, const OrbmBatchDevice* in, const float* invLevelSigma2, const uint8_t* active, int32_t* match,
+                                 uint8_t* claimed, int32_t* nmatches, double* pose7, float* Tcw7, uint8_t* discarded, int32_t* nmatchesMap) {
+    if (!h || !in || !batch_shape_ok(h->m, in->batch, in->kcap, in->mcap, in->nlevels) || !in->kps || !in->nK || !in->xyz || !in->hasObs ||
+        !in->Tcw7 || !invLevelSigma2 || !match || !claimed || !nmatches || !pose7 || !Tcw7 || !discarded || !nmatchesMap) {
+        set_error("orbm_motion_model_pose_batch: bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
+    }
+    Matcher& m = h->m;
+    const size_t B = in->batch, K = in->kcap, M = in->mcap;
+    for (size_t b = 0; b < B; ++b) {
+        if (active && !active[b]) continue;
+        if (in->nK[b] < 0 || in->nK[b] > in->kcap) { set_error("orbm_motion_model_pose_batch: nK out of range"); return ORB_ERR_ARG; }
+        for (int i = 0; i < in->nK[b]; ++i) {
+            const int oct = in->kps[b * K + i].octave, mt = match[b * K + i];
+            if (oct < 0 || oct >= in->nlevels) { set_error("orbm_motion_model_pose_batch: keypoint octave out of range"); return ORB_ERR_ARG; }
+            if (mt < -1 || mt >= in->mcap) { set_error("orbm_motion_model_pose_batch: match index out of range"); return ORB_ERR_ARG; }
+        }
+    }
+    CK(cudaSetDevice(m.device));
+    Staging& S = m.staging;
+    S.begin();
+    const int pKps = S.in(in->kps, 28 * B * K), pNK = S.in(in->nK, 4 * B), pXyz = S.in(in->xyz, 12 * B * M), pObs = S.in(in->hasObs, B * M),
+              pT = S.in(in->Tcw7, 28 * B), pIs = S.in(invLevelSigma2, 4 * (size_t)in->nlevels), pAct = S.in(active, active ? B : 0),
+              pMatch = S.inout(match, 4 * B * K), pCl = S.inout(claimed, B * K), pN = S.inout(nmatches, 4 * B), pPose = S.out(nullptr, 56 * B),
+              pTo = S.out(nullptr, 28 * B), pDis = S.out(nullptr, B * M), pMap = S.out(nullptr, 4 * B);
+    int rc = S.reserve();
+    if (rc) return rc;
+    OrbmBatchDevice d = *in;
+    d.kps = S.dev<OrbKeyPoint>(pKps); d.nK = S.dev<int>(pNK); d.xyz = S.dev<float>(pXyz); d.hasObs = S.dev(pObs); d.Tcw7 = S.dev<float>(pT);
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    rc = motion_model_pose_launch(m, &d, S.dev<float>(pIs), active ? S.dev(pAct) : nullptr, S.dev<int>(pMatch), S.dev(pCl), S.dev<int>(pN),
+                                  S.dev<double>(pPose), S.dev<float>(pTo), S.dev(pDis), S.dev<int>(pMap), st);
+    if (rc) return rc;
+    CK(S.download(st));
+    copy_active_rows(S, pPose, pose7, 56, in->batch, active);
+    copy_active_rows(S, pTo, Tcw7, 28, in->batch, active);
+    copy_active_rows(S, pDis, discarded, M, in->batch, active);
+    copy_active_rows(S, pMap, nmatchesMap, 4, in->batch, active);
+    return ORB_OK;
+}
+
+static int track_local_map_launch(Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, cudaStream_t st) {
+    int rc = m.track_scratch();
+    if (rc) return rc;
+    const Matcher::TrackScratch& ts = m.ts;
+    TrackLocalParams T; memset(&T, 0, sizeof(T));
+    T.batch = in->batch; T.kcap = in->kcap; T.mcap = in->mcap; T.mcapLast = in->lastToLocal ? in->mcapLast : 0;
+    T.active = in->active; T.nK = in->nK; T.nM = in->nM; T.match = out->match; T.claimed = out->claimed;
+    T.lastToLocal = in->lastToLocal; T.discarded = in->discarded; T.Tcw7 = in->Tcw7;
+    T.F.P = in->worldPos; T.F.N = in->normal; T.F.minD = in->minDistInv; T.F.maxD = in->maxDistInv; T.F.maxRaw = in->maxDistance;
+    memcpy(T.F.cam, in->cam, 16);
+    T.F.minX = in->minX; T.F.minY = in->minY; T.F.maxX = in->maxX; T.F.maxY = in->maxY; T.F.mbf = in->mbf; T.F.logSF = in->logScaleFactor;
+    T.F.cosLimit = in->viewingCosLimit; T.F.nLevels = in->nlevels;
+    T.bad = in->bad; T.hasObs = in->hasObs;
+    T.seen = ts.seen; T.inView = ts.inView; T.projX = ts.projX; T.projY = ts.projY; T.depth = ts.depth; T.viewCos = ts.viewCos; T.level = ts.level;
+    T.visible = out->visible; T.found = out->found; T.nToMatch = out->nToMatch;
+    tlm_frustum_kernel<<<in->batch, TL_NT, 0, st>>>(T);
+    CK(cudaGetLastError());
+    MatchParams P; memset(&P, 0, sizeof(P));
+    P.batch = in->batch; P.kcap = in->kcap; P.mcap = in->mcap; P.nlevels = in->nlevels; P.mode = 0;
+    P.kps = in->kps; P.desc = in->desc; P.nK = in->nK;
+    P.minX = in->minX; P.minY = in->minY; P.maxX = in->maxX; P.maxY = in->maxY;
+    P.scaleFactors = in->scaleFactors; P.nM = in->nM;
+    P.inView = ts.inView; P.bad = in->bad; P.depth = ts.depth; P.projX = ts.projX; P.projY = ts.projY; P.level = ts.level; P.viewCos = ts.viewCos;
+    P.hasObs = in->hasObs; P.mpDesc = in->mpDesc;
+    P.th = 1.0f; P.thBatch = in->th; P.nnratio = in->nnratio; P.bFar = in->bFarPoints; P.thFar = in->thFarPoints; P.active = in->active;
+    P.match = out->match; P.claimed = out->claimed; P.nmatches = out->nmatches;
+    if ((rc = m.run(P, in->kcap, in->mcap, st))) return rc;
+    poseopt::GatherArgs A; memset(&A, 0, sizeof(A));
+    A.batch = in->batch; A.kcap = in->kcap; A.pstride = in->mcap; A.nlevels = in->nlevels; A.mode = poseopt::LOCAL_MAP;
+    A.active = in->active; A.kps = in->kps; A.nK = in->nK; A.match = out->match; A.claimed = out->claimed;
+    A.xyz = in->worldPos; A.hasObs = in->hasObs; A.invLevelSigma2 = in->invLevelSigma2; memcpy(A.cam, in->cam, 16);
+    A.TcwIn = in->Tcw7; A.TcwOut = out->Tcw7; A.poseOut = out->pose7; A.nInliers = out->nInliers;
+    A.outlierKp = out->outlier; A.found = out->found; A.nMatchesInliers = out->nMatchesInliers;
+    m.bind_gather(A);
+    CK(poseopt::launch_gathered(A, st));
+    m.launches = 5;
+    return ORB_OK;
+}
+
+// Argument checks shared by the three forms that need no host-side data.  ORB_ERR_CAPACITY for a slab wider than the handle's capacities.
+static int local_map_shape(const Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, const char* who) {
+    if (!in || !out || !batch_shape_ok(m, in->batch, in->kcap, in->mcap, in->nlevels) || (in->lastToLocal && in->mcapLast < 1) || !in->kps ||
+        !in->desc || !in->nK || !in->scaleFactors || !in->invLevelSigma2 || !in->Tcw7 || !in->nM || !in->worldPos || !in->normal ||
+        !in->minDistInv || !in->maxDistInv || !in->maxDistance || !in->mpDesc || !in->hasObs || !in->bad || !in->th || !(in->maxX > in->minX) ||
+        !(in->maxY > in->minY) || !out->match || !out->claimed || !out->outlier || !out->visible || !out->found || !out->nToMatch ||
+        !out->nmatches || !out->nInliers || !out->nMatchesInliers || !out->pose7 || !out->Tcw7) {
+        set_error(std::string(who) + ": bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
+    }
+    if (in->mcap > m.mcap) { set_error(std::string(who) + ": more local map points than max_mappoints"); return ORB_ERR_CAPACITY; }
+    if (frame_smem_bytes(in->kcap, in->mcap, false) > 227 * 1024 - 2048) { set_error(std::string(who) + ": frame too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
+    return ORB_OK;
+}
+
+int orbm_track_local_map_batch_device(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, void* stream) {
+    if (!h) { set_error("orbm_track_local_map_batch_device: bad argument"); return ORB_ERR_ARG; }
+    if (int rc = local_map_shape(h->m, in, out, "orbm_track_local_map_batch_device")) return rc;
+    CK(cudaSetDevice(h->m.device));
+    return track_local_map_launch(h->m, in, out, (cudaStream_t)stream);
+}
+
+static int track_local_map_host(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, bool frameOnDevice) {
+    const char* who = frameOnDevice ? "orbm_track_local_map_batch_resident" : "orbm_track_local_map_batch";
+    if (!h) { set_error(std::string(who) + ": bad argument"); return ORB_ERR_ARG; }
+    if (int rc = local_map_shape(h->m, in, out, who)) return rc;
+    Matcher& m = h->m;
+    const size_t B = in->batch, K = in->kcap, M = in->mcap, ML = in->lastToLocal ? in->mcapLast : 0;
+    const uint8_t* active = in->active;
+    for (size_t b = 0; b < B; ++b) {
+        if (active && !active[b]) continue;
+        const int nM = in->nM[b];
+        if (nM < 0 || nM > in->mcap) { set_error(std::string(who) + ": nM out of range"); return ORB_ERR_ARG; }
+        if (!(in->th[b] > 0.0f)) { set_error(std::string(who) + ": th must be positive"); return ORB_ERR_ARG; }
+        if (!frameOnDevice) {
+            if (in->nK[b] < 0 || in->nK[b] > in->kcap) { set_error(std::string(who) + ": nK out of range"); return ORB_ERR_ARG; }
+            for (int i = 0; i < in->nK[b]; ++i) {
+                const int oct = in->kps[b * K + i].octave;
+                if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return ORB_ERR_ARG; }
+            }
+        }
+        for (size_t i = 0; i < K; ++i) {
+            const int mt = out->match[b * K + i];
+            if (mt < -1 || mt >= (in->lastToLocal ? in->mcapLast : in->mcap)) { set_error(std::string(who) + ": match index out of range"); return ORB_ERR_ARG; }
+        }
+        for (size_t j = 0; j < ML; ++j)
+            if (in->lastToLocal[b * ML + j] < -1 || in->lastToLocal[b * ML + j] >= nM) { set_error(std::string(who) + ": lastToLocal index out of range"); return ORB_ERR_ARG; }
+    }
+    CK(cudaSetDevice(m.device));
+    Staging& S = m.staging;
+    S.begin();
+    const size_t DL = in->discarded ? (in->lastToLocal ? ML : M) : 0;
+    const int pKps = S.in(frameOnDevice ? nullptr : in->kps, frameOnDevice ? 0 : 28 * B * K), pDesc = S.in(frameOnDevice ? nullptr : in->desc, frameOnDevice ? 0 : 32 * B * K),
+              pNK = S.in(frameOnDevice ? nullptr : in->nK, frameOnDevice ? 0 : 4 * B), pSf = S.in(in->scaleFactors, 4 * (size_t)in->nlevels),
+              pIs = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels), pT = S.in(in->Tcw7, 28 * B), pL2L = S.in(in->lastToLocal, 4 * B * ML),
+              pDis = S.in(in->discarded, B * DL), pNM = S.in(in->nM, 4 * B), pWp = S.in(in->worldPos, 12 * B * M), pNo = S.in(in->normal, 12 * B * M),
+              pMin = S.in(in->minDistInv, 4 * B * M), pMax = S.in(in->maxDistInv, 4 * B * M), pRaw = S.in(in->maxDistance, 4 * B * M),
+              pMd = S.in(in->mpDesc, 32 * B * M), pObs = S.in(in->hasObs, B * M), pBad = S.in(in->bad, B * M), pTh = S.in(in->th, 4 * B),
+              pAct = S.in(active, active ? B : 0), pMatch = S.inout(out->match, 4 * B * K), pCl = S.out(nullptr, B * K), pOut = S.out(nullptr, B * K),
+              pVis = S.out(nullptr, 4 * B * M), pFound = S.out(nullptr, 4 * B * M), pCounts = S.out(nullptr, 16 * B), pPose = S.out(nullptr, 56 * B),
+              pTo = S.out(nullptr, 28 * B);
+    int rc = S.reserve();
+    if (rc) return rc;
+    OrbmLocalMapBatch d = *in;
+    if (!frameOnDevice) { d.kps = S.dev<OrbKeyPoint>(pKps); d.desc = S.dev(pDesc); d.nK = S.dev<int>(pNK); }
+    d.scaleFactors = S.dev<float>(pSf); d.invLevelSigma2 = S.dev<float>(pIs); d.Tcw7 = S.dev<float>(pT);
+    d.lastToLocal = in->lastToLocal ? S.dev<int>(pL2L) : nullptr; d.discarded = in->discarded ? S.dev(pDis) : nullptr; d.nM = S.dev<int>(pNM);
+    d.worldPos = S.dev<float>(pWp); d.normal = S.dev<float>(pNo); d.minDistInv = S.dev<float>(pMin); d.maxDistInv = S.dev<float>(pMax);
+    d.maxDistance = S.dev<float>(pRaw); d.mpDesc = S.dev(pMd); d.hasObs = S.dev(pObs); d.bad = S.dev(pBad); d.th = S.dev<float>(pTh);
+    d.active = active ? S.dev(pAct) : nullptr;
+    int* counts = S.dev<int>(pCounts);      // nToMatch | nmatches | nInliers | nMatchesInliers, [B] each
+    OrbmLocalMapResult o = {S.dev<int>(pMatch), S.dev(pCl), S.dev(pOut), S.dev<int>(pVis), S.dev<int>(pFound), counts, counts + B, counts + 2 * B,
+                            counts + 3 * B, S.dev<double>(pPose), S.dev<float>(pTo)};
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    if ((rc = track_local_map_launch(m, &d, &o, st))) return rc;
+    CK(S.download(st));
+    copy_active_rows(S, pCl, out->claimed, K, in->batch, active);
+    copy_active_rows(S, pOut, out->outlier, K, in->batch, active);
+    copy_active_rows(S, pVis, out->visible, 4 * M, in->batch, active);
+    copy_active_rows(S, pFound, out->found, 4 * M, in->batch, active);
+    copy_active_rows(S, pPose, out->pose7, 56, in->batch, active);
+    copy_active_rows(S, pTo, out->Tcw7, 28, in->batch, active);
+    const int* hc = S.host<int>(pCounts);
+    int32_t* dst[4] = {out->nToMatch, out->nmatches, out->nInliers, out->nMatchesInliers};
+    for (size_t b = 0; b < B; ++b)
+        if (!active || active[b]) for (int k = 0; k < 4; ++k) dst[k][b] = hc[k * B + b];
+    return ORB_OK;
+}
+
+int orbm_track_local_map_batch(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out) {
+    return track_local_map_host(h, in, out, false);
+}
+int orbm_track_local_map_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out) {
+    return track_local_map_host(h, in, out, true);
 }
 
 }  // extern "C"

@@ -9,7 +9,9 @@
 #include <string>
 
 #include "../../include/orb_b200.h"
+#include "frame_pose.cuh"
 #include "inertial_dev.cuh"
+#include "pose_opt.h"
 #include "staging.h"
 
 using orbx::set_error;
@@ -188,6 +190,94 @@ __global__ void __launch_bounds__(NT) pose_opt_kernel(Params P) {
     }
     if (tid < 7) P.poseOut[7 * (size_t)f + tid] = s_T[tid];
     if (tid == 0) P.nInliers[f] = N - nBad;
+}
+
+// ---- The batched tracking calls (pose_opt.h): the matches of every stream are compacted into the packed arrays above, pose_opt_kernel
+// runs on them unchanged -- the very instructions pose_optimization_batch runs, so the poses equal its results bit for bit -- and a third
+// kernel applies SetPose and the Tracking loop that reads the outlier flags.  One CTA per stream in each.
+
+// Block-wide compaction of the matched keypoints in keypoint order (ballot + warp offsets per tile of NT keypoints), plus the initial
+// pose and the camera in pose_opt_kernel's layout.  An inactive stream gets N = 0.
+__global__ void __launch_bounds__(NT) gather_edges_kernel(GatherArgs A) {
+    __shared__ int s_cnt[NT / 32];
+    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (A.active && !A.active[f]) { if (tid == 0) A.N[f] = 0; return; }
+    const size_t kb = (size_t)f * A.kcap, pb = (size_t)f * A.pstride;
+    const int K = min(A.nK[f], A.kcap);
+    if (tid < 7) A.poseIn[7 * (size_t)f + tid] = (double)A.TcwIn[7 * (size_t)f + tid];
+    if (tid < 4) A.cam4[4 * f + tid] = A.cam[tid];
+    int base = 0;
+    for (int t0 = 0; t0 < K; t0 += NT) {
+        const int i = t0 + tid;
+        const int m = i < K ? A.match[kb + i] : -1;
+        const unsigned bits = __ballot_sync(0xffffffffu, m >= 0);
+        if (lane == 0) s_cnt[wid] = __popc(bits);
+        __syncthreads();
+        int off = 0, tot = 0;
+#pragma unroll
+        for (int w = 0; w < NT / 32; ++w) { off += w < wid ? s_cnt[w] : 0; tot += s_cnt[w]; }
+        if (m >= 0) {
+            const size_t e = kb + base + off + __popc(bits & ((1u << lane) - 1u));
+            const OrbKeyPoint kp = A.kps[kb + i];
+            const float* X = A.xyz + 3 * (pb + m);
+            A.Xw[3 * e] = (double)X[0]; A.Xw[3 * e + 1] = (double)X[1]; A.Xw[3 * e + 2] = (double)X[2];
+            A.obs[2 * e] = (double)kp.x; A.obs[2 * e + 1] = (double)kp.y;
+            A.invSigma2[e] = A.invLevelSigma2[min(max(kp.octave, 0), A.nlevels - 1)];   // the host entry points reject out-of-range octaves
+            A.edgeKp[e] = i;
+        }
+        base += tot;
+        __syncthreads();
+    }
+    if (tid == 0) A.N[f] = base;
+}
+
+// SetPose (none when PoseOptimization returned early with fewer than 3 edges), then the Tracking loop over the frame's matches.
+__global__ void __launch_bounds__(NT) gathered_finish_kernel(GatherArgs A) {
+    __shared__ int s_n[2];
+    const int f = blockIdx.x, tid = threadIdx.x;
+    if (A.active && !A.active[f]) return;
+    const size_t kb = (size_t)f * A.kcap, pb = (size_t)f * A.pstride;
+    const int N = A.N[f];
+    if (tid < 2) s_n[tid] = 0;
+    if (tid < 7) A.poseOut[7 * (size_t)f + tid] = A.poseTmp[7 * (size_t)f + tid];
+    if (tid == 0) A.nInliers[f] = A.nInlTmp[f];
+    if (N >= 3) { if (tid == 0) orbm::set_pose_from_double(A.poseTmp + 7 * (size_t)f, A.TcwOut + 7 * (size_t)f); }
+    else if (tid < 7) A.TcwOut[7 * (size_t)f + tid] = A.TcwIn[7 * (size_t)f + tid];
+    if (A.mode == MOTION_MODEL) for (int p = tid; p < A.pstride; p += NT) A.discarded[pb + p] = 0;
+    else for (int i = tid; i < A.kcap; i += NT) A.outlierKp[kb + i] = 0;
+    __syncthreads();
+    const uint8_t* outl = A.outlier + kb;
+    int nOut = 0, nObs = 0;
+    for (int e = tid; e < N; e += NT) {
+        const int i = A.edgeKp[kb + e];
+        const int p = A.match[kb + i];
+        if (A.mode == MOTION_MODEL) {
+            if (outl[e]) { A.match[kb + i] = -1; A.claimed[kb + i] = 0; A.discarded[pb + p] = 1; ++nOut; }
+            else nObs += A.hasObs[pb + p] != 0;
+        } else {
+            A.outlierKp[kb + i] = outl[e];
+            if (!outl[e]) { atomicAdd(&A.found[pb + p], 1); nObs += A.hasObs[pb + p] != 0; }
+        }
+    }
+    if (nOut) atomicAdd(&s_n[0], nOut);
+    if (nObs) atomicAdd(&s_n[1], nObs);
+    __syncthreads();
+    if (tid == 0) {
+        if (A.mode == MOTION_MODEL) { A.nmatches[f] -= s_n[0]; A.nmatchesMap[f] = s_n[1]; }
+        else A.nMatchesInliers[f] = s_n[1];
+    }
+}
+
+cudaError_t launch_gathered(const GatherArgs& A, cudaStream_t st) {
+    gather_edges_kernel<<<A.batch, NT, 0, st>>>(A);
+    Params P;
+    memset(&P, 0, sizeof(P));
+    P.count = A.batch; P.cap = A.kcap; P.N = A.N; P.pose7 = A.poseIn; P.cam4 = A.cam4;
+    P.Xw = A.Xw; P.obs = A.obs; P.invSigma2 = A.invSigma2; P.delta = (double)(float)sqrt(5.991);   // thHuberMono = sqrt(5.991), a float
+    P.err = A.err; P.poseOut = A.poseTmp; P.outlier = A.outlier; P.nInliers = A.nInlTmp;
+    pose_opt_kernel<<<A.batch, NT, 0, st>>>(P);
+    gathered_finish_kernel<<<A.batch, NT, 0, st>>>(A);
+    return cudaGetLastError();
 }
 
 }  // namespace poseopt
