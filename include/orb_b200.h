@@ -303,6 +303,52 @@ int orbm_track_local_map_batch(orbm_handle* h, const OrbmLocalMapBatch* in, cons
 /* Same with the current frame on the device (in->kps, in->desc, in->nK from orbx_resident_slabs, stride in->kcap). */
 int orbm_track_local_map_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out);
 
+/* Tracking::Track for a monocular-inertial frame once the IMU is initialised and the frame is past the relocalisation reset window, for
+ * `batch` streams (RECENTLY_LOST streams too, with th = 15): TrackWithMotionModel's PredictStateIMU and TrackLocalMap through the
+ * statistics loop.  The caller keeps PreintegrateIMU, UpdateLocalMap, the thresholds, IncreaseVisible / IncreaseFound and the choice of
+ * the streams that take this path (imu->mode).  On the device, per stream with mode 1 (mbMapUpdated: from the last keyframe) or 2 (from
+ * the last frame):
+ *   1. PredictStateIMU in float (source state, its bias and preintegration by mode; gravity (0, 0, -9.81f)) and
+ *      Frame::SetImuPoseVelocity: predState21 / predTcw7.
+ *   2. SearchLocalPoints with the frame holding no point (match starts at -1): isInFrustum + PredictScale for every non-bad local point,
+ *      visible += 1 when in view, then the local-map SearchByProjection with th[stream] (as orbm_track_local_map_batch*).
+ *   3. PoseInertialOptimizationLastKeyFrame (mode 1) or PoseInertialOptimizationLastFrame (mode 2), bRecInit = false, over the matches
+ *      in ascending keypoint order: Xw = local worldPos, obs = keypoint, invSigma2 = invLevelSigma2[octave], trackDepth = the depth the
+ *      frustum test just computed; the current frame's vertices are the double of predState21 (ImuCamPose(Frame*)), the fixed last
+ *      keyframe / free previous frame the double of kfState21 / lastState21, the prior (mode 2) prior21 / priorH.  A stream without
+ *      matches runs it with the inertial edges only.
+ *   4. SetImuPoseVelocity of the float estimate and mImuBias = the optimised bias (Tcw7, state21), mvbOutlier (outlier), mpcpi =
+ *      ConstraintPoseImu(double estimate, H) (prior21, priorH: symmetrised, eigenvalues below 1e-12 clamped), found += 1 per inlier,
+ *      nMatchesInliers = inliers whose point has observations, nInliers = the optimiser's return value.
+ * in: as orbm_track_local_map_batch* with in->Tcw7, in->lastToLocal, in->discarded and in->active NULL.  out: out->pose7 NULL,
+ * out->match output only.  Outputs of one call feed the next unchanged (state21 -> lastState21, prior21 / priorH -> the same fields).
+ * Streams with mode 0 are left untouched.  At most seven launches whatever the batch size (six with one optimiser variant). */
+typedef struct OrbmImuTrackBatch {
+    const uint8_t* mode;          /* HOST [batch] in every form: 0 skip, 1 map updated (last keyframe), 2 not updated (last frame) */
+    float Tcb7[7];                /* mImuCalib.mTcb as Sophus keeps it: unit quaternion (w, x, y, z) + t (one rig per call) */
+    const double* extrinsics24;   /* Rcb | tcb | Rbc | tbc, as the inertial optimisers take it */
+    const float* preintKF;        /* [batch][IMU_PREINT_FLOATS] mpImuPreintegratedFromLastKF (= mCurrentFrame.mpImuPreintegrated) */
+    const float* preintFrame;     /* [batch][IMU_PREINT_FLOATS] mCurrentFrame.mpImuPreintegratedFrame (mode 2) */
+    const float* kfState21;       /* [batch][21] mpLastKeyFrame: GetImuRotation | GetImuPosition | GetVelocity | gyro bias | acc bias (mode 1) */
+    const float* lastState21;     /* [batch][21] mLastFrame, same layout (mode 2) */
+    const double *prior21, *priorH;  /* [batch][21], [batch][225]: mLastFrame.mpcpi (mode 2) */
+} OrbmImuTrackBatch;
+typedef struct OrbmImuTrackResult {
+    float* predState21;           /* [batch][21] the frame after PredictStateIMU */
+    float* predTcw7;              /* [batch][7] its mTcw: the pose SearchLocalPoints projected with */
+    float* state21;               /* [batch][21] the frame after the write-back: the next call's lastState21 */
+    double *prior21, *priorH;     /* [batch][21], [batch][225]: the new mpcpi */
+} OrbmImuTrackResult;
+int orbm_track_local_map_inertial_batch_device(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu,
+                                               const OrbmLocalMapResult* out, const OrbmImuTrackResult* imuOut, void* stream);
+/* HOST pointers in `in`, `imu`, `out` and `imuOut` (one upload, the launches, one download); out-of-range octaves are rejected; a slab
+ * wider than max_mappoints is ORB_ERR_CAPACITY. */
+int orbm_track_local_map_inertial_batch(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu, const OrbmLocalMapResult* out,
+                                        const OrbmImuTrackResult* imuOut);
+/* Same with the current frame on the device (in->kps, in->desc, in->nK from orbx_resident_slabs, stride in->kcap). */
+int orbm_track_local_map_inertial_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu,
+                                                 const OrbmLocalMapResult* out, const OrbmImuTrackResult* imuOut);
+
 /* int ORBmatcher::SearchForInitialization(Frame &F1, Frame &F2, vector<cv::Point2f> &vbPrevMatched, vector<int> &vnMatches12,
  * int windowSize) (include/ORBmatcher.h:74, src/ORBmatcher.cc:648-763): the windowed brute-force search of the monocular
  * initialiser (Tracking::MonocularInitialization, src/Tracking.cc:2494-2495, nnratio 0.9, window 100).  F1.K <= max_mappoints and

@@ -217,9 +217,10 @@ protected:
     int device_;
 };
 
-// Tracking's per-frame steps after the last-frame search for a batch of streams (monocular, IMU not initialised; INTEGRATION.md §2):
-// TrackWithMotionModel's PoseOptimization + "discard outliers" loop, and TrackLocalMap from SearchLocalPoints through the statistics
-// loop.  Unlike ORBmatcher above it owns its matcher handle, sized for the batch; host pointers throughout.
+// Tracking's per-frame steps after the last-frame search for a batch of streams (INTEGRATION.md §2): monocular with the IMU not
+// initialised, TrackWithMotionModel's PoseOptimization + "discard outliers" loop and TrackLocalMap from SearchLocalPoints through the
+// statistics loop; monocular-inertial with the IMU initialised, PredictStateIMU and TrackLocalMap with the inertial pose optimisers.
+// Unlike ORBmatcher above it owns its matcher handle, sized for the batch; host pointers throughout.
 class BatchTracker {
 public:
     BatchTracker(int max_batch, int max_keypoints, int max_mappoints, int device = 0) {
@@ -236,6 +237,12 @@ public:
     }
     void TrackLocalMap(const OrbmLocalMapBatch& in, const OrbmLocalMapResult& out) {
         orb_check(orbm_track_local_map_batch(h_, &in, &out), "orbm_track_local_map_batch");
+    }
+    // Monocular-inertial frames once the IMU is initialised: PredictStateIMU, SearchLocalPoints, PoseInertialOptimizationLast{KeyFrame,Frame}
+    // and its write-back for every stream with imu.mode != 0 (in.Tcw7 / lastToLocal / discarded / active and out.pose7 NULL).  Feed
+    // imuOut.state21 / prior21 / priorH back as the next call's lastState21 / prior21 / priorH.
+    void TrackLocalMapInertial(const OrbmLocalMapBatch& in, const OrbmImuTrackBatch& imu, const OrbmLocalMapResult& out, const OrbmImuTrackResult& imuOut) {
+        orb_check(orbm_track_local_map_inertial_batch(h_, &in, &imu, &out, &imuOut), "orbm_track_local_map_inertial_batch");
     }
     int LastLaunchCount() const { return orbm_last_launch_count(h_); }
 

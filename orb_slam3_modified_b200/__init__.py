@@ -317,6 +317,18 @@ class _OrbmLocalMapResult(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _LOCAL_MAP_OUT]
 
 
+class _OrbmImuTrackBatch(C.Structure):
+    _fields_ = [('mode', C.c_void_p), ('Tcb7', C.c_float * 7)] + [(n, C.c_void_p) for n in ('extrinsics24', 'preintKF', 'preintFrame', 'kfState21',
+                                                                                            'lastState21', 'prior21', 'priorH')]
+
+
+_IMU_TRACK_OUT = ('predState21', 'predTcw7', 'state21', 'prior21', 'priorH')
+
+
+class _OrbmImuTrackResult(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in _IMU_TRACK_OUT]
+
+
 def _c(a, dt):
     return np.ascontiguousarray(a, dt)
 
@@ -575,6 +587,64 @@ class ORBmatcher:
         rc = L.orbm_track_local_map_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_local_map_batch_device')
+
+    _IMU_DT = dict(preintKF=np.float32, preintFrame=np.float32, kfState21=np.float32, lastState21=np.float32, prior21=np.float64, priorH=np.float64)
+
+    @staticmethod
+    def _imu_struct(imu, mode, get):
+        s = _OrbmImuTrackBatch()
+        s.mode = mode.ctypes.data
+        s.Tcb7 = (C.c_float * 7)(*[float(v) for v in np.asarray(imu['Tcb7'], np.float32)])
+        for k in ('extrinsics24',) + tuple(ORBmatcher._IMU_DT):
+            setattr(s, k, get(k))
+        return s
+
+    def track_local_map_inertial_batch(self, d, imu, resident=None):
+        """Tracking::Track for monocular-inertial frames once the IMU is initialised (PredictStateIMU, SearchLocalPoints, the inertial pose
+        optimiser and its write-back) for ``d['batch']`` streams, host numpy.  ``d``: the keys of :meth:`track_local_map_batch` without
+        Tcw7 / lastToLocal / discarded / active; ``imu``: mode [B] u8 (0 skip, 1 map updated, 2 not), Tcb7 [7], extrinsics24 [24], preintKF /
+        preintFrame [B, IMU_PREINT_FLOATS], kfState21 / lastState21 [B, 21] f32, prior21 [B, 21] / priorH [B, 15, 15] f64 (see
+        OrbmImuTrackBatch in include/orb_b200.h; arrays a call does not need may be None).  Returns dict(match, claimed, outlier [B, kcap],
+        visible, found [B, mcap], nToMatch, nmatches, nInliers, nMatchesInliers [B], Tcw7 [B, 7], predState21 [B, 21], predTcw7 [B, 7],
+        state21 [B, 21], prior21 [B, 21], priorH [B, 15, 15]); rows of mode-0 streams keep their initial values (match -1, the rest 0)."""
+        B, K, M = d['batch'], d['kcap'], d['mcap']
+        keep = {k: _c(d[k], dt) for k, dt in self._LOCAL_MAP_DT.items() if d.get(k) is not None}
+        if resident is not None:
+            assert resident[3] == K
+            keep.update(kps=resident[0], desc=resident[1], nK=resident[2])
+        s = self._local_map_struct(d, lambda k: (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None)
+        ik = {k: _c(imu[k], dt) for k, dt in dict(self._IMU_DT, extrinsics24=np.float64).items() if imu.get(k) is not None}
+        mode = _c(imu['mode'], np.uint8)
+        si = self._imu_struct(imu, mode, lambda k: ik[k].ctypes.data if k in ik else None)
+        out = dict(match=np.full((B, K), -1, np.int32), claimed=np.zeros((B, K), np.uint8), outlier=np.zeros((B, K), np.uint8),
+                   visible=np.zeros((B, M), np.int32), found=np.zeros((B, M), np.int32), nToMatch=np.zeros(B, np.int32), nmatches=np.zeros(B, np.int32),
+                   nInliers=np.zeros(B, np.int32), nMatchesInliers=np.zeros(B, np.int32), pose7=None, Tcw7=np.zeros((B, 7), np.float32))
+        io = dict(predState21=np.zeros((B, 21), np.float32), predTcw7=np.zeros((B, 7), np.float32), state21=np.zeros((B, 21), np.float32),
+                  prior21=np.zeros((B, 21)), priorH=np.zeros((B, 15, 15)))
+        r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
+        ri = _OrbmImuTrackResult(*[_ptr(io[k]) for k in _IMU_TRACK_OUT])
+        fn = lib().orbm_track_local_map_inertial_batch_resident if resident is not None else lib().orbm_track_local_map_inertial_batch
+        fn.argtypes = [C.c_void_p] * 5
+        rc = fn(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_track_local_map_inertial_batch')
+        del out['pose7']
+        out.update(io)
+        return out
+
+    def track_local_map_inertial_batch_device(self, d, imu, out, stream=0):
+        """Device form of :meth:`track_local_map_inertial_batch`: torch CUDA tensors in ``d``, ``imu`` (imu['mode'] stays a host numpy
+        array) and ``out`` (keys of OrbmLocalMapResult without pose7, and of OrbmImuTrackResult); enqueues on ``stream``."""
+        s = self._local_map_struct(d, lambda k: d[k].data_ptr() if d.get(k) is not None else None)
+        mode = _c(imu['mode'], np.uint8)
+        si = self._imu_struct(imu, mode, lambda k: imu[k].data_ptr() if imu.get(k) is not None else None)
+        r = _OrbmLocalMapResult(*[_ptr(out[k]) if k != 'pose7' else None for k in _LOCAL_MAP_OUT])
+        ri = _OrbmImuTrackResult(*[_ptr(out[k]) for k in _IMU_TRACK_OUT])
+        L = lib()
+        L.orbm_track_local_map_inertial_batch_device.argtypes = [C.c_void_p] * 6
+        rc = L.orbm_track_local_map_inertial_batch_device(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_track_local_map_inertial_batch_device')
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """``int ORBmatcher::SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize)`` (src/ORBmatcher.cc:648-763).

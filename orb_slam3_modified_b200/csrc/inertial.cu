@@ -18,6 +18,7 @@
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
 #include "inertial_dev.cuh"
+#include "pose_inertial.h"
 #include "staging.h"
 
 using orbx::set_error;
@@ -540,6 +541,32 @@ __global__ void __launch_bounds__(PI_NT) pose_inertial_opt_kernel(PoseInertialPa
     }
     __syncthreads();
     if (tid < 21) { Q.state[21 * (size_t)f + tid] = s_st[tid]; if (LF) Q.prevState[21 * (size_t)f + tid] = s_sp[tid]; }
+}
+
+// The two optimiser launches of the mono-inertial tracking call (pose_inertial.h): pose_inertial_opt_kernel<false> / <true> over the dense
+// sub-batches the gather stage of track_inertial.cu wrote, one launch per variant that has streams.
+int launch_inertial_optimisers(const ImuTrackArgs& A, cudaStream_t st) {
+    int launches = 0;
+    for (int v = 0; v < 2; ++v) {
+        const int n = A.count[v];
+        if (!n) continue;
+        const size_t g0 = v ? A.count[0] : 0, K = A.kcap;
+        PoseInertialParams Q;
+        Q.count = n; Q.cap = A.kcap; Q.recInit = 0;
+        Q.N = A.N + g0; Q.Xw = A.Xw + 3 * g0 * K; Q.obs = A.obs + 2 * g0 * K; Q.invSigma2 = A.invSigma2 + g0 * K; Q.trackDepth = A.trackDepth + g0 * K;
+        Q.cam4 = A.cam4 + 4 * g0; Q.extr = A.extr; Q.preint = A.preint + (size_t)P_SIZE * g0;
+        Q.state = A.state + 21 * g0; Q.err = A.err + 2 * g0 * K; Q.outlier = A.outlier + g0 * K; Q.H15 = A.H15 + 225 * g0; Q.ret = A.ret + g0;
+        if (v == 0) {
+            Q.kfState = A.fixedState; Q.preintKF = nullptr; Q.prior = nullptr; Q.priorH = nullptr; Q.prevState = nullptr;
+            pose_inertial_opt_kernel<false><<<n, PI_NT, 0, st>>>(Q);
+        } else {
+            Q.kfState = nullptr; Q.preintKF = A.preintKF2 + (size_t)P_SIZE * g0; Q.prior = A.prior + 21 * g0; Q.priorH = A.priorH + 225 * g0;
+            Q.prevState = A.fixedState + 21 * g0;          // the previous frame's estimate is discarded afterwards, as in the reference
+            pose_inertial_opt_kernel<true><<<n, PI_NT, 0, st>>>(Q);
+        }
+        ++launches;
+    }
+    return launches;
 }
 
 }  // namespace imu

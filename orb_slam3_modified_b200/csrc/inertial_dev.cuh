@@ -186,6 +186,26 @@ IMU_HD inline void inv_right_jacobian(const double* v, double* J) {
     }
 }
 
+// IMU::Preintegrated::GetDeltaRotation / Velocity / Position(b) (src/ImuTypes.cc:283-307) in float, like the reference: dbgf / dbaf are
+// b - the preintegration's own bias (gyro, acc).  Tracking::PredictStateIMU's deltas (track_inertial.cu).  edge_inertial_dev below
+// evaluates the same expressions inline: routing it through this function changed the register allocation and scheduling of
+// pose_inertial_opt_kernel, whose compiled code stays as it is.
+IMU_HD inline void preint_delta_f(const float* __restrict__ P, const float* dbgf, const float* dbaf, float* Rn, float* dVf, float* dPf) {
+    float w[3], W[9], W2[9], E[9], M[9];
+    m3vec(P + P_JRG, dbgf, w);
+    const float d2 = pm(w[0], w[0]) + pm(w[1], w[1]) + pm(w[2], w[2]), d = sqrtf(d2);
+    hat(w, W); m3mul(W, W, W2);
+    for (int i = 0; i < 9; ++i) {
+        const float I = (i % 4 == 0) ? 1.f : 0.f;
+        E[i] = d < 1e-5f ? I + W[i] + pm(0.5f, W2[i]) : I + pm(W[i], sinf(d)) / d + pm(W2[i], 1.0f - cosf(d)) / d2;
+    }
+    m3mul(P + P_DR, E, M);
+    normalize_rotation(M, Rn);
+    float g1[3], a1[3], g2[3], a2[3];
+    m3vec(P + P_JVG, dbgf, g1); m3vec(P + P_JVA, dbaf, a1); m3vec(P + P_JPG, dbgf, g2); m3vec(P + P_JPA, dbaf, a2);
+    for (int i = 0; i < 3; ++i) { dVf[i] = P[P_DV + i] + g1[i] + a1[i]; dPf[i] = P[P_DP + i] + g2[i] + a2[i]; }
+}
+
 // ---- EdgeInertial: residual, Jacobians, chi2 and robust weight; thread per edge.  states [count][36] doubles:
 //      Rwb1 9 | twb1 3 | v1 3 | bg 3 | ba 3 | Rwb2 9 | twb2 3 | v2 3 ----
 // EdgeInertial::computeError + linearizeOplus for one edge: S = Rwb1 9 | twb1 3 | v1 3 | bg 3 | ba 3 | Rwb2 9 | twb2 3 | v2 3; err [9]; J [9][24] or null

@@ -24,6 +24,7 @@
 #include "device_utils.cuh"
 #include "exact_math.h"
 #include "frame_pose.cuh"
+#include "pose_inertial.h"
 #include "pose_opt.h"
 #include "staging.h"
 
@@ -1267,11 +1268,16 @@ struct Matcher {
     Staging staging;                                     // the single-call host entry points' operands
     uint8_t* d_batch = nullptr; size_t batchBytes = 0;   // device staging of search_last_frame_batch_host (copied straight from the caller)
     int launches = 0;
+    // the device form of the mono-inertial call: pinned mirror of its route / active tables ([maxBatch] int + [maxBatch] u8) and the event
+    // of the copy that last read it (a new call waits for that copy only, never for the caller's stream)
+    uint8_t* h_route = nullptr; cudaEvent_t evRoute = nullptr;
 
     ~Matcher() {
         cudaSetDevice(device);
         void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_batch, d_track};
         for (void* p : ptrs) if (p) cudaFree(p);
+        if (h_route) cudaFreeHost(h_route);
+        if (evRoute) cudaEventDestroy(evRoute);
         if (evWait) cudaEventDestroy(evWait);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -1323,25 +1329,32 @@ struct Matcher {
     int lastCluster = 1;
 
     // The batched tracking calls' scratch, sized for max_batch x max_keypoints / max_mappoints: PoseOptimization's gathered edges
-    // ([B][kcap]), the frustum stage's per-point fields and flags ([B][mcap]) and the motion-model step's nInliers ([B]).
+    // ([B][kcap]), the frustum stage's per-point fields and flags ([B][mcap]) and the motion-model step's nInliers ([B]).  The
+    // mono-inertial call adds its float edges ([B][kcap]: Xw 3, obs 2, trackDepth; it shares is2, err, outl, edgeKp, N and cam4) and
+    // per-slot operands ([B]: route, two preintegrations, fixed / current state, prior, prior and optimised H, return value).
     struct TrackScratch {
         double *Xw, *obs, *err; float* is2; uint8_t* outl; int* edgeKp;
         uint8_t *seen, *inView; float *projX, *projY, *depth, *viewCos; int *level, *nInliers;
         int* N; double *poseIn, *poseTmp; float* cam4; int* nInlTmp;
+        float *iXw, *iObs, *iTd; int* route; uint8_t* active; float *preint, *preintKF2; double *fixedState, *state, *prior, *priorH, *H15; int* ret;
     } ts;
     int track_scratch() {
         if (d_track) return ORB_OK;
         const size_t BK = (size_t)maxBatch * kcap, BM = (size_t)maxBatch * mcap;
-        const size_t B = maxBatch;
-        const size_t sizes[] = {24 * BK, 16 * BK, 16 * BK, 4 * BK, BK, 4 * BK, BM, BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * B, 4 * B, 56 * B, 56 * B, 16 * B, 4 * B};
+        const size_t B = maxBatch, PS = 4 * IMU_PREINT_FLOATS;
+        const size_t sizes[] = {24 * BK, 16 * BK, 16 * BK, 4 * BK, BK, 4 * BK, BM, BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * B, 4 * B, 56 * B, 56 * B, 16 * B, 4 * B,
+                                12 * BK, 8 * BK, 4 * BK, 4 * B, B, PS * B, PS * B, 168 * B, 168 * B, 168 * B, 1800 * B, 1800 * B, 4 * B};
+        constexpr int nSlots = sizeof(sizes) / sizeof(sizes[0]);
         size_t total = 0;
         for (size_t b : sizes) total += (b + 255) & ~(size_t)255;
         CK(cudaMalloc(&d_track, total));
-        void** slots[] = {(void**)&ts.Xw, (void**)&ts.obs, (void**)&ts.err, (void**)&ts.is2, (void**)&ts.outl, (void**)&ts.edgeKp, (void**)&ts.seen,
+        void** slots[nSlots] = {(void**)&ts.Xw, (void**)&ts.obs, (void**)&ts.err, (void**)&ts.is2, (void**)&ts.outl, (void**)&ts.edgeKp, (void**)&ts.seen,
                           (void**)&ts.inView, (void**)&ts.projX, (void**)&ts.projY, (void**)&ts.depth, (void**)&ts.viewCos, (void**)&ts.level,
-                          (void**)&ts.nInliers, (void**)&ts.N, (void**)&ts.poseIn, (void**)&ts.poseTmp, (void**)&ts.cam4, (void**)&ts.nInlTmp};
+                          (void**)&ts.nInliers, (void**)&ts.N, (void**)&ts.poseIn, (void**)&ts.poseTmp, (void**)&ts.cam4, (void**)&ts.nInlTmp,
+                          (void**)&ts.iXw, (void**)&ts.iObs, (void**)&ts.iTd, (void**)&ts.route, (void**)&ts.active, (void**)&ts.preint, (void**)&ts.preintKF2,
+                          (void**)&ts.fixedState, (void**)&ts.state, (void**)&ts.prior, (void**)&ts.priorH, (void**)&ts.H15, (void**)&ts.ret};
         size_t off = 0;
-        for (int k = 0; k < 19; ++k) { *slots[k] = d_track + off; off += (sizes[k] + 255) & ~(size_t)255; }
+        for (int k = 0; k < nSlots; ++k) { *slots[k] = d_track + off; off += (sizes[k] + 255) & ~(size_t)255; }
         return ORB_OK;
     }
     void bind_gather(poseopt::GatherArgs& A) const {
@@ -2153,14 +2166,14 @@ int orbm_motion_model_pose_batch(orbm_handle* h, const OrbmBatchDevice* in, cons
     return ORB_OK;
 }
 
-static int track_local_map_launch(Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, cudaStream_t st) {
-    int rc = m.track_scratch();
-    if (rc) return rc;
+// SearchLocalPoints of both local-map calls: tlm_frustum_kernel, then the local-map search (two launches).  Tcw7: the frame's pose.
+static int search_local_points_launch(Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, const float* Tcw7, const uint8_t* active,
+                                      cudaStream_t st) {
     const Matcher::TrackScratch& ts = m.ts;
     TrackLocalParams T; memset(&T, 0, sizeof(T));
     T.batch = in->batch; T.kcap = in->kcap; T.mcap = in->mcap; T.mcapLast = in->lastToLocal ? in->mcapLast : 0;
-    T.active = in->active; T.nK = in->nK; T.nM = in->nM; T.match = out->match; T.claimed = out->claimed;
-    T.lastToLocal = in->lastToLocal; T.discarded = in->discarded; T.Tcw7 = in->Tcw7;
+    T.active = active; T.nK = in->nK; T.nM = in->nM; T.match = out->match; T.claimed = out->claimed;
+    T.lastToLocal = in->lastToLocal; T.discarded = in->discarded; T.Tcw7 = Tcw7;
     T.F.P = in->worldPos; T.F.N = in->normal; T.F.minD = in->minDistInv; T.F.maxD = in->maxDistInv; T.F.maxRaw = in->maxDistance;
     memcpy(T.F.cam, in->cam, 16);
     T.F.minX = in->minX; T.F.minY = in->minY; T.F.maxX = in->maxX; T.F.maxY = in->maxY; T.F.mbf = in->mbf; T.F.logSF = in->logScaleFactor;
@@ -2177,9 +2190,15 @@ static int track_local_map_launch(Matcher& m, const OrbmLocalMapBatch* in, const
     P.scaleFactors = in->scaleFactors; P.nM = in->nM;
     P.inView = ts.inView; P.bad = in->bad; P.depth = ts.depth; P.projX = ts.projX; P.projY = ts.projY; P.level = ts.level; P.viewCos = ts.viewCos;
     P.hasObs = in->hasObs; P.mpDesc = in->mpDesc;
-    P.th = 1.0f; P.thBatch = in->th; P.nnratio = in->nnratio; P.bFar = in->bFarPoints; P.thFar = in->thFarPoints; P.active = in->active;
+    P.th = 1.0f; P.thBatch = in->th; P.nnratio = in->nnratio; P.bFar = in->bFarPoints; P.thFar = in->thFarPoints; P.active = active;
     P.match = out->match; P.claimed = out->claimed; P.nmatches = out->nmatches;
-    if ((rc = m.run(P, in->kcap, in->mcap, st))) return rc;
+    return m.run(P, in->kcap, in->mcap, st);
+}
+
+static int track_local_map_launch(Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, cudaStream_t st) {
+    int rc = m.track_scratch();
+    if (rc) return rc;
+    if ((rc = search_local_points_launch(m, in, out, in->Tcw7, in->active, st))) return rc;
     poseopt::GatherArgs A; memset(&A, 0, sizeof(A));
     A.batch = in->batch; A.kcap = in->kcap; A.pstride = in->mcap; A.nlevels = in->nlevels; A.mode = poseopt::LOCAL_MAP;
     A.active = in->active; A.kps = in->kps; A.nK = in->nK; A.match = out->match; A.claimed = out->claimed;
@@ -2193,12 +2212,15 @@ static int track_local_map_launch(Matcher& m, const OrbmLocalMapBatch* in, const
 }
 
 // Argument checks shared by the three forms that need no host-side data.  ORB_ERR_CAPACITY for a slab wider than the handle's capacities.
-static int local_map_shape(const Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, const char* who) {
+// inertial: the mono-inertial call's form, where the pose is predicted and the frame holds nothing (Tcw7, lastToLocal, discarded,
+// active and pose7 must be NULL).
+static int local_map_shape(const Matcher& m, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, const char* who, bool inertial = false) {
     if (!in || !out || !batch_shape_ok(m, in->batch, in->kcap, in->mcap, in->nlevels) || (in->lastToLocal && in->mcapLast < 1) || !in->kps ||
-        !in->desc || !in->nK || !in->scaleFactors || !in->invLevelSigma2 || !in->Tcw7 || !in->nM || !in->worldPos || !in->normal ||
+        !in->desc || !in->nK || !in->scaleFactors || !in->invLevelSigma2 || (!in->Tcw7 != inertial) || !in->nM || !in->worldPos || !in->normal ||
         !in->minDistInv || !in->maxDistInv || !in->maxDistance || !in->mpDesc || !in->hasObs || !in->bad || !in->th || !(in->maxX > in->minX) ||
         !(in->maxY > in->minY) || !out->match || !out->claimed || !out->outlier || !out->visible || !out->found || !out->nToMatch ||
-        !out->nmatches || !out->nInliers || !out->nMatchesInliers || !out->pose7 || !out->Tcw7) {
+        !out->nmatches || !out->nInliers || !out->nMatchesInliers || (!out->pose7 != inertial) || !out->Tcw7 ||
+        (inertial && (in->lastToLocal || in->discarded || in->active))) {
         set_error(std::string(who) + ": bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
     }
     if (in->mcap > m.mcap) { set_error(std::string(who) + ": more local map points than max_mappoints"); return ORB_ERR_CAPACITY; }
@@ -2286,6 +2308,171 @@ int orbm_track_local_map_batch(orbm_handle* h, const OrbmLocalMapBatch* in, cons
 }
 int orbm_track_local_map_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out) {
     return track_local_map_host(h, in, out, true);
+}
+
+// ---- TrackLocalMap on the mono-inertial path, after PredictStateIMU, for a batch of streams (include/orb_b200.h) ----
+// From the host's mode array: each stream's slot (route; -1 = skipped), the map-updated streams first and the others after them, each
+// in stream order, and the device mask of the frustum and search stages.  Also the argument checks of the IMU operands.
+struct InertialRoutes {
+    std::vector<int> route; std::vector<uint8_t> active; int count[2] = {0, 0};
+};
+static int inertial_routes(const Matcher& m, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu, const OrbmLocalMapResult* out,
+                           const OrbmImuTrackResult* io, InertialRoutes& R, const char* who) {
+    if (int rc = local_map_shape(m, in, out, who, true)) return rc;
+    if (!imu || !io || !imu->mode || !imu->extrinsics24 || !imu->preintKF || !io->predState21 || !io->predTcw7 || !io->state21 || !io->prior21 || !io->priorH) {
+        set_error(std::string(who) + ": bad argument (null IMU arrays)"); return ORB_ERR_ARG;
+    }
+    R.route.assign(in->batch, -1); R.active.assign(in->batch, 0);
+    for (int b = 0; b < in->batch; ++b) {
+        if (imu->mode[b] > 2) { set_error(std::string(who) + ": mode must be 0, 1 or 2"); return ORB_ERR_ARG; }
+        if (imu->mode[b]) ++R.count[imu->mode[b] - 1];
+    }
+    if ((R.count[0] && !imu->kfState21) || (R.count[1] && (!imu->preintFrame || !imu->lastState21 || !imu->prior21 || !imu->priorH))) {
+        set_error(std::string(who) + ": a stream's mode needs an IMU array that is null"); return ORB_ERR_ARG;
+    }
+    int next[2] = {0, R.count[0]};
+    for (int b = 0; b < in->batch; ++b)
+        if (imu->mode[b]) { R.route[b] = next[imu->mode[b] - 1]++; R.active[b] = 1; }
+    return ORB_OK;
+}
+
+// Predict (1 launch), SearchLocalPoints (2), gather + optimisers + write-back (2 + one per variant with streams).
+static int track_inertial_launch(Matcher& m, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu, const OrbmLocalMapResult* out,
+                                 const OrbmImuTrackResult* io, const int* d_route, const uint8_t* d_active, const int count[2], cudaStream_t st) {
+    const Matcher::TrackScratch& ts = m.ts;
+    imu::ImuTrackArgs A; memset(&A, 0, sizeof(A));
+    A.batch = in->batch; A.kcap = in->kcap; A.pstride = in->mcap; A.nlevels = in->nlevels; A.count[0] = count[0]; A.count[1] = count[1];
+    A.route = d_route; memcpy(A.Tcb7, imu->Tcb7, sizeof(A.Tcb7)); A.extr = imu->extrinsics24;
+    A.preintKF = imu->preintKF; A.preintFrame = imu->preintFrame; A.kfState21 = imu->kfState21; A.lastState21 = imu->lastState21;
+    A.priorIn = imu->prior21; A.priorHIn = imu->priorH;
+    A.predState21 = io->predState21; A.predTcw7 = io->predTcw7; A.match = out->match;
+    A.kps = in->kps; A.nK = in->nK; A.xyz = in->worldPos; A.hasObs = in->hasObs; A.depth = ts.depth; A.invLevelSigma2 = in->invLevelSigma2;
+    memcpy(A.cam, in->cam, 16);
+    A.outlierKp = out->outlier; A.found = out->found; A.nInliers = out->nInliers; A.nMatchesInliers = out->nMatchesInliers;
+    A.Tcw7 = out->Tcw7; A.state21 = io->state21; A.priorOut = io->prior21; A.priorHOut = io->priorH;
+    A.Xw = ts.iXw; A.obs = ts.iObs; A.invSigma2 = ts.is2; A.trackDepth = ts.iTd; A.edgeKp = ts.edgeKp; A.err = ts.err; A.outlier = ts.outl;
+    A.N = ts.N; A.cam4 = ts.cam4; A.preint = ts.preint; A.preintKF2 = ts.preintKF2; A.fixedState = ts.fixedState; A.state = ts.state;
+    A.prior = ts.prior; A.priorH = ts.priorH; A.H15 = ts.H15; A.ret = ts.ret;
+    m.launches = 0;
+    if (!count[0] && !count[1]) return ORB_OK;           // every stream skipped
+    CK(imu::launch_predict_imu(A, st));
+    if (int rc = search_local_points_launch(m, in, out, io->predTcw7, d_active, st)) return rc;
+    int n = 0;
+    CK(imu::launch_gathered_inertial(A, st, &n));
+    m.launches = 3 + n;
+    return ORB_OK;
+}
+
+int orbm_track_local_map_inertial_batch_device(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu,
+                                               const OrbmLocalMapResult* out, const OrbmImuTrackResult* imuOut, void* stream) {
+    const char* who = "orbm_track_local_map_inertial_batch_device";
+    if (!h) { set_error(std::string(who) + ": bad argument"); return ORB_ERR_ARG; }
+    Matcher& m = h->m;
+    InertialRoutes R;
+    if (int rc = inertial_routes(m, in, imu, out, imuOut, R, who)) return rc;
+    CK(cudaSetDevice(m.device));
+    if (int rc = m.track_scratch()) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    // the route / active tables go through the handle's pinned mirror, so the copy is asynchronous; before the mirror is rewritten the
+    // call waits for the previous call's copy of it (an event, normally long complete), not for the caller's stream
+    const size_t B = in->batch, MB = m.maxBatch;
+    if (!m.h_route) {
+        CK(cudaMallocHost(&m.h_route, 5 * MB));
+        CK(cudaEventCreateWithFlags(&m.evRoute, cudaEventDisableTiming));
+    } else {
+        CK(cudaEventSynchronize(m.evRoute));
+    }
+    memcpy(m.h_route, R.route.data(), 4 * B);
+    memcpy(m.h_route + 4 * MB, R.active.data(), B);
+    CK(cudaMemcpyAsync(m.ts.route, m.h_route, 4 * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m.ts.active, m.h_route + 4 * MB, B, cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(m.evRoute, st));
+    return track_inertial_launch(m, in, imu, out, imuOut, m.ts.route, m.ts.active, R.count, st);
+}
+
+static int track_inertial_host(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu, const OrbmLocalMapResult* out,
+                               const OrbmImuTrackResult* io, bool frameOnDevice) {
+    const char* who = frameOnDevice ? "orbm_track_local_map_inertial_batch_resident" : "orbm_track_local_map_inertial_batch";
+    if (!h) { set_error(std::string(who) + ": bad argument"); return ORB_ERR_ARG; }
+    Matcher& m = h->m;
+    InertialRoutes R;
+    if (int rc = inertial_routes(m, in, imu, out, io, R, who)) return rc;
+    const size_t B = in->batch, K = in->kcap, M = in->mcap, PS = 4 * IMU_PREINT_FLOATS;
+    const uint8_t* active = R.active.data();
+    for (size_t b = 0; b < B; ++b) {
+        if (!active[b]) continue;
+        const int nM = in->nM[b];
+        if (nM < 0 || nM > in->mcap) { set_error(std::string(who) + ": nM out of range"); return ORB_ERR_ARG; }
+        if (!(in->th[b] > 0.0f)) { set_error(std::string(who) + ": th must be positive"); return ORB_ERR_ARG; }
+        if (!frameOnDevice) {
+            if (in->nK[b] < 0 || in->nK[b] > in->kcap) { set_error(std::string(who) + ": nK out of range"); return ORB_ERR_ARG; }
+            for (int i = 0; i < in->nK[b]; ++i) {
+                const int oct = in->kps[b * K + i].octave;
+                if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return ORB_ERR_ARG; }
+            }
+        }
+    }
+    CK(cudaSetDevice(m.device));
+    if (int rc = m.track_scratch()) return rc;
+    Staging& S = m.staging;
+    S.begin();
+    const bool lf = R.count[1] > 0, kf = R.count[0] > 0;
+    const int pKps = S.in(frameOnDevice ? nullptr : in->kps, frameOnDevice ? 0 : 28 * B * K), pDesc = S.in(frameOnDevice ? nullptr : in->desc, frameOnDevice ? 0 : 32 * B * K),
+              pNK = S.in(frameOnDevice ? nullptr : in->nK, frameOnDevice ? 0 : 4 * B), pSf = S.in(in->scaleFactors, 4 * (size_t)in->nlevels),
+              pIs = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels), pNM = S.in(in->nM, 4 * B), pWp = S.in(in->worldPos, 12 * B * M),
+              pNo = S.in(in->normal, 12 * B * M), pMin = S.in(in->minDistInv, 4 * B * M), pMax = S.in(in->maxDistInv, 4 * B * M),
+              pRaw = S.in(in->maxDistance, 4 * B * M), pMd = S.in(in->mpDesc, 32 * B * M), pObs = S.in(in->hasObs, B * M), pBad = S.in(in->bad, B * M),
+              pTh = S.in(in->th, 4 * B), pRoute = S.in(R.route.data(), 4 * B), pAct = S.in(active, B), pEx = S.in(imu->extrinsics24, 192),
+              pPk = S.in(imu->preintKF, PS * B), pPf = S.in(lf ? imu->preintFrame : nullptr, lf ? PS * B : 0),
+              pKs = S.in(kf ? imu->kfState21 : nullptr, kf ? 84 * B : 0), pLs = S.in(lf ? imu->lastState21 : nullptr, lf ? 84 * B : 0),
+              pPr = S.in(lf ? imu->prior21 : nullptr, lf ? 168 * B : 0), pPh = S.in(lf ? imu->priorH : nullptr, lf ? 1800 * B : 0),
+              pMatch = S.out(nullptr, 4 * B * K), pCl = S.out(nullptr, B * K), pOut = S.out(nullptr, B * K), pVis = S.out(nullptr, 4 * B * M),
+              pFound = S.out(nullptr, 4 * B * M), pCounts = S.out(nullptr, 16 * B), pTo = S.out(nullptr, 28 * B), pPs = S.out(nullptr, 84 * B),
+              pPt = S.out(nullptr, 28 * B), pSt = S.out(nullptr, 84 * B), pPo = S.out(nullptr, 168 * B), pHo = S.out(nullptr, 1800 * B);
+    int rc = S.reserve();
+    if (rc) return rc;
+    OrbmLocalMapBatch d = *in;
+    if (!frameOnDevice) { d.kps = S.dev<OrbKeyPoint>(pKps); d.desc = S.dev(pDesc); d.nK = S.dev<int>(pNK); }
+    d.scaleFactors = S.dev<float>(pSf); d.invLevelSigma2 = S.dev<float>(pIs); d.nM = S.dev<int>(pNM);
+    d.worldPos = S.dev<float>(pWp); d.normal = S.dev<float>(pNo); d.minDistInv = S.dev<float>(pMin); d.maxDistInv = S.dev<float>(pMax);
+    d.maxDistance = S.dev<float>(pRaw); d.mpDesc = S.dev(pMd); d.hasObs = S.dev(pObs); d.bad = S.dev(pBad); d.th = S.dev<float>(pTh);
+    OrbmImuTrackBatch di = *imu;
+    di.extrinsics24 = S.dev<double>(pEx); di.preintKF = S.dev<float>(pPk); di.preintFrame = lf ? S.dev<float>(pPf) : nullptr;
+    di.kfState21 = kf ? S.dev<float>(pKs) : nullptr; di.lastState21 = lf ? S.dev<float>(pLs) : nullptr;
+    di.prior21 = lf ? S.dev<double>(pPr) : nullptr; di.priorH = lf ? S.dev<double>(pPh) : nullptr;
+    int* counts = S.dev<int>(pCounts);      // nToMatch | nmatches | nInliers | nMatchesInliers, [B] each
+    OrbmLocalMapResult o = {S.dev<int>(pMatch), S.dev(pCl), S.dev(pOut), S.dev<int>(pVis), S.dev<int>(pFound), counts, counts + B, counts + 2 * B,
+                            counts + 3 * B, nullptr, S.dev<float>(pTo)};
+    OrbmImuTrackResult io2 = {S.dev<float>(pPs), S.dev<float>(pPt), S.dev<float>(pSt), S.dev<double>(pPo), S.dev<double>(pHo)};
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    if ((rc = track_inertial_launch(m, &d, &di, &o, &io2, S.dev<int>(pRoute), S.dev(pAct), R.count, st))) return rc;
+    CK(S.download(st));
+    copy_active_rows(S, pMatch, out->match, 4 * K, in->batch, active);
+    copy_active_rows(S, pCl, out->claimed, K, in->batch, active);
+    copy_active_rows(S, pOut, out->outlier, K, in->batch, active);
+    copy_active_rows(S, pVis, out->visible, 4 * M, in->batch, active);
+    copy_active_rows(S, pFound, out->found, 4 * M, in->batch, active);
+    copy_active_rows(S, pTo, out->Tcw7, 28, in->batch, active);
+    copy_active_rows(S, pPs, io->predState21, 84, in->batch, active);
+    copy_active_rows(S, pPt, io->predTcw7, 28, in->batch, active);
+    copy_active_rows(S, pSt, io->state21, 84, in->batch, active);
+    copy_active_rows(S, pPo, io->prior21, 168, in->batch, active);
+    copy_active_rows(S, pHo, io->priorH, 1800, in->batch, active);
+    const int* hc = S.host<int>(pCounts);
+    int32_t* dst[4] = {out->nToMatch, out->nmatches, out->nInliers, out->nMatchesInliers};
+    for (size_t b = 0; b < B; ++b)
+        if (active[b]) for (int k = 0; k < 4; ++k) dst[k][b] = hc[k * B + b];
+    return ORB_OK;
+}
+
+int orbm_track_local_map_inertial_batch(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu, const OrbmLocalMapResult* out,
+                                        const OrbmImuTrackResult* imuOut) {
+    return track_inertial_host(h, in, imu, out, imuOut, false);
+}
+int orbm_track_local_map_inertial_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu,
+                                                 const OrbmLocalMapResult* out, const OrbmImuTrackResult* imuOut) {
+    return track_inertial_host(h, in, imu, out, imuOut, true);
 }
 
 }  // extern "C"
