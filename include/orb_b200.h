@@ -379,6 +379,51 @@ int orbm_search_by_bow(orbm_handle* h, const OrbmBowFrame* KF, const uint8_t* kf
  * match12 [KF1.N] = feature of KF2 whose map point goes to vpMatches12[idx1] (-1 = NULL).  KF1.N <= max_mappoints, KF2.N <= max_keypoints. */
 int orbm_search_by_bow_kf(orbm_handle* h, const OrbmBowFrame* KF1, const uint8_t* point1, const OrbmBowFrame* KF2, const uint8_t* point2, float nnratio,
                           int checkOrientation, int32_t* match12, int* nmatches);
+
+/* bool Tracking::TrackReferenceKeyFrame() (reference src/Tracking.cc:2723, monocular; the mono-inertial path runs the same body before
+ * the IMU is initialised) after Frame::ComputeBoW, for `batch` streams in four launches whatever the batch size.  The caller computes the
+ * frame's BoW with orbv_transform_batch* (levelsup 4) and keeps the success test (nmatchesMap >= 10 monocular, true with an IMU).  Per stream:
+ *   1. SearchByBoW(mpReferenceKF, mCurrentFrame) with ORBmatcher(0.7, true): nmatches, match.
+ *   2. nmatches < 15: the stream stops there (the reference returns false without touching the frame).
+ *   3. Otherwise mvpMapPoints = the matches, SetPose(mLastFrame.GetPose()) = Tcw7, PoseOptimization (edges: the frame features i with
+ *      match[i] >= 0 in ascending i, Xw = (double)xyz[match[i]], obs = (double)kps[i].(x, y), invSigma2 = invLevelSigma2[kps[i].octave]),
+ *      SetPose of the result, and the "discard outliers" loop: an outlier loses its match and its keyframe feature is marked in discarded
+ *      (pMP->mnLastFrameSeen = current frame, mbTrackInView = false); nmatchesMap = inliers whose point has observations.
+ * Outputs: nmatches and match for every active stream (match after the discard loop for a stream that passed the gate, the search result
+ * otherwise); pose7, Tcw7, discarded and nmatchesMap only for active streams with nmatches >= 15.  Streams not in `active` are untouched.
+ * match / discarded feed orbm_track_local_map_batch* in the index space [keyframe features | last-frame points] (INTEGRATION.md §2). */
+typedef struct OrbmRefKeyFrameBatch {
+    int batch, kcap, mcap, nlevels;
+    /* current frame [batch][kcap] (device pointers in the resident form): mvKeysUn, mDescriptors, N, and the FeatureVector as
+     * orbv_transform_batch* writes it (fvNode / fvFeature [batch][kcap], nEntries [batch]) */
+    const OrbKeyPoint* kps; const uint8_t* desc; const int32_t* nK;
+    const int32_t* fvNode; const int32_t* fvFeature; const int32_t* nEntries;
+    const float* Tcw7;            /* [batch][7] mLastFrame.GetPose(): the pose SetPose gives the frame before PoseOptimization */
+    /* reference keyframe [batch][mcap], indexed by keyframe feature (mcap <= max_mappoints) */
+    const int32_t* kfN; const OrbKeyPoint* kfKps; const uint8_t* kfDesc;       /* N, mvKeysUn, mDescriptors */
+    const int32_t* kfFvNode; const int32_t* kfFvFeature; const int32_t* kfNEntries;  /* its FeatureVector */
+    const uint8_t* kfPoint;       /* 0 no map point, 1 a map point, 2 a bad one */
+    const float* xyz;             /* [batch][mcap][3] GetWorldPos() of the point at each feature */
+    const uint8_t* hasObs;        /* Observations() > 0 of that point */
+    float cam[4];                 /* fx fy cx cy */
+    const float* invLevelSigma2;  /* mvInvLevelSigma2 [nlevels] */
+    const uint8_t* active;        /* [batch] or NULL = all */
+} OrbmRefKeyFrameBatch;
+typedef struct OrbmRefKeyFrameResult {
+    int32_t* nmatches;            /* [batch] SearchByBoW's return value */
+    int32_t* match;               /* [batch][kcap] keyframe feature whose point each frame feature holds, -1 = none */
+    double* pose7; float* Tcw7;   /* [batch][7] PoseOptimization's pose and the float pose after SetPose */
+    uint8_t* discarded;           /* [batch][mcap] 1 = the outlier's point got mnLastFrameSeen = current frame */
+    int32_t* nmatchesMap;         /* [batch] */
+} OrbmRefKeyFrameResult;
+/* All pointers device pointers; enqueues on `stream`.  The FeatureVectors are trusted as orbv_transform_batch_device writes them. */
+int orbm_track_reference_keyframe_batch_device(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out, void* stream);
+/* HOST pointers in `in` and `out` (one upload, four launches, one download).  Out-of-range octaves and counts and unsorted or out-of-range
+ * FeatureVectors are ORB_ERR_ARG, slabs wider than the handle ORB_ERR_CAPACITY, both before any launch. */
+int orbm_track_reference_keyframe_batch(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out);
+/* Same with the current frame on the device (in->kps, desc, nK, fvNode, fvFeature, nEntries: e.g. the extractor's resident slabs and
+ * orbv_transform_batch_device's output on them); everything else host pointers. */
+int orbm_track_reference_keyframe_batch_resident(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out);
 /* int ORBmatcher::Fuse(KeyFrame* pKF, const vector<MapPoint*>& vpMapPoints, const float th, const bool bRight) (include/ORBmatcher.h:99,
  * src/ORBmatcher.cc:1148-1338, monocular keyframe; LocalMapping::SearchInNeighbors, src/LocalMapping.cc:878-1021): the SEARCH of every map
  * point -- projection with the keyframe pose, KeyFrame::IsInImage, distance / viewing-angle tests, MapPoint::PredictScale, the radius search

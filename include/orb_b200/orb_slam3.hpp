@@ -218,7 +218,7 @@ protected:
 };
 
 // Tracking's per-frame steps after the last-frame search for a batch of streams (INTEGRATION.md §2): monocular with the IMU not
-// initialised, TrackWithMotionModel's PoseOptimization + "discard outliers" loop and TrackLocalMap from SearchLocalPoints through the
+// initialised, TrackWithMotionModel's PoseOptimization + "discard outliers" loop, TrackReferenceKeyFrame, and TrackLocalMap from SearchLocalPoints through the
 // statistics loop; monocular-inertial with the IMU initialised, PredictStateIMU and TrackLocalMap with the inertial pose optimisers.
 // Unlike ORBmatcher above it owns its matcher handle, sized for the batch; host pointers throughout.
 class BatchTracker {
@@ -237,6 +237,12 @@ public:
     }
     void TrackLocalMap(const OrbmLocalMapBatch& in, const OrbmLocalMapResult& out) {
         orb_check(orbm_track_local_map_batch(h_, &in, &out), "orbm_track_local_map_batch");
+    }
+    // Tracking::TrackReferenceKeyFrame after Frame::ComputeBoW (the frame's FeatureVector from orbv_transform_batch): SearchByBoW, the
+    // 15-match gate, PoseOptimization from in.Tcw7 and the "discard outliers" loop.  The caller applies nmatchesMap >= 10 (monocular)
+    // and feeds out.match / out.discarded to TrackLocalMap in the index space [keyframe features | last-frame points].
+    void TrackReferenceKeyFrame(const OrbmRefKeyFrameBatch& in, const OrbmRefKeyFrameResult& out) {
+        orb_check(orbm_track_reference_keyframe_batch(h_, &in, &out), "orbm_track_reference_keyframe_batch");
     }
     // Monocular-inertial frames once the IMU is initialised: PredictStateIMU, SearchLocalPoints, PoseInertialOptimizationLast{KeyFrame,Frame}
     // and its write-back for every stream with imu.mode != 0 (in.Tcw7 / lastToLocal / discarded / active and out.pose7 NULL).  Feed

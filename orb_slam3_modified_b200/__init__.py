@@ -329,6 +329,22 @@ class _OrbmImuTrackResult(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _IMU_TRACK_OUT]
 
 
+_REF_KF_FRAME = ('kps', 'desc', 'nK', 'fvNode', 'fvFeature', 'nEntries')
+_REF_KF_IN = _REF_KF_FRAME + ('Tcw7', 'kfN', 'kfKps', 'kfDesc', 'kfFvNode', 'kfFvFeature', 'kfNEntries', 'kfPoint', 'xyz', 'hasObs')
+
+
+class _OrbmRefKeyFrameBatch(C.Structure):
+    _fields_ = ([(n, C.c_int) for n in ('batch', 'kcap', 'mcap', 'nlevels')] + [(n, C.c_void_p) for n in _REF_KF_IN] +
+                [('cam', C.c_float * 4), ('invLevelSigma2', C.c_void_p), ('active', C.c_void_p)])
+
+
+_REF_KF_OUT = ('nmatches', 'match', 'pose7', 'Tcw7', 'discarded', 'nmatchesMap')
+
+
+class _OrbmRefKeyFrameResult(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in _REF_KF_OUT]
+
+
 def _c(a, dt):
     return np.ascontiguousarray(a, dt)
 
@@ -645,6 +661,52 @@ class ORBmatcher:
         rc = L.orbm_track_local_map_inertial_batch_device(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri), C.c_void_p(stream))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_local_map_inertial_batch_device')
+
+    @staticmethod
+    def _ref_kf_struct(d, get):
+        s = _OrbmRefKeyFrameBatch()
+        s.batch, s.kcap, s.mcap, s.nlevels = d['batch'], d['kcap'], d['mcap'], d['nlevels']
+        for k in _REF_KF_IN + ('invLevelSigma2', 'active'):
+            setattr(s, k, get(k))
+        s.cam = (C.c_float * 4)(*d['cam'])
+        return s
+
+    _REF_KF_DT = dict(kps=KP_DTYPE, desc=np.uint8, nK=np.int32, fvNode=np.int32, fvFeature=np.int32, nEntries=np.int32, Tcw7=np.float32, kfN=np.int32,
+                      kfKps=KP_DTYPE, kfDesc=np.uint8, kfFvNode=np.int32, kfFvFeature=np.int32, kfNEntries=np.int32, kfPoint=np.uint8, xyz=np.float32,
+                      hasObs=np.uint8, invLevelSigma2=np.float32, active=np.uint8)
+
+    def track_reference_keyframe_batch(self, d, resident=None):
+        """Tracking::TrackReferenceKeyFrame after Frame::ComputeBoW for ``d['batch']`` streams, host numpy (see OrbmRefKeyFrameBatch in
+        include/orb_b200.h for the keys; 'active' may be None or absent).  SearchByBoW with ORBmatcher(0.7, true) and, for streams with
+        at least 15 matches, PoseOptimization from Tcw7 (mLastFrame's pose) and the "discard outliers" loop.  ``resident`` = (kps, desc, nK,
+        fvNode, fvFeature, nEntries) device pointers of the current frame with stride d['kcap'] (d's frame keys are then ignored).
+        Returns dict(nmatches [B], match [B, kcap] i32, pose7 [B, 7] f64, Tcw7 [B, 7] f32, discarded [B, mcap] u8, nmatchesMap [B] i32);
+        rows the call does not write keep their initial values (match -1, the rest 0)."""
+        B, K, M = d['batch'], d['kcap'], d['mcap']
+        keep = {k: _c(d[k], dt) for k, dt in self._REF_KF_DT.items() if d.get(k) is not None}
+        if resident is not None:
+            keep.update(zip(_REF_KF_FRAME, resident))
+        s = self._ref_kf_struct(d, lambda k: (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None)
+        out = dict(nmatches=np.zeros(B, np.int32), match=np.full((B, K), -1, np.int32), pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32),
+                   discarded=np.zeros((B, M), np.uint8), nmatchesMap=np.zeros(B, np.int32))
+        r = _OrbmRefKeyFrameResult(*[_ptr(out[k]) for k in _REF_KF_OUT])
+        fn = lib().orbm_track_reference_keyframe_batch_resident if resident is not None else lib().orbm_track_reference_keyframe_batch
+        fn.argtypes = [C.c_void_p] * 3
+        rc = fn(self._h, C.byref(s), C.byref(r))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_track_reference_keyframe_batch')
+        return out
+
+    def track_reference_keyframe_batch_device(self, d, out, stream=0):
+        """Device form of :meth:`track_reference_keyframe_batch`: torch CUDA tensors in ``d`` and ``out`` (keys of OrbmRefKeyFrameResult);
+        enqueues on ``stream``."""
+        s = self._ref_kf_struct(d, lambda k: d[k].data_ptr() if d.get(k) is not None else None)
+        r = _OrbmRefKeyFrameResult(*[_ptr(out[k]) for k in _REF_KF_OUT])
+        L = lib()
+        L.orbm_track_reference_keyframe_batch_device.argtypes = [C.c_void_p] * 4
+        rc = L.orbm_track_reference_keyframe_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_track_reference_keyframe_batch_device')
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """``int ORBmatcher::SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize)`` (src/ORBmatcher.cc:648-763).

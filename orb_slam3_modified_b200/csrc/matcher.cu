@@ -637,57 +637,69 @@ __global__ void __launch_bounds__(MF_NT) init_match_kernel(MatchParams P) {
 // src/Tracking.cc:2730 and relocalisation).  Features are matched only inside the same vocabulary node, so nodes are independent: one warp per
 // keyframe node walks its features in order (the claim rule "a frame feature that already holds a match is skipped" is sequential inside a
 // node only), lanes over the frame features of that node: top-2 by (distance, position).  The rotation histogram is resolved by the CTA.
-// One CTA per (keyframe, frame) pair.
+// One CTA per (keyframe, frame) pair: CTA f reads its operands at f times the strides (the single-pair entry points are the batch of one).
 // ---------------------------------------------------------------------------------------------
 struct BowMatchParams {
-    int nKF, nF, eKF, eF;
+    const int *nKF, *nF, *eKF, *eF;               // [grid]: features and FeatureVector entries of each keyframe / frame
+    int kfStride, fStride;                        // per-CTA stride of the keyframe-side / frame-side operands
     const OrbKeyPoint *kpsKF, *kpsF; const uint8_t *descKF, *descF, *kfPoint;
     const int *fvNodeKF, *fvFeatKF, *fvNodeF, *fvFeatF;
     float nnratio; int checkOri;
-    int* match; int* nmatches; int* groupStart; uint8_t* evBin;   // match [nF]; scratch: groupStart [eKF + 1], evBin [nF]
+    int* match; int* nmatches; int* groupStart; uint8_t* evBin;   // match [fStride], nmatches [1]; scratch: groupStart [kfStride + 1], evBin [fStride]
     // SearchByBoW(KeyFrame*, KeyFrame*) (src/ORBmatcher.cc:765-905): the second side is a keyframe too -- its features need a good map point
     // (fPoint, null for a Frame), the distance test is strict (bestDist1 < TH_LOW, :859) and the result is indexed by the first side (match12)
     const uint8_t* fPoint; int strictLow; int* match12;
+    // the batched TrackReferenceKeyFrame (orbm_track_reference_keyframe_batch*): streams not in `active` are skipped (null: all);
+    // poseActive[f] = the stream is active and nmatches >= gate, nmatchesCopy[f] = nmatches (both null elsewhere)
+    const uint8_t* active; uint8_t* poseActive; int* nmatchesCopy; int gate;
 };
 constexpr int BM_NT = 256;
 __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
     __shared__ int s_hist[HISTO_LENGTH], s_ind[3], s_acc, s_rem, s_ng;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    for (int i = tid; i < Q.nF; i += BM_NT) { Q.match[i] = -1; Q.evBin[i] = 0; }
-    if (Q.match12) for (int i = tid; i < Q.nKF; i += BM_NT) Q.match12[i] = -1;
+    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (Q.active && !Q.active[f]) { if (tid == 0 && Q.poseActive) Q.poseActive[f] = 0; return; }
+    const size_t kb = (size_t)f * Q.kfStride, fb = (size_t)f * Q.fStride;
+    const int nKF = min(Q.nKF[f], Q.kfStride), nF = min(Q.nF[f], Q.fStride), eKF = min(Q.eKF[f], nKF), eF = min(Q.eF[f], nF);
+    const OrbKeyPoint *kpsKF = Q.kpsKF + kb, *kpsF = Q.kpsF + fb;
+    const uint8_t *descKF = Q.descKF + 32 * kb, *descF = Q.descF + 32 * fb, *kfPoint = Q.kfPoint + kb, *fPoint = Q.fPoint ? Q.fPoint + fb : nullptr;
+    const int *fvNodeKF = Q.fvNodeKF + kb, *fvFeatKF = Q.fvFeatKF + kb, *fvNodeF = Q.fvNodeF + fb, *fvFeatF = Q.fvFeatF + fb;
+    int *match = Q.match + fb, *match12 = Q.match12 ? Q.match12 + kb : nullptr, *groupStart = Q.groupStart + (size_t)f * (Q.kfStride + 1);
+    uint8_t* evBin = Q.evBin + fb;
+    for (int i = tid; i < Q.fStride; i += BM_NT) { match[i] = -1; evBin[i] = 0; }
+    if (match12) for (int i = tid; i < nKF; i += BM_NT) match12[i] = -1;
     if (tid < HISTO_LENGTH) s_hist[tid] = 0;
     if (tid == 0) { s_acc = 0; s_rem = 0; s_ng = 0; }
     __syncthreads();
     // group heads of the keyframe's feature vector (entries are sorted by node id)
-    for (int e = tid; e < Q.eKF; e += BM_NT)
-        if (e == 0 || Q.fvNodeKF[e] != Q.fvNodeKF[e - 1]) Q.groupStart[atomicAdd(&s_ng, 1)] = e;     // order of groups is irrelevant: nodes are independent
+    for (int e = tid; e < eKF; e += BM_NT)
+        if (e == 0 || fvNodeKF[e] != fvNodeKF[e - 1]) groupStart[atomicAdd(&s_ng, 1)] = e;     // order of groups is irrelevant: nodes are independent
     __syncthreads();
     const int ng = s_ng;
     int acc = 0;
     for (int g = wid; g < ng; g += BM_NT / 32) {
-        const int a = Q.groupStart[g];
-        const int node = Q.fvNodeKF[a];
+        const int a = groupStart[g];
+        const int node = fvNodeKF[a];
         int a1 = a;
-        while (a1 < Q.eKF && Q.fvNodeKF[a1] == node) ++a1;
-        int lo = 0, hi = Q.eF;                                   // lower_bound / upper_bound of `node` in the frame's vector
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (Q.fvNodeF[mid] < node) lo = mid + 1; else hi = mid; }
+        while (a1 < eKF && fvNodeKF[a1] == node) ++a1;
+        int lo = 0, hi = eF;                                     // lower_bound / upper_bound of `node` in the frame's vector
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (fvNodeF[mid] < node) lo = mid + 1; else hi = mid; }
         const int b = lo;
-        hi = Q.eF;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (Q.fvNodeF[mid] <= node) lo = mid + 1; else hi = mid; }
+        hi = eF;
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (fvNodeF[mid] <= node) lo = mid + 1; else hi = mid; }
         const int b1 = lo;
         if (b1 == b) continue;
         for (int iKF = a; iKF < a1; ++iKF) {
-            const int realIdxKF = Q.fvFeatKF[iKF];
-            if (Q.kfPoint[realIdxKF] != 1) continue;             // no map point, or a bad one (:255-259)
-            const uint4* pk = reinterpret_cast<const uint4*>(Q.descKF + (size_t)realIdxKF * 32);
+            const int realIdxKF = fvFeatKF[iKF];
+            if (kfPoint[realIdxKF] != 1) continue;               // no map point, or a bad one (:255-259)
+            const uint4* pk = reinterpret_cast<const uint4*>(descKF + (size_t)realIdxKF * 32);
             const uint4 k0 = __ldg(pk), k1 = __ldg(pk + 1);
             const uint32_t dk[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
             Top2 t; t.init();
             for (int iF = b + lane; iF < b1; iF += 32) {
-                const int realIdxF = Q.fvFeatF[iF];
-                if (Q.match[realIdxF] >= 0) continue;            // already matched by an earlier keyframe feature of this node (:275-276)
-                if (Q.fPoint && Q.fPoint[realIdxF] != 1) continue;
-                const uint4* pf = reinterpret_cast<const uint4*>(Q.descF + (size_t)realIdxF * 32);
+                const int realIdxF = fvFeatF[iF];
+                if (match[realIdxF] >= 0) continue;              // already matched by an earlier keyframe feature of this node (:275-276)
+                if (fPoint && fPoint[realIdxF] != 1) continue;
+                const uint4* pf = reinterpret_cast<const uint4*>(descF + (size_t)realIdxF * 32);
                 const uint4 f0 = __ldg(pf), f1 = __ldg(pf + 1);
                 const uint32_t dfw[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
                 t.insert(((unsigned long long)hamming256(dk, dfw) << 32) | (unsigned)(iF - b), realIdxF);
@@ -696,11 +708,11 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
             const int bestDist1 = t.i[0] >= 0 ? (int)(t.k[0] >> 32) : 256, bestDist2 = t.i[1] >= 0 ? (int)(t.k[1] >> 32) : 256;
             if ((Q.strictLow ? bestDist1 < TH_LOW : bestDist1 <= TH_LOW) && (float)bestDist1 < fmul(Q.nnratio, (float)bestDist2)) {
                 if (lane == 0) {
-                    Q.match[t.i[0]] = realIdxKF;
-                    if (Q.match12) Q.match12[realIdxKF] = t.i[0];
+                    match[t.i[0]] = realIdxKF;
+                    if (match12) match12[realIdxKF] = t.i[0];
                     if (Q.checkOri) {
-                        const int bin = rot_bin(Q.kpsKF[realIdxKF].angle, Q.kpsF[t.i[0]].angle);
-                        Q.evBin[t.i[0]] = (uint8_t)(bin + 1);
+                        const int bin = rot_bin(kpsKF[realIdxKF].angle, kpsF[t.i[0]].angle);
+                        evBin[t.i[0]] = (uint8_t)(bin + 1);
                         atomicAdd(&s_hist[bin], 1);
                     }
                 }
@@ -726,14 +738,19 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
         }
         __syncthreads();
         int rem = 0;
-        for (int i = tid; i < Q.nF; i += BM_NT) {
-            const int bb = (int)Q.evBin[i] - 1;
-            if (bb >= 0 && bb != s_ind[0] && bb != s_ind[1] && bb != s_ind[2]) { if (Q.match12) Q.match12[Q.match[i]] = -1; Q.match[i] = -1; ++rem; }
+        for (int i = tid; i < nF; i += BM_NT) {
+            const int bb = (int)evBin[i] - 1;
+            if (bb >= 0 && bb != s_ind[0] && bb != s_ind[1] && bb != s_ind[2]) { if (match12) match12[match[i]] = -1; match[i] = -1; ++rem; }
         }
         if (rem) atomicAdd(&s_rem, rem);
         __syncthreads();
     }
-    if (tid == 0) *Q.nmatches = s_acc - s_rem;
+    if (tid == 0) {
+        const int n = s_acc - s_rem;
+        Q.nmatches[f] = n;
+        if (Q.nmatchesCopy) Q.nmatchesCopy[f] = n;
+        if (Q.poseActive) Q.poseActive[f] = n >= Q.gate ? 1 : 0;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1331,19 +1348,23 @@ struct Matcher {
     // The batched tracking calls' scratch, sized for max_batch x max_keypoints / max_mappoints: PoseOptimization's gathered edges
     // ([B][kcap]), the frustum stage's per-point fields and flags ([B][mcap]) and the motion-model step's nInliers ([B]).  The
     // mono-inertial call adds its float edges ([B][kcap]: Xw 3, obs 2, trackDepth; it shares is2, err, outl, edgeKp, N and cam4) and
-    // per-slot operands ([B]: route, two preintegrations, fixed / current state, prior, prior and optimised H, return value).
+    // per-slot operands ([B]: route, two preintegrations, fixed / current state, prior, prior and optimised H, return value).  The
+    // reference-keyframe call adds the search's group heads ([B][mcap + 1]) and histogram events ([B][kcap]), the streams that passed
+    // the match gate and the copy of nmatches the discard loop decrements ([B] each).
     struct TrackScratch {
         double *Xw, *obs, *err; float* is2; uint8_t* outl; int* edgeKp;
         uint8_t *seen, *inView; float *projX, *projY, *depth, *viewCos; int *level, *nInliers;
         int* N; double *poseIn, *poseTmp; float* cam4; int* nInlTmp;
         float *iXw, *iObs, *iTd; int* route; uint8_t* active; float *preint, *preintKF2; double *fixedState, *state, *prior, *priorH, *H15; int* ret;
+        int* groupStart; uint8_t *evBin, *poseActive; int* nmCopy;
     } ts;
     int track_scratch() {
         if (d_track) return ORB_OK;
         const size_t BK = (size_t)maxBatch * kcap, BM = (size_t)maxBatch * mcap;
         const size_t B = maxBatch, PS = 4 * IMU_PREINT_FLOATS;
         const size_t sizes[] = {24 * BK, 16 * BK, 16 * BK, 4 * BK, BK, 4 * BK, BM, BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * BM, 4 * B, 4 * B, 56 * B, 56 * B, 16 * B, 4 * B,
-                                12 * BK, 8 * BK, 4 * BK, 4 * B, B, PS * B, PS * B, 168 * B, 168 * B, 168 * B, 1800 * B, 1800 * B, 4 * B};
+                                12 * BK, 8 * BK, 4 * BK, 4 * B, B, PS * B, PS * B, 168 * B, 168 * B, 168 * B, 1800 * B, 1800 * B, 4 * B,
+                                4 * (BM + B), BK, B, 4 * B};
         constexpr int nSlots = sizeof(sizes) / sizeof(sizes[0]);
         size_t total = 0;
         for (size_t b : sizes) total += (b + 255) & ~(size_t)255;
@@ -1352,7 +1373,8 @@ struct Matcher {
                           (void**)&ts.inView, (void**)&ts.projX, (void**)&ts.projY, (void**)&ts.depth, (void**)&ts.viewCos, (void**)&ts.level,
                           (void**)&ts.nInliers, (void**)&ts.N, (void**)&ts.poseIn, (void**)&ts.poseTmp, (void**)&ts.cam4, (void**)&ts.nInlTmp,
                           (void**)&ts.iXw, (void**)&ts.iObs, (void**)&ts.iTd, (void**)&ts.route, (void**)&ts.active, (void**)&ts.preint, (void**)&ts.preintKF2,
-                          (void**)&ts.fixedState, (void**)&ts.state, (void**)&ts.prior, (void**)&ts.priorH, (void**)&ts.H15, (void**)&ts.ret};
+                          (void**)&ts.fixedState, (void**)&ts.state, (void**)&ts.prior, (void**)&ts.priorH, (void**)&ts.H15, (void**)&ts.ret,
+                          (void**)&ts.groupStart, (void**)&ts.evBin, (void**)&ts.poseActive, (void**)&ts.nmCopy};
         size_t off = 0;
         for (int k = 0; k < nSlots; ++k) { *slots[k] = d_track + off; off += (sizes[k] + 255) & ~(size_t)255; }
         return ORB_OK;
@@ -1714,14 +1736,20 @@ int orbm_search_last_frame_batch_resident(orbm_handle* h, const OrbmBatchDevice*
     return search_last_frame_batch_host(h, in, th, checkOri, match, claimed, nmatches, true);
 }
 
+// A FeatureVector of n entries over N features: node ids ascending, feature indices in [0, N).
+static bool fv_ok(const int32_t* node, const int32_t* feat, int n, int N) {
+    for (int e = 0; e < n; ++e) if (feat[e] < 0 || feat[e] >= N || (e && node[e] < node[e - 1])) return false;
+    return true;
+}
+
 static int search_by_bow_impl(orbm_handle* h, const OrbmBowFrame* KF, const uint8_t* kfPoint, const OrbmBowFrame* F, const uint8_t* fPoint, float nnratio,
                               int checkOrientation, int32_t* match, int32_t* match12, int* nmatches) {
     if (!h || !KF || !F || !kfPoint || (!match && !match12) || !nmatches || KF->N < 0 || F->N < 0 || KF->nEntries < 0 || F->nEntries < 0 || KF->nEntries > KF->N ||
         F->nEntries > F->N || KF->N > h->m.mcap || F->N > h->m.kcap) {
         set_error("orbm_search_by_bow: bad argument (KF.N <= max_mappoints, F.N <= max_keypoints of the handle)"); return ORB_ERR_ARG;
     }
-    for (int e = 0; e < KF->nEntries; ++e) if (KF->fvFeature[e] < 0 || KF->fvFeature[e] >= KF->N || (e && KF->fvNode[e] < KF->fvNode[e - 1])) { set_error("orbm_search_by_bow: keyframe feature vector not sorted / out of range"); return ORB_ERR_ARG; }
-    for (int e = 0; e < F->nEntries; ++e) if (F->fvFeature[e] < 0 || F->fvFeature[e] >= F->N || (e && F->fvNode[e] < F->fvNode[e - 1])) { set_error("orbm_search_by_bow: frame feature vector not sorted / out of range"); return ORB_ERR_ARG; }
+    if (!fv_ok(KF->fvNode, KF->fvFeature, KF->nEntries, KF->N)) { set_error("orbm_search_by_bow: keyframe feature vector not sorted / out of range"); return ORB_ERR_ARG; }
+    if (!fv_ok(F->fvNode, F->fvFeature, F->nEntries, F->N)) { set_error("orbm_search_by_bow: frame feature vector not sorted / out of range"); return ORB_ERR_ARG; }
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
     *nmatches = 0;
@@ -1735,11 +1763,14 @@ static int search_by_bow_impl(orbm_handle* h, const OrbmBowFrame* KF, const uint
               pNodeKF = S.in(KF->fvNode, 4 * eKF), pFeatKF = S.in(KF->fvFeature, 4 * eKF), pKpsF = S.in(F->keypoints, sizeof(OrbKeyPoint) * nF),
               pDescF = S.in(F->descriptors, 32 * nF), pNodeF = S.in(F->fvNode, 4 * eF), pFeatF = S.in(F->fvFeature, 4 * eF), pPtF = S.in(fPoint, fPoint ? nF : 0),
               pMatch = match ? S.out(match, 4 * nF) : S.scratch(4 * nF), pM12 = S.out(match12, match12 ? 4 * nKF : 0), pN = S.out(nmatches, 4),
-              pGs = S.scratch(4 * (eKF + 1)), pEv = S.scratch(nF);
+              pGs = S.scratch(4 * (nKF + 1)), pEv = S.scratch(nF), pCounts = S.in(nullptr, 16);
     int rc = S.reserve();
     if (rc) return rc;
+    int* counts = S.host<int>(pCounts);
+    counts[0] = KF->N; counts[1] = F->N; counts[2] = KF->nEntries; counts[3] = F->nEntries;
     BowMatchParams Q; memset(&Q, 0, sizeof(Q));
-    Q.nKF = KF->N; Q.nF = F->N; Q.eKF = KF->nEntries; Q.eF = F->nEntries; Q.nnratio = nnratio; Q.checkOri = checkOrientation;
+    Q.nKF = S.dev<int>(pCounts); Q.nF = Q.nKF + 1; Q.eKF = Q.nKF + 2; Q.eF = Q.nKF + 3; Q.kfStride = KF->N; Q.fStride = F->N;
+    Q.nnratio = nnratio; Q.checkOri = checkOrientation;
     Q.kpsKF = S.dev<OrbKeyPoint>(pKpsKF); Q.descKF = S.dev(pDescKF); Q.kfPoint = S.dev(pPtKF); Q.fvNodeKF = S.dev<int>(pNodeKF); Q.fvFeatKF = S.dev<int>(pFeatKF);
     Q.kpsF = S.dev<OrbKeyPoint>(pKpsF); Q.descF = S.dev(pDescF); Q.fvNodeF = S.dev<int>(pNodeF); Q.fvFeatF = S.dev<int>(pFeatF);
     if (fPoint) Q.fPoint = S.dev(pPtF);
@@ -2164,6 +2195,125 @@ int orbm_motion_model_pose_batch(orbm_handle* h, const OrbmBatchDevice* in, cons
     copy_active_rows(S, pDis, discarded, M, in->batch, active);
     copy_active_rows(S, pMap, nmatchesMap, 4, in->batch, active);
     return ORB_OK;
+}
+
+// ---- TrackReferenceKeyFrame for a batch of streams (include/orb_b200.h): the batched SearchByBoW, then PoseOptimization and the
+//      "discard outliers" loop -- the motion-model step's three launches -- on the streams that passed the match gate ----
+constexpr float TRK_REF_NNRATIO = 0.7f;     // TrackReferenceKeyFrame (src/Tracking.cc:2723): ORBmatcher matcher(0.7,true);
+constexpr int TRK_REF_MIN_MATCHES = 15;     //   and if(nmatches<15) return false;
+
+static int ref_kf_shape(const Matcher& m, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out, const char* who) {
+    if (!in || !out || in->batch < 1 || in->batch > m.maxBatch || in->kcap < 1 || in->mcap < 1 || in->nlevels < 1 || in->nlevels > 256 || !in->kps ||
+        !in->desc || !in->nK || !in->fvNode || !in->fvFeature || !in->nEntries || !in->Tcw7 || !in->kfN || !in->kfKps || !in->kfDesc || !in->kfFvNode ||
+        !in->kfFvFeature || !in->kfNEntries || !in->kfPoint || !in->xyz || !in->hasObs || !in->invLevelSigma2 || !out->nmatches || !out->match ||
+        !out->pose7 || !out->Tcw7 || !out->discarded || !out->nmatchesMap) {
+        set_error(std::string(who) + ": bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
+    }
+    if (in->kcap > m.kcap || in->mcap > m.mcap) { set_error(std::string(who) + ": slabs wider than max_keypoints / max_mappoints"); return ORB_ERR_CAPACITY; }
+    return ORB_OK;
+}
+
+// Four launches: bow_match_kernel (one CTA per stream; it also writes the gate mask and the copy of nmatches), then launch_gathered in
+// MOTION_MODEL mode over the keyframe slabs with the gate mask as its `active`.  Its `claimed` writes go to the search's histogram
+// events, which nothing reads after the search, and its nmatches-- to the copy: TrackReferenceKeyFrame returns before reading it.
+static int ref_kf_launch(Matcher& m, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out, cudaStream_t st) {
+    int rc = m.track_scratch();
+    if (rc) return rc;
+    const Matcher::TrackScratch& ts = m.ts;
+    BowMatchParams Q; memset(&Q, 0, sizeof(Q));
+    Q.nKF = in->kfN; Q.nF = in->nK; Q.eKF = in->kfNEntries; Q.eF = in->nEntries; Q.kfStride = in->mcap; Q.fStride = in->kcap;
+    Q.kpsKF = in->kfKps; Q.descKF = in->kfDesc; Q.kfPoint = in->kfPoint; Q.fvNodeKF = in->kfFvNode; Q.fvFeatKF = in->kfFvFeature;
+    Q.kpsF = in->kps; Q.descF = in->desc; Q.fvNodeF = in->fvNode; Q.fvFeatF = in->fvFeature;
+    Q.nnratio = TRK_REF_NNRATIO; Q.checkOri = 1;
+    Q.match = out->match; Q.nmatches = out->nmatches; Q.groupStart = ts.groupStart; Q.evBin = ts.evBin;
+    Q.active = in->active; Q.poseActive = ts.poseActive; Q.nmatchesCopy = ts.nmCopy; Q.gate = TRK_REF_MIN_MATCHES;
+    bow_match_kernel<<<in->batch, BM_NT, 0, st>>>(Q);
+    CK(cudaGetLastError());
+    poseopt::GatherArgs A; memset(&A, 0, sizeof(A));
+    A.batch = in->batch; A.kcap = in->kcap; A.pstride = in->mcap; A.nlevels = in->nlevels; A.mode = poseopt::MOTION_MODEL;
+    A.active = ts.poseActive; A.kps = in->kps; A.nK = in->nK; A.match = out->match; A.claimed = ts.evBin; A.nmatches = ts.nmCopy;
+    A.xyz = in->xyz; A.hasObs = in->hasObs; A.invLevelSigma2 = in->invLevelSigma2; memcpy(A.cam, in->cam, 16);
+    A.TcwIn = in->Tcw7; A.TcwOut = out->Tcw7; A.poseOut = out->pose7; A.nInliers = ts.nInliers; A.discarded = out->discarded;
+    A.nmatchesMap = out->nmatchesMap;
+    m.bind_gather(A);
+    CK(poseopt::launch_gathered(A, st));
+    m.launches = 4;
+    return ORB_OK;
+}
+
+int orbm_track_reference_keyframe_batch_device(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out, void* stream) {
+    const char* who = "orbm_track_reference_keyframe_batch_device";
+    if (!h) { set_error(std::string(who) + ": bad argument"); return ORB_ERR_ARG; }
+    if (int rc = ref_kf_shape(h->m, in, out, who)) return rc;
+    CK(cudaSetDevice(h->m.device));
+    return ref_kf_launch(h->m, in, out, (cudaStream_t)stream);
+}
+
+static int ref_kf_host(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out, bool frameOnDevice) {
+    const char* who = frameOnDevice ? "orbm_track_reference_keyframe_batch_resident" : "orbm_track_reference_keyframe_batch";
+    if (!h) { set_error(std::string(who) + ": bad argument"); return ORB_ERR_ARG; }
+    if (int rc = ref_kf_shape(h->m, in, out, who)) return rc;
+    Matcher& m = h->m;
+    const size_t B = in->batch, K = in->kcap, M = in->mcap;
+    const uint8_t* active = in->active;
+    for (size_t b = 0; b < B; ++b) {
+        if (active && !active[b]) continue;
+        const int nKF = in->kfN[b], eKF = in->kfNEntries[b];
+        if (nKF < 0 || nKF > in->mcap || eKF < 0 || eKF > nKF) { set_error(std::string(who) + ": keyframe N or nEntries out of range"); return ORB_ERR_ARG; }
+        if (!fv_ok(in->kfFvNode + b * M, in->kfFvFeature + b * M, eKF, nKF)) { set_error(std::string(who) + ": keyframe feature vector not sorted / out of range"); return ORB_ERR_ARG; }
+        if (frameOnDevice) continue;
+        const int nF = in->nK[b], eF = in->nEntries[b];
+        if (nF < 0 || nF > in->kcap || eF < 0 || eF > nF) { set_error(std::string(who) + ": frame N or nEntries out of range"); return ORB_ERR_ARG; }
+        if (!fv_ok(in->fvNode + b * K, in->fvFeature + b * K, eF, nF)) { set_error(std::string(who) + ": frame feature vector not sorted / out of range"); return ORB_ERR_ARG; }
+        for (int i = 0; i < nF; ++i) {
+            const int oct = in->kps[b * K + i].octave;
+            if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return ORB_ERR_ARG; }
+        }
+    }
+    CK(cudaSetDevice(m.device));
+    Staging& S = m.staging;
+    S.begin();
+    const size_t FK = frameOnDevice ? 0 : K, FB = frameOnDevice ? 0 : B;
+    const int pKps = S.in(frameOnDevice ? nullptr : in->kps, 28 * FB * FK), pDesc = S.in(frameOnDevice ? nullptr : in->desc, 32 * FB * FK),
+              pNK = S.in(frameOnDevice ? nullptr : in->nK, 4 * FB), pNode = S.in(frameOnDevice ? nullptr : in->fvNode, 4 * FB * FK),
+              pFeat = S.in(frameOnDevice ? nullptr : in->fvFeature, 4 * FB * FK), pNE = S.in(frameOnDevice ? nullptr : in->nEntries, 4 * FB),
+              pT = S.in(in->Tcw7, 28 * B), pKfN = S.in(in->kfN, 4 * B), pKfKps = S.in(in->kfKps, 28 * B * M), pKfDesc = S.in(in->kfDesc, 32 * B * M),
+              pKfNode = S.in(in->kfFvNode, 4 * B * M), pKfFeat = S.in(in->kfFvFeature, 4 * B * M), pKfNE = S.in(in->kfNEntries, 4 * B),
+              pPt = S.in(in->kfPoint, B * M), pXyz = S.in(in->xyz, 12 * B * M), pObs = S.in(in->hasObs, B * M),
+              pIs = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels), pAct = S.in(active, active ? B : 0),
+              pN = S.out(nullptr, 4 * B), pMatch = S.out(nullptr, 4 * B * K), pPose = S.out(nullptr, 56 * B), pTo = S.out(nullptr, 28 * B),
+              pDis = S.out(nullptr, B * M), pMap = S.out(nullptr, 4 * B);
+    int rc = S.reserve();
+    if (rc) return rc;
+    OrbmRefKeyFrameBatch d = *in;
+    if (!frameOnDevice) {
+        d.kps = S.dev<OrbKeyPoint>(pKps); d.desc = S.dev(pDesc); d.nK = S.dev<int>(pNK);
+        d.fvNode = S.dev<int>(pNode); d.fvFeature = S.dev<int>(pFeat); d.nEntries = S.dev<int>(pNE);
+    }
+    d.Tcw7 = S.dev<float>(pT); d.kfN = S.dev<int>(pKfN); d.kfKps = S.dev<OrbKeyPoint>(pKfKps); d.kfDesc = S.dev(pKfDesc);
+    d.kfFvNode = S.dev<int>(pKfNode); d.kfFvFeature = S.dev<int>(pKfFeat); d.kfNEntries = S.dev<int>(pKfNE); d.kfPoint = S.dev(pPt);
+    d.xyz = S.dev<float>(pXyz); d.hasObs = S.dev(pObs); d.invLevelSigma2 = S.dev<float>(pIs); d.active = active ? S.dev(pAct) : nullptr;
+    OrbmRefKeyFrameResult o = {S.dev<int>(pN), S.dev<int>(pMatch), S.dev<double>(pPose), S.dev<float>(pTo), S.dev(pDis), S.dev<int>(pMap)};
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    if ((rc = ref_kf_launch(m, &d, &o, st))) return rc;
+    CK(S.download(st));
+    copy_active_rows(S, pN, out->nmatches, 4, in->batch, active);
+    copy_active_rows(S, pMatch, out->match, 4 * K, in->batch, active);
+    std::vector<uint8_t> gated(B);               // the streams that ran PoseOptimization
+    for (size_t b = 0; b < B; ++b) gated[b] = (!active || active[b]) && S.host<int>(pN)[b] >= TRK_REF_MIN_MATCHES;
+    copy_active_rows(S, pPose, out->pose7, 56, in->batch, gated.data());
+    copy_active_rows(S, pTo, out->Tcw7, 28, in->batch, gated.data());
+    copy_active_rows(S, pDis, out->discarded, M, in->batch, gated.data());
+    copy_active_rows(S, pMap, out->nmatchesMap, 4, in->batch, gated.data());
+    return ORB_OK;
+}
+
+int orbm_track_reference_keyframe_batch(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out) {
+    return ref_kf_host(h, in, out, false);
+}
+int orbm_track_reference_keyframe_batch_resident(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const OrbmRefKeyFrameResult* out) {
+    return ref_kf_host(h, in, out, true);
 }
 
 // SearchLocalPoints of both local-map calls: tlm_frustum_kernel, then the local-map search (two launches).  Tcw7: the frame's pose.
