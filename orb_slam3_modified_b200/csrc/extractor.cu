@@ -64,9 +64,11 @@ struct Extractor {
     int rows = 0, cols = 0;
     ExtractParams P;
     std::vector<CellDesc> cells;
+    std::vector<FastBlock> fastBlocks;
     // device buffers
     uint8_t *d_pyr = nullptr, *d_blur = nullptr;
     CellDesc* d_cells = nullptr;
+    FastBlock* d_fastBlocks = nullptr;
     int* d_cellCount = nullptr;
     uint32_t* d_cellList = nullptr;
     uint32_t* d_cand = nullptr;
@@ -98,7 +100,7 @@ struct Extractor {
     ~Extractor() { release(); }
     void release() {
         cudaSetDevice(device);
-        void* ptrs[] = {d_pyr, d_blur, d_cells, d_cellCount, d_cellList, d_cand, d_nodeOf, d_sel, d_selCount, d_dstIndex,
+        void* ptrs[] = {d_pyr, d_blur, d_cells, d_fastBlocks, d_cellCount, d_cellList, d_cand, d_nodeOf, d_sel, d_selCount, d_dstIndex,
                         d_status, d_xtab, d_ytab, d_img, d_outKp, d_outDesc, d_outN, d_outMono, d_maps, d_blurMaps, d_stereoSad, d_stereoU, d_stereoD};
         for (void* p : ptrs) if (p) cudaFree(p);
         if (h_counts) cudaFreeHost(h_counts);
@@ -146,7 +148,7 @@ struct Extractor {
     int configure(int r, int c, std::vector<short4>& xtab, std::vector<short4>& ytab) {
         memset(&P, 0, sizeof(P));
         P.nlevels = nlevels; P.iniTh = iniTh; P.minTh = minTh; P.rows = r; P.cols = c;
-        cells.clear(); xtab.clear(); ytab.clear();
+        cells.clear(); fastBlocks.clear(); xtab.clear(); ytab.clear();
         size_t planeOff = 0, listOff = 0, candOff = 0;
         int selOff = 0, blurTiles = 0, maxNodes = 0, maxCells = 0;
         maxKp = 0;
@@ -188,18 +190,35 @@ struct Extractor {
                 }
             }
             G.nCells = (int)cells.size() - G.cellBase;
-            {   // TMA box covering the largest ROI of the level (width rounded up to 16 bytes)
-                int mw = 7, mh = 7;
-                int mwOff = 7;   // widest (x0 & 15) + rw: the box starts 16-byte aligned
-                for (int ci = G.cellBase; ci < (int)cells.size(); ++ci) {
-                    mw = std::max<int>(mw, cells[ci].rw); mh = std::max<int>(mh, cells[ci].rh);
-                    mwOff = std::max<int>(mwOff, (cells[ci].x0 & 15) + cells[ci].rw);
-                }
-                G.fastBoxW = (int)alignUp(mwOff, 16); G.fastBoxH = mh;
-                const int iwm = mw - 6, ihm = mh - 6;
-                const size_t spm = ((size_t)iwm + 2 + 3) & ~(size_t)3;
-                const size_t sm = alignUp((size_t)G.fastBoxW * G.fastBoxH, 128) + alignUp(((size_t)ihm + 2) * spm, 16) + 2 * (size_t)iwm * ihm;
-                smemFast = std::max(smemFast, sm);
+            {   // FAST blocks of 2 x 2 cells (partial at the right and bottom edges) and the TMA box covering the largest union window
+                // of the level (width rounded up to 16 bytes: the box starts 16-byte aligned).  The skipped cells are trailing rows and
+                // columns, so the listed cells form a row-major grid.
+                int gx = 0;
+                while (gx < G.nCells && cells[G.cellBase + gx].y0 == cells[G.cellBase].y0) ++gx;
+                const int gy = gx ? G.nCells / gx : 0;
+                int bw = 16, bh = 7, iwm = 0, ihm = 0;
+                for (int by = 0; by < gy; by += 2)
+                    for (int bx = 0; bx < gx; bx += 2) {
+                        FastBlock b = {};
+                        b.level = (uint16_t)l; b.ncx = (uint8_t)std::min(2, gx - bx); b.ncy = (uint8_t)std::min(2, gy - by);
+                        const CellDesc& c0 = cells[G.cellBase + by * gx + bx];
+                        b.x0 = c0.x0; b.y0 = c0.y0;
+                        int iw = 0, ih = 0;
+                        for (int k = 0; k < b.ncx * b.ncy; ++k) {
+                            b.cell[k] = G.cellBase + (by + k / b.ncx) * gx + bx + k % b.ncx;
+                            const CellDesc& c = cells[b.cell[k]];
+                            if (c.rw < 7 || c.rh < 7) continue;   // no interior: the kernel reports 0 corners
+                            iw = std::max(iw, c.x0 + c.rw - 3 - (b.x0 + 3)); ih = std::max(ih, c.y0 + c.rh - 3 - (b.y0 + 3));
+                        }
+                        b.iw = (uint16_t)iw; b.ih = (uint16_t)ih;
+                        if (iw > 0) {
+                            bw = std::max(bw, (b.x0 & 15) + iw + 6); bh = std::max(bh, ih + 6);
+                            iwm = std::max(iwm, iw); ihm = std::max(ihm, ih);
+                        }
+                        fastBlocks.push_back(b);
+                    }
+                G.fastBoxW = (int)alignUp(bw, 16); G.fastBoxH = bh;
+                smemFast = std::max(smemFast, (size_t)fast_smem_layout(G.fastBoxW, G.fastBoxH, iwm, ihm).total);
             }
             maxCells = std::max(maxCells, G.nCells);
             G.candOff = (uint32_t)candOff; G.candCap = (uint32_t)G.nCells * G.cellCap;
@@ -256,6 +275,7 @@ struct Extractor {
         }
         P.pyrFrameStride = planeOff;
         P.nCellsTotal = (int)cells.size();
+        P.nFastBlocks = (int)fastBlocks.size();
         P.cellCountStride = alignUp(cells.size(), 32);
         P.cellListStride = alignUp(listOff, 64);
         P.candStride = alignUp(candOff, 64);
@@ -285,6 +305,7 @@ struct Extractor {
         capCellList = P.cellListStride + P.cellListStride / 8; capCand = P.candStride + P.candStride / 8;
         capSel = P.selStride + 64; capX = xtab.size() + 64; capY = ytab.size() + 64;
         CK(cudaMalloc(&d_cells, sizeof(CellDesc) * capCells));
+        CK(cudaMalloc(&d_fastBlocks, sizeof(FastBlock) * capCells));   // never more blocks than cells
         CK(cudaMalloc(&d_cellCount, sizeof(int) * capCellCount * B));
         CK(cudaMalloc(&d_cellList, sizeof(uint32_t) * capCellList * B));
         CK(cudaMalloc(&d_cand, sizeof(uint32_t) * capCand * B));
@@ -312,7 +333,7 @@ struct Extractor {
         CK(cudaEventCreateWithFlags(&evJoin, cudaEventDisableTiming));
         CK(cudaMemcpyToSymbol(c_pattern, h_pattern, sizeof(h_pattern)));
         CK(cudaMemcpyToSymbol(c_umax, umax, sizeof(umax)));
-        maxSmemFast = 48 * 1024;   // worst-case cell is 76x76 in a 96-byte wide box: ~25 KB
+        maxSmemFast = 96 * 1024;   // a cell interior is at most 69 x 69 px, so a 2 x 2 block needs at most ~90 KB
         maxSmemQt = smemQt + 16 * 1024; maxSmemAs = 2 * capSel * sizeof(int);
         if (maxSmemQt > 200 * 1024) { set_error("nfeatures too large for the quadtree kernel's shared memory"); return ORB_ERR_ARG; }
         // process-wide monotonic maxima (device_utils.cuh): a smaller handle created later must not lower another handle's limit
@@ -342,9 +363,10 @@ struct Extractor {
         CK(cudaSetDevice(device));
         CK(cudaStreamSynchronize(stream));
         if (!cells.empty()) CK(cudaMemcpy(d_cells, cells.data(), sizeof(CellDesc) * cells.size(), cudaMemcpyHostToDevice));
+        if (!fastBlocks.empty()) CK(cudaMemcpy(d_fastBlocks, fastBlocks.data(), sizeof(FastBlock) * fastBlocks.size(), cudaMemcpyHostToDevice));
         if (!xtab.empty()) CK(cudaMemcpy(d_xtab, xtab.data(), sizeof(short4) * xtab.size(), cudaMemcpyHostToDevice));
         if (!ytab.empty()) CK(cudaMemcpy(d_ytab, ytab.data(), sizeof(short4) * ytab.size(), cudaMemcpyHostToDevice));
-        P.pyr = d_pyr; P.blur = d_blur; P.cells = d_cells; P.cellCount = d_cellCount; P.cellList = d_cellList;
+        P.pyr = d_pyr; P.blur = d_blur; P.cells = d_cells; P.fastBlocks = d_fastBlocks; P.cellCount = d_cellCount; P.cellList = d_cellList;
         P.cand = d_cand; P.nodeOf = d_nodeOf; P.sel = d_sel; P.selCount = d_selCount; P.dstIndex = d_dstIndex;
         P.status = d_status; P.xtab = d_xtab; P.ytab = d_ytab;
         for (int l = 0; l < nlevels; ++l) {
@@ -417,7 +439,7 @@ struct Extractor {
         ++launches;
         if (!profiling) CK(cudaEventRecord(evJoin, stream2));
         if (profiling) CK(cudaEventRecord(evStage[2], st));
-        fast_cells_kernel<<<dim3(Q.nCellsTotal, batch), FAST_NT, smemFast, st>>>(Q, map0, d_maps);
+        fast_cells_kernel<<<dim3(Q.nFastBlocks, batch), FAST_NT, smemFast, st>>>(Q, map0, d_maps);
         ++launches;
         if (profiling) CK(cudaEventRecord(evStage[3], st));
         quadtree_orient_kernel<<<dim3(nlevels, batch), QT_NT, smemQt, st>>>(Q);

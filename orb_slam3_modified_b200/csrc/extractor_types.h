@@ -39,6 +39,31 @@ struct CellDesc {
     uint32_t listOff;         // offset of this cell's list inside one frame's cell-list buffer
 };
 
+// Up to 2 x 2 neighbouring cells of one level that one FAST CTA detects together.  The cells' interiors tile the level, so their
+// union is one window: the ROI of the first cell grown to the bottom-right of the others.
+struct FastBlock {
+    uint16_t level;
+    uint16_t x0, y0;          // ROI origin of the first cell = origin of the union window
+    uint16_t iw, ih;          // union detection interior [3, 3 + iw) x [3, 3 + ih) of the window (0 x 0: every cell has rw or rh < 7)
+    uint8_t ncx, ncy;         // cells across / down
+    int cell[4];              // indices into the cell table, row-major inside the block
+};
+
+// Shared-memory carve-up of one FAST block CTA (byte offsets; the TMA tile is first, at 0).  Host and device both use it, so
+// the launch size is the maximum of exactly what the kernel addresses.
+struct FastSmem { int sp, nwp, score, bits, rowOff, list, total; };
+__host__ __device__ inline FastSmem fast_smem_layout(int boxW, int boxH, int iw, int ih) {
+    FastSmem L;
+    L.sp = 4 * ((iw + 3) >> 2) + 8;                    // score-map pitch: whole quads + 4-byte left margin + right ring
+    L.nwp = (iw + 31) >> 5;                            // keep-bitmap words per row
+    L.score = (boxW * boxH + 127) & ~127;              // (ih + 2) * sp: interior (y, x) at (y + 1) * sp + x + 4
+    L.bits = L.score + ((L.sp * (ih + 2) + 15) & ~15); // lo bitmap, then hi bitmap: ih * nwp words each
+    L.rowOff = L.bits + 8 * ih * L.nwp;                // one int per (cell, row): at most two cells share a row
+    L.list = L.rowOff + 8 * ih;                        // candidates (y << 8 | x), at most iw * ih
+    L.total = L.list + 2 * iw * ih;
+    return L;
+}
+
 // Selected keypoint before output assembly.
 struct SelKp {
     int16_t x, y;             // level coordinates (border offset already added)
@@ -58,6 +83,7 @@ struct ExtractParams {
     const uint8_t* lv0; size_t lv0Pitch, lv0FrameStride;
     int blurTilesTotal;
     const CellDesc* cells; int nCellsTotal;
+    const FastBlock* fastBlocks; int nFastBlocks;
     int* cellCount;        size_t cellCountStride;
     uint32_t* cellList;    size_t cellListStride;
     uint32_t* cand;        size_t candStride;       // gathered candidates (packed x|y|score)
