@@ -87,7 +87,11 @@ int orbx_extract_batch(orbx_handle* h, const uint8_t* images, int batch, int row
 
 /* Device-resident variant: every pointer is a device pointer, work is enqueued on `stream`
  * (cudaStream_t) and the call returns without synchronising.  Slabs have fixed capacity `cap`
- * per frame so that they can be all-gathered as-is (SURVEY.md 8e). */
+ * per frame so that they can be all-gathered as-is (SURVEY.md 8e).
+ * Capacity: a frame with K > cap keypoints gets no rows at all (its keypoint and descriptor rows
+ * keep what they held); d_nkeypoints[f] still receives K and d_monoIndex[f] the monoIndex, so
+ * d_nkeypoints[f] > cap is how the caller sees the overflow.  The other frames are written as usual
+ * and the call itself returns ORB_OK. */
 int orbx_extract_batch_device(orbx_handle* h, const uint8_t* d_images, int batch, int rows, int cols, size_t step,
                               size_t frame_stride, int lap0, int lap1, OrbKeyPoint* d_keypoints,
                               uint8_t* d_descriptors, int cap, int* d_nkeypoints, int* d_monoIndex, void* stream);
@@ -115,7 +119,9 @@ int orbx_stereo_matches_device(orbx_handle* left, orbx_handle* right, int batch,
 int orbx_copy_level_bordered(orbx_handle* h, int frame, int level, int border, uint8_t* dst);
 
 /* Debug/inspection taps used by the parity tests (mvImagePyramid is a public member of the reference class,
- * include/ORBextractor.h:84).  Copies level `level` of frame `frame` of the last call, unbordered, tightly packed. */
+ * include/ORBextractor.h:84).  Copies level `level` of frame `frame` of the last call, unbordered, tightly packed.
+ * Level 0 unblurred is read from the plane the last call read: after orbx_extract_batch_device with 16-byte aligned frames that
+ * is the caller's own device frames, which must then still hold the images; `frame` must be below that call's batch. */
 int orbx_get_level_size(const orbx_handle* h, int level, int* width, int* height);
 int orbx_copy_level(orbx_handle* h, int frame, int level, int blurred, uint8_t* dst);
 /* FAST candidates of one level of the last call as (x, y, score) int triples in the order the reference

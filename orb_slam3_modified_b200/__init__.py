@@ -244,6 +244,19 @@ class ORBextractor:
             raise OrbError(rc, 'orbx_stereo_matches')
         return ur, dep
 
+    def ComputeStereoMatchesDevice(self, right, d_kpsL, d_descL, d_nL, d_kpsR, d_descR, d_nR, mb, mbf, d_uRight, d_depth, stream=0):
+        """All-device ComputeStereoMatches (torch CUDA tensors) for the pairs both extractors processed in their last call (self = left):
+        the slabs as extract_batch_device wrote them (d_kps* [B, cap, 7], d_desc* [B, cap, 32] u8, d_n* [B] i32); d_uRight / d_depth
+        [B, capL] float32 receive mvuRight / mvDepth (-1 = no match).  Enqueues on ``stream`` and returns immediately."""
+        B, capL = d_descL.shape[:2]
+        capR = d_descR.shape[1]
+        lib().orbx_stereo_matches_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 3 + \
+            [C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 3
+        rc = lib().orbx_stereo_matches_device(self._h, right._h, B, _ptr(d_kpsL), _ptr(d_descL), _ptr(d_nL), capL, _ptr(d_kpsR), _ptr(d_descR),
+                                              _ptr(d_nR), capR, mb, mbf, _ptr(d_uRight), _ptr(d_depth), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbx_stereo_matches_device')
+
     def candidates(self, level, frame=0, cap=400000):
         out = np.zeros((cap, 3), np.int32)
         n = lib().orbx_copy_candidates(self._h, frame, level, _ptr(out), cap)

@@ -589,8 +589,12 @@ int orbx_copy_level(orbx_handle* h, int frame, int level, int blurred, uint8_t* 
     const LevelGeom& G = e.P.lv[level];
     const uint8_t* src;
     size_t pitch = G.pitch;
-    if (level == 0 && !blurred) { src = e.d_img + (size_t)frame * G.pitch * e.rows; }
-    else src = (blurred ? e.d_blur : e.d_pyr) + (size_t)frame * e.P.pyrFrameStride + G.planeOff;
+    if (level == 0 && !blurred) {
+        // the plane the last call read: the staging copy, the internal copy of unaligned frames, or the caller's own device frames
+        if (!e.hasLast || frame >= e.lastQ.batch) { set_error("orbx_copy_level: level 0 of a frame the last call did not process"); return ORB_ERR_ARG; }
+        src = e.lastQ.lv0 + (size_t)frame * e.lastQ.lv0FrameStride;
+        pitch = e.lastQ.lv0Pitch;
+    } else src = (blurred ? e.d_blur : e.d_pyr) + (size_t)frame * e.P.pyrFrameStride + G.planeOff;
     CK(cudaMemcpy2D(dst, G.w, src, pitch, G.w, G.h, cudaMemcpyDeviceToHost));
     return ORB_OK;
 }

@@ -13,14 +13,26 @@ cv2 = pytest.importorskip('cv2')
 EDGE_THRESHOLD = 19
 
 
-@pytest.mark.parametrize('t,ini,mn', [(4, 20, 7), (8, 20, 7), (8, 60, 12)])
+@pytest.mark.parametrize('t,ini,mn', [(4, 20, 7), (8, 20, 7), (8, 60, 12), (4, 12, 5), (4, 40, 7), (4, 20, 20), (4, 3, 1)])
 def test_pyramid_and_cell_candidates(t, ini, mn):
-    img = synth.frame(t)
-    ex = O.OracleExtractor(1000, 1.2, 8, ini, mn)
+    _pyramid_and_cell_candidates(t, ini, mn, 640, 480, 1.2, 8)
+
+
+# the geometries tests/test_extractor_paths_gpu.py runs (level 1 of the first four takes the bilinear resize, then 4095 px wide, one
+# level, 720p), plus a 1.9 scale factor whose levels are neither 2x decimations nor small steps
+@pytest.mark.parametrize('w,h,scaleFactor,nlevels', [(517, 389, 2.0, 3), (1241, 376, 2.0, 3), (640, 480, 2.5, 3), (640, 480, 3.0, 2),
+                                                     (4095, 300, 1.2, 8), (640, 480, 1.2, 1), (640, 480, 1.9, 4), (1280, 720, 1.2, 8)])
+def test_pyramid_and_cell_candidates_geometry(w, h, scaleFactor, nlevels):
+    _pyramid_and_cell_candidates(4, 20, 7, w, h, scaleFactor, nlevels)
+
+
+def _pyramid_and_cell_candidates(t, ini, mn, w, h, scaleFactor, nlevels):
+    img = synth.frame(t, w, h)
+    ex = O.OracleExtractor(1000, scaleFactor, nlevels, ini, mn)
     ex(img, (0, 1000))
     inv = np.asarray(ex.tables()['inv_scale'], np.float32)
     prev = img
-    for level in range(8):
+    for level in range(nlevels):
         if level:
             # ComputePyramid :1175-1183: Size(cvRound(cols * scale), cvRound(rows * scale)) with scale = mvInvScaleFactor[level]
             sz = (int(np.rint(np.float32(img.shape[1]) * inv[level])), int(np.rint(np.float32(img.shape[0]) * inv[level])))

@@ -9,13 +9,15 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, 'tests', 'cpp_example')
 
 
-def _build():
+def _build(out_dir):
+    """Compile tests/cpp_example.cpp into `out_dir` (never into the repository tree, which may not be writable) and return its path."""
+    exe = os.path.join(str(out_dir), 'cpp_example')
     lib = os.path.join(ROOT, 'orb_slam3_modified_b200')
     subprocess.check_call(['g++', '-std=c++14', '-O2', '-Wall', '-I', os.path.join(ROOT, 'include'), os.path.join(ROOT, 'tests', 'cpp_example.cpp'),
-                           '-o', EXE, '-L', lib, '-l:liborb_b200.so', '-Wl,-rpath,' + lib, '-lpthread'])
+                           '-o', exe, '-L', lib, '-l:liborb_b200.so', '-Wl,-rpath,' + lib, '-lpthread'])
+    return exe
 
 
 def _checksum(b):
@@ -25,9 +27,8 @@ def _checksum(b):
     return s
 
 
-def test_cpp_shim_compiles_and_links():
-    _build()
-    assert os.path.exists(EXE)
+def test_cpp_shim_compiles_and_links(tmp_path):
+    assert os.path.exists(_build(tmp_path))
 
 
 @pytest.mark.gpu
@@ -35,7 +36,7 @@ def test_cpp_shim_runs_like_the_oracle(tmp_path):
     import oracle_lib as O
     import matcher_scenes as S
     from orb_slam3_modified_b200 import synth
-    _build()
+    exe = _build(tmp_path)
     t = 12
     sc = S.last_frame_scene(t)
     img = synth.frame(t)
@@ -57,7 +58,7 @@ def test_cpp_shim_runs_like_the_oracle(tmp_path):
                           ('liba_is2', lp['inv_sigma2'], np.float32), ('liba_k1', lp['ie_kf1'], np.int32), ('liba_k2', lp['ie_kf2'], np.int32), ('liba_ep', lp['e_pt'], np.int32),
                           ('liba_ek', lp['e_kf'], np.int32)):
         (tmp_path / (name + '.raw')).write_bytes(np.ascontiguousarray(arr, dt).tobytes())
-    out = dict(l.split(' ', 1) for l in subprocess.check_output([EXE, str(tmp_path), '480', '640']).decode().strip().splitlines())
+    out = dict(l.split(' ', 1) for l in subprocess.check_output([exe, str(tmp_path), '480', '640']).decode().strip().splitlines())
     # extract
     mono, kps, desc = O.OracleExtractor()(img, (0, 1000))
     assert [int(v) for v in out['extract'].split()] == [mono, len(kps), _checksum(desc.tobytes())]

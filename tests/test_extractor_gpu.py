@@ -21,15 +21,22 @@ def synth():
 
 
 def _compare(ex, oe, img, lap, tag=''):
-    mono, kps, desc = ex(img, lap)
-    omono, okps, odesc = oe(img, lap)
+    return _check_frame(ex, 0, ex(img, lap), oe, oe(img, lap), tag)
+
+
+def _check_frame(ex, f, result, oe, oresult, tag=''):
+    """Frame `f` of `ex`'s last call, whose (mono, kps, desc) is `result`, against the oracle's last call on the same image."""
+    mono, kps, desc = result
+    omono, okps, odesc = oresult
     # stage taps first: they localise a failure
     for l in range(ex.nlevels):
-        lv, olv = ex.level(l), oe.level(l)
+        lv, olv = ex.level(l, f), oe.level(l)
         assert lv.shape == olv.shape, (tag, 'level shape', l)
         assert np.array_equal(lv, olv), (tag, 'pyramid level differs', l, int((lv != olv).sum()))
+        bl, obl = ex.level(l, f, blurred=True), O.blur7(olv)
+        assert np.array_equal(bl, obl), (tag, 'blurred level differs', l, int((bl != obl).sum()))
     for l in range(ex.nlevels):
-        c = ex.candidates(l)
+        c = ex.candidates(l, f)
         oc = oe.candidates(l)
         ocx = np.stack([oc['x'], oc['y'], oc['response']], 1).astype(np.int32)
         assert c.shape == ocx.shape, (tag, 'candidate count', l, c.shape, ocx.shape)
