@@ -1226,6 +1226,8 @@ struct Solver {
 
     int upload(int count, const LbaProblem* probs) {
         if (count < 1 || count > maxBatch) { set_error("lba: batch larger than max_batch"); return ORB_ERR_ARG; }
+        // from here on the slots' layouts and arena contents change: until this upload succeeds there is nothing to run or download
+        nLoaded = 0;
         uploadBytes.assign(maxBatch, 0); uploadOff.assign(maxBatch, 0);
         CK(cudaSetDevice(device));
         if (ranOnce) CK(cudaStreamWaitEvent(st, evRun, 0));   // a run may still be reading the arena on the caller's stream

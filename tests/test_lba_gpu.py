@@ -20,6 +20,11 @@ def opt():
 def _check(opt, p, **kw):
     ref = O.lba_solve(p, **kw)
     out = opt.LocalBundleAdjustment(p, **kw)
+    return _agrees(p, out, ref)
+
+
+def _agrees(p, out, ref):
+    """The GPU result `out` of problem p against the oracle's `ref` (the assertions of _check, for batched calls)."""
     assert out['iters'] == ref['iters'], (out['iters'], ref['iters'])
     assert out['trials'] == int(ref['stats'][3])
     r_ref = O.lba_residuals(p, ref['poses'], ref['points'])
