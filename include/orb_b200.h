@@ -445,6 +445,29 @@ typedef struct OrbmFusePoints {
 } OrbmFusePoints;
 int orbm_fuse_search(orbm_handle* h, const OrbmFrame* KF, const float* invLevelSigma2, float logScaleFactor, const float* Tcw7, const float* Ow3,
                      const float* cam4, const OrbmFusePoints* pts, float th, int32_t* bestIdx, int32_t* bestDist);
+/* The searches of several ORBmatcher::Fuse(KeyFrame*, vector<MapPoint*>, th) calls (each exactly orbm_fuse_search's) in ONE upload through the
+ * handle's staging, ONE launch and ONE download; orbm_last_launch_count() is 1 (0 when every item is empty).  Items with pts.M == 0 or KF.K == 0
+ * get -1 / 256 and take no CTA.  Host pointers.
+ * PRECONDITION: the items must not depend on each other's bookkeeping.  LocalMapping::SearchInNeighbors of several keyframes runs in lockstep
+ * rounds: round r holds target r of every keyframe (one keyframe per MAP: keyframes of different maps share no keyframe and no map point),
+ * with state and descriptors read after round r-1's walk; the Fuse(mpCurrentKeyFrame, vpFuseCandidates) of all keyframes is one more call
+ * (INTEGRATION.md §2, DESIGN.md §4).  Two keyframes of the same map in one call are NOT equivalent to the reference.
+ * ORB_ERR_ARG: an octave outside [0, nlevels), empty bounds, nlevels outside [1, 256], a null pointer an item needs (invLevelSigma2
+ * always; keypoints / descriptors when K > 0; the point arrays and the outputs when M > 0); ORB_ERR_CAPACITY: K > max_keypoints of the handle or
+ * a keyframe too large for the shared-memory grid.  Both before any launch. */
+typedef struct OrbmFuseItem {
+    OrbmFrame KF;                 /* the target keyframe: mvKeysUn, mDescriptors, bounds, mvScaleFactors */
+    const float* invLevelSigma2;  /* mvInvLevelSigma2 [KF.nlevels] */
+    float logScaleFactor;         /* mfLogScaleFactor */
+    float Tcw7[7];                /* GetPose(): unit quaternion (w, x, y, z) + t */
+    float Ow[3];                  /* GetCameraCenter() */
+    float cam[4];                 /* fx, fy, cx, cy */
+    float th;                     /* Fuse's th: 3 in SearchInNeighbors */
+    OrbmFusePoints pts;           /* the points to fuse into KF; state as for orbm_fuse_search */
+    int32_t* bestIdx;             /* [pts.M] out */
+    int32_t* bestDist;            /* [pts.M] out */
+} OrbmFuseItem;
+int orbm_fuse_search_batch(orbm_handle* h, int nItems, const OrbmFuseItem* items);
 /* int ORBmatcher::Fuse(KeyFrame* pKF, Sophus::Sim3f& Scw, const vector<MapPoint*>& vpPoints, float th, vector<MapPoint*>& vpReplacePoint)
  * (include/ORBmatcher.h:102, src/ORBmatcher.cc:1340-1455; LoopClosing::SearchAndFuse): the search of orbm_fuse_search without the chi-square
  * gate.  Tcw7 / Ow3: the caller's decomposition of Scw (:1349-1350: SE3f(Scw.rotationMatrix(), Scw.translation() / Scw.scale()) and its

@@ -200,6 +200,15 @@ public:
         orb_check(orbm_frustum_project(detail::matcher_handle(1, points.M, device_), &points, out.inView.data(), out.projX.data(), out.projY.data(),
                                        out.projXR.data(), out.depth.data(), out.level.data(), out.viewCos.data()), "orbm_frustum_project");
     }
+    // The searches of int Fuse(KeyFrame* pKF, const vector<MapPoint*>& vpMapPoints, const float th = 3.0) for several keyframes in one launch
+    // (orbm_fuse_search_batch): one round of LocalMapping::SearchInNeighbors for keyframes of DIFFERENT maps (INTEGRATION.md §2).  Every
+    // item's bestIdx / bestDist receive its search; the caller walks them in map-point order (src/ORBmatcher.cc:1310-1330), re-testing
+    // isBad() / IsInKeyFrame(pKF) when it reaches a point.
+    void FuseBatch(const std::vector<OrbmFuseItem>& items) {
+        int maxK = 1;
+        for (const OrbmFuseItem& it : items) if (it.KF.K > maxK) maxK = it.KF.K;
+        orb_check(orbm_fuse_search_batch(detail::matcher_handle(maxK, 1, device_), (int)items.size(), items.data()), "orbm_fuse_search_batch");
+    }
     // cv::BFMatcher(NORM_HAMMING).knnMatch(query, train, matches, 2)
     void knnMatch(const Descriptors& query, const Descriptors& train, std::vector<int32_t>& idx, std::vector<int32_t>& dist) {
         idx.assign((size_t)query.rows * 2, -1); dist.assign((size_t)query.rows * 2, -1);

@@ -358,6 +358,15 @@ class _OrbmRefKeyFrameResult(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _REF_KF_OUT]
 
 
+class _OrbmFusePoints(C.Structure):
+    _fields_ = [('M', C.c_int)] + [(n, C.c_void_p) for n in ('state', 'worldPos', 'normal', 'minDistance', 'maxDistance', 'descriptors')]
+
+
+class _OrbmFuseItem(C.Structure):
+    _fields_ = [('KF', _OrbmFrame), ('invLevelSigma2', C.c_void_p), ('logScaleFactor', C.c_float), ('Tcw7', C.c_float * 7), ('Ow', C.c_float * 3),
+                ('cam', C.c_float * 4), ('th', C.c_float), ('pts', _OrbmFusePoints), ('bestIdx', C.c_void_p), ('bestDist', C.c_void_p)]
+
+
 def _c(a, dt):
     return np.ascontiguousarray(a, dt)
 
@@ -797,6 +806,39 @@ class ORBmatcher:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_fuse_search_sim3')
         return bi, bd
+
+    FUSE_ITEM_KEYS = ('kps', 'desc', 'bounds', 'sf', 'isg', 'log_sf', 'Tcw', 'Ow', 'cam', 'state', 'xyz', 'normal', 'min_d', 'max_d', 'mp_desc')
+
+    def fuse_search_batch(self, items, th=3.0):
+        """The searches of several ``ORBmatcher::Fuse(KeyFrame*, const vector<MapPoint*>&, th)`` calls in one launch (orbm_fuse_search_batch).
+        Each item is a dict with the keys of ``FUSE_ITEM_KEYS`` (the arguments of :meth:`FuseSearch`) and optionally its own ``th``.  Returns
+        [(bestIdx [M], bestDist [M])] in item order, each equal to :meth:`FuseSearch` of that item.  The items must not depend on each other's
+        bookkeeping: at most one keyframe per map (see include/orb_b200.h)."""
+        keep, out = [], []
+        arr = (_OrbmFuseItem * max(len(items), 1))()
+        for j, it in enumerate(items):
+            k = [_c(it['kps'], KP_DTYPE), _c(it['desc'], np.uint8), _c(it['sf'], np.float32), _c(it['isg'], np.float32)]
+            m = [_c(it[n], dt) for n, dt in (('state', np.uint8), ('xyz', np.float32), ('normal', np.float32), ('min_d', np.float32), ('max_d', np.float32),
+                                             ('mp_desc', np.uint8))]
+            M = len(m[0])
+            bi = np.zeros(M, np.int32); bd = np.zeros(M, np.int32)
+            keep.append(k + m); out.append((bi, bd))
+            s = arr[j]
+            s.KF = _OrbmFrame(len(k[0]), k[0].ctypes.data, k[1].ctypes.data, *[float(b) for b in it['bounds']], k[2].ctypes.data, len(k[2]))
+            s.invLevelSigma2 = k[3].ctypes.data
+            s.logScaleFactor = float(it['log_sf'])
+            s.Tcw7[:] = [float(v) for v in np.asarray(it['Tcw'], np.float32)]
+            s.Ow[:] = [float(v) for v in np.asarray(it['Ow'], np.float32)]
+            s.cam[:] = [float(v) for v in np.asarray(it['cam'], np.float32)]
+            s.th = float(it.get('th', th))
+            s.pts = _OrbmFusePoints(M, *[a.ctypes.data for a in m])
+            s.bestIdx, s.bestDist = bi.ctypes.data, bd.ctypes.data
+        L = lib()
+        L.orbm_fuse_search_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        rc = L.orbm_fuse_search_batch(self._h, len(items), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_fuse_search_batch')
+        return out
 
     def SearchBySim3(self, kf1, kf2, bounds, scale_factors, log_scale_factor, cam4, pre12, th=7.5):
         """``int ORBmatcher::SearchBySim3(pKF1, pKF2, vpMatches12, S12, th)`` (src/ORBmatcher.cc:1457-1674).  kf = dict(kps, desc, state, pcam (the map points

@@ -759,6 +759,8 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
 // MapPoint::PredictScale, then the radius search of KeyFrame::GetFeaturesInArea (src/KeyFrame.cc:704-753) with the level window
 // [predicted - 1, predicted] and the chi-square gate e2 * invSigma2 > 5.99; first smallest distance wins.  No search depends on what Fuse does
 // with another map point's hit, so the AddObservation / Replace bookkeeping stays with the caller (in map-point order).
+// One launch serves a table of independent searches (items: keyframe, pose, points, outputs); item j owns CTAs
+// [ctaBegin, ctaBegin + nCta) and each of them builds that item's grid.  Single searches are tables of one.
 // ---------------------------------------------------------------------------------------------
 struct FuseParams {
     MatchParams P;          // keyframe: kps, desc, bounds, scaleFactors, nlevels, ks, descInSmem
@@ -768,16 +770,18 @@ struct FuseParams {
     float Tcw[7], Ow[3], logSF;
     int mode, gate;         // mode 0: world point + pose + normal test (Fuse); 2: point given in the camera frame (SearchBySim3).  gate: chi-square test
     int *bestIdx, *bestDist;
+    int ctaBegin, nCta;
 };
-__global__ void __launch_bounds__(MF_NT) fuse_search_kernel(FuseParams Q) {
+__global__ void __launch_bounds__(MF_NT) fuse_search_kernel(const FuseParams* __restrict__ items, const int* __restrict__ ctaItem) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     __shared__ int s_warp[33];
+    const FuseParams& Q = items[ctaItem[blockIdx.x]];
     const MatchParams& P = Q.P;
     const int tid = threadIdx.x, lane = tid & 31;
     const FrameSmem S = carve_frame_smem(smem_raw, P.ks, 1, P.descInSmem != 0);
     build_frame_smem(S, P.kps, P.desc, Q.K, P.minX, P.minY, P.gridWInv, P.gridHInv, s_warp);
-    const int nw = gridDim.x * (MF_NT / 32);
-    for (int i = blockIdx.x * (MF_NT / 32) + (tid >> 5); i < Q.M; i += nw) {
+    const int nw = Q.nCta * (MF_NT / 32);
+    for (int i = (blockIdx.x - Q.ctaBegin) * (MF_NT / 32) + (tid >> 5); i < Q.M; i += nw) {
         int bestIdx = -1, bestDist = 256;
         bool go = Q.state[i] == 1;
         float u = 0.f, v = 0.f, r = 0.f; int lvl = 0;
@@ -1795,52 +1799,117 @@ int orbm_search_by_bow_kf(orbm_handle* h, const OrbmBowFrame* KF1, const uint8_t
     return search_by_bow_impl(h, KF1, point1, KF2, point2, nnratio, checkOrientation, nullptr, match12, nmatches);
 }
 
+// One search of fuse_search_kernel's table, host pointers.  invLevelSigma2 == nullptr: no chi-square gate.
+struct FuseJob {
+    const OrbmFrame* KF; const float* invLevelSigma2; float logScaleFactor;
+    const float *Tcw7, *Ow3, *cam4;      // Tcw7 / Ow3 read in mode 0 only
+    const OrbmFusePoints* pts; float th; int mode;
+    int32_t *bestIdx, *bestDist;
+};
+
+// Runs the jobs (arguments already checked by the entry point) in ONE upload, ONE launch of fuse_search_kernel and ONE download.  Every
+// output starts as -1 / 256; jobs with M == 0 or K == 0 stop there and take no CTA.  Keypoint octaves and the shared-memory grid are checked
+// for all jobs before anything is staged.
+static int fuse_search_run(Matcher& m, int n, const FuseJob* jobs) {
+    CK(cudaSetDevice(m.device));
+    for (int j = 0; j < n; ++j)
+        for (int i = 0; i < jobs[j].pts->M; ++i) { jobs[j].bestIdx[i] = -1; jobs[j].bestDist[i] = 256; }
+    const size_t limit = 227 * 1024 - 2048;
+    std::vector<int> act;
+    size_t sm = 0;
+    int nCta = 0;
+    for (int j = 0; j < n; ++j) {
+        const OrbmFrame* KF = jobs[j].KF;
+        const int M = jobs[j].pts->M, K = KF->K;
+        if (M == 0 || K == 0) continue;
+        for (int k = 0; k < K; ++k) if (KF->keypoints[k].octave < 0 || KF->keypoints[k].octave >= KF->nlevels) { set_error("orbm_fuse_search: keypoint octave out of range"); return ORB_ERR_ARG; }
+        const size_t b = frame_smem_bytes(K, 1, frame_smem_bytes(K, 1, true) <= limit);
+        if (b > limit) { set_error("keyframe too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
+        sm = std::max(sm, b);
+        act.push_back(j);
+        nCta += std::min(16, (M + 127) / 128);          // every CTA rebuilds its item's grid: a few CTAs per item, ~8 map points per warp
+    }
+    if (act.empty()) return ORB_OK;
+    int rc = ensure_dynamic_smem(fuse_search_kernel, sm, m.device);
+    if (rc) return rc;
+    struct Pieces { int kp, de, sf, is, st, xy, no, mi, ma, md, bi, bd; };
+    std::vector<Pieces> pc(act.size());
+    Staging& S = m.staging;
+    S.begin();
+    for (size_t a = 0; a < act.size(); ++a) {
+        const FuseJob& J = jobs[act[a]];
+        const OrbmFusePoints* pts = J.pts;
+        const size_t M = (size_t)pts->M, K = (size_t)J.KF->K, nl = J.KF->nlevels;
+        Pieces& p = pc[a];
+        p.kp = S.in(J.KF->keypoints, sizeof(OrbKeyPoint) * K); p.de = S.in(J.KF->descriptors, 32 * K); p.sf = S.in(J.KF->scaleFactors, 4 * nl);
+        p.is = S.in(J.invLevelSigma2, J.invLevelSigma2 ? 4 * nl : 0); p.st = S.in(pts->state, M); p.xy = S.in(pts->worldPos, 12 * M);
+        p.no = S.in(pts->normal, J.mode == 0 ? 12 * M : 0); p.mi = S.in(pts->minDistance, 4 * M); p.ma = S.in(pts->maxDistance, 4 * M);
+        p.md = S.in(pts->descriptors, 32 * M); p.bi = S.out(J.bestIdx, 4 * M); p.bd = S.out(J.bestDist, 4 * M);
+    }
+    const int pTab = S.in(nullptr, sizeof(FuseParams) * act.size()), pCta = S.in(nullptr, sizeof(int) * nCta);
+    if ((rc = S.reserve())) return rc;
+    FuseParams* tab = S.host<FuseParams>(pTab);
+    int* ctaItem = S.host<int>(pCta);
+    for (size_t a = 0, c = 0; a < act.size(); ++a) {
+        const FuseJob& J = jobs[act[a]];
+        const OrbmFrame* KF = J.KF;
+        const Pieces& p = pc[a];
+        FuseParams& Q = tab[a];
+        memset(&Q, 0, sizeof(Q));
+        MatchParams& P = Q.P;
+        P.kps = S.dev<OrbKeyPoint>(p.kp); P.desc = S.dev(p.de); P.scaleFactors = S.dev<float>(p.sf); P.kcap = m.kcap; P.nlevels = KF->nlevels; P.batch = 1;
+        P.minX = KF->minX; P.minY = KF->minY; P.maxX = KF->maxX; P.maxY = KF->maxY;
+        P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX); P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
+        P.th = J.th; memcpy(P.cam, J.cam4, 16);
+        P.ks = KF->K; P.ms = 1;
+        P.descInSmem = frame_smem_bytes(P.ks, 1, true) <= limit ? 1 : 0;
+        Q.K = KF->K; Q.M = J.pts->M; Q.state = S.dev(p.st); Q.mpDesc = S.dev(p.md); Q.xyz = S.dev<float>(p.xy); Q.normal = S.dev<float>(p.no);
+        Q.minD = S.dev<float>(p.mi); Q.maxD = S.dev<float>(p.ma); Q.invSigma2 = S.dev<float>(p.is);
+        if (J.mode == 0) { memcpy(Q.Tcw, J.Tcw7, 28); memcpy(Q.Ow, J.Ow3, 12); }
+        Q.logSF = J.logScaleFactor; Q.mode = J.mode; Q.gate = J.invLevelSigma2 ? 1 : 0;
+        Q.bestIdx = S.dev<int>(p.bi); Q.bestDist = S.dev<int>(p.bd);
+        Q.ctaBegin = (int)c; Q.nCta = std::min(16, (Q.M + 127) / 128);
+        for (int k = 0; k < Q.nCta; ++k) ctaItem[c++] = (int)a;
+    }
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    fuse_search_kernel<<<nCta, MF_NT, sm, st>>>(S.dev<FuseParams>(pTab), S.dev<int>(pCta));
+    m.launches = 1;
+    CK(cudaGetLastError());
+    CK(S.download(st));
+    return ORB_OK;
+}
+
 static int project_search_impl(orbm_handle* h, const OrbmFrame* KF, const float* invLevelSigma2, float logScaleFactor, const float* Tcw7, const float* Ow3,
                                const float* cam4, const OrbmFusePoints* pts, float th, int mode, int32_t* bestIdx, int32_t* bestDist) {
     if (!h || !KF || (mode == 0 && (!Tcw7 || !Ow3)) || !cam4 || !pts || !bestIdx || !bestDist || pts->M < 0 || KF->K < 0 || KF->K > h->m.kcap ||
         !KF->scaleFactors || KF->nlevels < 1 || KF->nlevels > 256 || !(KF->maxX > KF->minX) || !(KF->maxY > KF->minY)) {
         set_error("orbm_fuse_search: bad argument (KF.K <= max_keypoints of the handle)"); return ORB_ERR_ARG;
     }
-    Matcher& m = h->m;
-    CK(cudaSetDevice(m.device));
-    const size_t M = (size_t)pts->M, K = (size_t)KF->K;
-    for (size_t i = 0; i < M; ++i) { bestIdx[i] = -1; bestDist[i] = 256; }
-    if (M == 0 || K == 0) return ORB_OK;
-    for (size_t k = 0; k < K; ++k) if (KF->keypoints[k].octave < 0 || KF->keypoints[k].octave >= KF->nlevels) { set_error("orbm_fuse_search: keypoint octave out of range"); return ORB_ERR_ARG; }
-    const size_t nl = KF->nlevels;
-    Staging& S = m.staging;
-    S.begin();
-    const int pKp = S.in(KF->keypoints, sizeof(OrbKeyPoint) * K), pDe = S.in(KF->descriptors, 32 * K), pSf = S.in(KF->scaleFactors, 4 * nl),
-              pIs = S.in(invLevelSigma2, invLevelSigma2 ? 4 * nl : 0), pSt = S.in(pts->state, M), pXy = S.in(pts->worldPos, 12 * M),
-              pNo = S.in(pts->normal, mode == 0 ? 12 * M : 0), pMi = S.in(pts->minDistance, 4 * M), pMa = S.in(pts->maxDistance, 4 * M),
-              pMd = S.in(pts->descriptors, 32 * M), pBi = S.out(bestIdx, 4 * M), pBd = S.out(bestDist, 4 * M);
-    int rc = S.reserve();
-    if (rc) return rc;
-    cudaStream_t st = m.stream;
-    FuseParams Q; memset(&Q, 0, sizeof(Q));
-    MatchParams& P = Q.P;
-    P.kps = S.dev<OrbKeyPoint>(pKp); P.desc = S.dev(pDe); P.scaleFactors = S.dev<float>(pSf); P.kcap = m.kcap; P.nlevels = KF->nlevels; P.batch = 1;
-    P.minX = KF->minX; P.minY = KF->minY; P.maxX = KF->maxX; P.maxY = KF->maxY;
-    P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX); P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
-    P.th = th; memcpy(P.cam, cam4, 16);
-    P.ks = (int)K; P.ms = 1;
-    const size_t limit = 227 * 1024 - 2048;
-    P.descInSmem = frame_smem_bytes(P.ks, 1, true) <= limit ? 1 : 0;
-    const size_t sm = frame_smem_bytes(P.ks, 1, P.descInSmem != 0);
-    if (sm > limit) { set_error("keyframe too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
-    if ((rc = ensure_dynamic_smem(fuse_search_kernel, sm, m.device))) return rc;
-    Q.K = (int)K; Q.M = (int)M; Q.state = S.dev(pSt); Q.mpDesc = S.dev(pMd); Q.xyz = S.dev<float>(pXy); Q.normal = S.dev<float>(pNo);
-    Q.minD = S.dev<float>(pMi); Q.maxD = S.dev<float>(pMa); Q.invSigma2 = S.dev<float>(pIs);
-    if (mode == 0) { memcpy(Q.Tcw, Tcw7, 28); memcpy(Q.Ow, Ow3, 12); }
-    Q.logSF = logScaleFactor; Q.mode = mode; Q.gate = invLevelSigma2 ? 1 : 0;
-    Q.bestIdx = S.dev<int>(pBi); Q.bestDist = S.dev<int>(pBd);
-    CK(S.upload(st));
-    const int grid = (int)std::min<size_t>(16, (M + 127) / 128);          // every CTA rebuilds the grid: a few CTAs, ~8 map points per warp
-    fuse_search_kernel<<<grid, MF_NT, sm, st>>>(Q);
-    m.launches = 1;
-    CK(cudaGetLastError());
-    CK(S.download(st));
-    return ORB_OK;
+    const FuseJob J = {KF, invLevelSigma2, logScaleFactor, Tcw7, Ow3, cam4, pts, th, mode, bestIdx, bestDist};
+    return fuse_search_run(h->m, 1, &J);
+}
+
+int orbm_fuse_search_batch(orbm_handle* h, int nItems, const OrbmFuseItem* items) {
+    if (!h || nItems < 0 || (nItems > 0 && !items)) { set_error("orbm_fuse_search_batch: bad argument"); return ORB_ERR_ARG; }
+    std::vector<FuseJob> jobs((size_t)nItems);
+    bool any = false;
+    for (int j = 0; j < nItems; ++j) {
+        const OrbmFuseItem& it = items[j];
+        const OrbmFrame& KF = it.KF;
+        const OrbmFusePoints& P = it.pts;
+        if (KF.K < 0 || P.M < 0 || !it.invLevelSigma2 || !KF.scaleFactors || KF.nlevels < 1 || KF.nlevels > 256 || !(KF.maxX > KF.minX) || !(KF.maxY > KF.minY) ||
+            (KF.K > 0 && (!KF.keypoints || !KF.descriptors)) ||
+            (P.M > 0 && (!P.state || !P.worldPos || !P.normal || !P.minDistance || !P.maxDistance || !P.descriptors || !it.bestIdx || !it.bestDist))) {
+            set_error("orbm_fuse_search_batch: bad argument in item " + std::to_string(j)); return ORB_ERR_ARG;
+        }
+        if (KF.K > h->m.kcap) { set_error("orbm_fuse_search_batch: item " + std::to_string(j) + " has more keypoints than max_keypoints of the handle"); return ORB_ERR_CAPACITY; }
+        jobs[j] = FuseJob{&it.KF, it.invLevelSigma2, it.logScaleFactor, it.Tcw7, it.Ow, it.cam, &it.pts, it.th, 0, it.bestIdx, it.bestDist};
+        any = any || (KF.K > 0 && P.M > 0);
+    }
+    const int rc = fuse_search_run(h->m, nItems, jobs.data());
+    if (rc == ORB_OK && !any) h->m.launches = 0;
+    return rc;
 }
 
 int orbm_fuse_search(orbm_handle* h, const OrbmFrame* KF, const float* invLevelSigma2, float logScaleFactor, const float* Tcw7, const float* Ow3,
