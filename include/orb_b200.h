@@ -524,6 +524,64 @@ int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNe
  * CreateNewMapPoints call it per point): the observed descriptors of point p are rows obsStart[p] .. obsStart[p+1] of `descriptors`;
  * best[p] = row (relative to obsStart[p]) with the least median Hamming distance to the others, -1 for a point without observations. */
 int orbm_distinctive_descriptors(orbm_handle* h, int nPoints, const int32_t* obsStart, const uint8_t* descriptors, int32_t* best);
+/* LocalMapping::KeyFrameCulling() (src/LocalMapping.cc, monocular and mono-inertial: redundant_th = 0.9, Nd = 21) for several maps: one CTA
+ * per map walks the map's local keyframes in GetVectorCovisibleKeyFrames() order, as the reference's loop does, and applies every cull to the
+ * map's state (point bad flags, Observations(), culled keyframes, prev / next links, KeyFramesInMap()) before it evaluates the next keyframe.
+ * ONE upload through the handle's staging, ONE launch, ONE download; orbm_last_launch_count() is 1 (0 when no map has a local keyframe).
+ * The caller replays the result on the host in `status` order (INTEGRATION.md §2): MergePrevious, the relink and SetBadFlag.
+ *
+ * Keyframe table [nKF]: every keyframe the call can touch -- the local keyframes, every observer of their points, every prev / next neighbour.
+ * Points [nPoints]: each point once per map, with isBad() and its observations (mObservations: the observing keyframe's table index and
+ * the observing keypoint's mvKeysUn[idx].octave); Observations() is the number of observations (monocular: nObs counts one per keyframe).
+ * PRECONDITIONS: a non-bad point in slot i of keyframe k lists k exactly once among its observations, and occupies no other slot of k;
+ * `local` holds each keyframe at most once; the maps of one call share nothing (their keyframes and points are distinct objects).
+ * Scalars are read once at the call, as the reference reads them before or during its loop: abortBA is mbAbortBA at the call (Tracking
+ * may set it while the loop runs; taking it at the start is one of the reference's own interleavings, a loop that ends before the flag
+ * is set).  lastId: the mnId reached from the current keyframe by following mPrevKF at most Nd times (inertial only).
+ * ORB_ERR_ARG before any launch: an index out of range (local, slotPoint, obsKF, prevKF / nextKF), slotStart / obsStart not starting
+ * at 0 or decreasing, an octave outside [0, 256), nLocal > nKF, a negative count, or a null pointer the map needs (the inertial arrays
+ * only when `inertial` is set; the outputs always, visited included). */
+enum {
+    ORBM_KFC_NOT_VISITED = 0,    /* after the loop's break */
+    ORBM_KFC_SKIPPED = 1,        /* the map's init keyframe or isBad() */
+    ORBM_KFC_KEPT = 2,           /* not redundant */
+    ORBM_KFC_KEPT_FEW_KFS = 3,   /* inertial: KeyFramesInMap() <= Nd */
+    ORBM_KFC_KEPT_RECENT = 4,    /* inertial: mnId > current mnId - 2 (unsigned) */
+    ORBM_KFC_KEPT_NO_LINK = 5,   /* inertial: mPrevKF or mNextKF is NULL */
+    ORBM_KFC_KEPT_IMU = 6,       /* inertial: neither the time rule nor the still rule holds */
+    ORBM_KFC_CULLED = 7,         /* monocular: SetBadFlag */
+    ORBM_KFC_CULLED_TIME = 8,    /* inertial: (bInitImu && mnId < last_ID && t < 3) || t < 0.5; merge, relink, SetBadFlag */
+    ORBM_KFC_CULLED_STILL = 9,   /* inertial: !GetIniertialBA2() && |p - p_prev| < 0.02 && t < 3; merge, relink, SetBadFlag */
+    ORBM_KFC_NOT_ERASE = 10      /* SetBadFlag called on a keyframe with mbNotErase: mbToBeErased set (inertial: after the relink) */
+};
+enum { ORBM_KF_BAD = 1, ORBM_KF_INIT = 2, ORBM_KF_NOT_ERASE = 4 };
+typedef struct OrbmCullingMap {
+    int nKF;
+    const uint64_t* mnId;          /* [nKF] */
+    const uint8_t* kfFlags;        /* [nKF] ORBM_KF_*: isBad(), mnId == GetMap()->GetInitKFid(), mbNotErase */
+    const int32_t* prevKF;         /* [nKF] inertial only: mPrevKF as a table index, -1 = NULL */
+    const int32_t* nextKF;         /* [nKF] inertial only: mNextKF */
+    const double* timeStamp;       /* [nKF] inertial only: mTimeStamp */
+    const float* imuPosition;      /* [nKF][3] inertial only: GetImuPosition() */
+    int nLocal;
+    const int32_t* local;          /* [nLocal] table indices in GetVectorCovisibleKeyFrames() order */
+    const int32_t* slotStart;      /* [nLocal + 1] the non-NULL slots of GetMapPointMatches(), in slot order */
+    const int32_t* slotPoint;      /* [slotStart[nLocal]] point index */
+    const int32_t* slotOctave;     /* [slotStart[nLocal]] mvKeysUn[i].octave */
+    int nPoints;
+    const uint8_t* pointBad;       /* [nPoints] isBad() */
+    const int32_t* obsStart;       /* [nPoints + 1] */
+    const int32_t* obsKF;          /* [obsStart[nPoints]] observing keyframe (table index) */
+    const int32_t* obsOctave;      /* [obsStart[nPoints]] its mvKeysUn[idx].octave */
+    int inertial, imuInitialized, inertialBA2, abortBA;   /* mbInertial, isImuInitialized(), GetIniertialBA2(), mbAbortBA */
+    int keyFramesInMap;            /* mpAtlas->KeyFramesInMap() */
+    uint64_t currentId, lastId;    /* mpCurrentKeyFrame->mnId, last_ID */
+    uint8_t* status;               /* [nLocal] out: ORBM_KFC_* */
+    int32_t* nMPs;                 /* [nLocal] out: -1 where not evaluated */
+    int32_t* nRedundant;           /* [nLocal] out: nRedundantObservations, -1 where not evaluated */
+    int32_t* visited;              /* [1] out: the reference's `count` when the loop ended */
+} OrbmCullingMap;
+int orbm_keyframe_culling_batch(orbm_handle* h, int nMaps, const OrbmCullingMap* maps);
 
 /* cv::BFMatcher(NORM_HAMMING).knnMatch(query, train, k=2) as used at src/Frame.cc:1144: idx/dist are Q x 2,
  * ordered by (distance, lower train index); missing neighbours are -1.  Q and T are unbounded.  Host pointers. */

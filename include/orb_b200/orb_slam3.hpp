@@ -209,6 +209,12 @@ public:
         for (const OrbmFuseItem& it : items) if (it.KF.K > maxK) maxK = it.KF.K;
         orb_check(orbm_fuse_search_batch(detail::matcher_handle(maxK, 1, device_), (int)items.size(), items.data()), "orbm_fuse_search_batch");
     }
+    // void LocalMapping::KeyFrameCulling() (monocular and mono-inertial) for several maps that share nothing, in one launch
+    // (orbm_keyframe_culling_batch).  Every map's status / nMPs / nRedundant / visited receive its walk; the caller replays the culls in
+    // status order: MergePrevious, the relink and SetBadFlag (INTEGRATION.md §2).
+    void KeyFrameCullingBatch(const std::vector<OrbmCullingMap>& maps) {
+        orb_check(orbm_keyframe_culling_batch(detail::matcher_handle(1, 1, device_), (int)maps.size(), maps.data()), "orbm_keyframe_culling_batch");
+    }
     // cv::BFMatcher(NORM_HAMMING).knnMatch(query, train, matches, 2)
     void knnMatch(const Descriptors& query, const Descriptors& train, std::vector<int32_t>& idx, std::vector<int32_t>& dist) {
         idx.assign((size_t)query.rows * 2, -1); dist.assign((size_t)query.rows * 2, -1);

@@ -367,6 +367,42 @@ class _OrbmFuseItem(C.Structure):
                 ('cam', C.c_float * 4), ('th', C.c_float), ('pts', _OrbmFusePoints), ('bestIdx', C.c_void_p), ('bestDist', C.c_void_p)]
 
 
+#: OrbmCullingMap's statuses (ORBM_KFC_*, include/orb_b200.h), by code
+KFC_STATUS = ('not visited', 'skipped', 'kept', 'kept: few keyframes', 'kept: recent', 'kept: no link', 'kept: imu', 'culled', 'culled: time',
+              'culled: still', 'not erase')
+KFC_NOT_VISITED, KFC_SKIPPED, KFC_KEPT, KFC_KEPT_FEW_KFS, KFC_KEPT_RECENT, KFC_KEPT_NO_LINK, KFC_KEPT_IMU, KFC_CULLED, KFC_CULLED_TIME, \
+    KFC_CULLED_STILL, KFC_NOT_ERASE = range(11)
+KF_BAD, KF_INIT, KF_NOT_ERASE = 1, 2, 4
+#: the arrays of one map of ORBmatcher.keyframe_culling_batch, with their dtypes (OrbmCullingMap)
+CULLING_ARRAYS = (('mnId', np.uint64), ('kfFlags', np.uint8), ('prevKF', np.int32), ('nextKF', np.int32), ('timeStamp', np.float64),
+                  ('imuPosition', np.float32), ('local', np.int32), ('slotStart', np.int32), ('slotPoint', np.int32), ('slotOctave', np.int32),
+                  ('pointBad', np.uint8), ('obsStart', np.int32), ('obsKF', np.int32), ('obsOctave', np.int32))
+CULLING_SCALARS = ('inertial', 'imuInitialized', 'inertialBA2', 'abortBA', 'keyFramesInMap', 'currentId', 'lastId')
+
+
+class OrbmCullingMap(C.Structure):
+    """One map of orbm_keyframe_culling_batch (include/orb_b200.h)."""
+    _fields_ = [('nKF', C.c_int)] + [(n, C.c_void_p) for n in ('mnId', 'kfFlags', 'prevKF', 'nextKF', 'timeStamp', 'imuPosition')] + \
+               [('nLocal', C.c_int)] + [(n, C.c_void_p) for n in ('local', 'slotStart', 'slotPoint', 'slotOctave')] + \
+               [('nPoints', C.c_int)] + [(n, C.c_void_p) for n in ('pointBad', 'obsStart', 'obsKF', 'obsOctave')] + \
+               [(n, C.c_int) for n in ('inertial', 'imuInitialized', 'inertialBA2', 'abortBA', 'keyFramesInMap')] + \
+               [('currentId', C.c_uint64), ('lastId', C.c_uint64)] + [(n, C.c_void_p) for n in ('status', 'nMPs', 'nRedundant', 'visited')]
+
+
+def culling_struct(m):
+    """OrbmCullingMap over map dict `m` (keys CULLING_ARRAYS + CULLING_SCALARS) with fresh outputs: (struct, out dict, arrays to keep alive).
+    The inertial arrays may be missing when m['inertial'] is false."""
+    a = {n: (_c(m[n], dt) if m.get(n) is not None else None) for n, dt in CULLING_ARRAYS}
+    nL = len(a['local'])
+    out = dict(status=np.zeros(nL, np.uint8), nMPs=np.zeros(nL, np.int32), nRedundant=np.zeros(nL, np.int32), visited=np.zeros(1, np.int32))
+    s = OrbmCullingMap(len(a['kfFlags']), *[_ptr(a[n]) for n in ('mnId', 'kfFlags', 'prevKF', 'nextKF', 'timeStamp', 'imuPosition')],
+                       nL, *[_ptr(a[n]) for n in ('local', 'slotStart', 'slotPoint', 'slotOctave')],
+                       len(a['pointBad']), *[_ptr(a[n]) for n in ('pointBad', 'obsStart', 'obsKF', 'obsOctave')],
+                       *[int(m[n]) for n in ('inertial', 'imuInitialized', 'inertialBA2', 'abortBA', 'keyFramesInMap')], int(m['currentId']),
+                       int(m['lastId']), *[_ptr(out[n]) for n in ('status', 'nMPs', 'nRedundant', 'visited')])
+    return s, out, a
+
+
 def _c(a, dt):
     return np.ascontiguousarray(a, dt)
 
@@ -937,6 +973,21 @@ class ORBmatcher:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_create_new_map_points')
         return out[:n.value].copy(), nm, nc
+
+    def keyframe_culling_batch(self, maps):
+        """``LocalMapping::KeyFrameCulling()`` (monocular and mono-inertial) for several maps in one launch (orbm_keyframe_culling_batch).
+        Each map is a dict with the arrays of ``CULLING_ARRAYS`` (the keyframe table, the local keyframes and their slots in CSR form, the
+        points and their observations in CSR form) and the scalars of ``CULLING_SCALARS``.  Returns, per map, dict(status [nLocal] (KFC_*),
+        nMPs [nLocal], nRedundant [nLocal], visited); the caller replays the culls in ``status`` order (INTEGRATION.md §2).  The maps must
+        share nothing (see include/orb_b200.h)."""
+        built = [culling_struct(m) for m in maps]
+        arr = (OrbmCullingMap * max(len(maps), 1))(*[b[0] for b in built])
+        L = lib()
+        L.orbm_keyframe_culling_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        rc = L.orbm_keyframe_culling_batch(self._h, len(maps), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_keyframe_culling_batch')
+        return [dict(b[1], visited=int(b[1]['visited'][0])) for b in built]
 
     def ComputeDistinctiveDescriptors(self, obs_list):
         """``MapPoint::ComputeDistinctiveDescriptors`` for a list of map points (each an [n, 32] u8 array of observed descriptors): index of the chosen row."""

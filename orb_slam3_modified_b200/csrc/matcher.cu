@@ -24,6 +24,7 @@
 #include "device_utils.cuh"
 #include "exact_math.h"
 #include "frame_pose.cuh"
+#include "matcher_context.h"
 #include "pose_inertial.h"
 #include "pose_opt.h"
 #include "staging.h"
@@ -1534,6 +1535,8 @@ __global__ void __launch_bounds__(TL_NT) tlm_frustum_kernel(TrackLocalParams T) 
 using namespace orbm;
 
 struct orbm_handle { Matcher m; };
+
+MatcherContext orbm::matcher_context(orbm_handle* h) { return {&h->m.staging, h->m.stream, h->m.device, &h->m.launches}; }
 
 extern "C" {
 
