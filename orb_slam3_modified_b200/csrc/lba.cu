@@ -54,6 +54,7 @@ struct Dev {
     const int* freePose;              // nF: pose index of Hessian block
     // edges in INTERNAL order = sorted by point (the edges of a point are contiguous)
     const int *ePt, *ePose;           // nE
+    const int* eH;                    // nE: Hessian block of the edge's pose (hidx[ePose]) or -1
     const int* eOrig;                 // nE: caller's edge index
     const double* obs;                // nE x 2
     const float* invSigma2;           // nE
@@ -100,8 +101,12 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long l
 #ifndef LBA_UNR
 #define LBA_UNR 4
 #endif
+#ifndef LBA_FLY
+#define LBA_FLY 1      /* items in flight per lane in the per-edge passes (build_points, build_poses, points_trial) */
+#endif
 constexpr int NT = LBA_NT;
 constexpr int NWARP = NT / 32;
+constexpr int FLY = LBA_FLY;
 constexpr int MAXC = 8;            // largest cluster
 constexpr int PSLOT = 24;          // doubles per partial slot: A[0..7], flag[8], B[9..16]
 constexpr int PC = 20;             // doubles per cached pose: q(4) t(3) R(9) fx fy cx cy
@@ -167,14 +172,20 @@ __device__ void load_pose_cache(const Dev& D, const double* poses, double* pc) {
     __syncthreads();
 }
 
-// one edge at pose P (cached: q t R cam) and point X: residual, robust chi2 and the edge factors of this state
-__device__ __forceinline__ double edge_error(const Dev& D, const double* P, const double* X, int e, double* __restrict__ Eout) {
+// The graph's index arrays and observations are written by lba_build_structure_kernel and stay fixed for the whole LM kernel:
+// they are read through the non-coherent path, which the compiler may also issue ahead of earlier stores
+template <typename T>
+__device__ __forceinline__ T ro(const T* p) { return __ldg(p); }
+__device__ __forceinline__ double2 ro_obs(const Dev& D, int e) { return ro(reinterpret_cast<const double2*>(D.obs) + e); }
+
+// one edge at pose P (cached: q t R cam) and point X with observation ob and 1/sigma^2 is2: residual, robust chi2 and the edge
+// factors of this state
+__device__ __forceinline__ double edge_error(const Dev& D, const double* P, const double* X, int e, double2 ob, double is2, double* __restrict__ Eout) {
     double r[3]; qrot(P, X, r);                                     // SE3Quat::map: _r * xyz + _t
     const double xc = r[0] + P[4], yc = r[1] + P[5], zc = r[2] + P[6];
     const double u = P[16] * xc / zc + P[18], v = P[17] * yc / zc + P[19];      // Pinhole::project(Vector3d)
-    const double e0 = D.obs[2 * (size_t)e] - u, e1 = D.obs[2 * (size_t)e + 1] - v;
+    const double e0 = ob.x - u, e1 = ob.y - v;
     *reinterpret_cast<double2*>(D.err + 2 * (size_t)e) = make_double2(e0, e1);
-    const double is2 = (double)D.invSigma2[e];
     double r0, r1;
     huber(is2 * (e0 * e0 + e1 * e1), D.delta, D.dsqr, r0, r1);
     const double iz = 1.0 / zc;
@@ -187,7 +198,8 @@ __device__ __forceinline__ double edge_error(const Dev& D, const double* P, cons
 //      Also leaves the edge factors (x/z, y/z, 1/z, rho' / sigma^2) of this state in Eout. ----
 __device__ double phase_errors(const Dev& D, const Ctx& c, double* __restrict__ Eout) {
     double acc = 0;
-    for (int e = c.wid; e < D.nE; e += c.nw) acc += edge_error(D, c.pc + PC * D.ePose[e], c.pts + 3 * (size_t)D.ePt[e], e, Eout);
+    for (int e = c.wid; e < D.nE; e += c.nw)
+        acc += edge_error(D, c.pc + PC * ro(D.ePose + e), c.pts + 3 * (size_t)ro(D.ePt + e), e, ro_obs(D, e), (double)ro(D.invSigma2 + e), Eout);
     return acc;
 }
 
@@ -195,10 +207,11 @@ __device__ double phase_errors(const Dev& D, const Ctx& c, double* __restrict__ 
 // EdgeSE3ProjectXYZ::linearizeOplus (-projectJac * R and -projectJac * [-[Xc]x | I], Pinhole.cpp:71-81) are
 //   A = -diag(fx iz, fy iz) t,   t = [R0 - xn R2 ; R1 - yn R2]                           (2x3)
 //   B =  diag(fx, fy) b,         b = [xn yn, -(1 + xn^2), yn, -iz, 0, xn iz ; 1 + yn^2, -xn yn, -xn, 0, -iz, yn iz]   (2x6)
-// A 32-byte record as two 128-bit global loads (LDG.E.128, the widest sm_90 has)
+// A 32-byte record as two 128-bit loads (the widest sm_90 has).  Plain loads, so that the compiler may issue them ahead of
+// stores it can tell apart from them
 __device__ __forceinline__ void ld256(const double* p, double& a, double& b, double& c, double& d) {
-    asm volatile("ld.global.v2.f64 {%0, %1}, [%2];" : "=d"(a), "=d"(b) : "l"(p));
-    asm volatile("ld.global.v2.f64 {%0, %1}, [%2];" : "=d"(c), "=d"(d) : "l"(p + 2));
+    const double2 u = reinterpret_cast<const double2*>(p)[0], v = reinterpret_cast<const double2*>(p)[1];
+    a = u.x; b = u.y; c = v.x; d = v.y;
 }
 __device__ __forceinline__ void load_e4(const double* __restrict__ E, int e, double& xn, double& yn, double& iz, double& w) {
     ld256(E + 4 * (size_t)e, xn, yn, iz, w);
@@ -246,40 +259,75 @@ __device__ __forceinline__ void warp_reduce_scatter(double* v, int lane, int& lo
 }
 
 __device__ __forceinline__ void point_record(const Dev& D, int p, const double* h, const double* bl3, double lambda);
+// The per-point passes give every group of 8 lanes the points p, p + G, p + 2G, ... (G groups) and take FLY of them per step:
+// a step first issues the loads of the lane's first edge of each of its points, then adds the points one after another,
+// each with the same per-lane order (edges sl, sl + 8, ...) and the same shuffle tree as one point per step.  The next step's
+// ptStart entries are loaded ahead.
+__device__ __forceinline__ void step_ranges(const int* ptStart, int nL, int p, int G, int* a, int* b) {
+#pragma unroll
+    for (int j = 0; j < FLY; ++j) {
+        const int q = p + j * G;
+        a[j] = q < nL ? ro(ptStart + q) : 0;
+        b[j] = q < nL ? ro(ptStart + q + 1) : 0;
+    }
+}
+// operands of one edge in the build pass: its pose, factors and error
+struct BuildEdge { int pose; double xn, yn, iz, w; double2 er; };
+__device__ __forceinline__ BuildEdge load_build_edge(const Dev& D, const double* __restrict__ E, int e) {
+    BuildEdge o;
+    o.pose = ro(D.ePose + e);
+    load_e4(E, e, o.xn, o.yn, o.iz, o.w);
+    o.er = *reinterpret_cast<const double2*>(D.err + 2 * (size_t)e);
+    return o;
+}
+__device__ __forceinline__ void add_build_edge(const double* pcache, const BuildEdge& o, double* h, double* g) {
+    const double* P = pcache + PC * o.pose;
+    double t[6];
+    edge_t(P + 7, o.xn, o.yn, t);
+    const double s0 = P[16] * o.iz, s1 = P[17] * o.iz;
+    const double c0 = o.w * s0 * s0, c1 = o.w * s1 * s1;          // w A^T A = c0 t0^T t0 + c1 t1^T t1
+    const double q0 = s0 * o.w * o.er.x, q1 = s1 * o.w * o.er.y;  // A^T r, r = -w err
+    g[0] += t[0] * q0 + t[3] * q1; g[1] += t[1] * q0 + t[4] * q1; g[2] += t[2] * q0 + t[5] * q1;
+    h[0] += c0 * t[0] * t[0] + c1 * t[3] * t[3]; h[1] += c0 * t[0] * t[1] + c1 * t[3] * t[4]; h[2] += c0 * t[0] * t[2] + c1 * t[3] * t[5];
+    h[3] += c0 * t[1] * t[1] + c1 * t[4] * t[4]; h[4] += c0 * t[1] * t[2] + c1 * t[4] * t[5]; h[5] += c0 * t[2] * t[2] + c1 * t[5] * t[5];
+}
 // ---- per point Hll, bl (and, when lambda is already known, the point record of phase_point_prep); 8 lanes per point
 //      (the edges of a point are contiguous) ----
 __device__ void phase_build_points(const Dev& D, const Ctx& c, const double* __restrict__ E, double lambda) {
     const int sl = c.tid & 7;
     const unsigned gmask = 0xFFu << (c.tid & 24);
-    for (int p = c.wid >> 3; p < D.nL; p += c.nw >> 3) {
-        const int a = D.ptStart[p], b = D.ptStart[p + 1];
-        double h[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0};
-        for (int e = a + sl; e < b; e += 8) {
-            const double* P = c.pc + PC * D.ePose[e];
-            double xn, yn, iz, w, t[6];
-            load_e4(E, e, xn, yn, iz, w);
-            edge_t(P + 7, xn, yn, t);
-            const double2 er = *reinterpret_cast<const double2*>(D.err + 2 * (size_t)e);
-            const double s0 = P[16] * iz, s1 = P[17] * iz;
-            const double c0 = w * s0 * s0, c1 = w * s1 * s1;          // w A^T A = c0 t0^T t0 + c1 t1^T t1
-            const double q0 = s0 * w * er.x, q1 = s1 * w * er.y;      // A^T r, r = -w err
-            g[0] += t[0] * q0 + t[3] * q1; g[1] += t[1] * q0 + t[4] * q1; g[2] += t[2] * q0 + t[5] * q1;
-            h[0] += c0 * t[0] * t[0] + c1 * t[3] * t[3]; h[1] += c0 * t[0] * t[1] + c1 * t[3] * t[4]; h[2] += c0 * t[0] * t[2] + c1 * t[3] * t[5];
-            h[3] += c0 * t[1] * t[1] + c1 * t[4] * t[4]; h[4] += c0 * t[1] * t[2] + c1 * t[4] * t[5]; h[5] += c0 * t[2] * t[2] + c1 * t[5] * t[5];
+    const int G = c.nw >> 3;
+    int a[FLY], b[FLY];
+    step_ranges(D.ptStart, D.nL, c.wid >> 3, G, a, b);
+    for (int p0 = c.wid >> 3; p0 < D.nL; p0 += FLY * G) {
+        BuildEdge first[FLY] = {};
+#pragma unroll
+        for (int j = 0; j < FLY; ++j) if (a[j] + sl < b[j]) first[j] = load_build_edge(D, E, a[j] + sl);
+        int na[FLY], nb[FLY];
+        step_ranges(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
+#pragma unroll
+        for (int j = 0; j < FLY; ++j) {
+            const int p = p0 + j * G;
+            if (p >= D.nL) break;
+            double h[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0};
+            if (a[j] + sl < b[j]) add_build_edge(c.pc, first[j], h, g);
+            for (int e = a[j] + sl + 8; e < b[j]; e += 8) add_build_edge(c.pc, load_build_edge(D, E, e), h, g);
+#pragma unroll
+            for (int o = 4; o; o >>= 1) {
+#pragma unroll
+                for (int i = 0; i < 6; ++i) h[i] += __shfl_xor_sync(gmask, h[i], o);
+#pragma unroll
+                for (int i = 0; i < 3; ++i) g[i] += __shfl_xor_sync(gmask, g[i], o);
+            }
+            if (sl == 0) {
+                double2* H = reinterpret_cast<double2*>(D.Hll + 6 * (size_t)p);
+                H[0] = make_double2(h[0], h[1]); H[1] = make_double2(h[2], h[3]); H[2] = make_double2(h[4], h[5]);
+                D.bl[3 * (size_t)p] = g[0]; D.bl[3 * (size_t)p + 1] = g[1]; D.bl[3 * (size_t)p + 2] = g[2];
+                if (lambda >= 0) point_record(D, p, h, g, lambda);
+            }
         }
 #pragma unroll
-        for (int o = 4; o; o >>= 1) {
-#pragma unroll
-            for (int i = 0; i < 6; ++i) h[i] += __shfl_xor_sync(gmask, h[i], o);
-#pragma unroll
-            for (int i = 0; i < 3; ++i) g[i] += __shfl_xor_sync(gmask, g[i], o);
-        }
-        if (sl == 0) {
-            double2* H = reinterpret_cast<double2*>(D.Hll + 6 * (size_t)p);
-            H[0] = make_double2(h[0], h[1]); H[1] = make_double2(h[2], h[3]); H[2] = make_double2(h[4], h[5]);
-            D.bl[3 * (size_t)p] = g[0]; D.bl[3 * (size_t)p + 1] = g[1]; D.bl[3 * (size_t)p + 2] = g[2];
-            if (lambda >= 0) point_record(D, p, h, g, lambda);
-        }
+        for (int j = 0; j < FLY; ++j) { a[j] = na[j]; b[j] = nb[j]; }
     }
 }
 
@@ -290,7 +338,9 @@ constexpr int UNR = LBA_UNR;       // items in flight per lane in the Schur chun
 // ---- per free pose Hpp, bp.  partial: warp per chunk of the pose's edges (the chunks of the diagonal Schur tasks), lane per
 //      edge, 21 + 6 sums reduce-scattered to Spart; combine: thread per (pose, entry), chunks added in order.
 //      The chunks cover every pose-major index once, so the partial step also writes the pose-major copy K of the factors
-//      that the Schur phase reads (coalesced stores; the factors stay fixed for all trials of an iteration) ----
+//      that the Schur phase reads (coalesced stores; the factors stay fixed for all trials of an iteration).
+//      As in the Schur chunks, the chunk's edge ids are loaded into registers up front; then the factors and errors of FLY
+//      items per lane are loaded before their K stores and their sums, which keep the item order of the lane. ----
 __device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const double* __restrict__ E) {
     const int lane = c.tid & 31;
     const int nDiag = D.taskChunkStart[D.nF];
@@ -298,27 +348,48 @@ __device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const doub
         const int4 h = D.chunkHdr[ch];
         const double* P = c.pc + PC * h.z;
         const double fx = P[16], fy = P[17];
+        int re[IPL];
+#pragma unroll
+        for (int j = 0; j < IPL; ++j) { const int i = lane + 32 * j; re[j] = i < h.y ? ro(D.poseEdges + h.x + i) : 0; }
         double acc[27];
 #pragma unroll
         for (int i = 0; i < 27; ++i) acc[i] = 0;
-        for (int i = lane; i < h.y; i += 32) {
-            const int k = h.x + i, e = D.poseEdges[k];
-            double xn, yn, iz, w, b0[6], b1[6];
-            load_e4(E, e, xn, yn, iz, w);
-            D.K[k] = make_double2(xn, yn); D.K[D.nE + k] = make_double2(iz, w);
-            edge_b(xn, yn, iz, b0, b1);
-            const double2 er = *reinterpret_cast<const double2*>(D.err + 2 * (size_t)e);
-            const double c0 = w * fx * fx, c1 = w * fy * fy;          // w B^T B = c0 b0^T b0 + c1 b1^T b1
-            const double q0 = fx * w * er.x, q1 = fy * w * er.y;      // B^T r = -(b0 q0 + b1 q1)
-            int t = 0;
 #pragma unroll
-            for (int a = 0; a < 6; ++a) {
-                const double u0 = c0 * b0[a], u1 = c1 * b1[a];
+        for (int j0 = 0; j0 < IPL; j0 += FLY) {
+            double f[FLY][4] = {}; double2 er[FLY] = {};
 #pragma unroll
-                for (int j = a; j < 6; ++j) acc[t++] += u0 * b0[j] + u1 * b1[j];
+            for (int u = 0; u < FLY; ++u) {
+                const int j = j0 + u;
+                if (j < IPL && lane + 32 * j < h.y) {
+                    load_e4(E, re[j], f[u][0], f[u][1], f[u][2], f[u][3]);
+                    er[u] = *reinterpret_cast<const double2*>(D.err + 2 * (size_t)re[j]);
+                }
             }
 #pragma unroll
-            for (int a = 0; a < 6; ++a) acc[21 + a] -= b0[a] * q0 + b1[a] * q1;
+            for (int u = 0; u < FLY; ++u) {
+                const int j = j0 + u, k = h.x + lane + 32 * j;
+                if (j < IPL && lane + 32 * j < h.y) { D.K[k] = make_double2(f[u][0], f[u][1]); D.K[D.nE + k] = make_double2(f[u][2], f[u][3]); }
+            }
+#pragma unroll
+            for (int u = 0; u < FLY; ++u) {
+                const int j = j0 + u;
+                if (j < IPL && lane + 32 * j < h.y) {
+                    const double xn = f[u][0], yn = f[u][1], iz = f[u][2], w = f[u][3];
+                    double b0[6], b1[6];
+                    edge_b(xn, yn, iz, b0, b1);
+                    const double c0 = w * fx * fx, c1 = w * fy * fy;          // w B^T B = c0 b0^T b0 + c1 b1^T b1
+                    const double q0 = fx * w * er[u].x, q1 = fy * w * er[u].y;  // B^T r = -(b0 q0 + b1 q1)
+                    int t = 0;
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) {
+                        const double u0 = c0 * b0[a], u1 = c1 * b1[a];
+#pragma unroll
+                        for (int i = a; i < 6; ++i) acc[t++] += u0 * b0[i] + u1 * b1[i];
+                    }
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) acc[21 + a] -= b0[a] * q0 + b1[a] * q1;
+                }
+            }
         }
         int lo, n;
         warp_reduce_scatter<27>(acc, lane, lo, n);
@@ -703,51 +774,93 @@ __device__ double phase_pose_trial(const Dev& D, const Ctx& c, const double* __r
 // ---- part 2, 8 lanes per point, one pass: landmark back-substitution x_l = Hll^-1 (bl - W^T x_p)
 //      (block_solver.hpp:461-483; W^T x_p = w A^T (B x_p) = -sum_k t_k g_k (b_k . x_p)), the point update into the trial
 //      buffer, its share of computeScale, and the residuals / robust chi2 / edge factors of the point's edges at the
-//      trial state (computeActiveErrors + activeRobustChi2).  Returns (scale share, chi2 share). ----
+//      trial state (computeActiveErrors + activeRobustChi2).  Returns (scale share, chi2 share).
+//      FLY points per step (see phase_build_points): the loads of the lane's first edge of each point (the edge's Hessian block
+//      eH, factors, observation) and the point's Dinv, bl and estimate are issued at the top of the step, then the pose
+//      increments x_p those edges need; the sums keep the per-lane edge order and the point order of one point per step. ----
+struct TrialEdge { int pose, h; double xn, yn, iz, w; double2 ob; double is2; };
+__device__ __forceinline__ TrialEdge load_trial_edge(const Dev& D, const double* __restrict__ E, int e) {
+    TrialEdge o;
+    o.pose = ro(D.ePose + e); o.h = ro(D.eH + e);
+    load_e4(E, e, o.xn, o.yn, o.iz, o.w);
+    o.ob = ro_obs(D, e); o.is2 = (double)ro(D.invSigma2 + e);
+    return o;
+}
+// the edge's share of W^T x_p, added into cl
+__device__ __forceinline__ void add_backsub_edge(const double* pcache, const TrialEdge& o, const double* xp, double* cl) {
+    const double* P = pcache + PC * o.pose;
+    double t[6], b0[6], b1[6];
+    edge_t(P + 7, o.xn, o.yn, t);
+    edge_b(o.xn, o.yn, o.iz, b0, b1);
+    double be0 = 0, be1 = 0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) { const double xa = xp[k]; be0 += b0[k] * xa; be1 += b1[k] * xa; }
+    const double q = o.iz * o.w;
+    be0 *= P[16] * P[16] * q; be1 *= P[17] * P[17] * q;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) cl[k] += t[k] * be0 + t[3 + k] * be1;
+}
 __device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* __restrict__ E, double* __restrict__ Eout, double* __restrict__ Xtr,
                                       const double* pcTr, double lambda) {
     const int sl = c.tid & 7;
     const unsigned gmask = 0xFFu << (c.tid & 24);
+    const int G = c.nw >> 3;
     double accS = 0, accC = 0;
-    for (int p = c.wid >> 3; p < D.nL; p += c.nw >> 3) {
-        const int a = D.ptStart[p], b = D.ptStart[p + 1];
-        double cl[3] = {0, 0, 0};
-        for (int e = a + sl; e < b; e += 8) {
-            const int ic = D.ePose[e];
-            const int h = D.hidx[ic];
-            if (h < 0) continue;
-            const double* P = c.pc + PC * ic;
-            double xn, yn, iz, w, t[6], b0[6], b1[6];
-            load_e4(E, e, xn, yn, iz, w);
-            edge_t(P + 7, xn, yn, t);
-            edge_b(xn, yn, iz, b0, b1);
-            const double* xp = D.x + 6 * (size_t)h;
-            double be0 = 0, be1 = 0;
+    int a[FLY], b[FLY];
+    step_ranges(D.ptStart, D.nL, c.wid >> 3, G, a, b);
+    for (int p0 = c.wid >> 3; p0 < D.nL; p0 += FLY * G) {
+        TrialEdge first[FLY] = {};
+        double Di[FLY][6] = {}, bl[FLY][3] = {}, X0[FLY][3] = {}, xp[FLY][6] = {};     // Di: 00 01 02 11 12 22
 #pragma unroll
-            for (int k = 0; k < 6; ++k) { const double xa = xp[k]; be0 += b0[k] * xa; be1 += b1[k] * xa; }
-            const double q = iz * w;
-            be0 *= P[16] * P[16] * q; be1 *= P[17] * P[17] * q;
+        for (int j = 0; j < FLY; ++j) if (a[j] + sl < b[j]) first[j] = load_trial_edge(D, E, a[j] + sl);
 #pragma unroll
-            for (int k = 0; k < 3; ++k) cl[k] += t[k] * be0 + t[3 + k] * be1;
+        for (int j = 0; j < FLY; ++j) {
+            const int p = p0 + j * G;
+            if (p < D.nL) {
+                load_dinv(D.PT, D.nL, p, Di[j]);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { bl[j][k] = D.bl[3 * (size_t)p + k]; X0[j][k] = c.pts[3 * (size_t)p + k]; }
+            }
         }
 #pragma unroll
-        for (int o = 4; o; o >>= 1) {
+        for (int j = 0; j < FLY; ++j)
+            if (a[j] + sl < b[j] && first[j].h >= 0) {
 #pragma unroll
-            for (int i = 0; i < 3; ++i) cl[i] += __shfl_xor_sync(gmask, cl[i], o);
+                for (int k = 0; k < 6; ++k) xp[j][k] = D.x[6 * (size_t)first[j].h + k];
+            }
+        int na[FLY], nb[FLY];
+        step_ranges(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
+#pragma unroll
+        for (int j = 0; j < FLY; ++j) {
+            const int p = p0 + j * G;
+            if (p >= D.nL) break;
+            const bool has = a[j] + sl < b[j];
+            double cl[3] = {0, 0, 0};
+            if (has && first[j].h >= 0) add_backsub_edge(c.pc, first[j], xp[j], cl);
+            for (int e = a[j] + sl + 8; e < b[j]; e += 8) {
+                const TrialEdge o = load_trial_edge(D, E, e);
+                if (o.h >= 0) add_backsub_edge(c.pc, o, D.x + 6 * (size_t)o.h, cl);
+            }
+#pragma unroll
+            for (int o = 4; o; o >>= 1) {
+#pragma unroll
+                for (int i = 0; i < 3; ++i) cl[i] += __shfl_xor_sync(gmask, cl[i], o);
+            }
+            const double* dv = Di[j];
+            const double bl0 = bl[j][0], bl1 = bl[j][1], bl2 = bl[j][2];
+            const double c0 = cl[0] + bl0, c1 = cl[1] + bl1, c2 = cl[2] + bl2;
+            const double u0 = dv[0] * c0 + dv[1] * c1 + dv[2] * c2, u1 = dv[1] * c0 + dv[3] * c1 + dv[4] * c2, u2 = dv[2] * c0 + dv[4] * c1 + dv[5] * c2;
+            double X[3] = {X0[j][0] + u0, X0[j][1] + u1, X0[j][2] + u2};
+            if (sl == 0) {
+                Xtr[3 * (size_t)p] = X[0]; Xtr[3 * (size_t)p + 1] = X[1]; Xtr[3 * (size_t)p + 2] = X[2];
+                accS += u0 * (lambda * u0 + bl0) + u1 * (lambda * u1 + bl1) + u2 * (lambda * u2 + bl2);
+            }
+            if (has) accC += edge_error(D, pcTr + PC * first[j].pose, X, a[j] + sl, first[j].ob, first[j].is2, Eout);
+            for (int e = a[j] + sl + 8; e < b[j]; e += 8)
+                accC += edge_error(D, pcTr + PC * ro(D.ePose + e), X, e, ro_obs(D, e), (double)ro(D.invSigma2 + e), Eout);
         }
-        double Di[6];      // 00 01 02 11 12 22
-        load_dinv(D.PT, D.nL, p, Di);
-        const double* b3 = D.bl + 3 * (size_t)p;
-        const double bl0 = b3[0], bl1 = b3[1], bl2 = b3[2];
-        const double c0 = cl[0] + bl0, c1 = cl[1] + bl1, c2 = cl[2] + bl2;
-        const double u0 = Di[0] * c0 + Di[1] * c1 + Di[2] * c2, u1 = Di[1] * c0 + Di[3] * c1 + Di[4] * c2, u2 = Di[2] * c0 + Di[4] * c1 + Di[5] * c2;
-        const double* X0 = c.pts + 3 * (size_t)p;
-        double X[3] = {X0[0] + u0, X0[1] + u1, X0[2] + u2};
-        if (sl == 0) {
-            Xtr[3 * (size_t)p] = X[0]; Xtr[3 * (size_t)p + 1] = X[1]; Xtr[3 * (size_t)p + 2] = X[2];
-            accS += u0 * (lambda * u0 + bl0) + u1 * (lambda * u1 + bl1) + u2 * (lambda * u2 + bl2);
-        }
-        for (int e = a + sl; e < b; e += 8) accC += edge_error(D, pcTr + PC * D.ePose[e], X, e, Eout);
+#pragma unroll
+        for (int j = 0; j < FLY; ++j) { a[j] = na[j]; b[j] = nb[j]; }
     }
     return make_double2(accS, accC);
 }
@@ -932,7 +1045,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     __shared__ int s_sm[32];
     __shared__ int s_err;
     int* ptStart = const_cast<int*>(D.ptStart);
-    int* ePt = const_cast<int*>(D.ePt); int* ePose = const_cast<int*>(D.ePose); int* eOrig = const_cast<int*>(D.eOrig);
+    int* ePt = const_cast<int*>(D.ePt); int* ePose = const_cast<int*>(D.ePose); int* eH = const_cast<int*>(D.eH); int* eOrig = const_cast<int*>(D.eOrig);
     double* obs = const_cast<double*>(D.obs); float* is2 = const_cast<float*>(D.invSigma2);
     int* poseEdges = const_cast<int*>(D.poseEdges); int* poseEdgePt = const_cast<int*>(D.poseEdgePt);
     int2* pairs = const_cast<int2*>(D.pairs); int* pairPt = const_cast<int*>(D.pairPt);
@@ -983,6 +1096,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
             obs[2 * (size_t)k] = D.rawObs[2 * (size_t)e]; obs[2 * (size_t)k + 1] = D.rawObs[2 * (size_t)e + 1];
             is2[k] = D.rawInvSigma2[e];
             const int h = D.hidx[c];
+            eH[k] = h;
             if (h >= 0 && atomicCAS(&D.bEid[(size_t)h * nL + p], -1, k) != -1) s_err = 2;
         }
     __syncthreads();
@@ -1116,7 +1230,7 @@ struct Solver {
         size_t b = outBlock(nP, nL, nE);                                          // poses, pts, chi2, depth flags, stats (downloaded in one copy)
         b += al(56 * nP) + al(24 * nL) + al(16 * nP) + 2 * al(4 * nP);            // uploaded: initial estimates, cam, hidx, freePose
         b += 2 * al(4 * nE) + al(16 * nE) + al(4 * nE);                           // uploaded: the caller's edges (point, pose, obs, invSigma2)
-        b += 3 * al(4 * nE) + al(16 * nE) + al(4 * nE) + al(4 * (nL + 1));        // edges sorted by point: ePt, ePose, eOrig, obs, invSigma2; ptStart
+        b += 4 * al(4 * nE) + al(16 * nE) + al(4 * nE) + al(4 * (nL + 1));        // edges sorted by point: ePt, ePose, eH, eOrig, obs, invSigma2; ptStart
         b += 2 * al(4 * nE) + al(8 * pc) + al(4 * pc);                            // poseEdges, poseEdgePt, pairs, pairPt
         b += al(16 * cc) + al(4 * (tasks + 1));                                   // chunk headers, task chunk starts
         b += 2 * al(4 * (nL + 1)) + al(4 * nE) + al(4 * nP * nL) + 2 * al(4 * tasks);   // structure-build scratch
@@ -1195,7 +1309,8 @@ struct Solver {
         o = carve(4 * (size_t)nE); put(o, P->invSigma2, 4 * (size_t)nE); D.rawInvSigma2 = (const float*)(d_arena + o);
         uploadOff[slot] = upBase; uploadBytes[slot] = off - upBase;
         // --- derived on the device ---
-        D.ePt = (const int*)(d_arena + carve(4 * (size_t)nE)); D.ePose = (const int*)(d_arena + carve(4 * (size_t)nE)); D.eOrig = (const int*)(d_arena + carve(4 * (size_t)nE));
+        D.ePt = (const int*)(d_arena + carve(4 * (size_t)nE)); D.ePose = (const int*)(d_arena + carve(4 * (size_t)nE));
+        D.eH = (const int*)(d_arena + carve(4 * (size_t)nE)); D.eOrig = (const int*)(d_arena + carve(4 * (size_t)nE));
         D.obs = (const double*)(d_arena + carve(16 * (size_t)nE)); D.invSigma2 = (const float*)(d_arena + carve(4 * (size_t)nE));
         D.ptStart = (const int*)(d_arena + carve(4 * (size_t)(nL + 1)));
         D.poseEdges = (const int*)(d_arena + carve(4 * (size_t)nE)); D.poseEdgePt = (const int*)(d_arena + carve(4 * (size_t)nE));

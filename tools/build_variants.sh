@@ -15,8 +15,9 @@ done
 wait
 for spec in "$@"; do
   name=${spec%%:*}; rest=${spec#*:}; unit=${rest%%:*}; defs=${rest#*:}
+  others=$(for f in orb_slam3_modified_b200/csrc/*.cu; do b=$(basename $f .cu); [ "$b" != "$unit" ] && echo build/obj/$b.o; done)
   ( nvcc $FLAGS $defs -c orb_slam3_modified_b200/csrc/$unit.cu -o build/obj/${unit}_$name.o
-    nvcc -shared -o build/liborb_$name.so build/obj/${unit}_$name.o $(ls build/obj/*.o | grep -v "_[^/]*\.o$" | grep -v "/$unit\.o$") -lcudart ) &
+    nvcc -shared -o build/liborb_$name.so build/obj/${unit}_$name.o $others -lcudart ) &
 done
 wait
 ls -la build/*.so
