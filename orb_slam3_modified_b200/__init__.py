@@ -407,6 +407,19 @@ def _c(a, dt):
     return np.ascontiguousarray(a, dt)
 
 
+def _host_call(d, dtypes, name, resident, frame_keys):
+    """(pointer getter, C function) of a batched call's host form.  The getter gives the address of ``d[k]`` made contiguous as
+    ``dtypes[k]`` (None for a missing key) and holds those arrays, so keep it until the call returns.  With ``resident``, device
+    pointers of the current frame in the order of ``frame_keys``, it gives those for the frame and the function is the _resident form."""
+    keep = {k: _c(d[k], dt) for k, dt in dtypes.items() if d.get(k) is not None}
+    if resident is not None:
+        keep.update(zip(frame_keys, resident))
+
+    def get(k):
+        return (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None
+    return get, getattr(lib(), name + '_resident' if resident is not None else name)
+
+
 class Frame:
     """The slice of ``ORB_SLAM3::Frame`` the matchers read: mvKeysUn, mDescriptors, image bounds, mvScaleFactors,
     and the in/out ``mvpMapPoints`` state as (match index, claimed flag) per keypoint."""
@@ -633,17 +646,14 @@ class ORBmatcher:
         Returns dict(claimed, outlier [B,kcap] u8, visible, found [B,mcap] i32, nToMatch, nmatches, nInliers, nMatchesInliers [B] i32,
         pose7 [B,7] f64, Tcw7 [B,7] f32); rows of inactive streams are zero."""
         B, K, M = d['batch'], d['kcap'], d['mcap']
-        keep = {k: _c(d[k], dt) for k, dt in self._LOCAL_MAP_DT.items() if d.get(k) is not None}
-        if resident is not None:
-            assert resident[3] == K
-            keep.update(kps=resident[0], desc=resident[1], nK=resident[2])
-        s = self._local_map_struct(d, lambda k: (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None)
+        assert resident is None or resident[3] == K
+        get, fn = _host_call(d, self._LOCAL_MAP_DT, 'orbm_track_local_map_batch', resident, ('kps', 'desc', 'nK'))
+        s = self._local_map_struct(d, get)
         assert match.dtype == np.int32 and match.flags.c_contiguous and match.shape == (B, K)
         out = dict(match=match, claimed=np.zeros((B, K), np.uint8), outlier=np.zeros((B, K), np.uint8), visible=np.zeros((B, M), np.int32),
                    found=np.zeros((B, M), np.int32), nToMatch=np.zeros(B, np.int32), nmatches=np.zeros(B, np.int32), nInliers=np.zeros(B, np.int32),
                    nMatchesInliers=np.zeros(B, np.int32), pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32))
         r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
-        fn = lib().orbm_track_local_map_batch_resident if resident is not None else lib().orbm_track_local_map_batch
         fn.argtypes = [C.c_void_p] * 3
         rc = fn(self._h, C.byref(s), C.byref(r))
         if rc != ORB_OK:
@@ -682,11 +692,9 @@ class ORBmatcher:
         visible, found [B, mcap], nToMatch, nmatches, nInliers, nMatchesInliers [B], Tcw7 [B, 7], predState21 [B, 21], predTcw7 [B, 7],
         state21 [B, 21], prior21 [B, 21], priorH [B, 15, 15]); rows of mode-0 streams keep their initial values (match -1, the rest 0)."""
         B, K, M = d['batch'], d['kcap'], d['mcap']
-        keep = {k: _c(d[k], dt) for k, dt in self._LOCAL_MAP_DT.items() if d.get(k) is not None}
-        if resident is not None:
-            assert resident[3] == K
-            keep.update(kps=resident[0], desc=resident[1], nK=resident[2])
-        s = self._local_map_struct(d, lambda k: (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None)
+        assert resident is None or resident[3] == K
+        get, fn = _host_call(d, self._LOCAL_MAP_DT, 'orbm_track_local_map_inertial_batch', resident, ('kps', 'desc', 'nK'))
+        s = self._local_map_struct(d, get)
         ik = {k: _c(imu[k], dt) for k, dt in dict(self._IMU_DT, extrinsics24=np.float64).items() if imu.get(k) is not None}
         mode = _c(imu['mode'], np.uint8)
         si = self._imu_struct(imu, mode, lambda k: ik[k].ctypes.data if k in ik else None)
@@ -697,7 +705,6 @@ class ORBmatcher:
                   prior21=np.zeros((B, 21)), priorH=np.zeros((B, 15, 15)))
         r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
         ri = _OrbmImuTrackResult(*[_ptr(io[k]) for k in _IMU_TRACK_OUT])
-        fn = lib().orbm_track_local_map_inertial_batch_resident if resident is not None else lib().orbm_track_local_map_inertial_batch
         fn.argtypes = [C.c_void_p] * 5
         rc = fn(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri))
         if rc != ORB_OK:
@@ -741,14 +748,11 @@ class ORBmatcher:
         Returns dict(nmatches [B], match [B, kcap] i32, pose7 [B, 7] f64, Tcw7 [B, 7] f32, discarded [B, mcap] u8, nmatchesMap [B] i32);
         rows the call does not write keep their initial values (match -1, the rest 0)."""
         B, K, M = d['batch'], d['kcap'], d['mcap']
-        keep = {k: _c(d[k], dt) for k, dt in self._REF_KF_DT.items() if d.get(k) is not None}
-        if resident is not None:
-            keep.update(zip(_REF_KF_FRAME, resident))
-        s = self._ref_kf_struct(d, lambda k: (keep[k] if isinstance(keep[k], int) else keep[k].ctypes.data) if k in keep else None)
+        get, fn = _host_call(d, self._REF_KF_DT, 'orbm_track_reference_keyframe_batch', resident, _REF_KF_FRAME)
+        s = self._ref_kf_struct(d, get)
         out = dict(nmatches=np.zeros(B, np.int32), match=np.full((B, K), -1, np.int32), pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32),
                    discarded=np.zeros((B, M), np.uint8), nmatchesMap=np.zeros(B, np.int32))
         r = _OrbmRefKeyFrameResult(*[_ptr(out[k]) for k in _REF_KF_OUT])
-        fn = lib().orbm_track_reference_keyframe_batch_resident if resident is not None else lib().orbm_track_reference_keyframe_batch
         fn.argtypes = [C.c_void_p] * 3
         rc = fn(self._h, C.byref(s), C.byref(r))
         if rc != ORB_OK:

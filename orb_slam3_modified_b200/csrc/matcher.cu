@@ -18,6 +18,7 @@
 #include <math.h>
 #include <string.h>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/orb_b200.h"
@@ -1538,6 +1539,39 @@ struct orbm_handle { Matcher m; };
 
 MatcherContext orbm::matcher_context(orbm_handle* h) { return {&h->m.staging, h->m.stream, h->m.device, &h->m.launches}; }
 
+// ---- the host forms of the batched tracking calls (below): what they share about the current frame ----
+// One stream's current frame: nK in [0, kcap] and every keypoint octave in [0, nlevels).
+template <class Batch> static bool stream_frame_ok(const Batch* in, size_t b, const char* who) {
+    const int n = in->nK[b];
+    if (n < 0 || n > in->kcap) { set_error(std::string(who) + ": nK out of range"); return false; }
+    for (int i = 0; i < n; ++i) {
+        const int oct = in->kps[b * in->kcap + i].octave;
+        if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return false; }
+    }
+    return true;
+}
+
+// The current frame's pieces: kps, desc and nK, and for TrackReferenceKeyFrame its FeatureVector (fvNode, fvFeature, nEntries).  A
+// _resident call reads the frame from device slabs, so its pieces are neither staged nor rebound.
+template <class Batch> class BatchFrame {
+    static constexpr bool FV = std::is_same<Batch, OrbmRefKeyFrameBatch>::value;
+    bool staged;
+    int kps = 0, desc = 0, nK = 0, fvNode = 0, fvFeature = 0, nEntries = 0;
+public:
+    BatchFrame(Staging& S, const Batch* in, bool frameOnDevice) : staged(!frameOnDevice) {
+        if (!staged) return;
+        const size_t B = in->batch, K = in->kcap;
+        kps = S.in(in->kps, 28 * B * K); desc = S.in(in->desc, 32 * B * K); nK = S.in(in->nK, 4 * B);
+        if constexpr (FV) { fvNode = S.in(in->fvNode, 4 * B * K); fvFeature = S.in(in->fvFeature, 4 * B * K); nEntries = S.in(in->nEntries, 4 * B); }
+    }
+    // Points the device copy `d` of the batch at the staged pieces.  The staging is reserved.
+    void bind(const Staging& S, Batch& d) const {
+        if (!staged) return;
+        d.kps = S.dev<OrbKeyPoint>(kps); d.desc = S.dev(desc); d.nK = S.dev<int>(nK);
+        if constexpr (FV) { d.fvNode = S.dev<int>(fvNode); d.fvFeature = S.dev<int>(fvFeature); d.nEntries = S.dev<int>(nEntries); }
+    }
+};
+
 extern "C" {
 
 int orbm_create(orbm_handle** out, int max_batch, int max_keypoints, int max_mappoints, int device) {
@@ -2208,13 +2242,23 @@ static int motion_model_pose_launch(Matcher& m, const OrbmBatchDevice* in, const
     return ORB_OK;
 }
 
+// Argument checks shared by both forms of the motion-model step.
+static int motion_model_shape(const orbm_handle* h, const OrbmBatchDevice* in, const float* invLevelSigma2, const int32_t* match,
+                              const uint8_t* claimed, const int32_t* nmatches, const double* pose7, const float* Tcw7, const uint8_t* discarded,
+                              const int32_t* nmatchesMap, const char* who) {
+    if (!h || !in || !batch_shape_ok(h->m, in->batch, in->kcap, in->mcap, in->nlevels) || !in->kps || !in->nK || !in->xyz || !in->hasObs ||
+        !in->Tcw7 || !invLevelSigma2 || !match || !claimed || !nmatches || !pose7 || !Tcw7 || !discarded || !nmatchesMap) {
+        set_error(std::string(who) + ": bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
+    }
+    return ORB_OK;
+}
+
 int orbm_motion_model_pose_batch_device(orbm_handle* h, const OrbmBatchDevice* in, const float* d_invLevelSigma2, const uint8_t* d_active,
                                         int32_t* d_match, uint8_t* d_claimed, int32_t* d_nmatches, double* d_pose7, float* d_Tcw7,
                                         uint8_t* d_discarded, int32_t* d_nmatchesMap, void* stream) {
-    if (!h || !in || !batch_shape_ok(h->m, in->batch, in->kcap, in->mcap, in->nlevels) || !in->kps || !in->nK || !in->xyz || !in->hasObs ||
-        !in->Tcw7 || !d_invLevelSigma2 || !d_match || !d_claimed || !d_nmatches || !d_pose7 || !d_Tcw7 || !d_discarded || !d_nmatchesMap) {
-        set_error("orbm_motion_model_pose_batch_device: bad argument (sizes or null slabs)"); return ORB_ERR_ARG;
-    }
+    if (int rc = motion_model_shape(h, in, d_invLevelSigma2, d_match, d_claimed, d_nmatches, d_pose7, d_Tcw7, d_discarded, d_nmatchesMap,
+                                    "orbm_motion_model_pose_batch_device"))
+        return rc;
     CK(cudaSetDevice(h->m.device));
     return motion_model_pose_launch(h->m, in, d_invLevelSigma2, d_active, d_match, d_claimed, d_nmatches, d_pose7, d_Tcw7, d_discarded,
                                     d_nmatchesMap, (cudaStream_t)stream);
@@ -2230,20 +2274,15 @@ static void copy_active_rows(const Staging& S, int piece, void* dst, size_t rowB
 
 int orbm_motion_model_pose_batch(orbm_handle* h, const OrbmBatchDevice* in, const float* invLevelSigma2, const uint8_t* active, int32_t* match,
                                  uint8_t* claimed, int32_t* nmatches, double* pose7, float* Tcw7, uint8_t* discarded, int32_t* nmatchesMap) {
-    if (!h || !in || !batch_shape_ok(h->m, in->batch, in->kcap, in->mcap, in->nlevels) || !in->kps || !in->nK || !in->xyz || !in->hasObs ||
-        !in->Tcw7 || !invLevelSigma2 || !match || !claimed || !nmatches || !pose7 || !Tcw7 || !discarded || !nmatchesMap) {
-        set_error("orbm_motion_model_pose_batch: bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
-    }
+    const char* who = "orbm_motion_model_pose_batch";
+    if (int rc = motion_model_shape(h, in, invLevelSigma2, match, claimed, nmatches, pose7, Tcw7, discarded, nmatchesMap, who)) return rc;
     Matcher& m = h->m;
     const size_t B = in->batch, K = in->kcap, M = in->mcap;
     for (size_t b = 0; b < B; ++b) {
         if (active && !active[b]) continue;
-        if (in->nK[b] < 0 || in->nK[b] > in->kcap) { set_error("orbm_motion_model_pose_batch: nK out of range"); return ORB_ERR_ARG; }
-        for (int i = 0; i < in->nK[b]; ++i) {
-            const int oct = in->kps[b * K + i].octave, mt = match[b * K + i];
-            if (oct < 0 || oct >= in->nlevels) { set_error("orbm_motion_model_pose_batch: keypoint octave out of range"); return ORB_ERR_ARG; }
-            if (mt < -1 || mt >= in->mcap) { set_error("orbm_motion_model_pose_batch: match index out of range"); return ORB_ERR_ARG; }
-        }
+        if (!stream_frame_ok(in, b, who)) return ORB_ERR_ARG;
+        for (int i = 0; i < in->nK[b]; ++i)
+            if (match[b * K + i] < -1 || match[b * K + i] >= in->mcap) { set_error(std::string(who) + ": match index out of range"); return ORB_ERR_ARG; }
     }
     CK(cudaSetDevice(m.device));
     Staging& S = m.staging;
@@ -2334,22 +2373,16 @@ static int ref_kf_host(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const Orb
         if (nKF < 0 || nKF > in->mcap || eKF < 0 || eKF > nKF) { set_error(std::string(who) + ": keyframe N or nEntries out of range"); return ORB_ERR_ARG; }
         if (!fv_ok(in->kfFvNode + b * M, in->kfFvFeature + b * M, eKF, nKF)) { set_error(std::string(who) + ": keyframe feature vector not sorted / out of range"); return ORB_ERR_ARG; }
         if (frameOnDevice) continue;
+        if (!stream_frame_ok(in, b, who)) return ORB_ERR_ARG;
         const int nF = in->nK[b], eF = in->nEntries[b];
-        if (nF < 0 || nF > in->kcap || eF < 0 || eF > nF) { set_error(std::string(who) + ": frame N or nEntries out of range"); return ORB_ERR_ARG; }
+        if (eF < 0 || eF > nF) { set_error(std::string(who) + ": frame nEntries out of range"); return ORB_ERR_ARG; }
         if (!fv_ok(in->fvNode + b * K, in->fvFeature + b * K, eF, nF)) { set_error(std::string(who) + ": frame feature vector not sorted / out of range"); return ORB_ERR_ARG; }
-        for (int i = 0; i < nF; ++i) {
-            const int oct = in->kps[b * K + i].octave;
-            if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return ORB_ERR_ARG; }
-        }
     }
     CK(cudaSetDevice(m.device));
     Staging& S = m.staging;
     S.begin();
-    const size_t FK = frameOnDevice ? 0 : K, FB = frameOnDevice ? 0 : B;
-    const int pKps = S.in(frameOnDevice ? nullptr : in->kps, 28 * FB * FK), pDesc = S.in(frameOnDevice ? nullptr : in->desc, 32 * FB * FK),
-              pNK = S.in(frameOnDevice ? nullptr : in->nK, 4 * FB), pNode = S.in(frameOnDevice ? nullptr : in->fvNode, 4 * FB * FK),
-              pFeat = S.in(frameOnDevice ? nullptr : in->fvFeature, 4 * FB * FK), pNE = S.in(frameOnDevice ? nullptr : in->nEntries, 4 * FB),
-              pT = S.in(in->Tcw7, 28 * B), pKfN = S.in(in->kfN, 4 * B), pKfKps = S.in(in->kfKps, 28 * B * M), pKfDesc = S.in(in->kfDesc, 32 * B * M),
+    const BatchFrame<OrbmRefKeyFrameBatch> frame(S, in, frameOnDevice);
+    const int pT = S.in(in->Tcw7, 28 * B), pKfN = S.in(in->kfN, 4 * B), pKfKps = S.in(in->kfKps, 28 * B * M), pKfDesc = S.in(in->kfDesc, 32 * B * M),
               pKfNode = S.in(in->kfFvNode, 4 * B * M), pKfFeat = S.in(in->kfFvFeature, 4 * B * M), pKfNE = S.in(in->kfNEntries, 4 * B),
               pPt = S.in(in->kfPoint, B * M), pXyz = S.in(in->xyz, 12 * B * M), pObs = S.in(in->hasObs, B * M),
               pIs = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels), pAct = S.in(active, active ? B : 0),
@@ -2358,10 +2391,7 @@ static int ref_kf_host(orbm_handle* h, const OrbmRefKeyFrameBatch* in, const Orb
     int rc = S.reserve();
     if (rc) return rc;
     OrbmRefKeyFrameBatch d = *in;
-    if (!frameOnDevice) {
-        d.kps = S.dev<OrbKeyPoint>(pKps); d.desc = S.dev(pDesc); d.nK = S.dev<int>(pNK);
-        d.fvNode = S.dev<int>(pNode); d.fvFeature = S.dev<int>(pFeat); d.nEntries = S.dev<int>(pNE);
-    }
+    frame.bind(S, d);
     d.Tcw7 = S.dev<float>(pT); d.kfN = S.dev<int>(pKfN); d.kfKps = S.dev<OrbKeyPoint>(pKfKps); d.kfDesc = S.dev(pKfDesc);
     d.kfFvNode = S.dev<int>(pKfNode); d.kfFvFeature = S.dev<int>(pKfFeat); d.kfNEntries = S.dev<int>(pKfNE); d.kfPoint = S.dev(pPt);
     d.xyz = S.dev<float>(pXyz); d.hasObs = S.dev(pObs); d.invLevelSigma2 = S.dev<float>(pIs); d.active = active ? S.dev(pAct) : nullptr;
@@ -2457,71 +2487,98 @@ int orbm_track_local_map_batch_device(orbm_handle* h, const OrbmLocalMapBatch* i
     return track_local_map_launch(h->m, in, out, (cudaStream_t)stream);
 }
 
+// One stream of a host form of either local-map call: nM in [0, mcap], a positive th and, unless the call is resident, the current frame.
+static bool local_map_stream_ok(const OrbmLocalMapBatch* in, size_t b, bool frameOnDevice, const char* who) {
+    if (in->nM[b] < 0 || in->nM[b] > in->mcap) { set_error(std::string(who) + ": nM out of range"); return false; }
+    if (!(in->th[b] > 0.0f)) { set_error(std::string(who) + ": th must be positive"); return false; }
+    return frameOnDevice || stream_frame_ok(in, b, who);
+}
+
+// The staging of what the host forms of both local-map calls share: the current frame, the local map and the results of
+// OrbmLocalMapResult.  Tcw7, lastToLocal, discarded and pose7 are staged when the caller gives them (the mono-inertial call predicts the
+// pose and gives none of them); match goes in and out when matchIn (TrackLocalMap remaps it), else only out.
+struct LocalMapPieces {
+    BatchFrame<OrbmLocalMapBatch> frame;
+    bool matchIn;
+    int sf, is, T, l2l, dis, nM, wp, no, minD, maxD, raw, md, obs, bad, th, match, cl, outl, vis, found, counts, pose, to;
+
+    LocalMapPieces(Staging& S, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, bool frameOnDevice, bool matchIn)
+        : frame(S, in, frameOnDevice), matchIn(matchIn) {
+        const size_t B = in->batch, K = in->kcap, M = in->mcap, ML = in->lastToLocal ? in->mcapLast : 0;
+        const size_t DL = in->discarded ? (in->lastToLocal ? ML : M) : 0;
+        sf = S.in(in->scaleFactors, 4 * (size_t)in->nlevels); is = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels);
+        T = S.in(in->Tcw7, in->Tcw7 ? 28 * B : 0); l2l = S.in(in->lastToLocal, 4 * B * ML); dis = S.in(in->discarded, B * DL);
+        nM = S.in(in->nM, 4 * B); wp = S.in(in->worldPos, 12 * B * M); no = S.in(in->normal, 12 * B * M);
+        minD = S.in(in->minDistInv, 4 * B * M); maxD = S.in(in->maxDistInv, 4 * B * M); raw = S.in(in->maxDistance, 4 * B * M);
+        md = S.in(in->mpDesc, 32 * B * M); obs = S.in(in->hasObs, B * M); bad = S.in(in->bad, B * M); th = S.in(in->th, 4 * B);
+        match = matchIn ? S.inout(out->match, 4 * B * K) : S.out(nullptr, 4 * B * K);
+        cl = S.out(nullptr, B * K); outl = S.out(nullptr, B * K); vis = S.out(nullptr, 4 * B * M); found = S.out(nullptr, 4 * B * M);
+        counts = S.out(nullptr, 16 * B); pose = S.out(nullptr, out->pose7 ? 56 * B : 0); to = S.out(nullptr, 28 * B);
+    }
+
+    // Points `d` and `o`, copies of the caller's batch and result, at the pieces.  The staging is reserved.
+    void bind(const Staging& S, OrbmLocalMapBatch& d, OrbmLocalMapResult& o) const {
+        frame.bind(S, d);
+        d.scaleFactors = S.dev<float>(sf); d.invLevelSigma2 = S.dev<float>(is); d.Tcw7 = d.Tcw7 ? S.dev<float>(T) : nullptr;
+        d.lastToLocal = d.lastToLocal ? S.dev<int>(l2l) : nullptr; d.discarded = d.discarded ? S.dev(dis) : nullptr; d.nM = S.dev<int>(nM);
+        d.worldPos = S.dev<float>(wp); d.normal = S.dev<float>(no); d.minDistInv = S.dev<float>(minD); d.maxDistInv = S.dev<float>(maxD);
+        d.maxDistance = S.dev<float>(raw); d.mpDesc = S.dev(md); d.hasObs = S.dev(obs); d.bad = S.dev(bad); d.th = S.dev<float>(th);
+        const size_t B = d.batch;
+        int* c = S.dev<int>(counts);      // nToMatch | nmatches | nInliers | nMatchesInliers, [B] each
+        o = {S.dev<int>(match), S.dev(cl), S.dev(outl), S.dev<int>(vis), S.dev<int>(found), c, c + B, c + 2 * B, c + 3 * B,
+             o.pose7 ? S.dev<double>(pose) : nullptr, S.dev<float>(to)};
+    }
+
+    // After the download: the rows of the active streams to the caller's `out` (an in / out match is already back whole).
+    void copy_back(const Staging& S, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, const uint8_t* active) const {
+        const size_t B = in->batch, K = in->kcap, M = in->mcap;
+        if (!matchIn) copy_active_rows(S, match, out->match, 4 * K, in->batch, active);
+        copy_active_rows(S, cl, out->claimed, K, in->batch, active);
+        copy_active_rows(S, outl, out->outlier, K, in->batch, active);
+        copy_active_rows(S, vis, out->visible, 4 * M, in->batch, active);
+        copy_active_rows(S, found, out->found, 4 * M, in->batch, active);
+        copy_active_rows(S, pose, out->pose7, 56, in->batch, active);
+        copy_active_rows(S, to, out->Tcw7, 28, in->batch, active);
+        const int* hc = S.host<int>(counts);
+        int32_t* dst[4] = {out->nToMatch, out->nmatches, out->nInliers, out->nMatchesInliers};
+        for (size_t b = 0; b < B; ++b)
+            if (!active || active[b]) for (int k = 0; k < 4; ++k) dst[k][b] = hc[k * B + b];
+    }
+};
+
 static int track_local_map_host(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmLocalMapResult* out, bool frameOnDevice) {
     const char* who = frameOnDevice ? "orbm_track_local_map_batch_resident" : "orbm_track_local_map_batch";
     if (!h) { set_error(std::string(who) + ": bad argument"); return ORB_ERR_ARG; }
     if (int rc = local_map_shape(h->m, in, out, who)) return rc;
     Matcher& m = h->m;
-    const size_t B = in->batch, K = in->kcap, M = in->mcap, ML = in->lastToLocal ? in->mcapLast : 0;
+    const size_t B = in->batch, K = in->kcap, ML = in->lastToLocal ? in->mcapLast : 0;
     const uint8_t* active = in->active;
     for (size_t b = 0; b < B; ++b) {
         if (active && !active[b]) continue;
-        const int nM = in->nM[b];
-        if (nM < 0 || nM > in->mcap) { set_error(std::string(who) + ": nM out of range"); return ORB_ERR_ARG; }
-        if (!(in->th[b] > 0.0f)) { set_error(std::string(who) + ": th must be positive"); return ORB_ERR_ARG; }
-        if (!frameOnDevice) {
-            if (in->nK[b] < 0 || in->nK[b] > in->kcap) { set_error(std::string(who) + ": nK out of range"); return ORB_ERR_ARG; }
-            for (int i = 0; i < in->nK[b]; ++i) {
-                const int oct = in->kps[b * K + i].octave;
-                if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return ORB_ERR_ARG; }
-            }
-        }
+        if (!local_map_stream_ok(in, b, frameOnDevice, who)) return ORB_ERR_ARG;
         for (size_t i = 0; i < K; ++i) {
             const int mt = out->match[b * K + i];
             if (mt < -1 || mt >= (in->lastToLocal ? in->mcapLast : in->mcap)) { set_error(std::string(who) + ": match index out of range"); return ORB_ERR_ARG; }
         }
         for (size_t j = 0; j < ML; ++j)
-            if (in->lastToLocal[b * ML + j] < -1 || in->lastToLocal[b * ML + j] >= nM) { set_error(std::string(who) + ": lastToLocal index out of range"); return ORB_ERR_ARG; }
+            if (in->lastToLocal[b * ML + j] < -1 || in->lastToLocal[b * ML + j] >= in->nM[b]) { set_error(std::string(who) + ": lastToLocal index out of range"); return ORB_ERR_ARG; }
     }
     CK(cudaSetDevice(m.device));
     Staging& S = m.staging;
     S.begin();
-    const size_t DL = in->discarded ? (in->lastToLocal ? ML : M) : 0;
-    const int pKps = S.in(frameOnDevice ? nullptr : in->kps, frameOnDevice ? 0 : 28 * B * K), pDesc = S.in(frameOnDevice ? nullptr : in->desc, frameOnDevice ? 0 : 32 * B * K),
-              pNK = S.in(frameOnDevice ? nullptr : in->nK, frameOnDevice ? 0 : 4 * B), pSf = S.in(in->scaleFactors, 4 * (size_t)in->nlevels),
-              pIs = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels), pT = S.in(in->Tcw7, 28 * B), pL2L = S.in(in->lastToLocal, 4 * B * ML),
-              pDis = S.in(in->discarded, B * DL), pNM = S.in(in->nM, 4 * B), pWp = S.in(in->worldPos, 12 * B * M), pNo = S.in(in->normal, 12 * B * M),
-              pMin = S.in(in->minDistInv, 4 * B * M), pMax = S.in(in->maxDistInv, 4 * B * M), pRaw = S.in(in->maxDistance, 4 * B * M),
-              pMd = S.in(in->mpDesc, 32 * B * M), pObs = S.in(in->hasObs, B * M), pBad = S.in(in->bad, B * M), pTh = S.in(in->th, 4 * B),
-              pAct = S.in(active, active ? B : 0), pMatch = S.inout(out->match, 4 * B * K), pCl = S.out(nullptr, B * K), pOut = S.out(nullptr, B * K),
-              pVis = S.out(nullptr, 4 * B * M), pFound = S.out(nullptr, 4 * B * M), pCounts = S.out(nullptr, 16 * B), pPose = S.out(nullptr, 56 * B),
-              pTo = S.out(nullptr, 28 * B);
+    const LocalMapPieces lm(S, in, out, frameOnDevice, true);
+    const int pAct = S.in(active, active ? B : 0);
     int rc = S.reserve();
     if (rc) return rc;
     OrbmLocalMapBatch d = *in;
-    if (!frameOnDevice) { d.kps = S.dev<OrbKeyPoint>(pKps); d.desc = S.dev(pDesc); d.nK = S.dev<int>(pNK); }
-    d.scaleFactors = S.dev<float>(pSf); d.invLevelSigma2 = S.dev<float>(pIs); d.Tcw7 = S.dev<float>(pT);
-    d.lastToLocal = in->lastToLocal ? S.dev<int>(pL2L) : nullptr; d.discarded = in->discarded ? S.dev(pDis) : nullptr; d.nM = S.dev<int>(pNM);
-    d.worldPos = S.dev<float>(pWp); d.normal = S.dev<float>(pNo); d.minDistInv = S.dev<float>(pMin); d.maxDistInv = S.dev<float>(pMax);
-    d.maxDistance = S.dev<float>(pRaw); d.mpDesc = S.dev(pMd); d.hasObs = S.dev(pObs); d.bad = S.dev(pBad); d.th = S.dev<float>(pTh);
+    OrbmLocalMapResult o = *out;
+    lm.bind(S, d, o);
     d.active = active ? S.dev(pAct) : nullptr;
-    int* counts = S.dev<int>(pCounts);      // nToMatch | nmatches | nInliers | nMatchesInliers, [B] each
-    OrbmLocalMapResult o = {S.dev<int>(pMatch), S.dev(pCl), S.dev(pOut), S.dev<int>(pVis), S.dev<int>(pFound), counts, counts + B, counts + 2 * B,
-                            counts + 3 * B, S.dev<double>(pPose), S.dev<float>(pTo)};
     cudaStream_t st = m.stream;
     CK(S.upload(st));
     if ((rc = track_local_map_launch(m, &d, &o, st))) return rc;
     CK(S.download(st));
-    copy_active_rows(S, pCl, out->claimed, K, in->batch, active);
-    copy_active_rows(S, pOut, out->outlier, K, in->batch, active);
-    copy_active_rows(S, pVis, out->visible, 4 * M, in->batch, active);
-    copy_active_rows(S, pFound, out->found, 4 * M, in->batch, active);
-    copy_active_rows(S, pPose, out->pose7, 56, in->batch, active);
-    copy_active_rows(S, pTo, out->Tcw7, 28, in->batch, active);
-    const int* hc = S.host<int>(pCounts);
-    int32_t* dst[4] = {out->nToMatch, out->nmatches, out->nInliers, out->nMatchesInliers};
-    for (size_t b = 0; b < B; ++b)
-        if (!active || active[b]) for (int k = 0; k < 4; ++k) dst[k][b] = hc[k * B + b];
+    lm.copy_back(S, in, out, active);
     return ORB_OK;
 }
 
@@ -2619,72 +2676,42 @@ static int track_inertial_host(orbm_handle* h, const OrbmLocalMapBatch* in, cons
     Matcher& m = h->m;
     InertialRoutes R;
     if (int rc = inertial_routes(m, in, imu, out, io, R, who)) return rc;
-    const size_t B = in->batch, K = in->kcap, M = in->mcap, PS = 4 * IMU_PREINT_FLOATS;
+    const size_t B = in->batch, PS = 4 * IMU_PREINT_FLOATS;
     const uint8_t* active = R.active.data();
-    for (size_t b = 0; b < B; ++b) {
-        if (!active[b]) continue;
-        const int nM = in->nM[b];
-        if (nM < 0 || nM > in->mcap) { set_error(std::string(who) + ": nM out of range"); return ORB_ERR_ARG; }
-        if (!(in->th[b] > 0.0f)) { set_error(std::string(who) + ": th must be positive"); return ORB_ERR_ARG; }
-        if (!frameOnDevice) {
-            if (in->nK[b] < 0 || in->nK[b] > in->kcap) { set_error(std::string(who) + ": nK out of range"); return ORB_ERR_ARG; }
-            for (int i = 0; i < in->nK[b]; ++i) {
-                const int oct = in->kps[b * K + i].octave;
-                if (oct < 0 || oct >= in->nlevels) { set_error(std::string(who) + ": keypoint octave out of range"); return ORB_ERR_ARG; }
-            }
-        }
-    }
+    for (size_t b = 0; b < B; ++b)
+        if (active[b] && !local_map_stream_ok(in, b, frameOnDevice, who)) return ORB_ERR_ARG;
     CK(cudaSetDevice(m.device));
     if (int rc = m.track_scratch()) return rc;
     Staging& S = m.staging;
     S.begin();
     const bool lf = R.count[1] > 0, kf = R.count[0] > 0;
-    const int pKps = S.in(frameOnDevice ? nullptr : in->kps, frameOnDevice ? 0 : 28 * B * K), pDesc = S.in(frameOnDevice ? nullptr : in->desc, frameOnDevice ? 0 : 32 * B * K),
-              pNK = S.in(frameOnDevice ? nullptr : in->nK, frameOnDevice ? 0 : 4 * B), pSf = S.in(in->scaleFactors, 4 * (size_t)in->nlevels),
-              pIs = S.in(in->invLevelSigma2, 4 * (size_t)in->nlevels), pNM = S.in(in->nM, 4 * B), pWp = S.in(in->worldPos, 12 * B * M),
-              pNo = S.in(in->normal, 12 * B * M), pMin = S.in(in->minDistInv, 4 * B * M), pMax = S.in(in->maxDistInv, 4 * B * M),
-              pRaw = S.in(in->maxDistance, 4 * B * M), pMd = S.in(in->mpDesc, 32 * B * M), pObs = S.in(in->hasObs, B * M), pBad = S.in(in->bad, B * M),
-              pTh = S.in(in->th, 4 * B), pRoute = S.in(R.route.data(), 4 * B), pAct = S.in(active, B), pEx = S.in(imu->extrinsics24, 192),
+    const LocalMapPieces lm(S, in, out, frameOnDevice, false);
+    const int pRoute = S.in(R.route.data(), 4 * B), pAct = S.in(active, B), pEx = S.in(imu->extrinsics24, 192),
               pPk = S.in(imu->preintKF, PS * B), pPf = S.in(lf ? imu->preintFrame : nullptr, lf ? PS * B : 0),
               pKs = S.in(kf ? imu->kfState21 : nullptr, kf ? 84 * B : 0), pLs = S.in(lf ? imu->lastState21 : nullptr, lf ? 84 * B : 0),
               pPr = S.in(lf ? imu->prior21 : nullptr, lf ? 168 * B : 0), pPh = S.in(lf ? imu->priorH : nullptr, lf ? 1800 * B : 0),
-              pMatch = S.out(nullptr, 4 * B * K), pCl = S.out(nullptr, B * K), pOut = S.out(nullptr, B * K), pVis = S.out(nullptr, 4 * B * M),
-              pFound = S.out(nullptr, 4 * B * M), pCounts = S.out(nullptr, 16 * B), pTo = S.out(nullptr, 28 * B), pPs = S.out(nullptr, 84 * B),
-              pPt = S.out(nullptr, 28 * B), pSt = S.out(nullptr, 84 * B), pPo = S.out(nullptr, 168 * B), pHo = S.out(nullptr, 1800 * B);
+              pPs = S.out(nullptr, 84 * B), pPt = S.out(nullptr, 28 * B), pSt = S.out(nullptr, 84 * B), pPo = S.out(nullptr, 168 * B),
+              pHo = S.out(nullptr, 1800 * B);
     int rc = S.reserve();
     if (rc) return rc;
     OrbmLocalMapBatch d = *in;
-    if (!frameOnDevice) { d.kps = S.dev<OrbKeyPoint>(pKps); d.desc = S.dev(pDesc); d.nK = S.dev<int>(pNK); }
-    d.scaleFactors = S.dev<float>(pSf); d.invLevelSigma2 = S.dev<float>(pIs); d.nM = S.dev<int>(pNM);
-    d.worldPos = S.dev<float>(pWp); d.normal = S.dev<float>(pNo); d.minDistInv = S.dev<float>(pMin); d.maxDistInv = S.dev<float>(pMax);
-    d.maxDistance = S.dev<float>(pRaw); d.mpDesc = S.dev(pMd); d.hasObs = S.dev(pObs); d.bad = S.dev(pBad); d.th = S.dev<float>(pTh);
+    OrbmLocalMapResult o = *out;
+    lm.bind(S, d, o);
     OrbmImuTrackBatch di = *imu;
     di.extrinsics24 = S.dev<double>(pEx); di.preintKF = S.dev<float>(pPk); di.preintFrame = lf ? S.dev<float>(pPf) : nullptr;
     di.kfState21 = kf ? S.dev<float>(pKs) : nullptr; di.lastState21 = lf ? S.dev<float>(pLs) : nullptr;
     di.prior21 = lf ? S.dev<double>(pPr) : nullptr; di.priorH = lf ? S.dev<double>(pPh) : nullptr;
-    int* counts = S.dev<int>(pCounts);      // nToMatch | nmatches | nInliers | nMatchesInliers, [B] each
-    OrbmLocalMapResult o = {S.dev<int>(pMatch), S.dev(pCl), S.dev(pOut), S.dev<int>(pVis), S.dev<int>(pFound), counts, counts + B, counts + 2 * B,
-                            counts + 3 * B, nullptr, S.dev<float>(pTo)};
     OrbmImuTrackResult io2 = {S.dev<float>(pPs), S.dev<float>(pPt), S.dev<float>(pSt), S.dev<double>(pPo), S.dev<double>(pHo)};
     cudaStream_t st = m.stream;
     CK(S.upload(st));
     if ((rc = track_inertial_launch(m, &d, &di, &o, &io2, S.dev<int>(pRoute), S.dev(pAct), R.count, st))) return rc;
     CK(S.download(st));
-    copy_active_rows(S, pMatch, out->match, 4 * K, in->batch, active);
-    copy_active_rows(S, pCl, out->claimed, K, in->batch, active);
-    copy_active_rows(S, pOut, out->outlier, K, in->batch, active);
-    copy_active_rows(S, pVis, out->visible, 4 * M, in->batch, active);
-    copy_active_rows(S, pFound, out->found, 4 * M, in->batch, active);
-    copy_active_rows(S, pTo, out->Tcw7, 28, in->batch, active);
+    lm.copy_back(S, in, out, active);
     copy_active_rows(S, pPs, io->predState21, 84, in->batch, active);
     copy_active_rows(S, pPt, io->predTcw7, 28, in->batch, active);
     copy_active_rows(S, pSt, io->state21, 84, in->batch, active);
     copy_active_rows(S, pPo, io->prior21, 168, in->batch, active);
     copy_active_rows(S, pHo, io->priorH, 1800, in->batch, active);
-    const int* hc = S.host<int>(pCounts);
-    int32_t* dst[4] = {out->nToMatch, out->nmatches, out->nInliers, out->nMatchesInliers};
-    for (size_t b = 0; b < B; ++b)
-        if (active[b]) for (int k = 0; k < 4; ++k) dst[k][b] = hc[k * B + b];
     return ORB_OK;
 }
 

@@ -179,19 +179,25 @@ def test_bad_arguments_and_capacity(orb):
     def l2l(lo, st): lo['lastToLocal'][0, 0] = 10 ** 6
     def match(lo, st): st['match'][1, 0] = lo['mcapLast']
     def nm(lo, st): lo['nM'][0] = lo['mcap'] + 1
+    def nk(lo, st): lo['nK'][1] = lo['kcap'] + 1
     def batch(lo, st):                                   # more streams than the handle's max_batch
         lo['batch'] = 3; st['match'] = np.full((3, lo['kcap']), -1, np.int32)
-    for f in (oct_, l2l, match, nm, batch):
+    for f in (oct_, l2l, match, nm, nk, batch):
         expect(orb.ORB_ERR_ARG, f=f)
     small = orb.ORBmatcher(0.8, False, max_batch=2, max_keypoints=2048, max_mappoints=100, device=0)
     mo, lo, st = T.batch(streams, g, [1, 1])            # local maps of 300+ points
     with pytest.raises(orb.OrbError) as ei:
         small.track_local_map_batch(lo, st['match'])
     assert ei.value.code == orb.ORB_ERR_CAPACITY
-    mo['kps']['octave'][0, 0] = -1
-    with pytest.raises(orb.OrbError) as ei:
-        m.motion_model_pose_batch(mo, g['invLevelSigma2'], st['match'], st['claimed'], st['nmatches'])
-    assert ei.value.code == orb.ORB_ERR_ARG
+    def mm_oct(mo, st): mo['kps']['octave'][0, 0] = -1
+    def mm_nk(mo, st): mo['nK'][1] = mo['kcap'] + 1
+    def mm_match(mo, st): st['match'][1, 0] = mo['mcap']
+    for f in (mm_oct, mm_nk, mm_match):
+        mo, lo, st = T.batch(streams, g, [1, 1])
+        f(mo, st)
+        with pytest.raises(orb.OrbError) as ei:
+            m.motion_model_pose_batch(mo, g['invLevelSigma2'], st['match'], st['claimed'], st['nmatches'])
+        assert ei.value.code == orb.ORB_ERR_ARG, f
     assert m.last_launch_count() == n0 == 5
 
 

@@ -141,9 +141,10 @@ def test_bad_arguments_and_capacity(orb, voc):
     def kf_feat_range(d): d['kfFvFeature'][0, 0] = -1
     def kf_n(d): d['kfN'][1] = d['mcap'] + 1
     def n_entries(d): d['nEntries'][0] = d['nK'][0] + 1
+    def n_k(d): d['nK'][1] = d['kcap'] + 1
     def batch(d):
         d['batch'] = 3
-    for f in (octave, unsorted, kf_unsorted, feat_range, kf_feat_range, kf_n, n_entries, batch):
+    for f in (octave, unsorted, kf_unsorted, feat_range, kf_feat_range, kf_n, n_entries, n_k, batch):
         expect(orb.ORB_ERR_ARG, f)
     small = orb.ORBmatcher(0.8, False, max_batch=2, max_keypoints=2048, max_mappoints=100, device=0)
     expect(orb.ORB_ERR_CAPACITY, lambda d: None, small)
