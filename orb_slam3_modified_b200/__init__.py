@@ -37,6 +37,93 @@ class OrbmNewPointsIn(C.Structure):
                 ('cam', C.c_void_p), ('scaleFactor', C.c_float), ('bCoarse', C.c_int), ('bInertial', C.c_int), ('thFarPoints', C.c_float)]
 
 
+_vp, _i, _f, _d, _sz, _out = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.POINTER(C.c_void_p)
+
+#: (restype, argtypes) of every liborb_b200.so function the package, its tests and its tools call, as include/orb_b200.h declares it.
+#: lib() applies it once when it loads the library; tests/test_abi_layout_cpu.py checks it against the header.
+SIGNATURES = {
+    'orb_last_error': (C.c_char_p, []),
+    'orb_abi_version': (_i, []),
+    'orb_compiled_sm': (_i, []),
+    # ORBextractor
+    'orbx_create': (_i, [_out, _i, _f, _i, _i, _i, _i, _i, _i, _i]),
+    'orbx_destroy': (None, [_vp]),
+    'orbx_get_levels': (_i, [_vp]),
+    'orbx_get_tables': (_i, [_vp] * 6),
+    'orbx_max_keypoints': (_i, [_vp]),
+    'orbx_extract': (_i, [_vp, _vp, _i, _i, _sz, _i, _i, _vp, _vp, _i, _vp, _vp]),
+    'orbx_extract_batch': (_i, [_vp, _vp, _i, _i, _i, _sz, _sz, _i, _i, _vp, _vp, _i, _vp, _vp]),
+    'orbx_extract_batch_device': (_i, [_vp, _vp, _i, _i, _i, _sz, _sz, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    'orbx_resident_slabs': (_i, [_vp] * 5),
+    'orbx_stereo_matches': (_i, [_vp, _vp, _i, _f, _f, _vp, _vp, _i]),
+    'orbx_stereo_matches_device': (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _f, _f, _vp, _vp, _vp]),
+    'orbx_copy_level_bordered': (_i, [_vp, _i, _i, _i, _vp]),
+    'orbx_get_level_size': (_i, [_vp, _i, _vp, _vp]),
+    'orbx_copy_level': (_i, [_vp, _i, _i, _i, _vp]),
+    'orbx_copy_candidates': (_i, [_vp, _i, _i, _vp, _i]),
+    'orbx_last_launch_count': (_i, [_vp]),
+    'orbx_set_profiling': (_i, [_vp, _i]),
+    'orbx_get_stage_ms': (_i, [_vp, _vp]),
+    # ORBmatcher
+    'orbm_create': (_i, [_out, _i, _i, _i, _i]),
+    'orbm_destroy': (None, [_vp]),
+    'orbm_search_local_map': (_i, [_vp, _vp, _vp, _f, _f, _i, _f, _vp, _vp, _vp]),
+    'orbm_search_last_frame': (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _vp, _vp, _vp]),
+    'orbm_frustum_project': (_i, [_vp] * 9),
+    'orbm_search_last_frame_batch_device': (_i, [_vp, _vp, _f, _i, _vp, _vp, _vp, _vp]),
+    'orbm_search_last_frame_batch': (_i, [_vp, _vp, _f, _i, _vp, _vp, _vp]),
+    'orbm_search_last_frame_batch_resident': (_i, [_vp, _vp, _f, _i, _vp, _vp, _vp]),
+    'orbm_motion_model_pose_batch_device': (_i, [_vp] * 12),
+    'orbm_motion_model_pose_batch': (_i, [_vp] * 11),
+    'orbm_track_local_map_batch_device': (_i, [_vp] * 4),
+    'orbm_track_local_map_batch': (_i, [_vp] * 3),
+    'orbm_track_local_map_batch_resident': (_i, [_vp] * 3),
+    'orbm_track_local_map_inertial_batch_device': (_i, [_vp] * 6),
+    'orbm_track_local_map_inertial_batch': (_i, [_vp] * 5),
+    'orbm_track_local_map_inertial_batch_resident': (_i, [_vp] * 5),
+    'orbm_track_reference_keyframe_batch_device': (_i, [_vp] * 4),
+    'orbm_track_reference_keyframe_batch': (_i, [_vp] * 3),
+    'orbm_track_reference_keyframe_batch_resident': (_i, [_vp] * 3),
+    'orbm_search_for_initialization': (_i, [_vp, _vp, _vp, _vp, _i, _f, _i, _vp, _vp]),
+    'orbm_search_by_bow': (_i, [_vp, _vp, _vp, _vp, _f, _i, _vp, _vp]),
+    'orbm_search_by_bow_kf': (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _vp, _vp]),
+    'orbm_fuse_search': (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
+    'orbm_fuse_search_batch': (_i, [_vp, _i, _vp]),
+    'orbm_fuse_search_sim3': (_i, [_vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
+    'orbm_search_by_sim3': (_i, [_vp] * 5 + [_f, _vp, _f, _vp, _vp, _vp]),
+    'orbm_search_for_triangulation': (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp]),
+    'orbm_create_new_map_points': (_i, [_vp] * 6),
+    'orbm_distinctive_descriptors': (_i, [_vp, _i, _vp, _vp, _vp]),
+    'orbm_keyframe_culling_batch': (_i, [_vp, _i, _vp]),
+    'orbm_bf_knn2': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp]),
+    'orbm_descriptor_distance': (_i, [_vp, _vp, _vp, _i, _vp]),
+    'orbm_last_launch_count': (_i, [_vp]),
+    # Optimizer
+    'lba_create': (_i, [_out, _i, _i, _i, _i]),
+    'lba_create_batch': (_i, [_out, _i, _i, _i, _i, _i]),
+    'lba_destroy': (None, [_vp]),
+    'lba_solve': (_i, [_vp] * 3),
+    'lba_solve_batch': (_i, [_vp, _i, _vp, _vp]),
+    'lba_upload_batch': (_i, [_vp, _i, _vp]),
+    'lba_run_batch_device': (_i, [_vp, _vp]),
+    'lba_download_batch': (_i, [_vp, _i, _vp]),
+    'lba_last_cluster_size': (_i, [_vp]),
+    'lba_set_cluster_size': (_i, [_vp, _i]),
+    'lba_get_phase_ns': (_i, [_vp, _i, _vp]),
+    'pose_optimization_batch': (_i, [_i, _i] + [_vp] * 6 + [_d] + [_vp] * 3 + [_i]),
+    'imu_preintegrate_batch': (_i, [_i, _vp, _i] + [_vp] * 6 + [_i]),
+    'imu_information_batch': (_i, [_i] + [_vp] * 4 + [_i]),
+    'imu_inertial_edges': (_i, [_i, _vp, _vp, _vp, _d, _vp, _vp, _vp, _vp, _i]),
+    'imu_mono_edges': (_i, [_vp] * 7 + [_i]),
+    'pose_inertial_optimization_last_kf_batch': (_i, [_i, _i] + [_vp] * 10 + [_i, _vp, _vp, _vp, _i]),
+    'pose_inertial_optimization_last_frame_batch': (_i, [_i, _i] + [_vp] * 13 + [_i, _vp, _vp, _vp, _i]),
+    'local_inertial_ba_batch': (_i, [_i, _vp, _vp, _vp, _i]),
+    # ORBVocabulary
+    'orbv_create': (_i, [_out, _vp, _i]),
+    'orbv_destroy': (None, [_vp]),
+    'orbv_transform_batch': (_i, [_vp, _i, _vp, _vp, _i, _i] + [_vp] * 6),
+}
+
 _lib = None
 
 
@@ -55,21 +142,9 @@ def lib():
             raise RuntimeError('liborb_b200.so is not built (run `python -c "import __graft_entry__ as g; g.build()"`); '
                                'this package has no fallback path')
         L = C.CDLL(LIB_PATH)
-        L.orb_last_error.restype = C.c_char_p
-        vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
-        L.orbx_create.argtypes = [C.POINTER(vp), i, f, i, i, i, i, i, i, i]
-        L.orbx_destroy.argtypes = [vp]
-        L.orbx_destroy.restype = None
-        L.orbx_get_levels.argtypes = [vp]
-        L.orbx_get_tables.argtypes = [vp, vp, vp, vp, vp, vp]
-        L.orbx_max_keypoints.argtypes = [vp]
-        L.orbx_extract.argtypes = [vp, vp, i, i, sz, i, i, vp, vp, i, vp, vp]
-        L.orbx_extract_batch.argtypes = [vp, vp, i, i, i, sz, sz, i, i, vp, vp, i, vp, vp]
-        L.orbx_extract_batch_device.argtypes = [vp, vp, i, i, i, sz, sz, i, i, vp, vp, i, vp, vp, vp]
-        L.orbx_get_level_size.argtypes = [vp, i, vp, vp]
-        L.orbx_copy_level.argtypes = [vp, i, i, i, vp]
-        L.orbx_copy_candidates.argtypes = [vp, i, i, vp, i]
-        L.orbx_last_launch_count.argtypes = [vp]
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _lib = L
     return _lib
 
@@ -193,7 +268,6 @@ class ORBextractor:
     def resident_slabs(self):
         """Device addresses (ints) of the slabs the last host-buffer call left in the handle: (kps, desc, n, cap)."""
         k, d, n, cap = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int()
-        lib().orbx_resident_slabs.argtypes = [C.c_void_p] + [C.c_void_p] * 4
         rc = lib().orbx_resident_slabs(self._h, C.byref(k), C.byref(d), C.byref(n), C.byref(cap))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbx_resident_slabs')
@@ -227,7 +301,6 @@ class ORBextractor:
         w, h = C.c_int(), C.c_int()
         lib().orbx_get_level_size(self._h, level, C.byref(w), C.byref(h))
         out = np.zeros((h.value + 2 * border, w.value + 2 * border), np.uint8)
-        lib().orbx_copy_level_bordered.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
         rc = lib().orbx_copy_level_bordered(self._h, frame, level, border, _ptr(out))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbx_copy_level_bordered')
@@ -238,7 +311,6 @@ class ORBextractor:
         (self = left).  Returns (mvuRight, mvDepth) as [batch, cap] float32, -1 = no match."""
         cap = self.max_keypoints
         ur = np.zeros((batch, cap), np.float32); dep = np.zeros((batch, cap), np.float32)
-        lib().orbx_stereo_matches.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_int]
         rc = lib().orbx_stereo_matches(self._h, right._h, batch, mb, mbf, _ptr(ur), _ptr(dep), cap)
         if rc != ORB_OK:
             raise OrbError(rc, 'orbx_stereo_matches')
@@ -250,8 +322,6 @@ class ORBextractor:
         [B, capL] float32 receive mvuRight / mvDepth (-1 = no match).  Enqueues on ``stream`` and returns immediately."""
         B, capL = d_descL.shape[:2]
         capR = d_descR.shape[1]
-        lib().orbx_stereo_matches_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 3 + \
-            [C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 3
         rc = lib().orbx_stereo_matches_device(self._h, right._h, B, _ptr(d_kpsL), _ptr(d_descL), _ptr(d_nL), capL, _ptr(d_kpsR), _ptr(d_descR),
                                               _ptr(d_nR), capR, mb, mbf, _ptr(d_uRight), _ptr(d_depth), C.c_void_p(stream))
         if rc != ORB_OK:
@@ -270,11 +340,9 @@ class ORBextractor:
     STAGES = ('pyramid', 'blur', 'fast_cells', 'quadtree_orient', 'assemble', 'brief')
 
     def set_profiling(self, on):
-        lib().orbx_set_profiling.argtypes = [C.c_void_p, C.c_int]
         lib().orbx_set_profiling(self._h, int(on))
 
     def stage_ms(self):
-        lib().orbx_get_stage_ms.argtypes = [C.c_void_p, C.c_void_p]
         ms = np.zeros(6, np.float32)
         rc = lib().orbx_get_stage_ms(self._h, _ptr(ms))
         if rc != ORB_OK:
@@ -288,6 +356,11 @@ class ORBextractor:
 class _OrbmFrame(C.Structure):
     _fields_ = [('K', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('minX', C.c_float), ('minY', C.c_float),
                 ('maxX', C.c_float), ('maxY', C.c_float), ('scaleFactors', C.c_void_p), ('nlevels', C.c_int)]
+
+
+class _OrbmBowFrame(C.Structure):
+    _fields_ = [('N', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('nEntries', C.c_int), ('fvNode', C.c_void_p),
+                ('fvFeature', C.c_void_p)]
 
 
 class _OrbmLocalPoints(C.Structure):
@@ -442,20 +515,9 @@ class ORBmatcher:
     TH_HIGH, TH_LOW, HISTO_LENGTH = 100, 50, 30   # src/ORBmatcher.cc:35-37
 
     def __init__(self, nnratio=0.6, checkOri=True, max_batch=1, max_keypoints=2048, max_mappoints=8192, device=0):
-        L = lib()
-        vp, i, f = C.c_void_p, C.c_int, C.c_float
-        L.orbm_create.argtypes = [C.POINTER(vp), i, i, i, i]
-        L.orbm_destroy.argtypes = [vp]
-        L.orbm_destroy.restype = None
-        L.orbm_search_local_map.argtypes = [vp, vp, vp, f, f, i, f, vp, vp, vp]
-        L.orbm_search_last_frame.argtypes = [vp, vp, vp, vp, vp, f, i, vp, vp, vp]
-        L.orbm_search_last_frame_batch_device.argtypes = [vp, vp, f, i, vp, vp, vp, vp]
-        L.orbm_bf_knn2.argtypes = [vp, vp, i, vp, i, vp, vp]
-        L.orbm_descriptor_distance.argtypes = [vp, vp, vp, i, vp]
-        L.orbm_last_launch_count.argtypes = [vp]
         self.mfNNratio, self.mbCheckOrientation = float(nnratio), bool(checkOri)
         self._h = C.c_void_p()
-        rc = L.orbm_create(C.byref(self._h), max_batch, max_keypoints, max_mappoints, device)
+        rc = lib().orbm_create(C.byref(self._h), max_batch, max_keypoints, max_mappoints, device)
         if rc != ORB_OK:
             self._h = None
             raise OrbError(rc, 'orbm_create')
@@ -495,9 +557,7 @@ class ORBmatcher:
                            float(np.float32(log_scale_factor)), int(n_levels), float(viewingCosLimit))
         out = dict(inView=np.zeros(M, np.uint8), projX=np.zeros(M, np.float32), projY=np.zeros(M, np.float32), projXR=np.zeros(M, np.float32),
                    depth=np.zeros(M, np.float32), level=np.zeros(M, np.int32), viewCos=np.zeros(M, np.float32))
-        L = lib()
-        L.orbm_frustum_project.argtypes = [C.c_void_p] * 9
-        rc = L.orbm_frustum_project(self._h, C.byref(s), *[_ptr(out[k]) for k in ('inView', 'projX', 'projY', 'projXR', 'depth', 'level', 'viewCos')])
+        rc = lib().orbm_frustum_project(self._h, C.byref(s), *[_ptr(out[k]) for k in ('inView', 'projX', 'projY', 'projXR', 'depth', 'level', 'viewCos')])
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_frustum_project')
         return out
@@ -541,15 +601,27 @@ class ORBmatcher:
             raise OrbError(rc, 'orbm_search_last_frame')
         return n.value
 
-    def search_last_frame_batch_device(self, d, th, d_match, d_claimed, d_nmatches, stream=0):
-        """Device-resident batch (torch CUDA tensors in dict ``d``; see OrbmBatchDevice in include/orb_b200.h)."""
+    _BATCH_DT = dict(kps=KP_DTYPE, desc=np.uint8, nK=np.int32, scaleFactors=np.float32, nM=np.int32, valid=np.uint8, xyz=np.float32, octave=np.int32,
+                     angle=np.float32, hasObs=np.uint8, mpDesc=np.uint8, Tcw7=np.float32)
+    _MOTION_IN = ('kps', 'nK', 'xyz', 'hasObs', 'Tcw7')
+    _MOTION_DT = dict(kps=KP_DTYPE, nK=np.int32, xyz=np.float32, hasObs=np.uint8, Tcw7=np.float32, invLevelSigma2=np.float32, active=np.uint8)
+
+    @staticmethod
+    def _batch_struct(d, get, keys, search=True):
+        """OrbmBatchDevice of ``d`` with the arrays ``keys`` at ``get(k)``; the bounds and the reset flag only for the last-frame search."""
         s = _OrbmBatchDevice()
         s.batch, s.kcap, s.mcap, s.nlevels = d['batch'], d['kcap'], d['mcap'], d['nlevels']
-        for k in ('kps', 'desc', 'nK', 'scaleFactors', 'nM', 'valid', 'xyz', 'octave', 'angle', 'hasObs', 'mpDesc', 'Tcw7'):
-            setattr(s, k, d[k].data_ptr())
-        s.minX, s.minY, s.maxX, s.maxY = d['bounds']
+        for k in keys:
+            setattr(s, k, get(k))
         s.cam = (C.c_float * 4)(*d['cam'])
-        s.resetState = int(d.get('reset', 0))
+        if search:
+            s.minX, s.minY, s.maxX, s.maxY = d['bounds']
+            s.resetState = int(d.get('reset', 0))
+        return s
+
+    def search_last_frame_batch_device(self, d, th, d_match, d_claimed, d_nmatches, stream=0):
+        """Device-resident batch (torch CUDA tensors in dict ``d``; see OrbmBatchDevice in include/orb_b200.h)."""
+        s = self._batch_struct(d, lambda k: d[k].data_ptr(), self._BATCH_DT)
         rc = lib().orbm_search_last_frame_batch_device(self._h, C.byref(s), th, int(self.mbCheckOrientation), _ptr(d_match),
                                                        _ptr(d_claimed), _ptr(d_nmatches), C.c_void_p(stream))
         if rc != ORB_OK:
@@ -559,21 +631,9 @@ class ORBmatcher:
         """Host-buffer batch (numpy arrays in dict ``d``, same keys as the device variant); in/out arrays are numpy.
         ``resident`` = ``ORBextractor.resident_slabs()`` of the extractor that just produced the frames: the current frame is then read
         from the device slabs (d['kps'], d['desc'], d['nK'] are ignored) instead of being uploaded again."""
-        s = _OrbmBatchDevice()
-        s.batch, s.kcap, s.mcap, s.nlevels = d['batch'], d['kcap'], d['mcap'], d['nlevels']
-        for k in ('scaleFactors', 'nM', 'valid', 'xyz', 'octave', 'angle', 'hasObs', 'mpDesc', 'Tcw7'):
-            setattr(s, k, d[k].ctypes.data)
-        if resident is not None:
-            s.kps, s.desc, s.nK = resident[0], resident[1], resident[2]
-            assert resident[3] == d['kcap']
-        else:
-            for k in ('kps', 'desc', 'nK'):
-                setattr(s, k, d[k].ctypes.data)
-        s.minX, s.minY, s.maxX, s.maxY = d['bounds']
-        s.cam = (C.c_float * 4)(*d['cam'])
-        s.resetState = int(d.get('reset', 0))
-        fn = lib().orbm_search_last_frame_batch_resident if resident is not None else lib().orbm_search_last_frame_batch
-        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        assert resident is None or resident[3] == d['kcap']
+        get, fn = _host_call(d, self._BATCH_DT, 'orbm_search_last_frame_batch', resident, ('kps', 'desc', 'nK'))
+        s = self._batch_struct(d, get, self._BATCH_DT)
         rc = fn(self._h, C.byref(s), th, int(self.mbCheckOrientation), _ptr(match), _ptr(claimed), _ptr(nmatches))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_last_frame_batch')
@@ -584,23 +644,14 @@ class ORBmatcher:
         ``d``: the dict ``search_last_frame_batch`` took (kps, nK, xyz, hasObs, Tcw7, cam, kcap, mcap, nlevels are read); ``match`` /
         ``claimed`` [B, kcap] and ``nmatches`` [B] are what the search wrote and are updated in place; ``active`` [B] u8 or None.
         Returns dict(pose7 [B,7] f64, Tcw7 [B,7] f32, discarded [B,mcap] u8, nmatchesMap [B] i32); rows of inactive streams are zero."""
-        B, K, M = d['batch'], d['kcap'], d['mcap']
-        s = _OrbmBatchDevice()
-        s.batch, s.kcap, s.mcap, s.nlevels = B, K, M, d['nlevels']
-        keep = dict(kps=_c(d['kps'], KP_DTYPE), nK=_c(d['nK'], np.int32), xyz=_c(d['xyz'], np.float32), hasObs=_c(d['hasObs'], np.uint8),
-                    Tcw7=_c(d['Tcw7'], np.float32))
-        for k, a in keep.items():
-            setattr(s, k, a.ctypes.data)
-        s.cam = (C.c_float * 4)(*d['cam'])
-        isg = _c(inv_level_sigma2, np.float32)
-        act = None if active is None else _c(active, np.uint8)
+        B, M = d['batch'], d['mcap']
+        get, fn = _host_call(dict(d, invLevelSigma2=inv_level_sigma2, active=active), self._MOTION_DT, 'orbm_motion_model_pose_batch', None, ())
+        s = self._batch_struct(d, get, self._MOTION_IN, search=False)
         out = dict(pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32), discarded=np.zeros((B, M), np.uint8), nmatchesMap=np.zeros(B, np.int32))
         for a, dt in ((match, np.int32), (claimed, np.uint8), (nmatches, np.int32)):
             assert a.dtype == dt and a.flags.c_contiguous
-        L = lib()
-        L.orbm_motion_model_pose_batch.argtypes = [C.c_void_p] * 11
-        rc = L.orbm_motion_model_pose_batch(self._h, C.byref(s), _ptr(isg), _ptr(act), _ptr(match), _ptr(claimed), _ptr(nmatches),
-                                            *[_ptr(out[k]) for k in ('pose7', 'Tcw7', 'discarded', 'nmatchesMap')])
+        rc = fn(self._h, C.byref(s), get('invLevelSigma2'), get('active'), _ptr(match), _ptr(claimed), _ptr(nmatches),
+                *[_ptr(out[k]) for k in ('pose7', 'Tcw7', 'discarded', 'nmatchesMap')])
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_motion_model_pose_batch')
         return out
@@ -608,15 +659,10 @@ class ORBmatcher:
     def motion_model_pose_batch_device(self, d, inv_level_sigma2, match, claimed, nmatches, pose7, Tcw7, discarded, nmatchesMap, active=None,
                                        stream=0):
         """Device form of :meth:`motion_model_pose_batch`: torch CUDA tensors in ``d`` and as arguments; enqueues on ``stream``."""
-        s = _OrbmBatchDevice()
-        s.batch, s.kcap, s.mcap, s.nlevels = d['batch'], d['kcap'], d['mcap'], d['nlevels']
-        for k in ('kps', 'nK', 'xyz', 'hasObs', 'Tcw7'):
-            setattr(s, k, d[k].data_ptr())
-        s.cam = (C.c_float * 4)(*d['cam'])
-        L = lib()
-        L.orbm_motion_model_pose_batch_device.argtypes = [C.c_void_p] * 12
-        rc = L.orbm_motion_model_pose_batch_device(self._h, C.byref(s), _ptr(inv_level_sigma2), _ptr(active), _ptr(match), _ptr(claimed),
-                                                   _ptr(nmatches), _ptr(pose7), _ptr(Tcw7), _ptr(discarded), _ptr(nmatchesMap), C.c_void_p(stream))
+        s = self._batch_struct(d, lambda k: d[k].data_ptr(), self._MOTION_IN, search=False)
+        rc = lib().orbm_motion_model_pose_batch_device(self._h, C.byref(s), _ptr(inv_level_sigma2), _ptr(active), _ptr(match), _ptr(claimed),
+                                                       _ptr(nmatches), _ptr(pose7), _ptr(Tcw7), _ptr(discarded), _ptr(nmatchesMap),
+                                                       C.c_void_p(stream))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_motion_model_pose_batch_device')
 
@@ -654,7 +700,6 @@ class ORBmatcher:
                    found=np.zeros((B, M), np.int32), nToMatch=np.zeros(B, np.int32), nmatches=np.zeros(B, np.int32), nInliers=np.zeros(B, np.int32),
                    nMatchesInliers=np.zeros(B, np.int32), pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32))
         r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
-        fn.argtypes = [C.c_void_p] * 3
         rc = fn(self._h, C.byref(s), C.byref(r))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_local_map_batch')
@@ -666,9 +711,7 @@ class ORBmatcher:
         is in / out); enqueues on ``stream``."""
         s = self._local_map_struct(d, lambda k: d[k].data_ptr() if d.get(k) is not None else None)
         r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
-        L = lib()
-        L.orbm_track_local_map_batch_device.argtypes = [C.c_void_p] * 4
-        rc = L.orbm_track_local_map_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
+        rc = lib().orbm_track_local_map_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_local_map_batch_device')
 
@@ -705,7 +748,6 @@ class ORBmatcher:
                   prior21=np.zeros((B, 21)), priorH=np.zeros((B, 15, 15)))
         r = _OrbmLocalMapResult(*[_ptr(out[k]) for k in _LOCAL_MAP_OUT])
         ri = _OrbmImuTrackResult(*[_ptr(io[k]) for k in _IMU_TRACK_OUT])
-        fn.argtypes = [C.c_void_p] * 5
         rc = fn(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_local_map_inertial_batch')
@@ -721,9 +763,7 @@ class ORBmatcher:
         si = self._imu_struct(imu, mode, lambda k: imu[k].data_ptr() if imu.get(k) is not None else None)
         r = _OrbmLocalMapResult(*[_ptr(out[k]) if k != 'pose7' else None for k in _LOCAL_MAP_OUT])
         ri = _OrbmImuTrackResult(*[_ptr(out[k]) for k in _IMU_TRACK_OUT])
-        L = lib()
-        L.orbm_track_local_map_inertial_batch_device.argtypes = [C.c_void_p] * 6
-        rc = L.orbm_track_local_map_inertial_batch_device(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri), C.c_void_p(stream))
+        rc = lib().orbm_track_local_map_inertial_batch_device(self._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri), C.c_void_p(stream))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_local_map_inertial_batch_device')
 
@@ -753,7 +793,6 @@ class ORBmatcher:
         out = dict(nmatches=np.zeros(B, np.int32), match=np.full((B, K), -1, np.int32), pose7=np.zeros((B, 7)), Tcw7=np.zeros((B, 7), np.float32),
                    discarded=np.zeros((B, M), np.uint8), nmatchesMap=np.zeros(B, np.int32))
         r = _OrbmRefKeyFrameResult(*[_ptr(out[k]) for k in _REF_KF_OUT])
-        fn.argtypes = [C.c_void_p] * 3
         rc = fn(self._h, C.byref(s), C.byref(r))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_reference_keyframe_batch')
@@ -764,9 +803,7 @@ class ORBmatcher:
         enqueues on ``stream``."""
         s = self._ref_kf_struct(d, lambda k: d[k].data_ptr() if d.get(k) is not None else None)
         r = _OrbmRefKeyFrameResult(*[_ptr(out[k]) for k in _REF_KF_OUT])
-        L = lib()
-        L.orbm_track_reference_keyframe_batch_device.argtypes = [C.c_void_p] * 4
-        rc = L.orbm_track_reference_keyframe_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
+        rc = lib().orbm_track_reference_keyframe_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_track_reference_keyframe_batch_device')
 
@@ -778,7 +815,6 @@ class ORBmatcher:
         n = C.c_int(0)
         f1, f2 = F1._struct(), F2._struct()
         L = lib()
-        L.orbm_search_for_initialization.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
         rc = L.orbm_search_for_initialization(self._h, C.byref(f1), C.byref(f2), _ptr(vbPrevMatched), int(windowSize), self.mfNNratio,
                                               int(self.mbCheckOrientation), _ptr(m12), C.byref(n))
         if rc != ORB_OK:
@@ -788,16 +824,13 @@ class ORBmatcher:
     def SearchByBoW(self, kf_kps, kf_desc, kf_point, kf_fv, f_kps, f_desc, f_fv):
         """``int ORBmatcher::SearchByBoW(KeyFrame*, Frame&, vector<MapPoint*>&)`` (src/ORBmatcher.cc:223-425).  ``*_fv`` = (node ids, feature indices) of
         the DBoW2 FeatureVector; ``kf_point`` [nKF]: 0 none / 1 map point / 2 bad.  Returns (nmatches, match [nF] = keyframe feature index or -1)."""
-        class _BF(C.Structure):
-            _fields_ = [('N', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('nEntries', C.c_int), ('fvNode', C.c_void_p), ('fvFeature', C.c_void_p)]
         keep = [_c(kf_kps, KP_DTYPE), _c(kf_desc, np.uint8), _c(kf_fv[0], np.int32), _c(kf_fv[1], np.int32), _c(f_kps, KP_DTYPE), _c(f_desc, np.uint8),
                 _c(f_fv[0], np.int32), _c(f_fv[1], np.int32), _c(kf_point, np.uint8)]
-        a = _BF(len(keep[0]), keep[0].ctypes.data, keep[1].ctypes.data, len(keep[2]), keep[2].ctypes.data, keep[3].ctypes.data)
-        b = _BF(len(keep[4]), keep[4].ctypes.data, keep[5].ctypes.data, len(keep[6]), keep[6].ctypes.data, keep[7].ctypes.data)
+        a = _OrbmBowFrame(len(keep[0]), keep[0].ctypes.data, keep[1].ctypes.data, len(keep[2]), keep[2].ctypes.data, keep[3].ctypes.data)
+        b = _OrbmBowFrame(len(keep[4]), keep[4].ctypes.data, keep[5].ctypes.data, len(keep[6]), keep[6].ctypes.data, keep[7].ctypes.data)
         match = np.full(len(keep[4]), -1, np.int32)
         n = C.c_int(0)
         L = lib()
-        L.orbm_search_by_bow.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
         rc = L.orbm_search_by_bow(self._h, C.byref(a), _ptr(keep[8]), C.byref(b), self.mfNNratio, int(self.mbCheckOrientation), _ptr(match), C.byref(n))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_by_bow')
@@ -807,41 +840,27 @@ class ORBmatcher:
                    mp_desc, th=3.0):
         """The search of ``int ORBmatcher::Fuse(KeyFrame*, const vector<MapPoint*>&, th)`` (src/ORBmatcher.cc:1148-1338): (bestIdx [M], bestDist [M]);
         Fuse's return value is ``(bestDist <= 50).sum()``; see include/orb_b200.h: orbm_fuse_search."""
-        class _Fr(C.Structure):
-            _fields_ = [('K', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('minX', C.c_float), ('minY', C.c_float), ('maxX', C.c_float),
-                        ('maxY', C.c_float), ('scaleFactors', C.c_void_p), ('nlevels', C.c_int)]
-        class _Pt(C.Structure):
-            _fields_ = [('M', C.c_int)] + [(n, C.c_void_p) for n in ('state', 'worldPos', 'normal', 'minDistance', 'maxDistance', 'descriptors')]
         k = [_c(kf_kps, KP_DTYPE), _c(kf_desc, np.uint8), _c(scale_factors, np.float32), _c(inv_level_sigma2, np.float32)]
         m = [_c(state, np.uint8), _c(xyz, np.float32), _c(normal, np.float32), _c(min_d, np.float32), _c(max_d, np.float32), _c(mp_desc, np.uint8)]
         o = [_c(Tcw7, np.float32), _c(Ow, np.float32), _c(cam4, np.float32)]
-        fr = _Fr(len(k[0]), k[0].ctypes.data, k[1].ctypes.data, *[float(b) for b in bounds], k[2].ctypes.data, len(k[2]))
-        pt = _Pt(len(m[0]), *[a.ctypes.data for a in m])
+        fr = _OrbmFrame(len(k[0]), k[0].ctypes.data, k[1].ctypes.data, *[float(b) for b in bounds], k[2].ctypes.data, len(k[2]))
+        pt = _OrbmFusePoints(len(m[0]), *[a.ctypes.data for a in m])
         bi = np.zeros(len(m[0]), np.int32); bd = np.zeros(len(m[0]), np.int32)
         L = lib()
-        L.orbm_fuse_search.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]
         rc = L.orbm_fuse_search(self._h, C.byref(fr), _ptr(k[3]), float(log_scale_factor), _ptr(o[0]), _ptr(o[1]), _ptr(o[2]), C.byref(pt), float(th), _ptr(bi), _ptr(bd))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_fuse_search')
         return bi, bd
-
-    class _Fr(C.Structure):
-        _fields_ = [('K', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('minX', C.c_float), ('minY', C.c_float), ('maxX', C.c_float),
-                    ('maxY', C.c_float), ('scaleFactors', C.c_void_p), ('nlevels', C.c_int)]
-
-    class _Pt(C.Structure):
-        _fields_ = [('M', C.c_int)] + [(n, C.c_void_p) for n in ('state', 'worldPos', 'normal', 'minDistance', 'maxDistance', 'descriptors')]
 
     def FuseSearchSim3(self, kf_kps, kf_desc, bounds, scale_factors, log_scale_factor, Tcw7, Ow, cam4, state, xyz, normal, min_d, max_d, mp_desc, th=3.0):
         """The search of ``ORBmatcher::Fuse(pKF, Scw, vpPoints, th, vpReplacePoint)`` (src/ORBmatcher.cc:1340-1455): (bestIdx, bestDist)."""
         k = [_c(kf_kps, KP_DTYPE), _c(kf_desc, np.uint8), _c(scale_factors, np.float32)]
         m = [_c(state, np.uint8), _c(xyz, np.float32), _c(normal, np.float32), _c(min_d, np.float32), _c(max_d, np.float32), _c(mp_desc, np.uint8)]
         o = [_c(Tcw7, np.float32), _c(Ow, np.float32), _c(cam4, np.float32)]
-        fr = self._Fr(len(k[0]), k[0].ctypes.data, k[1].ctypes.data, *[float(b) for b in bounds], k[2].ctypes.data, len(k[2]))
-        pt = self._Pt(len(m[0]), *[a.ctypes.data for a in m])
+        fr = _OrbmFrame(len(k[0]), k[0].ctypes.data, k[1].ctypes.data, *[float(b) for b in bounds], k[2].ctypes.data, len(k[2]))
+        pt = _OrbmFusePoints(len(m[0]), *[a.ctypes.data for a in m])
         bi = np.zeros(len(m[0]), np.int32); bd = np.zeros(len(m[0]), np.int32)
         L = lib()
-        L.orbm_fuse_search_sim3.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]
         rc = L.orbm_fuse_search_sim3(self._h, C.byref(fr), float(log_scale_factor), _ptr(o[0]), _ptr(o[1]), _ptr(o[2]), C.byref(pt), float(th), _ptr(bi), _ptr(bd))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_fuse_search_sim3')
@@ -874,7 +893,6 @@ class ORBmatcher:
             s.pts = _OrbmFusePoints(M, *[a.ctypes.data for a in m])
             s.bestIdx, s.bestDist = bi.ctypes.data, bd.ctypes.data
         L = lib()
-        L.orbm_fuse_search_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         rc = L.orbm_fuse_search_batch(self._h, len(items), arr)
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_fuse_search_batch')
@@ -889,14 +907,13 @@ class ORBmatcher:
             a = [_c(kf['kps'], KP_DTYPE), _c(kf['desc'], np.uint8), _c(scale_factors, np.float32), _c(kf['state'], np.uint8), _c(kf['pcam'], np.float32),
                  _c(kf['min_d'], np.float32), _c(kf['max_d'], np.float32), _c(kf['mp_desc'], np.uint8)]
             keep.append(a)
-            fr = self._Fr(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, *[float(b) for b in bounds], a[2].ctypes.data, len(a[2]))
-            pt = self._Pt(len(a[3]), a[3].ctypes.data, a[4].ctypes.data, None, a[5].ctypes.data, a[6].ctypes.data, a[7].ctypes.data)
+            fr = _OrbmFrame(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, *[float(b) for b in bounds], a[2].ctypes.data, len(a[2]))
+            pt = _OrbmFusePoints(len(a[3]), a[3].ctypes.data, a[4].ctypes.data, None, a[5].ctypes.data, a[6].ctypes.data, a[7].ctypes.data)
             return fr, pt
         f1, p1 = side(kf1); f2, p2 = side(kf2)
         cam = _c(cam4, np.float32); pre = _c(pre12, np.int32)
         m12 = np.zeros(f1.K, np.int32); n = C.c_int(0)
         L = lib()
-        L.orbm_search_by_sim3.argtypes = [C.c_void_p] * 5 + [C.c_float, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
         rc = L.orbm_search_by_sim3(self._h, C.byref(f1), C.byref(p1), C.byref(f2), C.byref(p2), float(log_scale_factor), _ptr(cam), float(th), _ptr(pre), _ptr(m12), C.byref(n))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_by_sim3')
@@ -904,42 +921,36 @@ class ORBmatcher:
 
     def SearchByBoWKF(self, k1, d1, point1, fv1, k2, d2, point2, fv2):
         """``int ORBmatcher::SearchByBoW(KeyFrame*, KeyFrame*, vector<MapPoint*>&)`` (src/ORBmatcher.cc:765-905): (nmatches, match12 [N1] = KF2 feature or -1)."""
-        class _BF(C.Structure):
-            _fields_ = [('N', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('nEntries', C.c_int), ('fvNode', C.c_void_p), ('fvFeature', C.c_void_p)]
         keep = [_c(k1, KP_DTYPE), _c(d1, np.uint8), _c(fv1[0], np.int32), _c(fv1[1], np.int32), _c(k2, KP_DTYPE), _c(d2, np.uint8),
                 _c(fv2[0], np.int32), _c(fv2[1], np.int32), _c(point1, np.uint8), _c(point2, np.uint8)]
-        a = _BF(len(keep[0]), keep[0].ctypes.data, keep[1].ctypes.data, len(keep[2]), keep[2].ctypes.data, keep[3].ctypes.data)
-        b = _BF(len(keep[4]), keep[4].ctypes.data, keep[5].ctypes.data, len(keep[6]), keep[6].ctypes.data, keep[7].ctypes.data)
+        a = _OrbmBowFrame(len(keep[0]), keep[0].ctypes.data, keep[1].ctypes.data, len(keep[2]), keep[2].ctypes.data, keep[3].ctypes.data)
+        b = _OrbmBowFrame(len(keep[4]), keep[4].ctypes.data, keep[5].ctypes.data, len(keep[6]), keep[6].ctypes.data, keep[7].ctypes.data)
         m12 = np.full(len(keep[0]), -1, np.int32)
         n = C.c_int(0)
         L = lib()
-        L.orbm_search_by_bow_kf.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
         rc = L.orbm_search_by_bow_kf(self._h, C.byref(a), _ptr(keep[8]), C.byref(b), _ptr(keep[9]), self.mfNNratio, int(self.mbCheckOrientation), _ptr(m12), C.byref(n))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_by_bow_kf')
         return n.value, m12
 
+    @staticmethod
+    def _tri_frame(kf, keep):
+        """OrbmTriFrame of keyframe dict ``kf`` (kps, desc, has_mp, fv=(nodes, features)); its arrays are appended to ``keep``."""
+        a = [_c(kf['kps'], KP_DTYPE), _c(kf['desc'], np.uint8), _c(kf['has_mp'], np.uint8), _c(kf['fv'][0], np.int32), _c(kf['fv'][1], np.int32)]
+        keep.append(a)
+        return OrbmTriFrame(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[3]), a[3].ctypes.data, a[4].ctypes.data)
+
     def SearchForTriangulation(self, kf1, kf2_list, scale_factors, level_sigma2, ep, F12, coarse=False):
         """``int ORBmatcher::SearchForTriangulation(pKF1, pKF2, vMatchedPairs, false, bCoarse)`` (src/ORBmatcher.cc:907-1146) for one keyframe against
         several neighbours.  A keyframe is a dict(kps, desc, has_mp, fv=(nodes, features)); ep [n, 2], F12 [n, 9].  Returns (nmatches [n], matches12 [n, N1])."""
-        class _TF(C.Structure):
-            _fields_ = [('N', C.c_int), ('keypoints', C.c_void_p), ('descriptors', C.c_void_p), ('hasMapPoint', C.c_void_p), ('nEntries', C.c_int),
-                        ('fvNode', C.c_void_p), ('fvFeature', C.c_void_p)]
         keep = []
-
-        def mk(kf):
-            a = [_c(kf['kps'], KP_DTYPE), _c(kf['desc'], np.uint8), _c(kf['has_mp'], np.uint8), _c(kf['fv'][0], np.int32), _c(kf['fv'][1], np.int32)]
-            keep.append(a)
-            return _TF(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[3]), a[3].ctypes.data, a[4].ctypes.data)
-        f1 = mk(kf1)
+        f1 = self._tri_frame(kf1, keep)
         n2 = len(kf2_list)
-        f2 = (_TF * max(n2, 1))(*[mk(k) for k in kf2_list])
+        f2 = (OrbmTriFrame * max(n2, 1))(*[self._tri_frame(k, keep) for k in kf2_list])
         sf, sg = _c(scale_factors, np.float32), _c(level_sigma2, np.float32)
         epa, Fa = _c(ep, np.float32).reshape(-1, 2), _c(F12, np.float32).reshape(-1, 9)
         m12 = np.full((n2, f1.N), -1, np.int32); nm = np.zeros(n2, np.int32)
         L = lib()
-        L.orbm_search_for_triangulation.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                                    C.c_void_p, C.c_void_p]
         rc = L.orbm_search_for_triangulation(self._h, C.byref(f1), n2, f2, _ptr(sf), _ptr(sg), len(sf), _ptr(epa), _ptr(Fa), int(coarse), int(self.mbCheckOrientation),
                                              _ptr(m12), _ptr(nm))
         if rc != ORB_OK:
@@ -954,14 +965,9 @@ class ORBmatcher:
         ``cam`` [1 + n, 4]; ``th_far_points`` 0 = off.  Returns (records, nmatches [n], ncreated [n]): ``records`` is a ``NEW_POINT_DTYPE``
         array in creation order.  The matcher's own settings are not used: the reference builds ``ORBmatcher(0.6f, false)`` here."""
         keep = []
-
-        def mk(kf):
-            a = [_c(kf['kps'], KP_DTYPE), _c(kf['desc'], np.uint8), _c(kf['has_mp'], np.uint8), _c(kf['fv'][0], np.int32), _c(kf['fv'][1], np.int32)]
-            keep.append(a)
-            return OrbmTriFrame(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[3]), a[3].ctypes.data, a[4].ctypes.data)
-        f1 = mk(kf1)
+        f1 = self._tri_frame(kf1, keep)
         n2 = len(kf2_list)
-        f2 = (OrbmTriFrame * max(n2, 1))(*[mk(k) for k in kf2_list])
+        f2 = (OrbmTriFrame * max(n2, 1))(*[self._tri_frame(k, keep) for k in kf2_list])
         arrs = [_c(scale_factors, np.float32), _c(level_sigma2, np.float32), _c(ep, np.float32).reshape(-1, 2), _c(F12, np.float32).reshape(-1, 9),
                 _c(Tcw, np.float32).reshape(-1, 12), _c(Ow, np.float32).reshape(-1, 3), _c(cam, np.float32).reshape(-1, 4)]
         assert len(arrs[4]) == len(arrs[5]) == len(arrs[6]) == n2 + 1 and len(arrs[2]) == len(arrs[3]) == n2
@@ -972,7 +978,6 @@ class ORBmatcher:
         nm, nc = np.zeros(n2, np.int32), np.zeros(n2, np.int32)
         n = C.c_int(0)
         L = lib()
-        L.orbm_create_new_map_points.argtypes = [C.c_void_p] * 6
         rc = L.orbm_create_new_map_points(self._h, C.byref(inp), _ptr(out), C.byref(n), _ptr(nm), _ptr(nc))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_create_new_map_points')
@@ -987,7 +992,6 @@ class ORBmatcher:
         built = [culling_struct(m) for m in maps]
         arr = (OrbmCullingMap * max(len(maps), 1))(*[b[0] for b in built])
         L = lib()
-        L.orbm_keyframe_culling_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         rc = L.orbm_keyframe_culling_batch(self._h, len(maps), arr)
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_keyframe_culling_batch')
@@ -1002,7 +1006,6 @@ class ORBmatcher:
         desc = np.ascontiguousarray(desc)
         best = np.zeros(len(obs_list), np.int32)
         L = lib()
-        L.orbm_distinctive_descriptors.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         rc = L.orbm_distinctive_descriptors(self._h, len(obs_list), _ptr(start), _ptr(desc), _ptr(best))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_distinctive_descriptors')
@@ -1046,15 +1049,6 @@ class Optimizer:
 
     def __init__(self, max_poses=64, max_points=8192, max_edges=65536, max_batch=1, device=0):
         L = lib()
-        L.lba_create_batch.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-        L.lba_destroy.argtypes = [C.c_void_p]
-        L.lba_destroy.restype = None
-        L.lba_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.lba_solve_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-        L.lba_upload_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        L.lba_run_batch_device.argtypes = [C.c_void_p, C.c_void_p]
-        L.lba_download_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        L.lba_last_cluster_size.argtypes = [C.c_void_p]
         self._h = C.c_void_p()
         rc = L.lba_create_batch(C.byref(self._h), max_poses, max_points, max_edges, max_batch, device)
         if rc != ORB_OK:
@@ -1123,7 +1117,6 @@ class Optimizer:
         return lib().lba_last_cluster_size(self._h)
 
     def set_cluster_size(self, ctas):
-        lib().lba_set_cluster_size.argtypes = [C.c_void_p, C.c_int]
         rc = lib().lba_set_cluster_size(self._h, ctas)
         if rc != ORB_OK:
             raise OrbError(rc, 'lba_set_cluster_size')
@@ -1158,7 +1151,6 @@ def PoseOptimization(frames, device=0):
         Xw[i, :N[i]] = f['Xw']; obs[i, :N[i]] = f['obs']; isg[i, :N[i]] = f['inv_sigma2']
     out_pose = np.zeros((count, 7)); outl = np.zeros((count, cap), np.uint8); ninl = np.zeros(count, np.int32)
     L = lib()
-    L.pose_optimization_batch.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_double] + [C.c_void_p] * 3 + [C.c_int]
     rc = L.pose_optimization_batch(count, cap, _ptr(N), _ptr(pose), _ptr(cam), _ptr(Xw), _ptr(obs), _ptr(isg),
                                    float(np.float32(np.sqrt(5.991))), _ptr(out_pose), _ptr(outl), _ptr(ninl), device)
     if rc != ORB_OK:
@@ -1183,7 +1175,6 @@ def imu_preintegrate(acc, gyr, dt, n_meas, bias6, noise4, device=0):
     count, mm = dt.shape
     out = np.zeros((count, IMU_PREINT_FLOATS), np.float32)
     L = lib()
-    L.imu_preintegrate_batch.argtypes = [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 6 + [C.c_int]
     rc = L.imu_preintegrate_batch(count, _ptr(n), mm, _ptr(acc), _ptr(gyr), _ptr(dt), _ptr(b), _ptr(nz), _ptr(out), device)
     if rc != ORB_OK:
         raise OrbError(rc, 'imu_preintegrate_batch')
@@ -1195,7 +1186,6 @@ def imu_information(preint, device=0):
     n = len(P)
     info = np.zeros((n, 9, 9)); ig = np.zeros((n, 3, 3)); ia = np.zeros((n, 3, 3))
     L = lib()
-    L.imu_information_batch.argtypes = [C.c_int] + [C.c_void_p] * 4 + [C.c_int]
     rc = L.imu_information_batch(n, _ptr(P), _ptr(info), _ptr(ig), _ptr(ia), device)
     if rc != ORB_OK:
         raise OrbError(rc, 'imu_information_batch')
@@ -1210,7 +1200,6 @@ def imu_inertial_edges(preint, states36, info9=None, huber_delta=0.0, jac=True, 
     info = _c(info9, np.float64) if info9 is not None else None
     chi2 = np.zeros(n); rho = np.zeros(n)
     L = lib()
-    L.imu_inertial_edges.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     rc = L.imu_inertial_edges(n, _ptr(P), _ptr(S), _ptr(info), float(huber_delta), _ptr(err), _ptr(J), _ptr(chi2), _ptr(rho), device)
     if rc != ORB_OK:
         raise OrbError(rc, 'imu_inertial_edges')
@@ -1228,7 +1217,6 @@ def imu_mono_edges(poses12, extrinsics24, cam, points, edge_point, edge_pose, ob
     err = np.zeros((n, 2)); Jp = np.zeros((n, 2, 3)) if jac else None; Jx = np.zeros((n, 2, 6)) if jac else None
     chi2 = np.zeros(n); rho = np.zeros(n); dp = np.zeros(n, np.uint8)
     L = lib()
-    L.imu_mono_edges.argtypes = [C.c_void_p] * 7 + [C.c_int]
     rc = L.imu_mono_edges(C.byref(s), _ptr(err), _ptr(Jp), _ptr(Jx), _ptr(chi2), _ptr(rho), _ptr(dp), device)
     if rc != ORB_OK:
         raise OrbError(rc, 'imu_mono_edges')
@@ -1250,7 +1238,6 @@ def PoseInertialOptimizationLastKeyFrame(frames, extrinsics24, rec_init=False, d
     ex = _c(extrinsics24, np.float64)
     out = np.zeros((n, cap), np.uint8); H = np.zeros((n, 15, 15)); ret = np.zeros(n, np.int32)
     L = lib()
-    L.pose_inertial_optimization_last_kf_batch.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 10 + [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     rc = L.pose_inertial_optimization_last_kf_batch(n, cap, _ptr(N), _ptr(Xw), _ptr(ob), _ptr(isg), _ptr(td), _ptr(cam), _ptr(ex), _ptr(P), _ptr(kf), _ptr(st), int(rec_init),
                                                     _ptr(out), _ptr(H), _ptr(ret), device)
     if rc != ORB_OK:
@@ -1274,7 +1261,6 @@ def PoseInertialOptimizationLastFrame(frames, extrinsics24, rec_init=False, devi
     ex = _c(extrinsics24, np.float64)
     out = np.zeros((n, cap), np.uint8); H = np.zeros((n, 15, 15)); ret = np.zeros(n, np.int32)
     L = lib()
-    L.pose_inertial_optimization_last_frame_batch.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 13 + [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     rc = L.pose_inertial_optimization_last_frame_batch(n, cap, _ptr(N), _ptr(Xw), _ptr(ob), _ptr(isg), _ptr(td), _ptr(cam), _ptr(ex), _ptr(Pf), _ptr(Pk), _ptr(prior), _ptr(pH),
                                                        _ptr(pv), _ptr(st), int(rec_init), _ptr(out), _ptr(H), _ptr(ret), device)
     if rc != ORB_OK:
@@ -1332,7 +1318,6 @@ def LocalInertialBA(probs, device=0):
     P, R, keep, outs = _liba_marshal(probs)
     iters = np.zeros(len(probs), np.int32)
     L = lib()
-    L.local_inertial_ba_batch.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     rc = L.local_inertial_ba_batch(len(probs), C.cast(P, C.c_void_p), C.cast(R, C.c_void_p), _ptr(iters), device)
     if rc != ORB_OK:
         raise OrbError(rc, 'local_inertial_ba_batch')
@@ -1352,7 +1337,6 @@ class ORBVocabulary:
         self._keep = [_c(child_start, np.int32), _c(children, np.int32), _c(desc, np.uint8), _c(weight, np.float64), _c(word_id, np.int32)]
         s = _OrbVocabulary(len(self._keep[4]), int(L), int(weighting), int(norm), *[a.ctypes.data for a in self._keep])
         self._h = C.c_void_p()
-        lib().orbv_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int]
         rc = lib().orbv_create(C.byref(self._h), C.byref(s), device)
         if rc != ORB_OK:
             self._h = None
@@ -1360,8 +1344,6 @@ class ORBVocabulary:
 
     def close(self):
         if getattr(self, '_h', None):
-            lib().orbv_destroy.argtypes = [C.c_void_p]
-            lib().orbv_destroy.restype = None
             lib().orbv_destroy(self._h)
             self._h = None
 
@@ -1382,7 +1364,6 @@ class ORBVocabulary:
         wid = np.zeros((B, cap), np.int32); wv = np.zeros((B, cap)); nw = np.zeros(B, np.int32)
         fn = np.zeros((B, cap), np.int32); ff = np.zeros((B, cap), np.int32); ne = np.zeros(B, np.int32)
         L = lib()
-        L.orbv_transform_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 6
         rc = L.orbv_transform_batch(self._h, B, _ptr(desc), _ptr(n), cap, int(levelsup), _ptr(wid), _ptr(wv), _ptr(nw), _ptr(fn), _ptr(ff), _ptr(ne))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbv_transform_batch')

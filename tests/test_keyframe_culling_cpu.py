@@ -1,7 +1,6 @@
 """CPU tests of LocalMapping::KeyFrameCulling's oracle (oracle/keyframe_culling_oracle.cpp) against the Python restatement and the host
 replay of tests/keyframe_culling_lib.py: seeded corridors, every status, the sequential rule, the float boundaries of the decision, the
 inertial guards and the break test.  No GPU needed."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -143,7 +142,6 @@ def test_new_entry_point_without_gpu():
     import orb_slam3_modified_b200 as orb
     L = orb.lib()
     assert hasattr(L, 'orbm_keyframe_culling_batch')
-    L.orbm_keyframe_culling_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     assert L.orbm_keyframe_culling_batch(None, 0, None) == orb.ORB_ERR_ARG
     if torch.cuda.is_available():
         pytest.skip('GPU present')

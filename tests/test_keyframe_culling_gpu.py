@@ -1,7 +1,6 @@
 """GPU tests of orbm_keyframe_culling_batch: per map, status / nMPs / nRedundant / visited equal the oracle's for batches of mono and
 inertial maps with empty maps mixed in; a batch equals per-map calls byte for byte; one launch per call; the host replay of the statuses
 gives the oracle's final map; the argument errors; the C++ mirror's digest equals the Python binding's."""
-import ctypes as C
 import os
 import subprocess
 
@@ -114,7 +113,6 @@ def test_launch_counts(orb, matcher):
 
 def test_bad_arguments(orb, matcher):
     L = orb.lib()
-    L.orbm_keyframe_culling_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     base = [K.flatten(K.corridor(5)), K.flatten(K.corridor(6, inertial=True, kf_extra=5))]
     matcher.keyframe_culling_batch(base)
     assert matcher.last_launch_count() == 1

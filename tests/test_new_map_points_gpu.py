@@ -73,7 +73,6 @@ def test_bad_arguments(orb, matcher, scenes):
     gpu(matcher, sc)
     assert matcher.last_launch_count() == 3
     L = orb.lib()
-    L.orbm_create_new_map_points.argtypes = [C.c_void_p] * 6
 
     def raw(s, out=True, n=True, nm=True, nc=True):
         o = np.zeros(2048, orb.NEW_POINT_DTYPE); a, b = np.zeros(8, np.int32), np.zeros(8, np.int32); k = C.c_int(0)

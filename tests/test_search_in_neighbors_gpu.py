@@ -1,7 +1,6 @@
 """GPU tests of orbm_fuse_search_batch: every round of the lockstep SearchInNeighbors driver (tests/search_in_neighbors_lib.py) equals
 orbm_fuse_search item by item, byte for byte, with empty items mixed in; the batched lockstep run equals the per-call GPU chain and the
 oracle chain in final map state; one launch per call; the argument errors; the C++ mirror's digest equals the Python binding's."""
-import ctypes as C
 import os
 import subprocess
 
@@ -105,7 +104,6 @@ def test_bad_arguments_and_capacity(orb, g):
     items = [j['map'].fuse_item(j['map'].kfs[j['targets'][0]], [int(p) for p in j['map'].kfs[j['cur']].mp if p >= 0]) for j in jobs]
     m = orb.ORBmatcher(0.6, True, max_batch=1, max_keypoints=2048, max_mappoints=64)
     L = orb.lib()
-    L.orbm_fuse_search_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     m.fuse_search_batch(items)
     assert m.last_launch_count() == 1
     m.fuse_search_batch([_empty_items(items)[0]])

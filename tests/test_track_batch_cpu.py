@@ -1,6 +1,5 @@
 """CPU tests of the batched tracking calls' reference: the float32 pose hand-off against float64, and the oracle chain of
 tests/track_lib.py on planted scenes that reach every rule of Tracking's glue.  No GPU needed."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -80,8 +79,8 @@ def test_new_symbols_exported_and_no_silent_path():
              'orbm_track_local_map_batch_device', 'orbm_track_local_map_batch_resident')
     for n in names:
         assert hasattr(L, n), n
-        getattr(L, n).argtypes = [C.c_void_p] * 3
-        assert getattr(L, n)(None, None, None) == orb.ORB_ERR_ARG       # no handle: rejected before anything runs
+        fn = getattr(L, n)
+        assert fn(*[None] * len(fn.argtypes)) == orb.ORB_ERR_ARG       # no handle: rejected before anything runs
     if torch.cuda.is_available():
         pytest.skip('GPU present')
     with pytest.raises(orb.OrbError) as ei:

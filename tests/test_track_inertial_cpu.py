@@ -1,6 +1,5 @@
 """CPU tests of the mono-inertial tracking call's reference (tests/track_inertial_lib.py): the PredictStateIMU restatement against float64
 and the truth, the oracle chain on scenes that reach every rule of the glue, and no silent path without a device.  No GPU needed."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -78,7 +77,6 @@ def test_new_symbols_exported_and_no_silent_path():
     for n, nargs in (('orbm_track_local_map_inertial_batch', 5), ('orbm_track_local_map_inertial_batch_device', 6),
                      ('orbm_track_local_map_inertial_batch_resident', 5)):
         assert hasattr(L, n), n
-        getattr(L, n).argtypes = [C.c_void_p] * nargs
         assert getattr(L, n)(*[None] * nargs) == orb.ORB_ERR_ARG     # no handle: rejected before anything runs
     # without a device the handle these calls need cannot be made: creating it fails with ORB_ERR_CUDA, so nothing runs on the CPU
     if torch.cuda.is_available():

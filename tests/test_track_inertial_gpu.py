@@ -233,7 +233,6 @@ def test_bad_arguments_and_capacity(orb):
     r = orb._OrbmLocalMapResult(*[b.ctypes.data for b in bufs[:11]])
     ri = orb._OrbmImuTrackResult(*[b.ctypes.data for b in bufs[11:]])
     L = orb.lib()
-    L.orbm_track_local_map_inertial_batch.argtypes = [C.c_void_p] * 5
     assert L.orbm_track_local_map_inertial_batch(m._h, C.byref(s), C.byref(si), C.byref(r), C.byref(ri)) == orb.ORB_ERR_ARG
 
 

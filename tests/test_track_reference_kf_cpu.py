@@ -1,7 +1,6 @@
 """CPU tests of the reference-keyframe path's reference: the oracle chain of tests/track_ref_lib.py (bow_transform + search_by_bow +
 pose_optimization, then TrackLocalMap) on planted scenes, checked against a literal restatement that follows mnLastFrameSeen and
 mbTrackInView per map point through TrackWithMotionModel (when it failed) -> TrackReferenceKeyFrame -> SearchLocalPoints.  No GPU needed."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -121,8 +120,8 @@ def test_new_symbols_exported_and_no_silent_path():
     L = orb.lib()
     for n in ('orbm_track_reference_keyframe_batch', 'orbm_track_reference_keyframe_batch_device', 'orbm_track_reference_keyframe_batch_resident'):
         assert hasattr(L, n), n
-        getattr(L, n).argtypes = [C.c_void_p] * 4
-        assert getattr(L, n)(None, None, None, None) == orb.ORB_ERR_ARG
+        fn = getattr(L, n)
+        assert fn(*[None] * len(fn.argtypes)) == orb.ORB_ERR_ARG
     if torch.cuda.is_available():
         pytest.skip('GPU present')
     with pytest.raises(orb.OrbError) as ei:

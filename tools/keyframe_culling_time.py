@@ -81,7 +81,6 @@ def main():
         rows.append(dict(maps=n, oracle_ms=oracle_ms(flat_all[:n], max(3, a.reps // 4))))
     mt = orb.ORBmatcher(0.6, True, max_batch=1, max_keypoints=64, max_mappoints=64)   # raises without a GPU: no CPU path
     L = orb.lib()
-    L.orbm_keyframe_culling_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     for row in rows:
         n = row['maps']
         got = mt.keyframe_culling_batch(flat_all[:n])

@@ -14,7 +14,7 @@ e0,e1=torch.cuda.Event(enable_timing=True),torch.cuda.Event(enable_timing=True)
 e0.record(); opt.run_device(torch.cuda.current_stream().cuda_stream); e1.record(); torch.cuda.synchronize()
 out = opt.download()
 ns = np.zeros(10)
-L = orb.lib(); L.lba_get_phase_ns.argtypes=[C.c_void_p,C.c_int,C.c_void_p]
+L = orb.lib()
 L.lba_get_phase_ns(opt._h, 0, ns.ctypes.data_as(C.c_void_p))
 names=['errors(it0)','build_points','build_poses','point_prep','schur_partial','ldlt','schur_combine','pose_trial','points_trial','-']
 print('batch',n,'cluster',opt.last_cluster_size(),'kernel ms',e0.elapsed_time(e1),'iters',out[0]['iters'],'trials',out[0]['trials'])

@@ -61,7 +61,6 @@ def main():
         out = np.zeros(len(sc['kf1']['kps']), orb.NEW_POINT_DTYPE)
         cnt, a1, a2 = C.c_int(0), np.zeros(n, np.int32), np.zeros(n, np.int32)
         G = orb.lib()
-        G.orbm_create_new_map_points.argtypes = [C.c_void_p] * 6
         tg = median_time(lambda: G.orbm_create_new_map_points(m._h, C.byref(inp.s), out.ctypes.data, C.byref(cnt), a1.ctypes.data, a2.ctypes.data), a.reps)
         tc = median_time(lambda: L.orbo_create_new_map_points(C.byref(inp.s), out.ctypes.data, C.byref(cnt), a1.ctypes.data, a2.ctypes.data, None),
                          max(5, a.reps // 5), warm=1)
