@@ -582,6 +582,77 @@ typedef struct OrbmCullingMap {
     int32_t* visited;              /* [1] out: the reference's `count` when the loop ended */
 } OrbmCullingMap;
 int orbm_keyframe_culling_batch(orbm_handle* h, int nMaps, const OrbmCullingMap* maps);
+/* LocalMapping::ProcessNewKeyFrame's map-point loop followed by KeyFrame::UpdateConnections (mode ORBM_UC_PROCESS_NEW_KEYFRAME), or the
+ * tail of LocalMapping::SearchInNeighbors -- ComputeDistinctiveDescriptors and UpdateNormalAndDepth of every good point of the keyframe,
+ * then UpdateConnections (mode ORBM_UC_SEARCH_IN_NEIGHBORS) -- for several keyframes (monocular observations), one CTA per item.
+ * ONE upload through the handle's staging, ONE launch, ONE download; orbm_last_launch_count() is 1 (0 when every item has nSlots == 0).
+ * The caller replays the result on the host (INTEGRATION.md §2): AddObservation for ADDED slots, the point fields of updated points,
+ * mlpRecentAddedMapPoints for IN_KEYFRAME slots, the connection maps and lists, AddChild.
+ *
+ * Keyframe table [nKF]: entry 0 is the current keyframe, then every observer of its points and every keyframe in the connection maps of
+ * those observers.  `order` is the std::map key the reference iterates by ((uint64_t)KeyFrame*); keys are distinct.  Observations and
+ * connections are listed in key order.  connStart / connKF / connWeight: mConnectedKeyFrameWeights as CSR; only keyframes that can receive
+ * AddConnection (good observers of the same map) need theirs, the others may be empty.  Every keyframe shares the current keyframe's
+ * mvScaleFactors (one ORB extractor per map).
+ * Points [nPoints]: each point of the keyframe's slots once, with isBad(), GetWorldPos(), mpRefKF (a table index: one of its observers)
+ * and mObservations as CSR in key order (keyframe, keypoint index, that keypoint's octave and descriptor row).
+ * PRECONDITIONS: at most one keyframe per map per call; the items share no keyframe and no point.
+ * ORB_ERR_ARG before any launch: an index, an octave or a CSR offset out of range, a CSR not starting at 0 or decreasing, keys not
+ * distinct or a list not in key order, a good point whose mpRefKF is not among its observers, a null pointer the item needs, or a
+ * negative count.  ORB_ERR_CAPACITY: a point with more than 65534 observations. */
+enum { ORBM_UC_PROCESS_NEW_KEYFRAME = 0, ORBM_UC_SEARCH_IN_NEIGHBORS = 1 };
+enum {
+    ORBM_UC_SLOT_NONE = 0,           /* NULL or isBad() */
+    ORBM_UC_SLOT_ADDED = 1,          /* ProcessNewKeyFrame: AddObservation(KF, i), UpdateNormalAndDepth, ComputeDistinctiveDescriptors */
+    ORBM_UC_SLOT_IN_KEYFRAME = 2,    /* ProcessNewKeyFrame: IsInKeyFrame(KF), mlpRecentAddedMapPoints.push_back */
+    ORBM_UC_SLOT_UPDATED = 3         /* SearchInNeighbors: ComputeDistinctiveDescriptors, UpdateNormalAndDepth */
+};
+enum { ORBM_KF_OTHER_MAP = 8 };
+typedef struct OrbmConnectionsItem {
+    int mode;                      /* ORBM_UC_* */
+    int nKF;                       /* >= 1 */
+    const uint64_t* order;         /* [nKF] the key of std::map<KeyFrame*, ...> */
+    const uint64_t* mnId;          /* [nKF] */
+    const uint8_t* kfFlags;        /* [nKF] ORBM_KF_BAD, ORBM_KF_OTHER_MAP (GetMap() != the current keyframe's); entry 0: ORBM_KF_INIT when
+                                      mnId == mpMap->GetInitKFid() */
+    const float* cameraCenter;     /* [nKF][3] GetCameraCenter() */
+    const int32_t* connStart;      /* [nKF + 1] */
+    const int32_t* connKF;         /* [connStart[nKF]] table index, in key order */
+    const int32_t* connWeight;     /* [connStart[nKF]] */
+    int firstConnection;           /* mbFirstConnection of the current keyframe */
+    int nlevels;                   /* mnScaleLevels */
+    const float* scaleFactors;     /* [nlevels] mvScaleFactors */
+    int nSlots;                    /* N of the current keyframe */
+    const int32_t* slotPoint;      /* [nSlots] point index, -1 = NULL */
+    const int32_t* slotOctave;     /* [nSlots] mvKeysUn[i].octave */
+    const uint8_t* slotDesc;       /* [nSlots][32] mDescriptors.row(i) */
+    int nPoints;
+    const uint8_t* pointBad;       /* [nPoints] isBad() */
+    const float* pointPos;         /* [nPoints][3] GetWorldPos() */
+    const int32_t* pointRefKF;     /* [nPoints] mpRefKF */
+    const int32_t* obsStart;       /* [nPoints + 1] */
+    const int32_t* obsKF;          /* [obsStart[nPoints]] observing keyframe (table index), in key order */
+    const int32_t* obsIdx;         /* [obsStart[nPoints]] its keypoint index */
+    const int32_t* obsOctave;      /* [obsStart[nPoints]] that keypoint's octave */
+    const uint8_t* obsDesc;        /* [obsStart[nPoints]][32] that keypoint's descriptor row */
+    uint8_t* slotStatus;           /* [nSlots] out: ORBM_UC_SLOT_* */
+    uint8_t* pointUpdated;         /* [nPoints] out: UpdateNormalAndDepth and ComputeDistinctiveDescriptors ran on the point */
+    float* normal;                 /* [nPoints][3] out: mNormalVector of an updated point, 0 otherwise */
+    float* minDistance;            /* [nPoints] out: mfMinDistance of an updated point, 0 otherwise */
+    float* maxDistance;            /* [nPoints] out: mfMaxDistance of an updated point, 0 otherwise */
+    int32_t* descKF;               /* [nPoints] out: the keyframe of the row mDescriptor takes, -1 = unchanged */
+    int32_t* descIdx;              /* [nPoints] out: that keyframe's keypoint index */
+    int32_t* counter;              /* [nKF] out: KFcounter, the current keyframe's new mConnectedKeyFrameWeights (0 = absent) */
+    int32_t* nConnected;           /* [1] out: length of the ordered list; -1 = empty counter, UpdateConnections changed nothing */
+    int32_t* orderedKF;            /* [nKF] out: mvpOrderedConnectedKeyFrames, -1 past the end */
+    int32_t* orderedWeight;        /* [nKF] out: mvOrderedWeights */
+    int32_t* parent;               /* [1] out: the new mpParent (mbFirstConnection becomes false), -1 = unchanged */
+    int32_t* nbrCount;             /* [nKF] out: per keyframe, -1 = no AddConnection or an equal weight (nothing changed), else the length
+                                      of its new ordered list; its weight for the current keyframe is then counter[k] */
+    int32_t* nbrKF;                /* [connStart[nKF] + nKF] out: keyframe k's new ordered list at offset connStart[k] + k */
+    int32_t* nbrWeight;            /* [connStart[nKF] + nKF] out: its weights */
+} OrbmConnectionsItem;
+int orbm_update_connections_batch(orbm_handle* h, int nItems, const OrbmConnectionsItem* items);
 
 /* cv::BFMatcher(NORM_HAMMING).knnMatch(query, train, k=2) as used at src/Frame.cc:1144: idx/dist are Q x 2,
  * ordered by (distance, lower train index); missing neighbours are -1.  Q and T are unbounded.  Host pointers. */

@@ -215,6 +215,13 @@ public:
     void KeyFrameCullingBatch(const std::vector<OrbmCullingMap>& maps) {
         orb_check(orbm_keyframe_culling_batch(detail::matcher_handle(1, 1, device_), (int)maps.size(), maps.data()), "orbm_keyframe_culling_batch");
     }
+    // LocalMapping::ProcessNewKeyFrame's map-point loop or the tail of SearchInNeighbors, each followed by KeyFrame::UpdateConnections, for
+    // several keyframes of different maps in one launch (orbm_update_connections_batch).  Every item's outputs receive its result; the caller
+    // replays it on the host: AddObservation, the point fields, mlpRecentAddedMapPoints, the connection maps and lists, AddChild
+    // (INTEGRATION.md §2).
+    void UpdateConnectionsBatch(const std::vector<OrbmConnectionsItem>& items) {
+        orb_check(orbm_update_connections_batch(detail::matcher_handle(1, 1, device_), (int)items.size(), items.data()), "orbm_update_connections_batch");
+    }
     // cv::BFMatcher(NORM_HAMMING).knnMatch(query, train, matches, 2)
     void knnMatch(const Descriptors& query, const Descriptors& train, std::vector<int32_t>& idx, std::vector<int32_t>& dist) {
         idx.assign((size_t)query.rows * 2, -1); dist.assign((size_t)query.rows * 2, -1);

@@ -95,6 +95,7 @@ SIGNATURES = {
     'orbm_create_new_map_points': (_i, [_vp] * 6),
     'orbm_distinctive_descriptors': (_i, [_vp, _i, _vp, _vp, _vp]),
     'orbm_keyframe_culling_batch': (_i, [_vp, _i, _vp]),
+    'orbm_update_connections_batch': (_i, [_vp, _i, _vp]),
     'orbm_bf_knn2': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp]),
     'orbm_descriptor_distance': (_i, [_vp, _vp, _vp, _i, _vp]),
     'orbm_last_launch_count': (_i, [_vp]),
@@ -474,6 +475,55 @@ def culling_struct(m):
                        *[int(m[n]) for n in ('inertial', 'imuInitialized', 'inertialBA2', 'abortBA', 'keyFramesInMap')], int(m['currentId']),
                        int(m['lastId']), *[_ptr(out[n]) for n in ('status', 'nMPs', 'nRedundant', 'visited')])
     return s, out, a
+
+
+#: OrbmConnectionsItem's modes and slot statuses (ORBM_UC_*), and the keyframe flag of another map (include/orb_b200.h)
+UC_PROCESS_NEW_KEYFRAME, UC_SEARCH_IN_NEIGHBORS = 0, 1
+UC_SLOT_NONE, UC_SLOT_ADDED, UC_SLOT_IN_KEYFRAME, UC_SLOT_UPDATED = range(4)
+KF_OTHER_MAP = 8
+#: the arrays of one item of ORBmatcher.update_connections_batch, with their dtypes (OrbmConnectionsItem)
+CONNECTIONS_ARRAYS = (('order', np.uint64), ('mnId', np.uint64), ('kfFlags', np.uint8), ('cameraCenter', np.float32), ('connStart', np.int32),
+                      ('connKF', np.int32), ('connWeight', np.int32), ('scaleFactors', np.float32), ('slotPoint', np.int32), ('slotOctave', np.int32),
+                      ('slotDesc', np.uint8), ('pointBad', np.uint8), ('pointPos', np.float32), ('pointRefKF', np.int32), ('obsStart', np.int32),
+                      ('obsKF', np.int32), ('obsIdx', np.int32), ('obsOctave', np.int32), ('obsDesc', np.uint8))
+CONNECTIONS_SCALARS = ('mode', 'firstConnection')
+#: its outputs, with their dtypes
+CONNECTIONS_OUTPUTS = (('slotStatus', np.uint8), ('pointUpdated', np.uint8), ('normal', np.float32), ('minDistance', np.float32),
+                       ('maxDistance', np.float32), ('descKF', np.int32), ('descIdx', np.int32), ('counter', np.int32), ('nConnected', np.int32),
+                       ('orderedKF', np.int32), ('orderedWeight', np.int32), ('parent', np.int32), ('nbrCount', np.int32), ('nbrKF', np.int32),
+                       ('nbrWeight', np.int32))
+
+
+class OrbmConnectionsItem(C.Structure):
+    """One keyframe of orbm_update_connections_batch (include/orb_b200.h)."""
+    _fields_ = [('mode', C.c_int), ('nKF', C.c_int)] + \
+               [(n, C.c_void_p) for n in ('order', 'mnId', 'kfFlags', 'cameraCenter', 'connStart', 'connKF', 'connWeight')] + \
+               [('firstConnection', C.c_int), ('nlevels', C.c_int), ('scaleFactors', C.c_void_p), ('nSlots', C.c_int)] + \
+               [(n, C.c_void_p) for n in ('slotPoint', 'slotOctave', 'slotDesc')] + [('nPoints', C.c_int)] + \
+               [(n, C.c_void_p) for n in ('pointBad', 'pointPos', 'pointRefKF', 'obsStart', 'obsKF', 'obsIdx', 'obsOctave', 'obsDesc')] + \
+               [(n, C.c_void_p) for n, _ in CONNECTIONS_OUTPUTS]
+
+
+def connections_struct(m):
+    """OrbmConnectionsItem over item dict `m` (keys CONNECTIONS_ARRAYS + CONNECTIONS_SCALARS) with fresh outputs: (struct, out dict, arrays
+    to keep alive).  Outputs: slotStatus [nSlots], pointUpdated / minDistance / maxDistance / descKF / descIdx [nPoints], normal [nPoints, 3],
+    counter / orderedKF / orderedWeight / nbrCount [nKF], nConnected / parent [1], nbrKF / nbrWeight [connStart[-1] + nKF]."""
+    a = {n: (_c(m[n], dt) if m.get(n) is not None else None) for n, dt in CONNECTIONS_ARRAYS}
+    nK, nS, nP = len(a['order']), len(a['slotPoint']), len(a['pointBad'])
+    a['cameraCenter'] = a['cameraCenter'].reshape(-1, 3)
+    sizes = dict(slotStatus=nS, pointUpdated=nP, normal=(nP, 3), minDistance=nP, maxDistance=nP, descKF=nP, descIdx=nP, counter=nK, nConnected=1,
+                 orderedKF=nK, orderedWeight=nK, parent=1, nbrCount=nK, nbrKF=int(a['connStart'][-1]) + nK, nbrWeight=int(a['connStart'][-1]) + nK)
+    out = {n: np.zeros(sizes[n], dt) for n, dt in CONNECTIONS_OUTPUTS}
+    s = OrbmConnectionsItem(int(m['mode']), nK, *[_ptr(a[n]) for n in ('order', 'mnId', 'kfFlags', 'cameraCenter', 'connStart', 'connKF', 'connWeight')],
+                            int(m['firstConnection']), len(a['scaleFactors']), _ptr(a['scaleFactors']), nS,
+                            *[_ptr(a[n]) for n in ('slotPoint', 'slotOctave', 'slotDesc')], nP,
+                            *[_ptr(a[n]) for n in ('pointBad', 'pointPos', 'pointRefKF', 'obsStart', 'obsKF', 'obsIdx', 'obsOctave', 'obsDesc')],
+                            *[_ptr(out[n]) for n, _ in CONNECTIONS_OUTPUTS])
+    return s, out, a
+
+
+def _connections_result(out):
+    return dict(out, nConnected=int(out['nConnected'][0]), parent=int(out['parent'][0]))
 
 
 def _c(a, dt):
@@ -996,6 +1046,20 @@ class ORBmatcher:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_keyframe_culling_batch')
         return [dict(b[1], visited=int(b[1]['visited'][0])) for b in built]
+
+    def update_connections_batch(self, items):
+        """``LocalMapping::ProcessNewKeyFrame``'s map-point loop (mode UC_PROCESS_NEW_KEYFRAME) or the tail of ``SearchInNeighbors`` (mode
+        UC_SEARCH_IN_NEIGHBORS), each followed by ``KeyFrame::UpdateConnections``, for several keyframes in one launch
+        (orbm_update_connections_batch).  Each item is a dict with the arrays of ``CONNECTIONS_ARRAYS`` (the keyframe table, current keyframe
+        first; its slots; the points and their observations in CSR form, key order) and the scalars of ``CONNECTIONS_SCALARS``.  Returns, per
+        item, the outputs of :func:`connections_struct` with ``nConnected`` and ``parent`` as ints; the caller replays them on the host
+        (INTEGRATION.md §2).  At most one keyframe per map, and the items share no keyframe or point (see include/orb_b200.h)."""
+        built = [connections_struct(m) for m in items]
+        arr = (OrbmConnectionsItem * max(len(items), 1))(*[b[0] for b in built])
+        rc = lib().orbm_update_connections_batch(self._h, len(items), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_update_connections_batch')
+        return [_connections_result(b[1]) for b in built]
 
     def ComputeDistinctiveDescriptors(self, obs_list):
         """``MapPoint::ComputeDistinctiveDescriptors`` for a list of map points (each an [n, 32] u8 array of observed descriptors): index of the chosen row."""

@@ -113,6 +113,35 @@ __device__ __forceinline__ int hamming256(const uint32_t* a, const uint32_t* b) 
     return d;
 }
 
+// MapPoint::ComputeDistinctiveDescriptors' choice (src/MapPoint.cc:329-403) among n <= 65535 rows, for one warp: lane l takes rows
+// l, l + 32, ...; row(j) gives the address of row j (32 bytes, 16-byte aligned, not written by the kernel).  Every lane returns the first
+// row with the least median distance to the others; the median (element (int)(0.5 (n - 1)) of the sorted row) is found by bisection on the
+// distance value.  Used by distinctive_kernel and update_connections_kernel.
+template <class Row>
+__device__ __forceinline__ int distinctive_best(int n, int lane, Row row) {
+    const int k = (int)(0.5 * (double)(n - 1));
+    unsigned bestKey = 0xFFFFFFFFu;
+    for (int i = lane; i < n; i += 32) {
+        const uint4* pi = reinterpret_cast<const uint4*>(row(i));
+        const uint4 x0 = __ldg(pi), x1 = __ldg(pi + 1);
+        const uint32_t di[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+        int lo = 0, hi = 256;                                    // smallest v with #{j : d(i, j) <= v} >= k + 1
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            int cnt = 0;
+            for (int j = 0; j < n; ++j) {
+                const uint4* pj = reinterpret_cast<const uint4*>(row(j));
+                const uint4 y0 = __ldg(pj), y1 = __ldg(pj + 1);
+                const uint32_t dj[8] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y, y1.z, y1.w};
+                cnt += (i == j ? 0 : hamming256(di, dj)) <= mid;
+            }
+            if (cnt >= k + 1) hi = mid; else lo = mid + 1;
+        }
+        bestKey = min(bestKey, ((unsigned)lo << 16) | (unsigned)i);
+    }
+    return (int)(__reduce_min_sync(0xffffffffu, bestKey) & 0xFFFFu);
+}
+
 // Wait for a stream from a host thread that has nothing else to do: through an event created with cudaEventBlockingSync the thread sleeps
 // instead of spinning in cudaStreamSynchronize (a server runs several such threads per GPU and several GPUs per host; spinning threads
 // take the cores the other ranks' threads need).  Used by the BATCH host entry points; single-frame calls keep the low-latency spin.

@@ -1212,36 +1212,16 @@ __global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsPara
 }
 
 // ---------------------------------------------------------------------------------------------
-// MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:329-403) for a batch of map points: warp per map point, lane per observation row;
-// the row's median distance (element (int)(0.5 (n - 1)) of the sorted row) by bisection on the distance value; first minimum wins.
+// MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:329-403) for a batch of map points: warp per map point, lane per observation row
+// (distinctive_best, device_utils.cuh).
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) distinctive_kernel(int nPoints, const int* __restrict__ ptStart, const uint8_t* __restrict__ desc, int* __restrict__ best) {
     const int p = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (p >= nPoints) return;
     const int a = ptStart[p], n = ptStart[p + 1] - a;
     if (n <= 0) { if (lane == 0) best[p] = -1; return; }
-    const int k = (int)(0.5 * (double)(n - 1));
-    unsigned bestKey = 0xFFFFFFFFu;
-    for (int i = lane; i < n; i += 32) {
-        const uint4* pi = reinterpret_cast<const uint4*>(desc + (size_t)(a + i) * 32);
-        const uint4 x0 = __ldg(pi), x1 = __ldg(pi + 1);
-        const uint32_t di[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-        int lo = 0, hi = 256;                                    // smallest v with #{j : d(i, j) <= v} >= k + 1
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            int cnt = 0;
-            for (int j = 0; j < n; ++j) {
-                const uint4* pj = reinterpret_cast<const uint4*>(desc + (size_t)(a + j) * 32);
-                const uint4 y0 = __ldg(pj), y1 = __ldg(pj + 1);
-                const uint32_t dj[8] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y, y1.z, y1.w};
-                cnt += (i == j ? 0 : hamming256(di, dj)) <= mid;
-            }
-            if (cnt >= k + 1) hi = mid; else lo = mid + 1;
-        }
-        bestKey = min(bestKey, ((unsigned)lo << 16) | (unsigned)i);
-    }
-    bestKey = __reduce_min_sync(0xffffffffu, bestKey);
-    if (lane == 0) best[p] = (int)(bestKey & 0xFFFFu);
+    const int b = distinctive_best(n, lane, [&](int j) { return desc + (size_t)(a + j) * 32; });
+    if (lane == 0) best[p] = b;
 }
 
 // cv::BFMatcher(NORM_HAMMING).knnMatch(k=2): warp per query, lanes over train rows
