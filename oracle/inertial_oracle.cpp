@@ -241,7 +241,7 @@ static bool invert(int n, const double* A, double* out) {   // Gauss-Jordan with
     for (int c = 0; c < n; ++c) {
         int piv = c;
         for (int r = c + 1; r < n; ++r) if (std::fabs(M[r * 2 * n + c]) > std::fabs(M[piv * 2 * n + c])) piv = r;
-        if (M[piv * 2 * n + c] == 0) return false;
+        if (M[piv * 2 * n + c] == 0) { for (int i = 0; i < n * n; ++i) out[i] = NAN; return false; }   // PartialPivLU divides by the zero pivot: not finite
         if (piv != c) for (int j = 0; j < 2 * n; ++j) std::swap(M[c * 2 * n + j], M[piv * 2 * n + j]);
         const double inv = 1.0 / M[c * 2 * n + c];
         for (int j = 0; j < 2 * n; ++j) M[c * 2 * n + j] *= inv;

@@ -303,7 +303,8 @@ extern "C" {
 //   mono edge e: point ePt[e], keyframe eKf[e], obs2, invSigma2; trackDepth [nL] = pMP->mTrackDepth.
 //   eraseOut [nE]: the (keyframe, point) pairs of vToErase; edgeChi2Out [nE].
 //   stats [8]: err, err_end (as the reference's floats), failed, final lambda, LM trials, outer iterations.
-// Returns optimize()'s iteration count.  When the FAIL test fires the states and points are left as they came in (the reference returns before the write-back).
+// Returns optimize()'s iteration count.  When the FAIL test fires the states and points are left as they came in and eraseOut is all zero (the reference
+// returns before the erasure and the write-back).
 int orbo_local_inertial_ba(int nKF, int nOpt, double* kfState21, double* kfTcw12, const float* cam4, const double* extr24, int nI, const int* ieKf1, const int* ieKf2,
                            const float* preint, const uint8_t* ieRobust, const double* ieInfoScale, int nL, double* points3, const float* trackDepth, int nE,
                            const int* ePt, const int* eKf, const double* obs2, const float* invSigma2, int iterations, double lambdaInit, int bLarge,
@@ -408,7 +409,8 @@ int orbo_local_inertial_ba(int nKF, int nOpt, double* kfState21, double* kfTcw12
         eraseOut[e] = ((c2 > chi2Mono2 && !bClose) || (c2 > 1.5f * chi2Mono2 && bClose) || !depthPos) ? 1 : 0;
     }
     const bool failed = (2 * err < errEnd || std::isnan(err) || std::isnan(errEnd)) && !bLarge;
-    if (failed) { L.kf = kf0; L.pts = pts0; }
+    // on FAIL the reference returns before it erases any observation (:2884-2888): no flag is set
+    if (failed) { L.kf = kf0; L.pts = pts0; if (nE) std::memset(eraseOut, 0, (size_t)nE); }
     for (int k = 0; k < nKF; ++k) {
         double* s = kfState21 + 21 * (size_t)k;
         const KF& f = L.kf[k];

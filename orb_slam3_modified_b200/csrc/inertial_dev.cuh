@@ -108,13 +108,15 @@ template <class T> IMU_HD inline void normalize_rotation(const T* R, T* out) {
 
 // ---- information matrices: inverse of the covariance blocks (Gauss-Jordan with partial pivoting, like Eigen's PartialPivLU inverse),
 //      symmetrised, eigenvalues below 1e-12 clamped to zero (cyclic Jacobi eigen-decomposition) ----
+// On an exactly zero pivot (a singular matrix, e.g. the covariance of an interval with one IMU sample) the result is all NaN and false is
+// returned: PartialPivLU's inverse divides by that pivot, so the reference's information matrix is not finite either.
 template <int N> IMU_HD inline bool invert_n(const double* A, double* out) {
     double M[N * 2 * N];
     for (int i = 0; i < N; ++i) for (int j = 0; j < N; ++j) { M[i * 2 * N + j] = A[i * N + j]; M[i * 2 * N + N + j] = i == j ? 1.0 : 0.0; }
     for (int c = 0; c < N; ++c) {
         int piv = c;
         for (int r = c + 1; r < N; ++r) if (fabs(M[r * 2 * N + c]) > fabs(M[piv * 2 * N + c])) piv = r;
-        if (M[piv * 2 * N + c] == 0) return false;
+        if (M[piv * 2 * N + c] == 0) { for (int i = 0; i < N * N; ++i) out[i] = NAN; return false; }
         if (piv != c) for (int j = 0; j < 2 * N; ++j) { const double t = M[c * 2 * N + j]; M[c * 2 * N + j] = M[piv * 2 * N + j]; M[piv * 2 * N + j] = t; }
         const double inv = 1.0 / M[c * 2 * N + c];
         for (int j = 0; j < 2 * N; ++j) M[c * 2 * N + j] *= inv;

@@ -113,8 +113,9 @@ IMU_HD inline void inv3_cof(const double* m, double* o) {                       
 // of its eigen-decomposition.  The eigen step only changes the matrix when an eigenvalue is below 1e-12.  lambda_min(Info) = 1 / lambda_max(C) >=
 // 1 / trace(C), so for a positive definite Info (Cholesky succeeds) and trace(C) < 1e11 nothing is clamped and V diag(w) V^T reproduces the
 // symmetrised inverse up to rounding: the serial Jacobi sweeps (~3 ms on one thread) are then skipped.  Otherwise the full path runs.
-IMU_HD inline void information_matrices(const float* __restrict__ P, double* __restrict__ I9, double* __restrict__ IG, double* __restrict__ IA) {
-    double C9[81], A[81], Lc[81];
+// information_fast_path: that test; true leaves the symmetrised inverse in A.
+IMU_HD inline bool information_fast_path(const float* __restrict__ P, double* __restrict__ A) {
+    double C9[81], Lc[81];
     double trace = 0;
     for (int i = 0; i < 9; ++i) for (int j = 0; j < 9; ++j) C9[i * 9 + j] = (double)P[P_C + i * 15 + j];
     for (int i = 0; i < 9; ++i) trace += C9[i * 10];
@@ -134,7 +135,11 @@ IMU_HD inline void information_matrices(const float* __restrict__ P, double* __r
             }
         }
     }
-    if (!ok) { imu_information_dev(P, I9, IG, IA); return; }
+    return ok;
+}
+IMU_HD inline void information_matrices(const float* __restrict__ P, double* __restrict__ I9, double* __restrict__ IG, double* __restrict__ IA) {
+    double A[81];
+    if (!information_fast_path(P, A)) { imu_information_dev(P, I9, IG, IA); return; }
     for (int i = 0; i < 81; ++i) I9[i] = A[i];
     double G[9], Aa[9];
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) { G[i * 3 + j] = (double)P[P_C + (9 + i) * 15 + 9 + j]; Aa[i * 3 + j] = (double)P[P_C + (12 + i) * 15 + 12 + j]; }

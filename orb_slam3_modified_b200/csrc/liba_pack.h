@@ -26,6 +26,7 @@ inline size_t bump(size_t& off, size_t bytes) { const size_t at = off; off = (of
 // returns an error text ("" = ok)
 inline std::string check(const LocalInertialBAProblem& p) {
     if (p.nKF < 1 || p.nOpt < 0 || p.nOpt > p.nKF || p.nInertial < 0 || p.nPoints < 0 || p.nEdges < 0 || p.iterations < 0) return "LocalInertialBA: negative or inconsistent sizes";
+    if (p.nOpt < 1) return "LocalInertialBA: empty temporal window (the reference's window always holds the current keyframe)";
     if (p.nOpt > 64) return "LocalInertialBA: more than 64 keyframes in the temporal window";
     if (!p.kfState21 || !p.kfTcw12 || !p.cam4 || !p.extrinsics24) return "LocalInertialBA: null keyframe arrays";
     if (p.nInertial && (!p.ieKf1 || !p.ieKf2 || !p.preint || !p.ieRobust || !p.ieInfoScale)) return "LocalInertialBA: null inertial-edge arrays";

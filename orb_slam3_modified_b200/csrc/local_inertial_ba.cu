@@ -1,5 +1,5 @@
 // Optimizer::LocalInertialBA (reference src/Optimizer.cc:2383-2958; SURVEY.md 8f rank 1) on the H100: local_inertial_ba_batch.
-// One persistent CTA (256 threads) per local map runs the whole g2o Levenberg-Marquardt loop of liba_core.cuh on the device; a batch
+// One persistent CTA (NT = 512 threads) per local map runs the whole g2o Levenberg-Marquardt loop of liba_core.cuh on the device; a batch
 // of maps (one per stream of a multi-stream server) fills the SMs.  The host side flattens the graph (liba_pack.h: layout, CSR lists),
 // uploads one packed input buffer, launches ONE kernel and downloads one packed output buffer.
 //

@@ -48,6 +48,12 @@ extern "C" int liba_emulate(const LocalInertialBAProblem* p, const LocalInertial
     return liba::unpack_outputs(*p, *r, L, out.data());
 }
 
+// Whether information_matrices takes its fast path (no Jacobi sweeps) for one IMU::Preintegrated record.
+extern "C" int liba_information_fast_path(const float* P) {
+    double A[81];
+    return liba::information_fast_path(P, A) ? 1 : 0;
+}
+
 // The batch form of the host side (layout, threaded packing into ONE staging buffer, per-problem views) followed by the serial executor per map.
 extern "C" int liba_emulate_batch(int count, const LocalInertialBAProblem* p, const LocalInertialBAResult* r, int* iterations, char* errText, int errCap) {
     std::vector<liba::Layout> lay(count);

@@ -151,7 +151,7 @@ def test_local_inertial_ba_from_initialize_to_the_fail_test():
         seen_fail |= want['failed']
         if not want['failed']:
             assert np.array_equal(erase, want['erase']) and st.tobytes() == want['state'].tobytes()
-        else:                                                # the oracle hands the inputs back and clears the flags on FAIL; the text computed its vToErase before returning
+        else:                                                # on FAIL the text returns before it erases (:2884-2888): the oracle hands the inputs back and sets no flag
             assert np.array_equal(want['state'], pr['state']) and want['erase'].sum() == 0
     assert seen_fail
 
