@@ -25,6 +25,7 @@
 #include <string.h>
 #include <algorithm>
 #include <atomic>
+#include <new>
 #include <string>
 #include <thread>
 #include <vector>
@@ -101,23 +102,37 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long l
 #ifndef LBA_UNR
 #define LBA_UNR 4
 #endif
-#ifndef LBA_FLY
-#define LBA_FLY 1      /* items in flight per lane in the per-edge passes (build_points, build_poses, points_trial) */
+/* items in flight per lane in the per-edge passes: points per 8-lane group and step (build_points, points_trial), edges per
+   lane of a build_poses chunk */
+#ifndef LBA_FLY_BP
+#define LBA_FLY_BP 2
+#endif
+#ifndef LBA_FLY_BPP
+#define LBA_FLY_BPP 2
+#endif
+#ifndef LBA_FLY_PT
+#define LBA_FLY_PT 1
 #endif
 constexpr int NT = LBA_NT;
 constexpr int NWARP = NT / 32;
-constexpr int FLY = LBA_FLY;
+constexpr int FLY_BP = LBA_FLY_BP, FLY_BPP = LBA_FLY_BPP, FLY_PT = LBA_FLY_PT;
 constexpr int MAXC = 8;            // largest cluster
 constexpr int PSLOT = 24;          // doubles per partial slot: A[0..7], flag[8], B[9..16]
 constexpr int PC = 20;             // doubles per cached pose: q(4) t(3) R(9) fx fy cx cy
 
+// The thread's place in the cluster is read from the special registers where a phase starts (asm volatile, so that the
+// compiler does not merge the reads into one value held in registers across every phase)
+__device__ __forceinline__ int sreg_ctarank() { int r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ int sreg_nctarank() { int r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
 struct Ctx {
-    int crank, csize, tid;
-    int wid, nw;           // worker id / count over the cluster
     int slot;              // rotating partial slot
     double* sm;            // NT doubles of scratch
     const double* pc;      // pose cache in shared memory (state at the linearisation point), PC doubles per pose
-    const double* pts;     // point estimates of that state
+    __device__ __forceinline__ int crank() const { return sreg_ctarank(); }
+    __device__ __forceinline__ int csize() const { return sreg_nctarank(); }
+    __device__ __forceinline__ int tid() const { return (int)threadIdx.x; }
+    __device__ __forceinline__ int wid() const { return sreg_ctarank() * NT + (int)threadIdx.x; }   // worker id / count over the cluster
+    __device__ __forceinline__ int nw() const { return sreg_nctarank() * NT; }
 };
 
 // cluster-wide ordered sum (per-CTA partials -> global slot -> cluster barrier -> added in rank order by every thread);
@@ -125,13 +140,13 @@ struct Ctx {
 __device__ __forceinline__ double cluster_sum(const Dev& D, Ctx& c, double local, int flagIn, int& flagOut) {
     const double s = block_sum<NT>(local, c.sm);
     double* slot = D.partial + (size_t)(c.slot & 3) * PSLOT;
-    if (c.tid == 0) {
-        slot[c.crank] = s;
-        if (c.crank == 0) slot[MAXC] = (double)flagIn;
+    if (c.tid() == 0) {
+        slot[c.crank()] = s;
+        if (c.crank() == 0) slot[MAXC] = (double)flagIn;
     }
     cg::this_cluster().sync();
     double tot = 0;
-    for (int r = 0; r < c.csize; ++r) tot += slot[r];
+    for (int r = 0; r < c.csize(); ++r) tot += slot[r];
     flagOut = (int)slot[MAXC];
     ++c.slot;
     return tot;
@@ -147,12 +162,12 @@ __device__ __forceinline__ void cluster_sum2(const Dev& D, Ctx& c, double a, dou
     if (tid == 0) {
         double ra = 0, rb = 0;
         for (int w = 0; w < NWARP; ++w) { ra += c.sm[w]; rb += c.sm[NWARP + w]; }
-        slot[c.crank] = ra; slot[MAXC + 1 + c.crank] = rb;
-        if (c.crank == 0) slot[MAXC] = (double)flagIn;
+        slot[c.crank()] = ra; slot[MAXC + 1 + c.crank()] = rb;
+        if (c.crank() == 0) slot[MAXC] = (double)flagIn;
     }
     cg::this_cluster().sync();
     totA = 0; totB = 0;
-    for (int r = 0; r < c.csize; ++r) { totA += slot[r]; totB += slot[MAXC + 1 + r]; }
+    for (int r = 0; r < c.csize(); ++r) { totA += slot[r]; totB += slot[MAXC + 1 + r]; }
     flagOut = (int)slot[MAXC];
     ++c.slot;
 }
@@ -196,10 +211,11 @@ __device__ __forceinline__ double edge_error(const Dev& D, const double* P, cons
 }
 // ---- residuals + robust chi2 (SparseOptimizer::computeActiveErrors + activeRobustChi2), thread per edge.
 //      Also leaves the edge factors (x/z, y/z, 1/z, rho' / sigma^2) of this state in Eout. ----
-__device__ double phase_errors(const Dev& D, const Ctx& c, double* __restrict__ Eout) {
+__device__ double phase_errors(const Dev& D, const Ctx& c, const double* pts, double* __restrict__ Eout) {
     double acc = 0;
-    for (int e = c.wid; e < D.nE; e += c.nw)
-        acc += edge_error(D, c.pc + PC * ro(D.ePose + e), c.pts + 3 * (size_t)ro(D.ePt + e), e, ro_obs(D, e), (double)ro(D.invSigma2 + e), Eout);
+    const int nw = c.nw();
+    for (int e = c.wid(); e < D.nE; e += nw)
+        acc += edge_error(D, c.pc + PC * ro(D.ePose + e), pts + 3 * (size_t)ro(D.ePt + e), e, ro_obs(D, e), (double)ro(D.invSigma2 + e), Eout);
     return acc;
 }
 
@@ -263,6 +279,7 @@ __device__ __forceinline__ void point_record(const Dev& D, int p, const double* 
 // a step first issues the loads of the lane's first edge of each of its points, then adds the points one after another,
 // each with the same per-lane order (edges sl, sl + 8, ...) and the same shuffle tree as one point per step.  The next step's
 // ptStart entries are loaded ahead.
+template <int FLY>
 __device__ __forceinline__ void step_ranges(const int* ptStart, int nL, int p, int G, int* a, int* b) {
 #pragma unroll
     for (int j = 0; j < FLY; ++j) {
@@ -294,17 +311,18 @@ __device__ __forceinline__ void add_build_edge(const double* pcache, const Build
 // ---- per point Hll, bl (and, when lambda is already known, the point record of phase_point_prep); 8 lanes per point
 //      (the edges of a point are contiguous) ----
 __device__ void phase_build_points(const Dev& D, const Ctx& c, const double* __restrict__ E, double lambda) {
-    const int sl = c.tid & 7;
-    const unsigned gmask = 0xFFu << (c.tid & 24);
-    const int G = c.nw >> 3;
+    constexpr int FLY = FLY_BP;
+    const int sl = c.tid() & 7;
+    const unsigned gmask = 0xFFu << (c.tid() & 24);
+    const int G = c.nw() >> 3;
     int a[FLY], b[FLY];
-    step_ranges(D.ptStart, D.nL, c.wid >> 3, G, a, b);
-    for (int p0 = c.wid >> 3; p0 < D.nL; p0 += FLY * G) {
+    step_ranges<FLY>(D.ptStart, D.nL, c.wid() >> 3, G, a, b);
+    for (int p0 = c.wid() >> 3; p0 < D.nL; p0 += FLY * G) {
         BuildEdge first[FLY] = {};
 #pragma unroll
         for (int j = 0; j < FLY; ++j) if (a[j] + sl < b[j]) first[j] = load_build_edge(D, E, a[j] + sl);
         int na[FLY], nb[FLY];
-        step_ranges(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
+        step_ranges<FLY>(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
 #pragma unroll
         for (int j = 0; j < FLY; ++j) {
             const int p = p0 + j * G;
@@ -342,9 +360,10 @@ constexpr int UNR = LBA_UNR;       // items in flight per lane in the Schur chun
 //      As in the Schur chunks, the chunk's edge ids are loaded into registers up front; then the factors and errors of FLY
 //      items per lane are loaded before their K stores and their sums, which keep the item order of the lane. ----
 __device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const double* __restrict__ E) {
-    const int lane = c.tid & 31;
-    const int nDiag = D.taskChunkStart[D.nF];
-    for (int ch = c.crank * NWARP + (c.tid >> 5); ch < nDiag; ch += c.csize * NWARP) {
+    constexpr int FLY = FLY_BPP;
+    const int lane = c.tid() & 31;
+    const int nDiag = D.taskChunkStart[D.nF], step = c.csize() * NWARP;
+    for (int ch = c.crank() * NWARP + (c.tid() >> 5); ch < nDiag; ch += step) {
         const int4 h = D.chunkHdr[ch];
         const double* P = c.pc + PC * h.z;
         const double fx = P[16], fy = P[17];
@@ -397,7 +416,8 @@ __device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const doub
     }
 }
 __device__ void phase_build_poses_combine(const Dev& D, const Ctx& c) {
-    for (int idx = c.wid; idx < D.nF * 27; idx += c.nw) {
+    const int nw = c.nw();
+    for (int idx = c.wid(); idx < D.nF * 27; idx += nw) {
         const int hI = idx / 27, ent = idx - hI * 27;
         double s = 0;
         for (int ch = D.taskChunkStart[hI]; ch < D.taskChunkStart[hI + 1]; ++ch) s += D.Ppart[28 * (size_t)ch + ent];
@@ -413,12 +433,12 @@ __device__ void phase_build_poses_combine(const Dev& D, const Ctx& c) {
 // ---- max |diag| over all Hessian blocks (computeLambdaInit); every CTA computes it redundantly ----
 __device__ double phase_maxdiag(const Dev& D, const Ctx& c) {
     double m = 0;
-    for (int i = c.tid; i < D.n; i += NT) m = fmax(m, fabs(D.Hpp[36 * (size_t)(i / 6) + 7 * (i % 6)]));
-    for (int i = c.tid; i < 3 * D.nL; i += NT) { const int k = i % 3; m = fmax(m, fabs(D.Hll[6 * (size_t)(i / 3) + (k == 0 ? 0 : k == 1 ? 3 : 5)])); }
+    for (int i = c.tid(); i < D.n; i += NT) m = fmax(m, fabs(D.Hpp[36 * (size_t)(i / 6) + 7 * (i % 6)]));
+    for (int i = c.tid(); i < 3 * D.nL; i += NT) { const int k = i % 3; m = fmax(m, fabs(D.Hll[6 * (size_t)(i / 3) + (k == 0 ? 0 : k == 1 ? 3 : 5)])); }
 #pragma unroll
     for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
     __syncthreads();
-    if ((c.tid & 31) == 0) c.sm[c.tid >> 5] = m;
+    if ((c.tid() & 31) == 0) c.sm[c.tid() >> 5] = m;
     __syncthreads();
     double r = 0;
     for (int w = 0; w < NWARP; ++w) r = fmax(r, c.sm[w]);
@@ -446,7 +466,8 @@ __device__ __forceinline__ void load_dinv(const double2* __restrict__ PT, size_t
     dv[0] = a.x; dv[1] = a.y; dv[2] = b.x; dv[3] = b.y; dv[4] = c.x; dv[5] = c.y;
 }
 __device__ void phase_point_prep(const Dev& D, const Ctx& c, double lambda) {
-    for (int p = c.wid; p < D.nL; p += c.nw) {
+    const int nw = c.nw();
+    for (int p = c.wid(); p < D.nL; p += nw) {
         const double2* H = reinterpret_cast<const double2*>(D.Hll + 6 * (size_t)p);
         const double2 h01 = H[0], h23 = H[1], h45 = H[2];
         const double h[6] = {h01.x, h01.y, h23.x, h23.y, h45.x, h45.y};
@@ -573,7 +594,8 @@ __device__ void phase_schur_partial(const Dev& D, const Ctx& c, const double2* _
     // CTA barrier at entry: the previous phase (combine of the pose sums) leaves the warps of a CTA out of step, and warps that
     // enter this gather-bound phase out of step ran it 3x slower (measured); a barrier per round of chunks on top was slower again.
     __syncthreads();
-    for (int ch = c.crank * NWARP + (c.tid >> 5); ch < D.nChunks; ch += c.csize * NWARP) {
+    const int step = c.csize() * NWARP;
+    for (int ch = c.crank() * NWARP + (c.tid() >> 5); ch < D.nChunks; ch += step) {
         const int4 h = D.chunkHdr[ch];      // first item, items, pose A, pose B (-1: diagonal task)
         if (h.w >= 0) schur_chunk_offdiag(D.pairs, D.pairPt, D.PT, D.nL, K, D.nE, c.pc, D.Spart + 42 * (size_t)ch, h);
         else schur_chunk_diag(D.poseEdgePt, D.PT, D.nL, K, D.nE, c.pc, D.Spart + 42 * (size_t)ch, h);
@@ -581,7 +603,8 @@ __device__ void phase_schur_partial(const Dev& D, const Ctx& c, const double2* _
 }
 __device__ void phase_schur_combine(const Dev& D, const Ctx& c, double lambda, double* Hs, int ld) {
     const int nOff = D.nF * (D.nF - 1) / 2, nTasks = D.nF + nOff;
-    for (int idx = c.wid; idx < nTasks * 42; idx += c.nw) {
+    const int nw = c.nw();
+    for (int idx = c.wid(); idx < nTasks * 42; idx += nw) {
         const int task = idx / 42, ent = idx - task * 42;
         if (task >= D.nF && ent >= 36) continue;
         double s = 0;
@@ -641,7 +664,7 @@ __device__ __forceinline__ void ldlt_factor6(double* A, int ld, int k0, double* 
     if (bad) *sFail = 1;
 }
 __device__ int phase_ldlt(const Dev& D, const Ctx& c, double* A, int ld, double* scratch, double* brow) {
-    const int n = D.n, tid = c.tid, lane = tid & 31, warp = tid >> 5;
+    const int n = D.n, tid = c.tid(), lane = tid & 31, warp = tid >> 5;
     const int n1 = n + 1;
     double* Xs = scratch;               // 6 x (n + 1): unscaled panel, column-major by panel column (conflict-free for lanes over rows)
     double* Ls = scratch + 6 * n1;      // 6 x (n + 1): scaled panel (= the final L entries)
@@ -744,7 +767,8 @@ __device__ int phase_ldlt(const Dev& D, const Ctx& c, double* A, int ld, double*
 //      residuals); CTA 0 also writes them to the trial buffer and returns the poses' share of computeScale ----
 __device__ double phase_pose_trial(const Dev& D, const Ctx& c, const double* __restrict__ Pcur, double* __restrict__ Ptr, double* pcTr, double lambda) {
     double acc = 0;
-    for (int v = c.tid; v < D.nP; v += NT) {
+    const bool rank0 = c.crank() == 0;
+    for (int v = c.tid(); v < D.nP; v += NT) {
         double T[7];
 #pragma unroll
         for (int i = 0; i < 7; ++i) T[i] = Pcur[7 * (size_t)v + i];
@@ -752,12 +776,12 @@ __device__ double phase_pose_trial(const Dev& D, const Ctx& c, const double* __r
         if (h >= 0) {
             const double* u = D.x + 6 * (size_t)h;
             pose_oplus(T, u);
-            if (c.crank == 0) {
+            if (rank0) {
 #pragma unroll
                 for (int i = 0; i < 6; ++i) acc += u[i] * (lambda * u[i] + D.bp[6 * (size_t)h + i]);
             }
         }
-        if (c.crank == 0) {
+        if (rank0) {
 #pragma unroll
             for (int i = 0; i < 7; ++i) Ptr[7 * (size_t)v + i] = T[i];
         }
@@ -800,15 +824,16 @@ __device__ __forceinline__ void add_backsub_edge(const double* pcache, const Tri
 #pragma unroll
     for (int k = 0; k < 3; ++k) cl[k] += t[k] * be0 + t[3 + k] * be1;
 }
-__device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* __restrict__ E, double* __restrict__ Eout, double* __restrict__ Xtr,
-                                      const double* pcTr, double lambda) {
-    const int sl = c.tid & 7;
-    const unsigned gmask = 0xFFu << (c.tid & 24);
-    const int G = c.nw >> 3;
+__device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* __restrict__ E, double* __restrict__ Eout, const double* Xcur,
+                                      double* __restrict__ Xtr, const double* pcTr, double lambda) {
+    constexpr int FLY = FLY_PT;
+    const int sl = c.tid() & 7;
+    const unsigned gmask = 0xFFu << (c.tid() & 24);
+    const int G = c.nw() >> 3;
     double accS = 0, accC = 0;
     int a[FLY], b[FLY];
-    step_ranges(D.ptStart, D.nL, c.wid >> 3, G, a, b);
-    for (int p0 = c.wid >> 3; p0 < D.nL; p0 += FLY * G) {
+    step_ranges<FLY>(D.ptStart, D.nL, c.wid() >> 3, G, a, b);
+    for (int p0 = c.wid() >> 3; p0 < D.nL; p0 += FLY * G) {
         TrialEdge first[FLY] = {};
         double Di[FLY][6] = {}, bl[FLY][3] = {}, X0[FLY][3] = {}, xp[FLY][6] = {};     // Di: 00 01 02 11 12 22
 #pragma unroll
@@ -819,7 +844,7 @@ __device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* 
             if (p < D.nL) {
                 load_dinv(D.PT, D.nL, p, Di[j]);
 #pragma unroll
-                for (int k = 0; k < 3; ++k) { bl[j][k] = D.bl[3 * (size_t)p + k]; X0[j][k] = c.pts[3 * (size_t)p + k]; }
+                for (int k = 0; k < 3; ++k) { bl[j][k] = D.bl[3 * (size_t)p + k]; X0[j][k] = Xcur[3 * (size_t)p + k]; }
             }
         }
 #pragma unroll
@@ -829,7 +854,7 @@ __device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* 
                 for (int k = 0; k < 6; ++k) xp[j][k] = D.x[6 * (size_t)first[j].h + k];
             }
         int na[FLY], nb[FLY];
-        step_ranges(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
+        step_ranges<FLY>(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
 #pragma unroll
         for (int j = 0; j < FLY; ++j) {
             const int p = p0 + j * G;
@@ -864,149 +889,167 @@ __device__ double2 phase_points_trial(const Dev& D, const Ctx& c, const double* 
     }
     return make_double2(accS, accC);
 }
-__device__ void phase_finalize(const Dev& D, const Ctx& c) {
-    for (int e = c.wid; e < D.nE; e += c.nw) {
+__device__ void phase_finalize(const Dev& D, const Ctx& c, const double* pts) {
+    const int nw = c.nw();
+    for (int e = c.wid(); e < D.nE; e += nw) {
         const double e0 = D.err[2 * (size_t)e], e1 = D.err[2 * (size_t)e + 1];
         const int o = D.eOrig[e];
         D.outChi2[o] = (double)D.invSigma2[e] * (e0 * e0 + e1 * e1);   // e->chi2() from the last computed _error (Optimizer.cc:1425)
         const double* P = c.pc + PC * D.ePose[e];
-        double r[3]; qrot(P, c.pts + 3 * (size_t)D.ePt[e], r);
+        double r[3]; qrot(P, pts + 3 * (size_t)D.ePt[e], r);
         D.outDepthPos[o] = r[2] + P[6] > 0.0;
     }
     // the estimate ends in whichever buffer was current last; the caller reads D.poses / D.pts
-    if (c.pts != D.pts) for (int i = c.wid; i < 3 * D.nL; i += c.nw) D.pts[i] = c.pts[i];
+    if (pts != D.pts) for (int i = c.wid(); i < 3 * D.nL; i += nw) D.pts[i] = pts[i];
 }
 
 // =============================================================================================
 // The persistent kernel: SparseOptimizer::optimize (sparse_optimizer.cpp:354-418) around
 // OptimizationAlgorithmLevenberg::solve (optimization_algorithm_levenberg.cpp:61-168), one cluster per problem.
-// Every thread carries the (uniform) LM state; decisions use values every CTA reads identically after a cluster barrier.
+// The LM state is uniform: thread 0 of every CTA runs the policy on the CTA's copy in shared memory, from values every CTA
+// reads identically after a cluster barrier, and the other threads read the outcome after the next CTA barrier.  The
+// descriptor and that state stay in shared memory so that the registers (128 per thread) go to the phases.
 // Dynamic shared memory: 2 pose caches (PC x maxP doubles each, maxP = most poses of any loaded problem, fixed keyframes included) |
 // LDLT panel scratch (2 x 6 x (6 maxF + 1), maxF = most FREE poses) | rhs row (6 maxF) | reduced camera system (smemMatrixN^2).
 // =============================================================================================
+struct LoopState {
+    Levenberg lm;
+    double currentChi = 0, firstChi = 0, iniChi = 0, rho = 0;
+    int cj = 0, trials = 0, qmax = 0, term = 0, ok = 1;
+    int cur = 0;                        // the side of the double buffers that holds the current state: 0 = (E4a, poses, pts), 1 = (E4b, posesB, ptsB)
+    bool accepted = false, more = false;   // the last trial was accepted / the iteration runs another trial
+};
 __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __restrict__ probs, const volatile int* stop, int smemMatrixN, int maxP, int maxF) {
     extern __shared__ double s_dyn[];
     __shared__ double s_red[NT];
-    cg::cluster_group cluster = cg::this_cluster();
+    __shared__ Dev s_D;
+    __shared__ alignas(LoopState) unsigned char s_state[sizeof(LoopState)];   // constructed by thread 0 (a __shared__ variable has no initialiser)
+    LoopState& S = *reinterpret_cast<LoopState*>(s_state);
     Ctx c;
-    c.crank = (int)cluster.block_rank(); c.csize = (int)cluster.num_blocks(); c.tid = threadIdx.x;
-    c.wid = c.crank * NT + c.tid; c.nw = c.csize * NT; c.slot = 0; c.sm = s_red;
+    c.slot = 0; c.sm = s_red;
     double* s_pc = s_dyn;                        // pose cache, linearisation state
     double* s_pcT = s_pc + PC * maxP;            // pose cache, trial state
     double* s_col = s_pcT + PC * maxP;           // 2 x 6 x (6 maxF + 1) panel scratch
     double* s_rhs = s_col + 72 * maxF + 12;      // 6 maxF: rhs row of the LDLT
     double* s_mat = s_rhs + 6 * maxF + 2;
-    const Dev D = probs[blockIdx.x / c.csize];
-    const bool matInSmem = D.n <= smemMatrixN && D.n > 0;
-    // reduced camera system: CTA 0's shared memory; the other CTAs of the cluster reach it as distributed shared memory
-    double* HsRemote = matInSmem ? cluster.map_shared_rank(s_mat, 0) : D.Hs;
-    double* HsLocal = matInSmem ? s_mat : D.Hs;
-    const int ld = D.n;
-    const int stopIdx = blockIdx.x / c.csize;
-    const bool poller = c.crank == 0 && c.tid == 0;
+    c.pc = s_pc;
+    if (c.tid() == 0) {
+        s_D = probs[blockIdx.x / c.csize()];
+        new (&S) LoopState();
+    }
+    __syncthreads();
+    const Dev& D = s_D;
     // double-buffered state: the trial of an LM step is written next to the current estimate and the two swap when the
     // step is accepted, so a rejected step needs no restore ("pop") pass
-    double *Elin = D.E4a, *Etrial = D.E4b;       // edge factors at the linearisation point / at the trial state
-    double *Pcur = D.poses, *Ptr = D.posesB;     // poses
-    double *Xcur = D.pts, *Xtr = D.ptsB;         // points
-    c.pc = s_pc; c.pts = Xcur;
+    auto cur = [&](double* a, double* b) { return S.cur ? b : a; };
+    auto trial = [&](double* a, double* b) { return S.cur ? a : b; };
+    auto poll = [&]() { return (c.crank() == 0 && c.tid() == 0 && stop && stop[blockIdx.x / c.csize()]) ? 1 : 0; };
 
-    for (int i = c.wid; i < D.nP; i += c.nw) {
+    const int nw = c.nw();
+    for (int i = c.wid(); i < D.nP; i += nw) {
         double* T = D.poses + 7 * (size_t)i;
 #pragma unroll
         for (int k = 0; k < 7; ++k) T[k] = D.initPoses[7 * (size_t)i + k];
         qnormalize(T);                                              // SE3Quat(q, t) constructor
     }
-    for (int i = c.wid; i < 3 * D.nL; i += c.nw) D.pts[i] = D.initPts[i];
-    for (int i = c.wid; i < 2 * D.nE; i += c.nw) D.err[i] = 0.0;
-    for (int i = c.wid; i < D.n; i += c.nw) D.x[i] = 0.0;
-    int term = 0, dummy;
-    cluster_sum(D, c, 0.0, (poller && stop && stop[stopIdx]) ? 1 : 0, term);   // initial terminate() poll + publishes the poses
-    load_pose_cache(D, Pcur, s_pc);
+    for (int i = c.wid(); i < 3 * D.nL; i += nw) D.pts[i] = D.initPts[i];
+    for (int i = c.wid(); i < 2 * D.nE; i += nw) D.err[i] = 0.0;
+    for (int i = c.wid(); i < D.n; i += nw) D.x[i] = 0.0;
+    int flag;
+    cluster_sum(D, c, 0.0, poll(), flag);        // initial terminate() poll + publishes the poses
+    if (c.tid() == 0) S.term = flag;
+    load_pose_cache(D, D.poses, s_pc);
 
-    Levenberg lm;
-    double currentChi = 0, firstChi = 0;
-    int cj = 0, trials = 0;
-    bool ok = true;
     __shared__ unsigned long long s_tph[11];     // per-phase ns of CTA 0 (thread 0), [10] = tick
-    if (c.tid < 11) s_tph[c.tid] = 0;
+    if (c.tid() < 11) s_tph[c.tid()] = 0;
     __syncthreads();
-#define TICK() do { if (c.wid == 0) s_tph[10] = globaltimer_ns(); } while (0)
-#define TOCK(i) do { if (c.wid == 0) s_tph[i] += globaltimer_ns() - s_tph[10]; } while (0)
-    for (int it = 0; it < D.iterations && !term && ok; ++it) {
+#define TICK() do { if (c.wid() == 0) s_tph[10] = globaltimer_ns(); } while (0)
+#define TOCK(i) do { if (c.wid() == 0) s_tph[i] += globaltimer_ns() - s_tph[10]; } while (0)
+    for (int it = 0; it < D.iterations && !S.term && S.ok; ++it) {
+        // the first iteration starts the LM policy: with the user's lambda before the build, else with H's largest diagonal entry after it
+        const bool lambdaKnown = it > 0 || D.userLambdaInit > 0;
         // computeActiveErrors at the start of solve(): after an accepted step the state, the errors and the edge factors are
         // exactly those of the accepted trial (same arithmetic), so only the first iteration evaluates them
         if (it == 0) {
+            if (lambdaKnown && c.tid() == 0) S.lm.start(D.userLambdaInit, 0.0);
             TICK();
-            currentChi = cluster_sum(D, c, phase_errors(D, c, Elin), 0, dummy);
+            const double chi = cluster_sum(D, c, phase_errors(D, c, cur(D.pts, D.ptsB), cur(D.E4a, D.E4b)), 0, flag);
+            if (c.tid() == 0) S.currentChi = chi;
             TOCK(0);
         }
-        const double iniChi = currentChi;
-        if (it == 0) firstChi = iniChi;
-        // the first iteration starts the LM policy: with the user's lambda before the build, else with H's largest diagonal entry after it
-        const bool lambdaKnown = it > 0 || D.userLambdaInit > 0;
-        if (it == 0 && lambdaKnown) lm.start(D.userLambdaInit, 0.0);
+        if (c.tid() == 0) {
+            S.iniChi = S.currentChi;
+            if (it == 0) S.firstChi = S.iniChi;
+            S.rho = 0; S.qmax = 0;
+        }
         TICK();
-        phase_build_points(D, c, Elin, lambdaKnown ? lm.lambda : -1.0);
+        phase_build_points(D, c, cur(D.E4a, D.E4b), lambdaKnown ? S.lm.lambda : -1.0);
         TOCK(1); TICK();
-        phase_build_poses_partial(D, c, Elin);
+        phase_build_poses_partial(D, c, cur(D.E4a, D.E4b));
         csync();
         phase_build_poses_combine(D, c);
         TOCK(2);
-        if (!lambdaKnown) { csync(); lm.start(0.0, phase_maxdiag(D, c)); }
+        if (!lambdaKnown) {
+            csync();
+            const double maxDiag = phase_maxdiag(D, c);
+            if (c.tid() == 0) S.lm.start(0.0, maxDiag);
+            __syncthreads();
+        }
         bool needPrep = !lambdaKnown;
-        double rho = 0;
-        int qmax = 0;
         do {
             if (needPrep) {
                 TICK();
-                phase_point_prep(D, c, lm.lambda);
+                phase_point_prep(D, c, S.lm.lambda);
                 csync();
                 TOCK(3);
             }
             int ok2 = 1;
             if (D.nF) {
+                // reduced camera system: CTA 0's shared memory; the other CTAs of the cluster reach it as distributed shared memory
+                const bool matInSmem = D.n <= smemMatrixN && D.n > 0;
                 TICK();
                 phase_schur_partial(D, c, D.K);
                 csync();
                 TOCK(4); TICK();
-                phase_schur_combine(D, c, lm.lambda, HsRemote, ld);   // every CTA writes entries into CTA 0's shared memory through DSMEM
+                phase_schur_combine(D, c, S.lm.lambda, matInSmem ? cg::this_cluster().map_shared_rank(s_mat, 0) : D.Hs, D.n);   // every CTA writes entries into CTA 0's shared memory through DSMEM
                 csync();
                 TOCK(6); TICK();
-                if (c.crank == 0) {
-                    ok2 = phase_ldlt(D, c, HsLocal, ld, s_col, s_rhs);
-                    if (c.tid == 0) D.partial[4 * PSLOT] = (double)ok2;
+                if (c.crank() == 0) {
+                    ok2 = phase_ldlt(D, c, matInSmem ? s_mat : D.Hs, D.n, s_col, s_rhs);
+                    if (c.tid() == 0) D.partial[4 * PSLOT] = (double)ok2;
                 }
                 csync();
                 ok2 = (int)D.partial[4 * PSLOT];
                 TOCK(5);
             }
             TICK();
-            const double sP = phase_pose_trial(D, c, Pcur, Ptr, s_pcT, lm.lambda);
+            const double sP = phase_pose_trial(D, c, cur(D.poses, D.posesB), trial(D.poses, D.posesB), s_pcT, S.lm.lambda);
             TOCK(7); TICK();
-            const double2 sc = phase_points_trial(D, c, Elin, Etrial, Xtr, s_pcT, lm.lambda);
+            const double2 sc = phase_points_trial(D, c, cur(D.E4a, D.E4b), trial(D.E4a, D.E4b), cur(D.pts, D.ptsB), trial(D.pts, D.ptsB), s_pcT,
+                                                  S.lm.lambda);
             double scale0, tempChi;
-            cluster_sum2(D, c, sP + sc.x, sc.y, (poller && stop && stop[stopIdx]) ? 1 : 0, term, scale0, tempChi);
+            cluster_sum2(D, c, sP + sc.x, sc.y, poll(), flag, scale0, tempChi);
             TOCK(8);
-            if (lm.trial(currentChi, tempChi, scale0, ok2, rho)) {
-                double* sw;
-                sw = Elin; Elin = Etrial; Etrial = sw;
-                sw = Pcur; Pcur = Ptr; Ptr = sw;
-                sw = Xcur; Xcur = Xtr; Xtr = sw;
-                c.pts = Xcur;
-                for (int i = c.tid; i < PC * D.nP; i += NT) s_pc[i] = s_pcT[i];
+            if (c.tid() == 0) {
+                S.term = flag;
+                S.accepted = S.lm.trial(S.currentChi, tempChi, scale0, ok2, S.rho);
+                if (S.accepted) S.cur ^= 1;                     // a rejected trial's buffers are simply abandoned (pop)
+                ++S.qmax; ++S.trials;
+                S.more = S.rho < 0 && S.qmax < Levenberg::maxTrials && !S.term;
+                if (!S.more) { ++S.cj; S.ok = S.lm.iteration_done(S.qmax, S.rho, S.iniChi, S.currentChi); }
+            }
+            __syncthreads();
+            if (S.accepted) {
+                for (int i = c.tid(); i < PC * D.nP; i += NT) s_pc[i] = s_pcT[i];
                 __syncthreads();
-            }                                                   // a rejected trial's buffers are simply abandoned (pop)
+            }
             needPrep = true;
-            ++qmax; ++trials;
-        } while (rho < 0 && qmax < Levenberg::maxTrials && !term);
-        ++cj;
-        ok = lm.iteration_done(qmax, rho, iniChi, currentChi);
+        } while (S.more);
     }
-    phase_finalize(D, c);
-    if (Pcur != D.poses) for (int i = c.wid; i < 7 * D.nP; i += c.nw) D.poses[i] = Pcur[i];
-    if (c.wid == 0) for (int i = 0; i < 10; ++i) D.stats[8 + i] = (double)s_tph[i];
-    if (c.wid == 0) { D.stats[0] = cj; D.stats[1] = trials; D.stats[2] = lm.lambda; D.stats[3] = currentChi; D.stats[4] = firstChi; }
+    phase_finalize(D, c, cur(D.pts, D.ptsB));
+    if (S.cur) for (int i = c.wid(); i < 7 * D.nP; i += nw) D.poses[i] = D.posesB[i];
+    if (c.wid() == 0) for (int i = 0; i < 10; ++i) D.stats[8 + i] = (double)s_tph[i];
+    if (c.wid() == 0) { D.stats[0] = S.cj; D.stats[1] = S.trials; D.stats[2] = S.lm.lambda; D.stats[3] = S.currentChi; D.stats[4] = S.firstChi; }
 }
 
 // =============================================================================================
