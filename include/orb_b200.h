@@ -520,6 +520,24 @@ typedef struct OrbmNewPoint {
 /* out [KF1.N]: the new points in the order the reference creates them ((neighbour, idx1) ascending), *nNew of them.  nmatches [nKF2]: the
  * reference's vMatchedIndices.size() per neighbour; ncreated [nKF2]: points created from each neighbour.  Host pointers; 3 launches. */
 int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNewPoint* out, int* nNew, int32_t* nmatches, int32_t* ncreated);
+/* orbm_create_new_map_points for several new keyframes (items) in ONE upload through the handle's staging, 3 launches and ONE download; every
+ * item's outputs are byte-identical to what orbm_create_new_map_points gives it alone.  Every per-keyframe setting (level tables, nlevels,
+ * scaleFactor, bCoarse, bInertial, thFarPoints) is per item.  An item with nKF2 == 0 or KF1.N == 0 gets zero counts and takes no CTA;
+ * orbm_last_launch_count() is 3, or 0 when every item is empty.  Host pointers.
+ * PRECONDITION: at most one keyframe per MAP.  CreateNewMapPoints of keyframe A calls AddMapPoint on A and on its neighbours, which changes
+ * the hasMapPoint another keyframe of the same map may search; keyframes of different maps share no keyframe and no map point.  Two
+ * keyframes of the same map in one call are NOT equivalent to the reference.  CheckNewKeyFrames stays with the caller: read it once per item
+ * and cut that item's neighbour list to its first entry when a keyframe is queued (INTEGRATION.md §2).
+ * ORB_ERR_ARG: any item failing a check of orbm_create_new_map_points, nItems < 0, or items NULL with nItems > 0; ORB_ERR_CAPACITY: more than
+ * 65535 (keyframe, neighbour) pairs over the items with KF1.N > 0.  Both before anything is staged; the message names the item. */
+typedef struct OrbmNewPointsItem {
+    OrbmNewPointsIn in;           /* exactly what orbm_create_new_map_points takes, per keyframe */
+    OrbmNewPoint* out;            /* [in.KF1->N] out: records in creation order */
+    int* nNew;                    /* [1] out */
+    int32_t* nmatches;            /* [in.nKF2] out */
+    int32_t* ncreated;            /* [in.nKF2] out */
+} OrbmNewPointsItem;
+int orbm_create_new_map_points_batch(orbm_handle* h, int nItems, const OrbmNewPointsItem* items);
 /* void MapPoint::ComputeDistinctiveDescriptors() (src/MapPoint.cc:329-403) for nPoints map points at once (LocalMapping::ProcessNewKeyFrame /
  * CreateNewMapPoints call it per point): the observed descriptors of point p are rows obsStart[p] .. obsStart[p+1] of `descriptors`;
  * best[p] = row (relative to obsStart[p]) with the least median Hamming distance to the others, -1 for a point without observations. */

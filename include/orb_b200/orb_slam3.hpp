@@ -209,6 +209,14 @@ public:
         for (const OrbmFuseItem& it : items) if (it.KF.K > maxK) maxK = it.KF.K;
         orb_check(orbm_fuse_search_batch(detail::matcher_handle(maxK, 1, device_), (int)items.size(), items.data()), "orbm_fuse_search_batch");
     }
+    // void LocalMapping::CreateNewMapPoints() (monocular, the vpNeighKFs loop) for several new keyframes of DIFFERENT maps in three launches
+    // (orbm_create_new_map_points_batch).  Every item's out / nNew / nmatches / ncreated receive exactly what orbm_create_new_map_points
+    // gives it alone; the caller picks the neighbours, cuts a list to one entry when CheckNewKeyFrames() holds, and replays the records in
+    // order (INTEGRATION.md §2).
+    void CreateNewMapPointsBatch(const std::vector<OrbmNewPointsItem>& items) {
+        orb_check(orbm_create_new_map_points_batch(detail::matcher_handle(1, 1, device_), (int)items.size(), items.data()),
+                  "orbm_create_new_map_points_batch");
+    }
     // void LocalMapping::KeyFrameCulling() (monocular and mono-inertial) for several maps that share nothing, in one launch
     // (orbm_keyframe_culling_batch).  Every map's status / nMPs / nRedundant / visited receive its walk; the caller replays the culls in
     // status order: MergePrevious, the relink and SetBadFlag (INTEGRATION.md §2).

@@ -37,6 +37,11 @@ class OrbmNewPointsIn(C.Structure):
                 ('cam', C.c_void_p), ('scaleFactor', C.c_float), ('bCoarse', C.c_int), ('bInertial', C.c_int), ('thFarPoints', C.c_float)]
 
 
+class OrbmNewPointsItem(C.Structure):
+    """One new keyframe of orbm_create_new_map_points_batch (include/orb_b200.h); ``in_`` is the header's ``in``."""
+    _fields_ = [('in_', OrbmNewPointsIn), ('out', C.c_void_p), ('nNew', C.c_void_p), ('nmatches', C.c_void_p), ('ncreated', C.c_void_p)]
+
+
 _vp, _i, _f, _d, _sz, _out = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.POINTER(C.c_void_p)
 
 #: (restype, argtypes) of every liborb_b200.so function the package, its tests and its tools call, as include/orb_b200.h declares it.
@@ -93,6 +98,7 @@ SIGNATURES = {
     'orbm_search_by_sim3': (_i, [_vp] * 5 + [_f, _vp, _f, _vp, _vp, _vp]),
     'orbm_search_for_triangulation': (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp]),
     'orbm_create_new_map_points': (_i, [_vp] * 6),
+    'orbm_create_new_map_points_batch': (_i, [_vp, _i, _vp]),
     'orbm_distinctive_descriptors': (_i, [_vp, _i, _vp, _vp, _vp]),
     'orbm_keyframe_culling_batch': (_i, [_vp, _i, _vp]),
     'orbm_update_connections_batch': (_i, [_vp, _i, _vp]),
@@ -1015,23 +1021,53 @@ class ORBmatcher:
         ``cam`` [1 + n, 4]; ``th_far_points`` 0 = off.  Returns (records, nmatches [n], ncreated [n]): ``records`` is a ``NEW_POINT_DTYPE``
         array in creation order.  The matcher's own settings are not used: the reference builds ``ORBmatcher(0.6f, false)`` here."""
         keep = []
-        f1 = self._tri_frame(kf1, keep)
-        n2 = len(kf2_list)
-        f2 = (OrbmTriFrame * max(n2, 1))(*[self._tri_frame(k, keep) for k in kf2_list])
-        arrs = [_c(scale_factors, np.float32), _c(level_sigma2, np.float32), _c(ep, np.float32).reshape(-1, 2), _c(F12, np.float32).reshape(-1, 9),
-                _c(Tcw, np.float32).reshape(-1, 12), _c(Ow, np.float32).reshape(-1, 3), _c(cam, np.float32).reshape(-1, 4)]
-        assert len(arrs[4]) == len(arrs[5]) == len(arrs[6]) == n2 + 1 and len(arrs[2]) == len(arrs[3]) == n2
-        inp = OrbmNewPointsIn(C.pointer(f1), n2, C.cast(f2, C.POINTER(OrbmTriFrame)), arrs[2].ctypes.data, arrs[3].ctypes.data, arrs[0].ctypes.data,
-                              arrs[1].ctypes.data, len(arrs[0]), arrs[4].ctypes.data, arrs[5].ctypes.data, arrs[6].ctypes.data, float(scale_factor),
-                              int(coarse), int(inertial), float(th_far_points))
-        out = np.zeros(max(f1.N, 1), NEW_POINT_DTYPE)
-        nm, nc = np.zeros(n2, np.int32), np.zeros(n2, np.int32)
+        inp = self._new_points_in(kf1, kf2_list, scale_factors, level_sigma2, ep, F12, Tcw, Ow, cam, scale_factor, coarse, inertial, th_far_points, keep)
+        out, nm, nc = self._new_points_out(inp)
         n = C.c_int(0)
         L = lib()
         rc = L.orbm_create_new_map_points(self._h, C.byref(inp), _ptr(out), C.byref(n), _ptr(nm), _ptr(nc))
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_create_new_map_points')
         return out[:n.value].copy(), nm, nc
+
+    def create_new_map_points_batch(self, items):
+        """:meth:`CreateNewMapPoints` for several new keyframes in one call of 3 launches (orbm_create_new_map_points_batch).  Each item is a
+        dict of :meth:`CreateNewMapPoints`' arguments by name (``kf1``, ``kf2_list``, ``scale_factors``, ... ; ``coarse``, ``inertial`` and
+        ``th_far_points`` optional).  Returns [(records, nmatches, ncreated)] in item order, each byte-identical to :meth:`CreateNewMapPoints`
+        of that item.  At most one keyframe per map (see include/orb_b200.h)."""
+        keep, res = [], []
+        arr = (OrbmNewPointsItem * max(len(items), 1))()
+        for j, it in enumerate(items):
+            inp = self._new_points_in(it['kf1'], it['kf2_list'], it['scale_factors'], it['level_sigma2'], it['ep'], it['F12'], it['Tcw'], it['Ow'],
+                                      it['cam'], it['scale_factor'], it.get('coarse', False), it.get('inertial', False), it.get('th_far_points', 0.0), keep)
+            out, nm, nc = self._new_points_out(inp)
+            n = np.zeros(1, np.int32)
+            res.append((out, nm, nc, n))
+            arr[j] = OrbmNewPointsItem(inp, out.ctypes.data, n.ctypes.data, nm.ctypes.data, nc.ctypes.data)
+        L = lib()
+        rc = L.orbm_create_new_map_points_batch(self._h, len(items), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_create_new_map_points_batch')
+        return [(out[:n[0]].copy(), nm, nc) for out, nm, nc, n in res]
+
+    def _new_points_in(self, kf1, kf2_list, scale_factors, level_sigma2, ep, F12, Tcw, Ow, cam, scale_factor, coarse, inertial, th_far_points, keep):
+        """OrbmNewPointsIn of one CreateNewMapPoints call; every array it points to is appended to ``keep``."""
+        f1 = self._tri_frame(kf1, keep)
+        n2 = len(kf2_list)
+        f2 = (OrbmTriFrame * max(n2, 1))(*[self._tri_frame(k, keep) for k in kf2_list])
+        arrs = [_c(scale_factors, np.float32), _c(level_sigma2, np.float32), _c(ep, np.float32).reshape(-1, 2), _c(F12, np.float32).reshape(-1, 9),
+                _c(Tcw, np.float32).reshape(-1, 12), _c(Ow, np.float32).reshape(-1, 3), _c(cam, np.float32).reshape(-1, 4)]
+        assert len(arrs[4]) == len(arrs[5]) == len(arrs[6]) == n2 + 1 and len(arrs[2]) == len(arrs[3]) == n2
+        f1p = C.pointer(f1)
+        keep.append((f1p, f2, arrs))
+        return OrbmNewPointsIn(f1p, n2, C.cast(f2, C.POINTER(OrbmTriFrame)), arrs[2].ctypes.data, arrs[3].ctypes.data, arrs[0].ctypes.data,
+                               arrs[1].ctypes.data, len(arrs[0]), arrs[4].ctypes.data, arrs[5].ctypes.data, arrs[6].ctypes.data, float(scale_factor),
+                               int(coarse), int(inertial), float(th_far_points))
+
+    @staticmethod
+    def _new_points_out(inp):
+        """(records [max(KF1.N, 1)], nmatches [nKF2], ncreated [nKF2]) buffers for ``inp``."""
+        return np.zeros(max(inp.KF1.contents.N, 1), NEW_POINT_DTYPE), np.zeros(inp.nKF2, np.int32), np.zeros(inp.nKF2, np.int32)
 
     def keyframe_culling_batch(self, maps):
         """``LocalMapping::KeyFrameCulling()`` (monocular and mono-inertial) for several maps in one launch (orbm_keyframe_culling_batch).

@@ -851,23 +851,30 @@ __global__ void __launch_bounds__(MF_NT) fuse_search_kernel(const FuseParams* __
 // the smallest distance wins, the last candidate on ties (:1008 is strict).  The reference never sets vbMatched2, so KF1 features are
 // independent.  The epipole and the fundamental matrix are inputs (Eigen / Sophus expressions in the caller); the scalar float expressions
 // are contracted as the reference's build contracts them (oracle/matcher_oracle.cpp: orbo_search_for_triangulation).
+// The pairs may belong to several new keyframes (items): each pair names its item, whose KF1 operands sit in the item table.
 // ---------------------------------------------------------------------------------------------
+struct TriItem {
+    int N1, E1, coarse;
+    const OrbKeyPoint* kps1; const uint8_t *desc1, *hasMP1; const int *fvNode1, *fvFeat1;
+    const float *scaleFactors, *levelSigma2;
+};
 struct TriPair {
-    int N2, E2;
+    int item, N2, E2;
     const OrbKeyPoint* kps2; const uint8_t *desc2, *hasMP2; const int *fvNode2, *fvFeat2;
     float ep[2], F12[9];
     int* matches12; int* nmatches; uint8_t* evBin;
 };
 struct TriParams {
-    int N1, E1, coarse, checkOri;
-    const OrbKeyPoint* kps1; const uint8_t *desc1, *hasMP1; const int *fvNode1, *fvFeat1;
-    const float *scaleFactors, *levelSigma2;
+    int checkOri;
+    const TriItem* items;
     const TriPair* pairs;
 };
 constexpr int TM_NT = 256;
-__global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams Q) {
+__global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams P) {
     __shared__ int s_hist[HISTO_LENGTH], s_ind[3], s_acc, s_rem;
-    const TriPair R = Q.pairs[blockIdx.x];
+    const TriPair& R = P.pairs[blockIdx.x];
+    const TriItem& Q = P.items[R.item];
+    const int checkOri = P.checkOri;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     for (int i = tid; i < Q.N1; i += TM_NT) { R.matches12[i] = -1; R.evBin[i] = 0; }
     if (tid < HISTO_LENGTH) s_hist[tid] = 0;
@@ -922,7 +929,7 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams Q) {
             if (lane == 0) {
                 const int idx2 = R.fvFeat2[b + (int)(0xFFFFFFFFu - (unsigned)best)];
                 R.matches12[idx1] = idx2;
-                if (Q.checkOri) {
+                if (checkOri) {
                     const int bin = rot_bin(kp1.angle, R.kps2[idx2].angle);
                     R.evBin[idx1] = (uint8_t)(bin + 1);
                     atomicAdd(&s_hist[bin], 1);
@@ -933,7 +940,7 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams Q) {
     }
     if (lane == 0 && acc) atomicAdd(&s_acc, acc);
     __syncthreads();
-    if (Q.checkOri) {
+    if (checkOri) {
         if (tid == 0) {
             int ind1 = -1, ind2 = -1, ind3 = -1, max1 = 0, max2 = 0, max3 = 0;
             for (int bb = 0; bb < HISTO_LENGTH; ++bb) {
@@ -965,18 +972,23 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams Q) {
 // new_points_commit_kernel applies the sequential rule (DESIGN.md section 4): the point of idx1 comes from the first k whose match
 // passes, and a match of a later neighbour at that idx1 is one the reference never sees.  Every rounding and contraction is the
 // oracle's (oracle/mapping_oracle.cpp), which documents the evaluation order.
+// A launch serves several new keyframes (items) of different maps: the pairs of tri_match_kernel, item after item, carry the item; each
+// item owns the [nKF2][N1] block of slots from `slot0` in matches12 / reason / recs and its own outputs.
 // ---------------------------------------------------------------------------------------------
 enum : uint8_t { NP_NO_MATCH = 0, NP_LOW_PARALLAX, NP_SVD_W0, NP_DEPTH1, NP_DEPTH2, NP_REPROJ1, NP_REPROJ2, NP_ZERO_DIST, NP_FAR, NP_SCALE, NP_CREATED };
 constexpr int NP_MAX_SWEEPS = 64;       // Eigen has no limit; a float 4x4 converges in a handful of sweeps (oracle)
 constexpr int NP_NT = 128, NPC_NT = 1024;
 
-struct NewPointsParams {
-    int N1, nKF2, nlevels, bInertial;
+struct NpItem {
+    int pair0, nKF2, nlevels, bInertial;                                     // pair0: the item's first pair
     float ratioFactor, thFar;
-    const OrbKeyPoint* kps1; const TriPair* pairs; const int* matches12;     // [nKF2][N1]
-    const float *scaleFactors, *levelSigma2, *Tcw, *Ow, *cam;                // Tcw / Ow / cam: [1 + nKF2] keyframes, KF1 first
-    uint8_t* reason; OrbmNewPoint* recs; int* winner;                        // [nKF2][N1], [nKF2][N1], [N1]
-    int* counts; OrbmNewPoint* out;                                          // nNew, nmatches [nKF2], ncreated [nKF2]; out [N1]
+    size_t slot0;
+    const float *Tcw, *Ow, *cam;                                             // [1 + nKF2] keyframes, KF1 first
+    int* winner; int* counts; OrbmNewPoint* out;                             // [N1]; nNew, nmatches [nKF2], ncreated [nKF2]; out [N1]
+};
+struct NewPointsParams {
+    const TriItem* tri; const NpItem* items; const TriPair* pairs;
+    const int* matches12; uint8_t* reason; OrbmNewPoint* recs;               // every item's slots
 };
 
 struct NpRot { float c, s; };
@@ -1102,21 +1114,27 @@ __device__ __forceinline__ float np_row(const float* T, int r, const float* x) {
 }
 __device__ __forceinline__ float np_norm(const float* a) { return __fsqrt_rn(fadd(fadd(fmul(a[0], a[0]), fmul(a[1], a[1])), fmul(a[2], a[2]))); }
 
+// Grid (x: idx1 blocks of the widest item, y: pair); a thread beyond its item's N1 exits.
 __global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
-    const int idx1 = blockIdx.x * NP_NT + threadIdx.x, k = blockIdx.y;
-    if (idx1 >= P.N1) return;
-    const size_t slot = (size_t)k * P.N1 + idx1;
+    const TriPair* R = P.pairs + blockIdx.y;
+    const int it = R->item, N1 = P.tri[it].N1, idx1 = blockIdx.x * NP_NT + threadIdx.x;
+    if (idx1 >= N1) return;
+    const NpItem* I = P.items + it;
+    const int k = (int)blockIdx.y - I->pair0;
+    const size_t slot = I->slot0 + (size_t)k * N1 + idx1;
     const int idx2 = P.matches12[slot];
     uint8_t why = NP_NO_MATCH;
     if (idx2 >= 0) {
-        const OrbKeyPoint kp1 = P.kps1[idx1], kp2 = P.pairs[k].kps2[idx2];
+        const float *scaleFactors = P.tri[it].scaleFactors, *levelSigma2 = P.tri[it].levelSigma2;
+        const OrbKeyPoint kp1 = P.tri[it].kps1[idx1], kp2 = R->kps2[idx2];
+        const float *Tcw = I->Tcw, *Ow = I->Ow, *cam = I->cam;
         float T1[12], T2[12], O1[3], O2[3], c1[4], c2[4];
 #pragma unroll
-        for (int i = 0; i < 12; ++i) { T1[i] = P.Tcw[i]; T2[i] = P.Tcw[12 * (k + 1) + i]; }
+        for (int i = 0; i < 12; ++i) { T1[i] = Tcw[i]; T2[i] = Tcw[12 * (k + 1) + i]; }
 #pragma unroll
-        for (int i = 0; i < 3; ++i) { O1[i] = P.Ow[i]; O2[i] = P.Ow[3 * (k + 1) + i]; }
+        for (int i = 0; i < 3; ++i) { O1[i] = Ow[i]; O2[i] = Ow[3 * (k + 1) + i]; }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) { c1[i] = P.cam[i]; c2[i] = P.cam[4 * (k + 1) + i]; }
+        for (int i = 0; i < 4; ++i) { c1[i] = cam[i]; c2[i] = cam[4 * (k + 1) + i]; }
         const float xn1[3] = {fdiv(fsub(kp1.x, c1[2]), c1[0]), fdiv(fsub(kp1.y, c1[3]), c1[1]), 1.0f};
         const float xn2[3] = {fdiv(fsub(kp2.x, c2[2]), c2[0]), fdiv(fsub(kp2.y, c2[3]), c2[1]), 1.0f};
         float ray1[3], ray2[3];
@@ -1128,7 +1146,8 @@ __global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
         const float dot = fadd(fadd(fmul(ray1[0], ray2[0]), fmul(ray1[1], ray2[1])), fmul(ray1[2], ray2[2]));
         const float cp = fdiv(dot, fmul(np_norm(ray1), np_norm(ray2)));
         float x3D[3];
-        if (!(cp < fadd(cp, 1.0f) && cp > 0.0f && ((P.bInertial && (double)cp < 0.9996) || (!P.bInertial && (double)cp < 0.9998)))) why = NP_LOW_PARALLAX;
+        const int bInertial = I->bInertial;
+        if (!(cp < fadd(cp, 1.0f) && cp > 0.0f && ((bInertial && (double)cp < 0.9996) || (!bInertial && (double)cp < 0.9998)))) why = NP_LOW_PARALLAX;
         else if (!np_triangulate(xn1[0], xn1[1], xn2[0], xn2[1], T1, T2, x3D)) why = NP_SVD_W0;
         else {
             const float z1 = np_row(T1, 2, x3D), z2 = np_row(T2, 2, x3D);
@@ -1139,16 +1158,17 @@ __global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
             const float nv1[3] = {fsub(x3D[0], O1[0]), fsub(x3D[1], O1[1]), fsub(x3D[2], O1[2])};
             const float nv2[3] = {fsub(x3D[0], O2[0]), fsub(x3D[1], O2[1]), fsub(x3D[2], O2[2])};
             const float dist1 = np_norm(nv1), dist2 = np_norm(nv2);
-            const float sf1 = P.scaleFactors[kp1.octave];
+            const float sf1 = scaleFactors[kp1.octave], thFar = I->thFar;
             if (z1 <= 0.0f) why = NP_DEPTH1;
             else if (z2 <= 0.0f) why = NP_DEPTH2;
-            else if ((double)__fmaf_rn(ex1, ex1, fmul(ey1, ey1)) > 5.991 * (double)P.levelSigma2[kp1.octave]) why = NP_REPROJ1;   // one FMA, see oracle
-            else if ((double)__fmaf_rn(ex2, ex2, fmul(ey2, ey2)) > 5.991 * (double)P.levelSigma2[kp2.octave]) why = NP_REPROJ2;
+            else if ((double)__fmaf_rn(ex1, ex1, fmul(ey1, ey1)) > 5.991 * (double)levelSigma2[kp1.octave]) why = NP_REPROJ1;   // one FMA, see oracle
+            else if ((double)__fmaf_rn(ex2, ex2, fmul(ey2, ey2)) > 5.991 * (double)levelSigma2[kp2.octave]) why = NP_REPROJ2;
             else if (dist1 == 0.0f || dist2 == 0.0f) why = NP_ZERO_DIST;
-            else if (P.thFar > 0.0f && (dist1 >= P.thFar || dist2 >= P.thFar)) why = NP_FAR;
+            else if (thFar > 0.0f && (dist1 >= thFar || dist2 >= thFar)) why = NP_FAR;
             else {
-                const float ratioDist = fdiv(dist2, dist1), ratioOctave = fdiv(sf1, P.scaleFactors[kp2.octave]);
-                if (fmul(ratioDist, P.ratioFactor) < ratioOctave || ratioDist > fmul(ratioOctave, P.ratioFactor)) why = NP_SCALE;
+                const float ratioFactor = I->ratioFactor;
+                const float ratioDist = fdiv(dist2, dist1), ratioOctave = fdiv(sf1, scaleFactors[kp2.octave]);
+                if (fmul(ratioDist, ratioFactor) < ratioOctave || ratioDist > fmul(ratioOctave, ratioFactor)) why = NP_SCALE;
                 else {
                     why = NP_CREATED;
                     OrbmNewPoint r;
@@ -1156,7 +1176,7 @@ __global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
 #pragma unroll
                     for (int i = 0; i < 3; ++i) { r.x3D[i] = x3D[i]; r.normal[i] = fdiv(fadd(fadd(0.0f, fdiv(nv1[i], dist1)), fdiv(nv2[i], dist2)), 2.0f); }
                     r.maxDistance = fmul(dist1, sf1);
-                    r.minDistance = fdiv(r.maxDistance, P.scaleFactors[P.nlevels - 1]);
+                    r.minDistance = fdiv(r.maxDistance, scaleFactors[I->nlevels - 1]);
                     P.recs[slot] = r;
                 }
             }
@@ -1165,15 +1185,20 @@ __global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
     P.reason[slot] = why;
 }
 
-// One CTA: winner[idx1] = first neighbour that created idx1's point; then per neighbour, in order, the counts and the records compacted in
-// idx1 order (thread t owns a contiguous run of idx1, a block scan gives each run its place).
+// One CTA per item: winner[idx1] = first neighbour that created idx1's point; then per neighbour, in order, the counts and the records
+// compacted in idx1 order (thread t owns a contiguous run of idx1, a block scan gives each run its place).
 __global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsParams P) {
     __shared__ int s_scan[NPC_NT / 32], s_msum[NPC_NT / 32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, N1 = P.N1, K = P.nKF2;
+    const NpItem& I = P.items[blockIdx.x];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, N1 = P.tri[blockIdx.x].N1, K = I.nKF2;
+    const int* matches12 = P.matches12 + I.slot0;
+    const uint8_t* reason = P.reason + I.slot0;
+    const OrbmNewPoint* recs = P.recs + I.slot0;
+    int* winner = I.winner;
     for (int i = tid; i < N1; i += NPC_NT) {
         int w = -1;
-        for (int k = 0; k < K && w < 0; ++k) if (P.reason[(size_t)k * N1 + i] == NP_CREATED) w = k;
-        P.winner[i] = w;
+        for (int k = 0; k < K && w < 0; ++k) if (reason[(size_t)k * N1 + i] == NP_CREATED) w = k;
+        winner[i] = w;
     }
     __syncthreads();
     const int per = (N1 + NPC_NT - 1) / NPC_NT, i0 = min(N1, tid * per), i1 = min(N1, i0 + per);
@@ -1181,9 +1206,9 @@ __global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsPara
     for (int k = 0; k < K; ++k) {
         int c = 0, mt = 0;
         for (int i = i0; i < i1; ++i) {
-            const int w = P.winner[i];
+            const int w = winner[i];
             c += w == k;
-            mt += P.matches12[(size_t)k * N1 + i] >= 0 && (w < 0 || w >= k);     // the reference's search skips idx1 once an earlier k made its point
+            mt += matches12[(size_t)k * N1 + i] >= 0 && (w < 0 || w >= k);     // the reference's search skips idx1 once an earlier k made its point
         }
         int incl = c;
 #pragma unroll
@@ -1202,13 +1227,13 @@ __global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsPara
         }
         __syncthreads();
         int pos = base + (wid ? s_scan[wid - 1] : 0) + incl - c;
-        for (int i = i0; i < i1; ++i) if (P.winner[i] == k) P.out[pos++] = P.recs[(size_t)k * N1 + i];
+        for (int i = i0; i < i1; ++i) if (winner[i] == k) I.out[pos++] = recs[(size_t)k * N1 + i];
         const int created = s_scan[NPC_NT / 32 - 1];
-        if (tid == 0) { P.counts[1 + k] = s_msum[0]; P.counts[1 + K + k] = created; }
+        if (tid == 0) { I.counts[1 + k] = s_msum[0]; I.counts[1 + K + k] = created; }
         base += created;
         __syncthreads();
     }
-    if (tid == 0) P.counts[0] = base;
+    if (tid == 0) I.counts[0] = base;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1976,19 +2001,18 @@ static bool tri_frame_ok(const OrbmTriFrame* f) {
     for (int e = 0; e < f->nEntries; ++e) if (f->fvFeature[e] < 0 || f->fvFeature[e] >= f->N || (e && f->fvNode[e] < f->fvNode[e - 1])) return false;
     return true;
 }
-// The SearchForTriangulation part (KF1 against nKF2 neighbours) shared by orbm_search_for_triangulation and
-// orbm_create_new_map_points.  tri_stage declares its pieces on the matcher's staging: the level tables, KF1, every neighbour's
-// arrays and the pair table in, nmatches [nKF2] and matches12 [nKF2][N1] out to the given destinations (device only when null).
-// After the caller has declared its own pieces and reserved, tri_launch fills the pair table, uploads everything in ONE copy
-// and runs tri_match_kernel on the handle's stream.
+// The SearchForTriangulation part (KF1 against nKF2 neighbours) shared by orbm_search_for_triangulation and the CreateNewMapPoints
+// calls.  tri_stage declares one item's inputs on the matcher's staging: the level tables, KF1 and every neighbour's arrays.  After the
+// caller has declared the item and pair tables and its own pieces and reserved, tri_fill writes the item's TriItem and its nKF2 TriPairs
+// into the tables' host mirrors; the caller then uploads everything in ONE copy and runs tri_match_kernel over all pairs.
 struct TriPieces {
-    int sf, sg, kp1, de1, mp1, fn1, ff1, tab, cnt, m12, ev;
+    int sf, sg, kp1, de1, mp1, fn1, ff1;
     struct Neighbour { int kp, de, mp, fn, ff; };
     std::vector<Neighbour> kf2;
 };
 static TriPieces tri_stage(Staging& S, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
-                           int nlevels, int32_t* nmatches, int32_t* matches12) {
-    const size_t N1 = (size_t)KF1->N, E1 = (size_t)KF1->nEntries, K = (size_t)nKF2;
+                           int nlevels) {
+    const size_t N1 = (size_t)KF1->N, E1 = (size_t)KF1->nEntries;
     TriPieces t;
     t.sf = S.in(scaleFactors, 4 * (size_t)nlevels); t.sg = S.in(levelSigma2, 4 * (size_t)nlevels);
     t.kp1 = S.in(KF1->keypoints, sizeof(OrbKeyPoint) * N1); t.de1 = S.in(KF1->descriptors, 32 * N1); t.mp1 = S.in(KF1->hasMapPoint, N1);
@@ -1998,35 +2022,26 @@ static TriPieces tri_stage(Staging& S, const OrbmTriFrame* KF1, int nKF2, const 
         t.kf2.push_back({S.in(KF2[k].keypoints, sizeof(OrbKeyPoint) * N2), S.in(KF2[k].descriptors, 32 * N2), S.in(KF2[k].hasMapPoint, N2),
                          S.in(KF2[k].fvNode, 4 * E2), S.in(KF2[k].fvFeature, 4 * E2)});
     }
-    t.tab = S.in(nullptr, sizeof(TriPair) * K);
-    t.cnt = nmatches ? S.out(nmatches, 4 * K) : S.scratch(4 * K);
-    t.m12 = matches12 ? S.out(matches12, 4 * N1 * K) : S.scratch(4 * N1 * K);
-    t.ev = S.scratch(N1 * K);
     return t;
 }
-static int tri_launch(Matcher& m, const TriPieces& t, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* ep2, const float* F12,
-                      int bCoarse, int checkOrientation, TriParams* Q) {
-    Staging& S = m.staging;
+// item: the item's row in the item table; m12 / cnt / ev: device addresses of its matches12 [nKF2][N1], nmatches [nKF2] and bins [nKF2][N1].
+static void tri_fill(const Staging& S, const TriPieces& t, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* ep2, const float* F12,
+                     int bCoarse, int item, int* m12, int* cnt, uint8_t* ev, TriItem* itemRow, TriPair* pairRows) {
     const size_t N1 = (size_t)KF1->N;
-    TriPair* tab = S.host<TriPair>(t.tab);
+    TriItem Q; memset(&Q, 0, sizeof(Q));
+    Q.N1 = (int)N1; Q.E1 = KF1->nEntries; Q.coarse = bCoarse;
+    Q.kps1 = S.dev<OrbKeyPoint>(t.kp1); Q.desc1 = S.dev(t.de1); Q.hasMP1 = S.dev(t.mp1); Q.fvNode1 = S.dev<int>(t.fn1); Q.fvFeat1 = S.dev<int>(t.ff1);
+    Q.scaleFactors = S.dev<float>(t.sf); Q.levelSigma2 = S.dev<float>(t.sg);
+    memcpy(itemRow, &Q, sizeof(Q));
     for (int k = 0; k < nKF2; ++k) {
         const TriPieces::Neighbour& p = t.kf2[k];
         TriPair T; memset(&T, 0, sizeof(T));
-        T.N2 = KF2[k].N; T.E2 = KF2[k].nEntries;
+        T.item = item; T.N2 = KF2[k].N; T.E2 = KF2[k].nEntries;
         T.kps2 = S.dev<OrbKeyPoint>(p.kp); T.desc2 = S.dev(p.de); T.hasMP2 = S.dev(p.mp); T.fvNode2 = S.dev<int>(p.fn); T.fvFeat2 = S.dev<int>(p.ff);
         memcpy(T.ep, ep2 + 2 * (size_t)k, 8); memcpy(T.F12, F12 + 9 * (size_t)k, 36);
-        T.matches12 = S.dev<int>(t.m12) + (size_t)k * N1; T.nmatches = S.dev<int>(t.cnt) + k; T.evBin = S.dev(t.ev) + (size_t)k * N1;
-        memcpy(tab + k, &T, sizeof(T));
+        T.matches12 = m12 + (size_t)k * N1; T.nmatches = cnt + k; T.evBin = ev + (size_t)k * N1;
+        memcpy(pairRows + k, &T, sizeof(T));
     }
-    cudaStream_t st = m.stream;
-    CK(S.upload(st));
-    memset(Q, 0, sizeof(*Q));
-    Q->N1 = (int)N1; Q->E1 = KF1->nEntries; Q->coarse = bCoarse; Q->checkOri = checkOrientation;
-    Q->kps1 = S.dev<OrbKeyPoint>(t.kp1); Q->desc1 = S.dev(t.de1); Q->hasMP1 = S.dev(t.mp1); Q->fvNode1 = S.dev<int>(t.fn1); Q->fvFeat1 = S.dev<int>(t.ff1);
-    Q->scaleFactors = S.dev<float>(t.sf); Q->levelSigma2 = S.dev<float>(t.sg); Q->pairs = S.dev<TriPair>(t.tab);
-    tri_match_kernel<<<nKF2, TM_NT, 0, st>>>(*Q);
-    CK(cudaGetLastError());
-    return ORB_OK;
 }
 
 int orbm_search_for_triangulation(orbm_handle* h, const OrbmTriFrame* KF1, int nKF2, const OrbmTriFrame* KF2, const float* scaleFactors, const float* levelSigma2,
@@ -2041,70 +2056,140 @@ int orbm_search_for_triangulation(orbm_handle* h, const OrbmTriFrame* KF1, int n
     if (nKF2 == 0) return ORB_OK;
     Matcher& m = h->m;
     CK(cudaSetDevice(m.device));
-    const size_t N1 = (size_t)KF1->N;
-    for (size_t i = 0; i < (size_t)nKF2 * N1; ++i) matches12[i] = -1;
+    const size_t N1 = (size_t)KF1->N, K = (size_t)nKF2;
+    for (size_t i = 0; i < K * N1; ++i) matches12[i] = -1;
     for (int k = 0; k < nKF2; ++k) nmatches[k] = 0;
     if (N1 == 0) return ORB_OK;
-    m.staging.begin();
-    const TriPieces t = tri_stage(m.staging, KF1, nKF2, KF2, scaleFactors, levelSigma2, nlevels, nmatches, matches12);
-    int rc = m.staging.reserve();
+    Staging& S = m.staging;
+    S.begin();
+    const TriPieces t = tri_stage(S, KF1, nKF2, KF2, scaleFactors, levelSigma2, nlevels);
+    const int pItem = S.in(nullptr, sizeof(TriItem)), pPairs = S.in(nullptr, sizeof(TriPair) * K), pCnt = S.out(nmatches, 4 * K),
+              pM12 = S.out(matches12, 4 * N1 * K), pEv = S.scratch(N1 * K);
+    int rc = S.reserve();
     if (rc) return rc;
+    tri_fill(S, t, KF1, nKF2, KF2, ep2, F12, bCoarse, 0, S.dev<int>(pM12), S.dev<int>(pCnt), S.dev(pEv), S.host<TriItem>(pItem), S.host<TriPair>(pPairs));
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
     TriParams Q;
-    if ((rc = tri_launch(m, t, KF1, nKF2, KF2, ep2, F12, bCoarse, checkOrientation, &Q))) return rc;
+    Q.checkOri = checkOrientation; Q.items = S.dev<TriItem>(pItem); Q.pairs = S.dev<TriPair>(pPairs);
+    tri_match_kernel<<<nKF2, TM_NT, 0, st>>>(Q);
     m.launches = 1;
-    CK(m.staging.download(m.stream));
+    CK(cudaGetLastError());
+    CK(S.download(st));
+    return ORB_OK;
+}
+
+// LocalMapping::CreateNewMapPoints for nItems new keyframes, the single call being a batch of one.  Every item is checked before anything
+// is staged; then one upload, tri_match_kernel over every (item, neighbour) pair, new_points_kernel over every (pair, idx1), one
+// new_points_commit_kernel CTA per item, one download.  An item with nKF2 == 0 or KF1.N == 0 gets zero counts and takes no CTA.
+static int new_points_run(orbm_handle* h, int nItems, const OrbmNewPointsItem* items, bool batch) {
+    const std::string who = batch ? "orbm_create_new_map_points_batch" : "orbm_create_new_map_points";
+    auto fail = [&](int rc, int j, const char* what) {
+        set_error(who + (batch ? ": item " + std::to_string(j) + ": " : std::string(": ")) + what);
+        return rc;
+    };
+    constexpr size_t MAX_PAIRS = 65535;       // new_points_kernel's gridDim.y
+    size_t nPairs = 0;
+    int over = -1;
+    for (int j = 0; j < nItems; ++j) {
+        const OrbmNewPointsItem& it = items[j];
+        const OrbmNewPointsIn& in = it.in;
+        if (!it.nNew || in.nKF2 < 0 || !tri_frame_ok(in.KF1) || (in.KF1->N && !it.out) ||
+            (in.nKF2 && (!in.KF2 || !in.ep2 || !in.F12 || !it.nmatches || !it.ncreated)) || !in.scaleFactors || !in.levelSigma2 || in.nlevels < 1 ||
+            in.nlevels > 256 || !in.Tcw || !in.Ow || !in.cam || !(in.scaleFactor > 0.0f) || !(in.thFarPoints >= 0.0f))
+            return fail(ORB_ERR_ARG, j, "bad argument (feature vectors must be sorted by node id, indices in range; Tcw / Ow / cam for 1 + nKF2 keyframes)");
+        const OrbmTriFrame* KF1 = in.KF1;
+        const int nl = in.nlevels;
+        for (int i = 0; i < KF1->N; ++i) if (KF1->keypoints[i].octave < 0 || KF1->keypoints[i].octave >= nl) return fail(ORB_ERR_ARG, j, "keypoint octave out of range");
+        for (int k = 0; k < in.nKF2; ++k) {
+            if (!tri_frame_ok(in.KF2 + k)) return fail(ORB_ERR_ARG, j, "bad KF2 entry");
+            for (int i = 0; i < in.KF2[k].N; ++i) if (in.KF2[k].keypoints[i].octave < 0 || in.KF2[k].keypoints[i].octave >= nl) return fail(ORB_ERR_ARG, j, "keypoint octave out of range");
+        }
+        if (KF1->N > 0) nPairs += (size_t)in.nKF2;
+        if (nPairs > MAX_PAIRS && over < 0) over = j;
+    }
+    if (over >= 0) return fail(ORB_ERR_CAPACITY, over, "more than 65535 (keyframe, neighbour) pairs in one call");
+    std::vector<int> act;
+    for (int j = 0; j < nItems; ++j) {
+        const OrbmNewPointsItem& it = items[j];
+        *it.nNew = 0;
+        for (int k = 0; k < it.in.nKF2; ++k) { it.nmatches[k] = 0; it.ncreated[k] = 0; }
+        if (it.in.nKF2 > 0 && it.in.KF1->N > 0) act.push_back(j);
+    }
+    Matcher& m = h->m;
+    if (act.empty()) {
+        if (batch) m.launches = 0;
+        return ORB_OK;
+    }
+    CK(cudaSetDevice(m.device));
+    Staging& S = m.staging;
+    S.begin();
+    // per item: its search inputs, Tcw / Ow / cam, counts = {nNew, nmatches [K], ncreated [K]} and its records (the first nNew go to `out`)
+    struct Pieces { TriPieces t; int tcw, ow, cam, cnt, out; };
+    std::vector<Pieces> pc(act.size());
+    size_t nSlots = 0, sumN1 = 0;
+    int maxN1 = 0;
+    for (size_t a = 0; a < act.size(); ++a) {
+        const OrbmNewPointsIn& in = items[act[a]].in;
+        const size_t N1 = (size_t)in.KF1->N, K = (size_t)in.nKF2;
+        Pieces& p = pc[a];
+        p.t = tri_stage(S, in.KF1, in.nKF2, in.KF2, in.scaleFactors, in.levelSigma2, in.nlevels);
+        p.tcw = S.in(in.Tcw, 48 * (K + 1)); p.ow = S.in(in.Ow, 12 * (K + 1)); p.cam = S.in(in.cam, 16 * (K + 1));
+        p.cnt = S.out(nullptr, 4 * (1 + 2 * K)); p.out = S.out(nullptr, sizeof(OrbmNewPoint) * N1);
+        nSlots += K * N1; sumN1 += N1; maxN1 = std::max(maxN1, in.KF1->N);
+    }
+    const int pTri = S.in(nullptr, sizeof(TriItem) * act.size()), pNp = S.in(nullptr, sizeof(NpItem) * act.size()), pPairs = S.in(nullptr, sizeof(TriPair) * nPairs),
+              pM12 = S.scratch(4 * nSlots), pEv = S.scratch(nSlots), pNm = S.scratch(4 * nPairs), pReason = S.scratch(nSlots),
+              pRecs = S.scratch(sizeof(OrbmNewPoint) * nSlots), pWin = S.scratch(4 * sumN1);
+    int rc = S.reserve();
+    if (rc) return rc;
+    size_t pair = 0, slot = 0, win = 0;
+    for (size_t a = 0; a < act.size(); ++a) {
+        const OrbmNewPointsIn& in = items[act[a]].in;
+        const Pieces& p = pc[a];
+        tri_fill(S, p.t, in.KF1, in.nKF2, in.KF2, in.ep2, in.F12, in.bCoarse, (int)a, S.dev<int>(pM12) + slot, S.dev<int>(pNm) + pair, S.dev(pEv) + slot,
+                 S.host<TriItem>(pTri) + a, S.host<TriPair>(pPairs) + pair);
+        NpItem J; memset(&J, 0, sizeof(J));
+        J.pair0 = (int)pair; J.nKF2 = in.nKF2; J.nlevels = in.nlevels; J.bInertial = in.bInertial ? 1 : 0;
+        J.ratioFactor = 1.5f * in.scaleFactor; J.thFar = in.thFarPoints; J.slot0 = slot;
+        J.Tcw = S.dev<float>(p.tcw); J.Ow = S.dev<float>(p.ow); J.cam = S.dev<float>(p.cam);
+        J.winner = S.dev<int>(pWin) + win; J.counts = S.dev<int>(p.cnt); J.out = S.dev<OrbmNewPoint>(p.out);
+        memcpy(S.host<NpItem>(pNp) + a, &J, sizeof(J));
+        pair += (size_t)in.nKF2; slot += (size_t)in.nKF2 * in.KF1->N; win += (size_t)in.KF1->N;
+    }
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    TriParams Q;
+    Q.checkOri = 0; Q.items = S.dev<TriItem>(pTri); Q.pairs = S.dev<TriPair>(pPairs);
+    tri_match_kernel<<<(unsigned)nPairs, TM_NT, 0, st>>>(Q);
+    NewPointsParams P;
+    P.tri = Q.items; P.items = S.dev<NpItem>(pNp); P.pairs = Q.pairs;
+    P.matches12 = S.dev<int>(pM12); P.reason = S.dev(pReason); P.recs = S.dev<OrbmNewPoint>(pRecs);
+    new_points_kernel<<<dim3((unsigned)((maxN1 + NP_NT - 1) / NP_NT), (unsigned)nPairs), NP_NT, 0, st>>>(P);
+    new_points_commit_kernel<<<(unsigned)act.size(), NPC_NT, 0, st>>>(P);
+    m.launches = 3;
+    CK(cudaGetLastError());
+    CK(S.download(st));
+    for (size_t a = 0; a < act.size(); ++a) {
+        const OrbmNewPointsItem& it = items[act[a]];
+        const size_t K = (size_t)it.in.nKF2;
+        const int* cnt = S.host<int>(pc[a].cnt);
+        *it.nNew = cnt[0];
+        memcpy(it.nmatches, cnt + 1, 4 * K); memcpy(it.ncreated, cnt + 1 + K, 4 * K);
+        memcpy(it.out, S.host(pc[a].out), sizeof(OrbmNewPoint) * (size_t)cnt[0]);
+    }
     return ORB_OK;
 }
 
 int orbm_create_new_map_points(orbm_handle* h, const OrbmNewPointsIn* in, OrbmNewPoint* out, int* nNew, int32_t* nmatches, int32_t* ncreated) {
-    if (!h || !in || !nNew || in->nKF2 < 0 || !tri_frame_ok(in->KF1) || (in->KF1->N && !out) ||
-        (in->nKF2 && (!in->KF2 || !in->ep2 || !in->F12 || !nmatches || !ncreated)) || !in->scaleFactors || !in->levelSigma2 || in->nlevels < 1 ||
-        in->nlevels > 256 || !in->Tcw || !in->Ow || !in->cam || !(in->scaleFactor > 0.0f) || !(in->thFarPoints >= 0.0f)) {
-        set_error("orbm_create_new_map_points: bad argument (feature vectors must be sorted by node id, indices in range; Tcw / Ow / cam for 1 + nKF2 keyframes)");
-        return ORB_ERR_ARG;
-    }
-    const OrbmTriFrame* KF1 = in->KF1;
-    const int nKF2 = in->nKF2, nl = in->nlevels;
-    for (int i = 0; i < KF1->N; ++i) if (KF1->keypoints[i].octave < 0 || KF1->keypoints[i].octave >= nl) { set_error("orbm_create_new_map_points: keypoint octave out of range"); return ORB_ERR_ARG; }
-    for (int k = 0; k < nKF2; ++k) {
-        if (!tri_frame_ok(in->KF2 + k)) { set_error("orbm_create_new_map_points: bad KF2 entry"); return ORB_ERR_ARG; }
-        for (int i = 0; i < in->KF2[k].N; ++i) if (in->KF2[k].keypoints[i].octave < 0 || in->KF2[k].keypoints[i].octave >= nl) { set_error("orbm_create_new_map_points: keypoint octave out of range"); return ORB_ERR_ARG; }
-    }
-    *nNew = 0;
-    for (int k = 0; k < nKF2; ++k) { nmatches[k] = 0; ncreated[k] = 0; }
-    const size_t N1 = (size_t)KF1->N, K = (size_t)nKF2;
-    if (K == 0 || N1 == 0) return ORB_OK;
-    Matcher& m = h->m;
-    CK(cudaSetDevice(m.device));
-    Staging& S = m.staging;
-    S.begin();
-    const TriPieces t = tri_stage(S, KF1, nKF2, in->KF2, in->scaleFactors, in->levelSigma2, nl, nullptr, nullptr);
-    // counts = {nNew, nmatches [K], ncreated [K]}; only the first nNew records go to `out`
-    const int pTcw = S.in(in->Tcw, 48 * (K + 1)), pOw = S.in(in->Ow, 12 * (K + 1)), pCam = S.in(in->cam, 16 * (K + 1)), pReason = S.scratch(K * N1),
-              pRecs = S.scratch(sizeof(OrbmNewPoint) * K * N1), pWin = S.scratch(4 * N1), pCounts = S.out(nullptr, 4 * (1 + 2 * K)),
-              pOut = S.out(nullptr, sizeof(OrbmNewPoint) * N1);
-    int rc = S.reserve();
-    if (rc) return rc;
-    TriParams Q;
-    if ((rc = tri_launch(m, t, KF1, nKF2, in->KF2, in->ep2, in->F12, in->bCoarse, 0, &Q))) return rc;
-    NewPointsParams P; memset(&P, 0, sizeof(P));
-    P.N1 = (int)N1; P.nKF2 = nKF2; P.nlevels = nl; P.bInertial = in->bInertial ? 1 : 0;
-    P.ratioFactor = 1.5f * in->scaleFactor; P.thFar = in->thFarPoints;
-    P.kps1 = Q.kps1; P.pairs = Q.pairs; P.matches12 = S.dev<int>(t.m12);
-    P.scaleFactors = Q.scaleFactors; P.levelSigma2 = Q.levelSigma2;
-    P.Tcw = S.dev<float>(pTcw); P.Ow = S.dev<float>(pOw); P.cam = S.dev<float>(pCam);
-    P.reason = S.dev(pReason); P.recs = S.dev<OrbmNewPoint>(pRecs); P.winner = S.dev<int>(pWin); P.counts = S.dev<int>(pCounts); P.out = S.dev<OrbmNewPoint>(pOut);
-    cudaStream_t st = m.stream;
-    new_points_kernel<<<dim3((unsigned)((N1 + NP_NT - 1) / NP_NT), (unsigned)K), NP_NT, 0, st>>>(P);
-    new_points_commit_kernel<<<1, NPC_NT, 0, st>>>(P);
-    m.launches = 3;
-    CK(cudaGetLastError());
-    CK(S.download(st));
-    const int* cnt = S.host<int>(pCounts);
-    *nNew = cnt[0];
-    memcpy(nmatches, cnt + 1, 4 * K); memcpy(ncreated, cnt + 1 + K, 4 * K);
-    memcpy(out, S.host(pOut), sizeof(OrbmNewPoint) * (size_t)cnt[0]);
-    return ORB_OK;
+    if (!h || !in) { set_error("orbm_create_new_map_points: bad argument"); return ORB_ERR_ARG; }
+    const OrbmNewPointsItem it = {*in, out, nNew, nmatches, ncreated};
+    return new_points_run(h, 1, &it, false);
+}
+
+int orbm_create_new_map_points_batch(orbm_handle* h, int nItems, const OrbmNewPointsItem* items) {
+    if (!h || nItems < 0 || (nItems > 0 && !items)) { set_error("orbm_create_new_map_points_batch: bad argument"); return ORB_ERR_ARG; }
+    return new_points_run(h, nItems, items, true);
 }
 
 int orbm_distinctive_descriptors(orbm_handle* h, int nPoints, const int32_t* obsStart, const uint8_t* descriptors, int32_t* best) {
