@@ -738,9 +738,14 @@ int lba_download_batch(lba_handle* h, int count, LbaResult* results);
 int lba_last_cluster_size(const lba_handle* h);
 /* Force the cluster size (1..8 CTAs per problem; 0 = automatic: the largest for which every problem's cluster is resident at once). */
 int lba_set_cluster_size(lba_handle* h, int ctas);
-/* Device-side phase timers (ns, CTA 0) of problem i of the last downloaded run: errors (first iteration), build_points,
- * build_poses, point_prep (after a rejected step), schur_partial, ldlt, schur_combine, pose_trial, points_trial (back-substitution +
- * update + residuals), spare. */
+/* Helper clusters: a batch whose clusters leave SMs idle is launched with extra clusters of the same size that serve the chunked
+ * phases (build, point records, Schur partial sums) of every problem; results do not depend on them.  -1 (default): as many as
+ * are resident beside the batch; 0: none; n > 0: at most n.  lba_last_helpers: helper clusters of the last run. */
+int lba_set_helpers(lba_handle* h, int clusters);
+int lba_last_helpers(const lba_handle* h);
+/* Device-side phase timers (ns, CTA 0) of problem i of the last downloaded run: errors (first iteration), build_points +
+ * build_poses partial sums, build_poses combine, point_prep (after a rejected step), schur_partial, ldlt, schur_combine, pose_trial, points_trial
+ * (back-substitution + update + residuals), and last a count instead of a time: the chunks helper clusters served for problem i. */
 int lba_get_phase_ns(const lba_handle* h, int i, double* ns10);
 
 /* ------------------------------------------------------------------------------------------

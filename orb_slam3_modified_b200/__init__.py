@@ -116,6 +116,8 @@ SIGNATURES = {
     'lba_download_batch': (_i, [_vp, _i, _vp]),
     'lba_last_cluster_size': (_i, [_vp]),
     'lba_set_cluster_size': (_i, [_vp, _i]),
+    'lba_last_helpers': (_i, [_vp]),
+    'lba_set_helpers': (_i, [_vp, _i]),
     'lba_get_phase_ns': (_i, [_vp, _i, _vp]),
     'pose_optimization_batch': (_i, [_i, _i] + [_vp] * 6 + [_d] + [_vp] * 3 + [_i]),
     'imu_preintegrate_batch': (_i, [_i, _vp, _i] + [_vp] * 6 + [_i]),
@@ -1220,6 +1222,14 @@ class Optimizer:
         rc = lib().lba_set_cluster_size(self._h, ctas)
         if rc != ORB_OK:
             raise OrbError(rc, 'lba_set_cluster_size')
+
+    def last_helpers(self):
+        return lib().lba_last_helpers(self._h)
+
+    def set_helpers(self, clusters):
+        rc = lib().lba_set_helpers(self._h, clusters)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'lba_set_helpers')
 
     def LocalBundleAdjustment(self, prob, iterations=10, user_lambda_init=0.0, stop_flag=None):
         keep = dict(poses=_c(prob['poses'], np.float64), fixed=_c(prob['fixed'], np.uint8), cam=_c(prob['cam'], np.float32),

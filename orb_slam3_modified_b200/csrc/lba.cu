@@ -5,6 +5,8 @@
 // (1..8 CTAs, chosen so that the batch fills the 132 SMs); the whole Levenberg-Marquardt loop -- accept/reject,
 // lambda schedule, stop rules, stop-flag polling -- runs on the device, phases are separated by cluster barriers,
 // and the host only uploads the flattened graph and downloads the result.  All arithmetic is FP64 (g2o is double).
+// SMs the batch's clusters leave idle run helper clusters, which serve chunks of the build, point-record and Schur phases of
+// any problem (owner_phase / helper_loop); the results do not depend on which CTA serves a chunk.
 // The linearisation is kept FACTORED: an edge stores only (x/z, y/z, 1/z, robust weight) at the linearisation point (32 B);
 // its Jacobians are A = -S t (2x3, t = [R0 - xn R2; R1 - yn R2], S = diag(fx, fy)/z) and B = F b (2x6, F = diag(fx, fy),
 // b a polynomial in xn, yn, 1/z), so the Hpl block W = w B^T A is rank 2 and is never materialised: every product that
@@ -42,8 +44,24 @@ namespace lba {
 using namespace g2o;
 using orbx::block_sum;
 
+// The open data-parallel phase of one problem, in global memory: CTA 0 of the problem's cluster opens a phase, and the owner CTAs
+// and any helper CTA claim its chunks NWARP at a time.  `word` = tag (16 bits) | chunks (24) | next unclaimed chunk (24): one
+// atomicAdd claims, and a claim whose next chunk is past the count gets nothing.  A granted chunk pins the phase (its fields and
+// the pose-cache mirror) until `done` counts it, so a claimer reads them after the claim.
+struct Job {
+    unsigned long long word;
+    unsigned done;                    // chunks finished this launch, all phases (each phase's join waits for its running total)
+    unsigned helped;                  // of those, chunks served by helper CTAs
+    unsigned seq;                     // phases opened this launch
+    int phase, side;                  // PH_*, which side of the double buffers is current (LoopState::cur)
+    double lambda;
+};
+constexpr int PH_BUILD = 0, PH_PREP = 1, PH_SCHUR = 2;
+
 struct Dev {
     int nP, nL, nE, nF, n;            // n = 6 nF
+    Job* job;
+    double* pcm;                      // nP x PC: the pose cache of the open phase, for helper CTAs
     double *poses, *posesB, *pts, *ptsB;        // nP x 7, nL x 3: estimate / second buffer (trial state; the two swap when a step is accepted)
     const double *initPoses, *initPts;          // the uploaded initial estimates (a run always restarts from them)
     // the caller's graph as uploaded (caller's edge order); lba_build_structure_kernel derives everything below from it
@@ -308,28 +326,29 @@ __device__ __forceinline__ void add_build_edge(const double* pcache, const Build
     h[0] += c0 * t[0] * t[0] + c1 * t[3] * t[3]; h[1] += c0 * t[0] * t[1] + c1 * t[3] * t[4]; h[2] += c0 * t[0] * t[2] + c1 * t[3] * t[5];
     h[3] += c0 * t[1] * t[1] + c1 * t[4] * t[4]; h[4] += c0 * t[1] * t[2] + c1 * t[4] * t[5]; h[5] += c0 * t[2] * t[2] + c1 * t[5] * t[5];
 }
-// ---- per point Hll, bl (and, when lambda is already known, the point record of phase_point_prep); 8 lanes per point
-//      (the edges of a point are contiguous) ----
-__device__ void phase_build_points(const Dev& D, const Ctx& c, const double* __restrict__ E, double lambda) {
-    constexpr int FLY = FLY_BP;
-    const int sl = c.tid() & 7;
-    const unsigned gmask = 0xFFu << (c.tid() & 24);
-    const int G = c.nw() >> 3;
+constexpr int PCH = 32;            // points per chunk of the per-point phases (build_points, point_prep)
+// ---- per point Hll, bl (and, when lambda is already known, the point record of point_prep_chunk); 8 lanes per point
+//      (the edges of a point are contiguous); one warp per chunk of PCH points ----
+__device__ __forceinline__ void build_points_chunk(const Dev& D, const double* pc, const double* __restrict__ E, double lambda, int ch) {
+    constexpr int FLY = FLY_BP, G = 4;
+    const int sl = threadIdx.x & 7;
+    const unsigned gmask = 0xFFu << (threadIdx.x & 24);
+    const int first = ch * PCH + ((threadIdx.x & 31) >> 3), end = min(D.nL, (ch + 1) * PCH);
     int a[FLY], b[FLY];
-    step_ranges<FLY>(D.ptStart, D.nL, c.wid() >> 3, G, a, b);
-    for (int p0 = c.wid() >> 3; p0 < D.nL; p0 += FLY * G) {
+    step_ranges<FLY>(D.ptStart, end, first, G, a, b);
+    for (int p0 = first; p0 < end; p0 += FLY * G) {
         BuildEdge first[FLY] = {};
 #pragma unroll
         for (int j = 0; j < FLY; ++j) if (a[j] + sl < b[j]) first[j] = load_build_edge(D, E, a[j] + sl);
         int na[FLY], nb[FLY];
-        step_ranges<FLY>(D.ptStart, D.nL, p0 + FLY * G, G, na, nb);
+        step_ranges<FLY>(D.ptStart, end, p0 + FLY * G, G, na, nb);
 #pragma unroll
         for (int j = 0; j < FLY; ++j) {
             const int p = p0 + j * G;
-            if (p >= D.nL) break;
+            if (p >= end) break;
             double h[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0};
-            if (a[j] + sl < b[j]) add_build_edge(c.pc, first[j], h, g);
-            for (int e = a[j] + sl + 8; e < b[j]; e += 8) add_build_edge(c.pc, load_build_edge(D, E, e), h, g);
+            if (a[j] + sl < b[j]) add_build_edge(pc, first[j], h, g);
+            for (int e = a[j] + sl + 8; e < b[j]; e += 8) add_build_edge(pc, load_build_edge(D, E, e), h, g);
 #pragma unroll
             for (int o = 4; o; o >>= 1) {
 #pragma unroll
@@ -359,13 +378,12 @@ constexpr int UNR = LBA_UNR;       // items in flight per lane in the Schur chun
 //      that the Schur phase reads (coalesced stores; the factors stay fixed for all trials of an iteration).
 //      As in the Schur chunks, the chunk's edge ids are loaded into registers up front; then the factors and errors of FLY
 //      items per lane are loaded before their K stores and their sums, which keep the item order of the lane. ----
-__device__ void phase_build_poses_partial(const Dev& D, const Ctx& c, const double* __restrict__ E) {
+__device__ __forceinline__ void build_poses_chunk(const Dev& D, const double* pc, const double* __restrict__ E, int ch) {
     constexpr int FLY = FLY_BPP;
-    const int lane = c.tid() & 31;
-    const int nDiag = D.taskChunkStart[D.nF], step = c.csize() * NWARP;
-    for (int ch = c.crank() * NWARP + (c.tid() >> 5); ch < nDiag; ch += step) {
+    const int lane = threadIdx.x & 31;
+    {
         const int4 h = D.chunkHdr[ch];
-        const double* P = c.pc + PC * h.z;
+        const double* P = pc + PC * h.z;
         const double fx = P[16], fy = P[17];
         int re[IPL];
 #pragma unroll
@@ -465,9 +483,9 @@ __device__ __forceinline__ void load_dinv(const double2* __restrict__ PT, size_t
     const double2 a = PT[p], b = PT[nL + p], c = PT[2 * nL + p];
     dv[0] = a.x; dv[1] = a.y; dv[2] = b.x; dv[3] = b.y; dv[4] = c.x; dv[5] = c.y;
 }
-__device__ void phase_point_prep(const Dev& D, const Ctx& c, double lambda) {
-    const int nw = c.nw();
-    for (int p = c.wid(); p < D.nL; p += nw) {
+__device__ __forceinline__ void point_prep_chunk(const Dev& D, double lambda, int ch) {
+    const int p = ch * PCH + (threadIdx.x & 31);
+    if (p < D.nL) {
         const double2* H = reinterpret_cast<const double2*>(D.Hll + 6 * (size_t)p);
         const double2 h01 = H[0], h23 = H[1], h45 = H[2];
         const double h[6] = {h01.x, h01.y, h23.x, h23.y, h45.x, h45.y};
@@ -590,17 +608,37 @@ __device__ __forceinline__ void schur_chunk_diag(const int* __restrict__ poseEdg
     if (n > 0) out[0] = acc[0];
     if (n > 1) out[1] = acc[1];
 }
-__device__ void phase_schur_partial(const Dev& D, const Ctx& c, const double2* __restrict__ K) {
-    // CTA barrier at entry: the previous phase (combine of the pose sums) leaves the warps of a CTA out of step, and warps that
-    // enter this gather-bound phase out of step ran it 3x slower (measured); a barrier per round of chunks on top was slower again.
-    __syncthreads();
-    const int step = c.csize() * NWARP;
-    for (int ch = c.crank() * NWARP + (c.tid() >> 5); ch < D.nChunks; ch += step) {
+// ---- one chunk of the open phase of a problem, by one warp.  Owner CTAs and helper CTAs both serve chunks through this one
+//      function, kept out of line so that there is one compiled copy of every chunk's arithmetic: ptxas contracts products into
+//      FMAs depending on the surrounding code, and a chunk must give the same bits whichever CTA serves it.
+//      BUILD: chunks [0, nPointChunks) are build_points chunks, the rest the build_poses chunks (the diagonal Schur chunks). ----
+__device__ __noinline__ void serve_chunk(const Dev& D, const double* pc, int phase, int side, double lambda, int ch) {
+    if (phase == PH_SCHUR) {
         const int4 h = D.chunkHdr[ch];      // first item, items, pose A, pose B (-1: diagonal task)
-        if (h.w >= 0) schur_chunk_offdiag(D.pairs, D.pairPt, D.PT, D.nL, K, D.nE, c.pc, D.Spart + 42 * (size_t)ch, h);
-        else schur_chunk_diag(D.poseEdgePt, D.PT, D.nL, K, D.nE, c.pc, D.Spart + 42 * (size_t)ch, h);
+        if (h.w >= 0) schur_chunk_offdiag(D.pairs, D.pairPt, D.PT, D.nL, D.K, D.nE, pc, D.Spart + 42 * (size_t)ch, h);
+        else schur_chunk_diag(D.poseEdgePt, D.PT, D.nL, D.K, D.nE, pc, D.Spart + 42 * (size_t)ch, h);
+    } else if (phase == PH_PREP) {
+        point_prep_chunk(D, lambda, ch);
+    } else {
+        const double* E = side ? D.E4b : D.E4a;
+        const int nPtCh = (D.nL + PCH - 1) / PCH;
+        if (ch < nPtCh) build_points_chunk(D, pc, E, lambda, ch);
+        else build_poses_chunk(D, pc, E, ch - nPtCh);
     }
 }
+
+__device__ __forceinline__ unsigned long long ld_acquire(const unsigned long long* p) {
+    unsigned long long v; asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
+    unsigned v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ unsigned long long ld_relaxed(const unsigned long long* p) {
+    unsigned long long v; asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ unsigned job_tag(unsigned long long w) { return (unsigned)(w >> 48); }
+__device__ __forceinline__ int job_count(unsigned long long w) { return (int)((w >> 24) & 0xFFFFFF); }
+__device__ __forceinline__ int job_next(unsigned long long w) { return (int)(w & 0xFFFFFF); }
 __device__ void phase_schur_combine(const Dev& D, const Ctx& c, double lambda, double* Hs, int ld) {
     const int nOff = D.nF * (D.nF - 1) / 2, nTasks = D.nF + nOff;
     const int nw = c.nw();
@@ -918,8 +956,120 @@ struct LoopState {
     int cj = 0, trials = 0, qmax = 0, term = 0, ok = 1;
     int cur = 0;                        // the side of the double buffers that holds the current state: 0 = (E4a, poses, pts), 1 = (E4b, posesB, ptsB)
     bool accepted = false, more = false;   // the last trial was accepted / the iteration runs another trial
+    unsigned seq = 0, doneTarget = 0;      // phases opened so far (Job::seq) and the chunks they hold (Job::done once they are joined)
 };
-__global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __restrict__ probs, const volatile int* stop, int smemMatrixN, int maxP, int maxF) {
+__shared__ int2 s_grant;                   // the claim group of a helper CTA: chunks [x, y)
+__device__ __forceinline__ unsigned long long job_word(unsigned seq, int nCh) {
+    return ((unsigned long long)(seq % 65535u + 1u) << 48) | ((unsigned long long)nCh << 24);
+}
+// ---- a data-parallel phase of nCh chunks in the owner cluster: CTA 0 opens it (pose-cache mirror, phase fields, then the claim
+//      word with release semantics), every owner CTA claims and serves chunks until the word is exhausted, then waits with its
+//      own acquire until the problem's done count holds every chunk of the phase (helper CTAs may have served some).  The owners
+//      never wait for a helper to start, so the result and the progress do not depend on helpers being resident. ----
+__device__ void owner_phase(const Dev& D, LoopState& S, const double* pc, int phase, int side, double lambda, int nCh) {
+    Job* J = D.job;
+    const int tid = threadIdx.x;
+    if (sreg_ctarank() == 0) {
+        for (int i = tid; i < PC * D.nP; i += NT) D.pcm[i] = pc[i];
+        if (tid == 0) { J->phase = phase; J->side = side; J->lambda = lambda; J->seq = S.seq + 1; }
+        __syncthreads();
+        if (tid == 0) { __threadfence(); atomicExch(&J->word, job_word(S.seq + 1, nCh)); }
+    }
+    if (tid == 0) {
+        ++S.seq; S.doneTarget += nCh;
+        const unsigned tag = (unsigned)(job_word(S.seq, 0) >> 48);
+        while (job_tag(ld_acquire(&J->word)) != tag) __nanosleep(32);      // ranks > 0 may arrive before CTA 0 has opened it
+    }
+    __syncthreads();
+    // the owner's warps claim one chunk at a time on their own: no CTA barrier inside the loop, and a warp's release of its
+    // chunk stalls only that warp.  (Every claim an owner makes is of this phase: CTA 0 opens the next one only after a
+    // cluster barrier that every owner thread reaches after leaving this loop.)
+    const int lane = tid & 31;
+    for (;;) {
+        int ch = 0;
+        if (lane == 0) {
+            const unsigned long long old = atomicAdd(&J->word, 1ull);
+            ch = job_next(old) < job_count(old) ? job_next(old) : -1;
+        }
+        ch = __shfl_sync(0xffffffffu, ch, 0);
+        if (ch < 0) break;
+        serve_chunk(D, pc, phase, side, lambda, ch);
+        __syncwarp();
+        if (lane == 0) { __threadfence(); atomicAdd(&J->done, 1u); }
+    }
+    __syncthreads();
+    if (tid == 0) while (ld_acquire(&J->done) < S.doneTarget) __nanosleep(32);
+    __syncthreads();
+}
+// ---- a helper CTA: scans the problems round-robin from its own index (one lane per problem), claims a group of chunks of any
+//      open phase, loads that problem's descriptor and pose-cache mirror into its shared memory when the problem or the phase
+//      changed, and serves the group.  It leaves once every problem has finished. ----
+__device__ void helper_loop(const Dev* __restrict__ probs, int nProb, const unsigned long long* finished, Dev& sD, double* spc, int hIdx) {
+    __shared__ int s_q, s_phase, s_side; __shared__ unsigned s_seq; __shared__ double s_lambda;
+    const int tid = threadIdx.x, lane = tid & 31;
+    int start = hIdx % nProb, cachedQ = -1;
+    unsigned cachedSeq = 0;
+    for (;;) {
+        if (tid < 32) {
+            int q = -1;
+            if (ld_acquire(finished) >= (unsigned long long)nProb) q = -2;
+            for (int b = 0; b < nProb && q == -1; b += 32) {
+                const int qi = (start + b + lane) % nProb;
+                Job* J = b + lane < nProb ? probs[qi].job : nullptr;
+                bool avail = false;
+                if (J) { const unsigned long long w = ld_relaxed(&J->word); avail = job_next(w) < job_count(w); }
+                unsigned m = __ballot_sync(0xffffffffu, avail);
+                while (m && q == -1) {
+                    const int src = __ffs(m) - 1;
+                    m &= m - 1;
+                    int got = 0;
+                    if (lane == src) {
+                        const unsigned long long old = atomicAdd(&J->word, (unsigned long long)NWARP);
+                        const int k0 = job_next(old), n = job_count(old);
+                        if (k0 < n) {
+                            got = 1;
+                            __threadfence();
+                            s_grant = make_int2(k0, min(k0 + NWARP, n));
+                            s_seq = *(volatile unsigned*)&J->seq; s_phase = *(volatile int*)&J->phase; s_side = *(volatile int*)&J->side;
+                            s_lambda = *(volatile double*)&J->lambda;
+                        }
+                    }
+                    if (__shfl_sync(0xffffffffu, got, src)) q = __shfl_sync(0xffffffffu, qi, src);
+                }
+            }
+            if (lane == 0) { s_q = q; if (q == -1) __nanosleep(256); }
+        }
+        __syncthreads();
+        const int q = s_q;
+        if (q == -2) break;
+        if (q >= 0) {
+            if (q != cachedQ || s_seq != cachedSeq) {
+                static_assert(sizeof(Dev) % 8 == 0, "Dev is copied in 8-byte words");
+                for (int i = tid; i < (int)(sizeof(Dev) / 8); i += NT)
+                    reinterpret_cast<unsigned long long*>(&sD)[i] = reinterpret_cast<const unsigned long long*>(probs + q)[i];
+                __syncthreads();
+                for (int i = tid; i < PC * sD.nP; i += NT) spc[i] = sD.pcm[i];
+                cachedQ = q; cachedSeq = s_seq;
+                __syncthreads();
+            }
+            // the group: warp w serves chunk g.x + w; then the CTA counts the group (helped, then done, each after a release fence)
+            const int2 g = s_grant;
+            const int ch = g.x + (tid >> 5);
+            if (ch < g.y) serve_chunk(sD, spc, s_phase, s_side, s_lambda, ch);
+            __syncthreads();
+            if (tid == 0) {
+                __threadfence(); atomicAdd(&sD.job->helped, (unsigned)(g.y - g.x));
+                __threadfence(); atomicAdd(&sD.job->done, (unsigned)(g.y - g.x));
+            }
+            start = q;
+        }
+        __syncthreads();
+    }
+}
+// Grid: nProb owner clusters (problem blockIdx.x / cluster size), then helper clusters of the same size, each of whose CTAs serves
+// chunks of any problem on its own (helper_loop) until `finished` counts every problem.
+__global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __restrict__ probs, const volatile int* stop, int smemMatrixN, int maxP, int maxF,
+                                                                   int nProb, unsigned long long* finished) {
     extern __shared__ double s_dyn[];
     __shared__ double s_red[NT];
     __shared__ Dev s_D;
@@ -933,9 +1083,17 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
     double* s_rhs = s_col + 72 * maxF + 12;      // 6 maxF: rhs row of the LDLT
     double* s_mat = s_rhs + 6 * maxF + 2;
     c.pc = s_pc;
+    if ((int)blockIdx.x >= nProb * c.csize()) {
+        helper_loop(probs, nProb, finished, s_D, s_pc, (int)blockIdx.x - nProb * c.csize());
+        return;
+    }
     if (c.tid() == 0) {
         s_D = probs[blockIdx.x / c.csize()];
         new (&S) LoopState();
+        if (c.crank() == 0) {     // the claim word was left exhausted by the last run (or zeroed by the upload): no claim succeeds before the first phase opens
+            Job* J = s_D.job;
+            J->done = 0; J->helped = 0; J->seq = 0;
+        }
     }
     __syncthreads();
     const Dev& D = s_D;
@@ -982,11 +1140,11 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
             if (it == 0) S.firstChi = S.iniChi;
             S.rho = 0; S.qmax = 0;
         }
+        const int nPtCh = (D.nL + PCH - 1) / PCH;
         TICK();
-        phase_build_points(D, c, cur(D.E4a, D.E4b), lambdaKnown ? S.lm.lambda : -1.0);
-        TOCK(1); TICK();
-        phase_build_poses_partial(D, c, cur(D.E4a, D.E4b));
+        owner_phase(D, S, s_pc, PH_BUILD, S.cur, lambdaKnown ? S.lm.lambda : -1.0, nPtCh + D.taskChunkStart[D.nF]);
         csync();
+        TOCK(1); TICK();
         phase_build_poses_combine(D, c);
         TOCK(2);
         if (!lambdaKnown) {
@@ -999,7 +1157,7 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
         do {
             if (needPrep) {
                 TICK();
-                phase_point_prep(D, c, S.lm.lambda);
+                owner_phase(D, S, s_pc, PH_PREP, S.cur, S.lm.lambda, nPtCh);
                 csync();
                 TOCK(3);
             }
@@ -1008,7 +1166,7 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
                 // reduced camera system: CTA 0's shared memory; the other CTAs of the cluster reach it as distributed shared memory
                 const bool matInSmem = D.n <= smemMatrixN && D.n > 0;
                 TICK();
-                phase_schur_partial(D, c, D.K);
+                owner_phase(D, S, s_pc, PH_SCHUR, S.cur, S.lm.lambda, D.nChunks);
                 csync();
                 TOCK(4); TICK();
                 phase_schur_combine(D, c, S.lm.lambda, matInSmem ? cg::this_cluster().map_shared_rank(s_mat, 0) : D.Hs, D.n);   // every CTA writes entries into CTA 0's shared memory through DSMEM
@@ -1048,8 +1206,13 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
     }
     phase_finalize(D, c, cur(D.pts, D.ptsB));
     if (S.cur) for (int i = c.wid(); i < 7 * D.nP; i += nw) D.poses[i] = D.posesB[i];
-    if (c.wid() == 0) for (int i = 0; i < 10; ++i) D.stats[8 + i] = (double)s_tph[i];
-    if (c.wid() == 0) { D.stats[0] = S.cj; D.stats[1] = S.trials; D.stats[2] = S.lm.lambda; D.stats[3] = S.currentChi; D.stats[4] = S.firstChi; }
+    if (c.wid() == 0) for (int i = 0; i < 9; ++i) D.stats[8 + i] = (double)s_tph[i];
+    if (c.wid() == 0) {
+        D.stats[0] = S.cj; D.stats[1] = S.trials; D.stats[2] = S.lm.lambda; D.stats[3] = S.currentChi; D.stats[4] = S.firstChi;
+        D.stats[17] = (double)*(volatile unsigned*)&D.job->helped;   // complete: every phase has been joined
+        __threadfence();
+        atomicAdd(finished, 1ull);
+    }
 }
 
 // =============================================================================================
@@ -1093,7 +1256,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     int* poseEdges = const_cast<int*>(D.poseEdges); int* poseEdgePt = const_cast<int*>(D.poseEdgePt);
     int2* pairs = const_cast<int2*>(D.pairs); int* pairPt = const_cast<int*>(D.pairPt);
     int4* chunkHdr = const_cast<int4*>(D.chunkHdr); int* taskChunkStart = const_cast<int*>(D.taskChunkStart);
-    if (tid == 0) s_err = 0;
+    if (tid == 0) { s_err = 0; *D.job = Job{}; }     // an exhausted claim word: no claim succeeds before the LM kernel opens a phase
     for (int i = tid; i <= nL; i += BT) D.bCnt[i] = 0;
     for (size_t i = tid; i < (size_t)nF * nL; i += BT) D.bEid[i] = -1;
     __syncthreads();
@@ -1252,8 +1415,10 @@ struct Solver {
     cudaEvent_t evWait = nullptr;                    // blocking-sync event: upload / download sleep on it instead of spinning (device_utils.cuh)
     bool ranOnce = false;
     int nLoaded = 0, launches = 0, numSMs = 132;
+    unsigned long long* d_finished = nullptr;        // problems finished in the running launch (helper CTAs leave when it reaches the batch)
     ~Solver() {
         cudaSetDevice(device);
+        if (d_finished) cudaFree(d_finished);
         if (d_arena) cudaFree(d_arena);
         if (h_arena) cudaFreeHost(h_arena);
         if (d_probs) cudaFree(d_probs);
@@ -1282,6 +1447,7 @@ struct Solver {
         b += al(288 * nP) + al(48 * nP) + al(48 * nL) + al(72 * nL) + al(24 * nL);   // Hpp, bp, Hll, PT, bl
         b += al(8 * 42 * cc) + al(8 * 28 * (nP + nE / SCH + 1));                  // Spart, Ppart
         b += al(8 * n * n) + al(8 * n) + al(8 * (n + 3 * nL)) + al(8 * (4 * PSLOT + 8));   // Hs, bs, x, partial
+        b += al(sizeof(Job)) + al(8 * PC * nP);                                   // open phase, pose-cache mirror
         return b;
     }
     int init() {
@@ -1298,6 +1464,7 @@ struct Solver {
             CK(cudaMallocHost(&h_arena, arenaBytes));
         }
         CK(cudaMalloc(&d_probs, sizeof(Dev) * maxBatch));
+        CK(cudaMalloc(&d_finished, sizeof(unsigned long long)));
         CK(cudaHostAlloc(&h_stop, sizeof(int) * maxBatch, cudaHostAllocMapped));
         CK(cudaHostGetDevicePointer(&d_stop, h_stop, 0));
         CK(cudaHostAlloc(&h_status, sizeof(int) * maxBatch, cudaHostAllocMapped));
@@ -1376,6 +1543,8 @@ struct Solver {
         D.Hs = (double*)(d_arena + carve(8 * (size_t)n * n)); D.bs = (double*)(d_arena + carve(8 * (size_t)std::max(n, 1)));
         D.x = (double*)(d_arena + carve(8 * ((size_t)n + 3 * (size_t)nL)));
         D.partial = (double*)(d_arena + carve(8 * (4 * PSLOT + 8)));
+        D.job = (Job*)(d_arena + carve(sizeof(Job))); D.pcm = (double*)(d_arena + carve(8 * PC * (size_t)nP));
+        if (cc + ((size_t)nL + PCH - 1) / PCH >= ((size_t)1 << 23)) { set_error("lba: more chunks in one phase than the claim word counts"); return ORB_ERR_CAPACITY; }
         if (off - base > perProblem) { set_error("lba: arena too small (internal sizing error)"); return ORB_ERR_CAPACITY; }
         D.delta = P->huberDelta; D.dsqr = P->huberDelta * P->huberDelta; D.userLambdaInit = P->userLambdaInit; D.iterations = P->iterations;
         return ORB_OK;
@@ -1470,16 +1639,27 @@ struct Solver {
         (void)cudaGetLastError();
         if (forcedCluster > 0) csize = forcedCluster;
         attr[0].val.clusterDim.x = csize;
-        cfg.gridDim = dim3(nLoaded * csize);
-        const Dev* dp = d_probs; const volatile int* ds = d_stop; int mn = matN;
-        CK(cudaLaunchKernelEx(&cfg, lba_cluster_kernel, dp, ds, mn, mp, mf));
+        // helper clusters: as many more clusters of this size as are resident beside the batch's own
+        int nHelp = 0;
+        if (helpers != 0) {
+            cfg.gridDim = dim3(csize);
+            int maxActive = 0;
+            if (cudaOccupancyMaxActiveClusters(&maxActive, lba_cluster_kernel, &cfg) == cudaSuccess) nHelp = std::max(0, maxActive - nLoaded);
+            (void)cudaGetLastError();
+            if (helpers > 0) nHelp = std::min(nHelp, helpers);
+        }
+        cfg.gridDim = dim3((nLoaded + nHelp) * csize);
+        CK(cudaMemsetAsync(d_finished, 0, sizeof(unsigned long long), s));
+        const Dev* dp = d_probs; const volatile int* ds = d_stop; int mn = matN, np = nLoaded; unsigned long long* fin = d_finished;
+        CK(cudaLaunchKernelEx(&cfg, lba_cluster_kernel, dp, ds, mn, mp, mf, np, fin));
         CK(cudaEventRecord(evRun, s));
         ranOnce = true;
         launches = 1;
-        lastCluster = csize;
+        lastCluster = csize; lastHelpers = nHelp;
         return ORB_OK;
     }
     int lastCluster = 1, forcedCluster = 0;
+    int helpers = -1, lastHelpers = 0;
     int download(int count, LbaResult* res, cudaStream_t s) {
         for (int i = 0; i < count; ++i)
             if (!res[i].poses || !res[i].points || !res[i].edgeChi2 || !res[i].edgeDepthPositive) { set_error("lba: null result arrays"); return ORB_ERR_ARG; }
@@ -1544,7 +1724,13 @@ int lba_set_cluster_size(lba_handle* h, int ctas) {
     h->s.forcedCluster = ctas;
     return ORB_OK;
 }
-/* ns spent by CTA 0 of problem `i` in each phase of the last downloaded run: errors, build_points, build_poses, point_prep, schur, ldlt, backsub, update, errors(trial) */
+int lba_last_helpers(const lba_handle* h) { return h ? h->s.lastHelpers : ORB_ERR_ARG; }
+int lba_set_helpers(lba_handle* h, int clusters) {
+    if (!h || clusters < -1) { set_error("lba_set_helpers: -1 (fill the GPU), 0 (none) or a maximum"); return ORB_ERR_ARG; }
+    h->s.helpers = clusters;
+    return ORB_OK;
+}
+/* ns spent by CTA 0 of problem `i` in each phase of the last downloaded run (include/orb_b200.h), then the chunks helpers served */
 int lba_get_phase_ns(const lba_handle* h, int i, double* ns10) {
     if (!h || !ns10 || i < 0 || i >= h->s.nLoaded) return ORB_ERR_ARG;
     const double* stt = (const double*)(h->s.h_arena + h->s.packed[i].statsOff);
