@@ -754,8 +754,8 @@ int lba_get_phase_ns(const lba_handle* h, int i, double* ns10);
  *   pose7 [count][7]: pFrame->GetPose() as unit quaternion (w,x,y,z) + translation, cast to double (:829-830)
  *   cam4  [count][4]: fx, fy, cx, cy;  Xw [count][cap][3]: pMP->GetWorldPos() (:884);  obs [count][cap][2]: mvKeysUn[i].pt
  *   invSigma2 [count][cap]: mvInvLevelSigma2[octave] (:877);  huberDelta = (float)sqrt(5.991)
- * Out: poseOut [count][7] (pFrame->SetPose), outlier [count][cap] (pFrame->mvbOutlier), nInliers[count] = the return value
- * nInitialCorrespondences - nBad.  Host pointers.
+ * Out: poseOut [count][7] (pFrame->SetPose), outlier [count][cap] (pFrame->mvbOutlier in slots [0, N[f]), 0 in the slots past N[f]),
+ * nInliers[count] = the return value nInitialCorrespondences - nBad.  N[f] outside [0, cap] is refused (ORB_ERR_ARG).  Host pointers.
  * ------------------------------------------------------------------------------------------ */
 int pose_optimization_batch(int count, int cap, const int32_t* N, const double* pose7, const float* cam4, const double* Xw,
                             const double* obs, const float* invSigma2, double huberDelta, double* poseOut, uint8_t* outlier,
@@ -795,8 +795,9 @@ int imu_inertial_edges(int count, const float* preint, const double* states36, c
  *   preint [count][IMU_PREINT_FLOATS]: pFrame->mpImuPreintegrated (from the last keyframe);
  *   kfState21 / state21 [count][21]: Rwb 9 | twb 3 | velocity 3 | gyro bias 3 | acc bias 3 of the last keyframe (fixed) and of the frame
  *   (in: VertexPose / Velocity / GyroBias / AccBias(pFrame); out: what SetImuPoseVelocity / mImuBias receive, :4813-4817).
- * Out: outlier [count][cap] = mvbOutlier, H15 [count][225] = the Hessian handed to ConstraintPoseImu (:4819-4870, row-major, order pose 6 |
- * velocity | gyro bias | acc bias), ret [count] = nInitialCorrespondences - nBad.  Host pointers. */
+ * Out: outlier [count][cap] = mvbOutlier in slots [0, N[f]) and 0 in the slots past N[f], H15 [count][225] = the Hessian handed to
+ * ConstraintPoseImu (:4819-4870, row-major, order pose 6 | velocity | gyro bias | acc bias), ret [count] = nInitialCorrespondences - nBad.
+ * N[f] outside [0, cap] is refused (ORB_ERR_ARG).  Host pointers. */
 int pose_inertial_optimization_last_kf_batch(int count, int cap, const int32_t* N, const float* Xw, const float* obs, const float* invSigma2, const float* trackDepth,
                                              const float* cam4, const double* extrinsics24, const float* preint, const double* kfState21, double* state21, int bRecInit,
                                              uint8_t* outlier, double* H15, int32_t* ret, int device);

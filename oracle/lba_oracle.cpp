@@ -491,7 +491,8 @@ void orbo_lba_residuals(int nP, const double* poses7, const float* cam4, int nL,
 // BaseUnaryEdge::constructQuadraticForm (g2o/core/base_unary_edge.hpp:43-72), LinearSolverDense (6x6 LDLT).
 // 4 rounds x optimize(10), every round restarts from the frame's pose; outliers (chi2 > 5.991) leave the active set
 // (level 1) and can come back; the Huber kernel is removed after the third round (:1040-1041).
-// Returns nInitialCorrespondences - nBad.  pose7 in/out, outlier[N] out.
+// Returns nInitialCorrespondences - nBad.  pose7 in/out, outlier[N] out.  stats (optional, 4 doubles): LM trials, LM iterations that
+// ended after maxTrials rejected trials (qmax == 10), iterations that ended with rho == 0, rounds run.
 // ---------------------------------------------------------------------------------------------------------
 }  // extern "C" (reopened below: the pose-only problem is a struct shared by the solver and its step-by-step form)
 
@@ -551,7 +552,7 @@ int orbo_pose_optimization(double* pose7, const float* cam4, int N, const double
                            double huberDelta, uint8_t* outlier, double* stats) {
     if (N < 3) {   // if(nInitialCorrespondences<3) return 0; (src/Optimizer.cc:996-997): the frame's pose is not touched
         for (int i = 0; i < N; ++i) outlier[i] = 0;
-        if (stats) stats[0] = 0;
+        if (stats) for (int i = 0; i < 4; ++i) stats[i] = 0;
         return 0;
     }
     PoseOpt P;
@@ -561,8 +562,9 @@ int orbo_pose_optimization(double* pose7, const float* cam4, int N, const double
     P.err.assign(2 * (size_t)N, 0.0); P.level.assign(N, 0); P.robust.assign(N, 1);
     for (double& v : P.xs) v = 0;
     for (int i = 0; i < N; ++i) outlier[i] = 0;
-    int nBad = 0, totalTrials = 0;
+    int nBad = 0, totalTrials = 0, nExhausted = 0, nRhoZero = 0, rounds = 0;
     for (int round = 0; round < 4; ++round) {
+        ++rounds;
         P.T = T0;
         const int nActive = P.n_active();
         // optimizer.optimize(10)
@@ -589,6 +591,7 @@ int orbo_pose_optimization(double* pose7, const float* cam4, int N, const double
                 } else { lambda *= ni; ni *= 2; P.T = P.Tbk; }
                 ++qmax; ++totalTrials;
             } while (rho < 0 && qmax < 10);
+            nExhausted += qmax == 10; nRhoZero += rho == 0;
             if (qmax == 10 || rho == 0) ok = false;
             else { if ((iniChi - currentChi) * 1e3 < iniChi) ++nBadLM; else nBadLM = 0; if (nBadLM >= 3) ok = false; }
         }
@@ -602,7 +605,7 @@ int orbo_pose_optimization(double* pose7, const float* cam4, int N, const double
         if (N < 10) break;
     }
     pose7[0] = P.T.q.w; pose7[1] = P.T.q.x; pose7[2] = P.T.q.y; pose7[3] = P.T.q.z; pose7[4] = P.T.t[0]; pose7[5] = P.T.t[1]; pose7[6] = P.T.t[2];
-    if (stats) { stats[0] = totalTrials; }
+    if (stats) { stats[0] = totalTrials; stats[1] = nExhausted; stats[2] = nRhoZero; stats[3] = rounds; }
     return N - nBad;
 }
 

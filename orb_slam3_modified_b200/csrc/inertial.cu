@@ -642,9 +642,11 @@ int pose_inertial_optimization_last_kf_batch(int count, int cap, const int32_t* 
     if (count < 1 || cap < 1 || !N || !Xw || !obs || !invSigma2 || !trackDepth || !cam4 || !extrinsics24 || !preint || !kfState21 || !state21 || !outlier || !H15 || !ret) {
         set_error("pose_inertial_optimization_last_kf_batch: bad argument"); return ORB_ERR_ARG;
     }
+    int rc = orbx::check_row_counts("pose_inertial_optimization_last_kf_batch", N, count, cap);
+    if (rc) return rc;
     const size_t C = count, K = cap;
     ThreadStaging* S;
-    int rc = orbx::thread_staging(device, &S);
+    rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
     S->begin();
     const int pN = S->in(N, 4 * C), pX = S->in(Xw, 12 * C * K), pO = S->in(obs, 8 * C * K), pS = S->in(invSigma2, 4 * C * K), pT = S->in(trackDepth, 4 * C * K),
@@ -662,6 +664,7 @@ int pose_inertial_optimization_last_kf_batch(int count, int cap, const int32_t* 
     pose_inertial_opt_kernel<false><<<count, PI_NT, 0, st>>>(Q);
     CK(cudaGetLastError());
     CK(S->download(st));
+    orbx::zero_row_tails(outlier, N, count, cap);
     return ORB_OK;
 }
 
@@ -673,9 +676,11 @@ int pose_inertial_optimization_last_frame_batch(int count, int cap, const int32_
         !state21 || !outlier || !H15 || !ret) {
         set_error("pose_inertial_optimization_last_frame_batch: bad argument"); return ORB_ERR_ARG;
     }
+    int rc = orbx::check_row_counts("pose_inertial_optimization_last_frame_batch", N, count, cap);
+    if (rc) return rc;
     const size_t C = count, K = cap;
     ThreadStaging* S;
-    int rc = orbx::thread_staging(device, &S);
+    rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
     S->begin();
     const int pN = S->in(N, 4 * C), pX = S->in(Xw, 12 * C * K), pO = S->in(obs, 8 * C * K), pS = S->in(invSigma2, 4 * C * K), pT = S->in(trackDepth, 4 * C * K),
@@ -694,6 +699,7 @@ int pose_inertial_optimization_last_frame_batch(int count, int cap, const int32_
     pose_inertial_opt_kernel<true><<<count, PI_NT, 0, st>>>(Q);
     CK(cudaGetLastError());
     CK(S->download(st));
+    orbx::zero_row_tails(outlier, N, count, cap);
     return ORB_OK;
 }
 

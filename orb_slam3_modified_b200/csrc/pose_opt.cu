@@ -293,9 +293,11 @@ int pose_optimization_batch(int count, int cap, const int32_t* N, const double* 
     if (count < 1 || cap < 1 || !N || !pose7 || !cam4 || !Xw || !obs || !invSigma2 || !poseOut || !outlier || !nInliers) {
         set_error("pose_optimization_batch: bad argument"); return ORB_ERR_ARG;
     }
+    int rc = orbx::check_row_counts("pose_optimization_batch", N, count, cap);
+    if (rc) return rc;
     const size_t C = count, K = cap;
     orbx::ThreadStaging* S;
-    int rc = orbx::thread_staging(device, &S);
+    rc = orbx::thread_staging(device, &S);
     if (rc) return rc;
     S->begin();
     const int pN = S->in(N, 4 * C), pP = S->in(pose7, 56 * C), pC = S->in(cam4, 16 * C), pX = S->in(Xw, 24 * C * K), pO = S->in(obs, 16 * C * K),
@@ -311,6 +313,7 @@ int pose_optimization_batch(int count, int cap, const int32_t* N, const double* 
     pose_opt_kernel<<<count, NT, 0, st>>>(P);
     CK(cudaGetLastError());
     CK(S->download(st));
+    orbx::zero_row_tails(outlier, N, count, cap);
     return ORB_OK;
 }
 

@@ -108,6 +108,18 @@ private:
     size_t dcap_ = 0, hcap_ = 0;
 };
 
+// Per-row counts of the pose optimisers' [count][cap] slot arrays: N[f] in [0, cap], checked before anything is staged.
+inline int check_row_counts(const char* where, const int32_t* N, int count, int cap) {
+    for (int f = 0; f < count; ++f)
+        if (N[f] < 0 || N[f] > cap) { set_error(std::string(where) + ": N[f] outside [0, cap]"); return ORB_ERR_ARG; }
+    return ORB_OK;
+}
+// The kernels write the slots [0, N[f]) of an output row only and download copies the whole row, so the slots past N[f] would carry
+// whatever the staging buffer last held there: they are set to 0 after download.
+inline void zero_row_tails(uint8_t* rows, const int32_t* N, int count, int cap) {
+    for (int f = 0; f < count; ++f) memset(rows + (size_t)f * cap + N[f], 0, (size_t)(cap - N[f]));
+}
+
 // The staging and stream of the stateless batch entry points (inertial.cu, pose_opt.cu, local_inertial_ba.cu; static functions
 // in the reference, so no object owns them): one per host thread, moved when a call names another device.
 struct ThreadStaging : Staging {

@@ -242,7 +242,7 @@ def pose_optimization(frame):
     L = lib()
     L.orbo_pose_optimization.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]
     n = L.orbo_pose_optimization(_p(pose), _p(cam), N, _p(Xw), _p(obs), _p(isg), float(np.float32(np.sqrt(5.991))), _p(outl), _p(stats))
-    return dict(pose=pose, outlier=outl[:N].copy(), inliers=n, trials=int(stats[0]))
+    return dict(pose=pose, outlier=outl[:N].copy(), inliers=n, trials=int(stats[0]), exhausted=int(stats[1]), rho_zero=int(stats[2]), rounds=int(stats[3]))
 
 
 # ---------------------------------------------------------------------------------------------

@@ -159,11 +159,10 @@ def test_pose_inertial_opt_noise_free_fixed_point():
     assert r5['ret'] == 5 and np.isfinite(r5['state']).all()
 
 
-def test_pose_inertial_opt_first_step_is_the_gauss_newton_step():
+def check_first_step_last_kf(pr, P):
     """One Gauss-Newton step of the oracle = the dense normal-equation step built from NUMERICAL derivatives of the stacked, whitened residuals
-    (mono edges without robust weight: inliers only, inertial edge, random-walk edges) under ImuCamPose::Update."""
-    pr = synth.pose_inertial_problem(seed=5, n=60, outlier_frac=0.0, perturb=0.05, noise_px=0.2)
-    P = O.imu_preintegrate(pr['acc'], pr['gyr'], pr['dt'], pr['bias6'], synth.IMU_NOISE)
+    (mono edges without robust weight: inliers only, inertial edge, random-walk edges) under ImuCamPose::Update.  For a frame where no
+    Huber weight is active at the start."""
     info9, ig, ia = O.imu_information(P)
     ex = pr['extr']
 
@@ -189,7 +188,7 @@ def test_pose_inertial_opt_first_step_is_the_gauss_newton_step():
         return np.concatenate(out)
     s0 = pr['state']
     r0 = residuals(s0)
-    assert (r0[:2 * len(pr['Xw'])].reshape(-1, 2) ** 2).sum(1).max() < 5.99      # no Huber weight at the linearisation point
+    assert (r0[:2 * len(pr['Xw'])].reshape(-1, 2) ** 2).sum(1).max(initial=0.0) < 5.99      # no Huber weight at the linearisation point
     J = np.zeros((len(r0), 15))
     for k in range(15):
         h = 1e-6
@@ -200,6 +199,11 @@ def test_pose_inertial_opt_first_step_is_the_gauss_newton_step():
     # the oracle with ONE iteration: emulate by comparing against its first update through a 1-iteration copy (huge Huber never active at this noise level)
     got = O.pose_inertial_opt_one_step(pr, P)
     assert np.allclose(got, want, rtol=0, atol=2e-6), np.abs(got - want).max()
+
+
+def test_pose_inertial_opt_first_step_is_the_gauss_newton_step():
+    pr = synth.pose_inertial_problem(seed=5, n=60, outlier_frac=0.0, perturb=0.05, noise_px=0.2)
+    check_first_step_last_kf(pr, O.imu_preintegrate(pr['acc'], pr['gyr'], pr['dt'], pr['bias6'], synth.IMU_NOISE))
 
 
 # ---- Optimizer::PoseInertialOptimizationLastFrame (src/Optimizer.cc:4875-5289) ----
@@ -237,9 +241,8 @@ def test_pose_inertial_opt_last_frame_with_a_rigid_prior_is_the_last_keyframe_va
     assert np.abs(a['H'] - b['H']).max() < 1e-4 * np.abs(b['H']).max()          # H_cc - H_cb H_bb^-1 H_bc with H_bb ~ 1e16
 
 
-def test_pose_inertial_opt_last_frame_first_step_is_the_gauss_newton_step():
-    pr = synth.pose_inertial_problem_last_frame(seed=6, n=50, outlier_frac=0.0, perturb=0.05, noise_px=0.2)
-    Pf, Pk = _preints(pr)
+def check_first_step_last_frame(pr, Pf, Pk):
+    """As check_first_step_last_kf over the 30 unknowns of the frame and the previous frame, with the prior edge."""
     info9 = O.imu_information(Pf)[0]; _, ig, ia = O.imu_information(Pk)
     ex = pr['extr']
     Lp = np.linalg.cholesky(pr['prior_H'])
@@ -270,7 +273,7 @@ def test_pose_inertial_opt_last_frame_first_step_is_the_gauss_newton_step():
     chi2_prior = []
     c0, p0 = pr['state'], pr['prev_state']
     r0 = residuals(c0, p0)
-    assert chi2_prior[0] < 25.0 and (r0[:2 * len(pr['Xw'])].reshape(-1, 2) ** 2).sum(1).max() < 5.99      # no Huber weight at the linearisation point
+    assert chi2_prior[0] < 25.0 and (r0[:2 * len(pr['Xw'])].reshape(-1, 2) ** 2).sum(1).max(initial=0.0) < 5.99      # no Huber weight at the linearisation point
     J = np.zeros((len(r0), 30))
     for k in range(30):
         h = 2e-3 if k % 15 >= 9 else 1e-6      # the preintegration applies bias changes in float (src/ImuTypes.cc:283-307): a bias step must stand out of its rounding
@@ -280,3 +283,8 @@ def test_pose_inertial_opt_last_frame_first_step_is_the_gauss_newton_step():
     got = O.pose_inertial_opt_last_frame(pr, Pf, Pk, rounds=1, iters=1)
     assert np.allclose(got['state'], apply(c0, dx[:15]), rtol=0, atol=3e-6), np.abs(got['state'] - apply(c0, dx[:15])).max()
     assert np.allclose(got['prev_state'], apply(p0, dx[15:]), rtol=0, atol=3e-6), np.abs(got['prev_state'] - apply(p0, dx[15:])).max()
+
+
+def test_pose_inertial_opt_last_frame_first_step_is_the_gauss_newton_step():
+    pr = synth.pose_inertial_problem_last_frame(seed=6, n=50, outlier_frac=0.0, perturb=0.05, noise_px=0.2)
+    check_first_step_last_frame(pr, *_preints(pr))

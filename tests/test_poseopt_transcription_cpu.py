@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as O
+import pose_scenes as S
 from orb_slam3_modified_b200 import synth
 from test_lba_dense_cpu import _R, _exp
 
@@ -18,6 +19,8 @@ def _pose_opt(f):
     delta = float(np.float32(np.sqrt(5.991))); dsqr = delta * delta
     q = f['pose'][:4] / np.linalg.norm(f['pose'][:4])
     R0, t0 = _R(q), f['pose'][4:].astype(np.float64)
+    if N < 3:                                             # if(nInitialCorrespondences<3) return 0; (:996-997)
+        return R0, t0, np.zeros(N, bool), 0, 0
 
     def resid(R, t):
         xc = X @ R.T + t
@@ -91,12 +94,13 @@ def _pose_opt(f):
     return R, t, outlier, N - nBad, trials
 
 
-@pytest.mark.parametrize('kw', [dict(n=300, seed=1), dict(n=120, seed=5, outlier_frac=0.3), dict(n=40, seed=9, pose_noise=(0.1, 4.0))])
+# the layouts of tests/pose_scenes.py, by name
+@pytest.mark.parametrize('kw', [dict(n=300, seed=1), dict(n=120, seed=5, outlier_frac=0.3), dict(n=40, seed=9, pose_noise=(0.1, 4.0))] + list(S.PO_LAYOUTS))
 def test_pose_optimization_second_transcription(kw):
-    f = synth.pose_opt_problem(**kw)
+    f = S.PO_LAYOUTS[kw]() if isinstance(kw, str) else synth.pose_opt_problem(**kw)
     ref = O.pose_optimization(f)
     R, t, outl, inl, trials = _pose_opt(f)
     assert inl == ref['inliers'] and np.array_equal(outl.astype(np.uint8), ref['outlier'])
-    assert trials > 0 and ref['trials'] > 0
+    assert (trials > 0) == (ref['trials'] > 0) == (len(f['obs']) >= 3)
     qo = ref['pose'][:4]
     assert np.abs(_R(qo / np.linalg.norm(qo)) - R).max() < 1e-6 and np.abs(ref['pose'][4:] - t).max() < 1e-6
