@@ -266,8 +266,8 @@ int orbm_motion_model_pose_batch(orbm_handle* h, const OrbmBatchDevice* in, cons
                                  uint8_t* claimed, int32_t* nmatches, double* pose7, float* Tcw7, uint8_t* discarded, int32_t* nmatchesMap);
 
 /* Tracking::TrackLocalMap (reference src/Tracking.cc:2952) from SearchLocalPoints (:3346) through the statistics loop that sets
- * mnMatchesInliers, for `batch` streams; monocular, IMU not initialised (so PoseOptimization runs), not only-tracking.  The caller keeps
- * UpdateLocalMap (it provides the local map and lastToLocal), the thresholds, and the IncreaseVisible / IncreaseFound calls (visible /
+ * mnMatchesInliers, for `batch` streams; monocular, IMU not initialised (so PoseOptimization runs), not only-tracking.  The local map and
+ * lastToLocal come from UpdateLocalMap (orbm_update_local_map_batch*, or the caller's own); the caller keeps the thresholds, and the IncreaseVisible / IncreaseFound calls (visible /
  * found say how many).  Precondition: every non-bad point the frame holds is in its local map (true on this path: UpdateLocalKeyFrames votes
  * with the frame's matches), so a match without a local index is one the reference dropped.  On the device, per stream:
  *   1. SearchLocalPoints' first loop: match[i] is remapped to its local index (lastToLocal[match[i]]; -1 or a bad point: match = -1);
@@ -311,7 +311,8 @@ int orbm_track_local_map_batch_resident(orbm_handle* h, const OrbmLocalMapBatch*
 
 /* Tracking::Track for a monocular-inertial frame once the IMU is initialised and the frame is past the relocalisation reset window, for
  * `batch` streams (RECENTLY_LOST streams too, with th = 15): TrackWithMotionModel's PredictStateIMU and TrackLocalMap through the
- * statistics loop.  The caller keeps PreintegrateIMU, UpdateLocalMap, the thresholds, IncreaseVisible / IncreaseFound and the choice of
+ * statistics loop.  The local map comes from UpdateLocalMap (orbm_update_local_map_batch*, or the caller's own).  The caller keeps
+ * PreintegrateIMU, the thresholds, IncreaseVisible / IncreaseFound and the choice of
  * the streams that take this path (imu->mode).  On the device, per stream with mode 1 (mbMapUpdated: from the last keyframe) or 2 (from
  * the last frame):
  *   1. PredictStateIMU in float (source state, its bias and preintegration by mode; gravity (0, 0, -9.81f)) and
@@ -354,6 +355,81 @@ int orbm_track_local_map_inertial_batch(orbm_handle* h, const OrbmLocalMapBatch*
 /* Same with the current frame on the device (in->kps, in->desc, in->nK from orbx_resident_slabs, stride in->kcap). */
 int orbm_track_local_map_inertial_batch_resident(orbm_handle* h, const OrbmLocalMapBatch* in, const OrbmImuTrackBatch* imu,
                                                  const OrbmLocalMapResult* out, const OrbmImuTrackResult* imuOut);
+
+/* Tracking::UpdateLocalMap's UpdateLocalKeyFrames and UpdateLocalPoints (reference src/Tracking.cc; monocular and mono-inertial, Nleft == -1)
+ * for `batch` streams, one CTA per stream in ONE launch.  Its outputs are the local map in exactly the slabs OrbmLocalMapBatch takes, so
+ * orbm_track_local_map_batch_device and orbm_track_local_map_inertial_batch_device can read them with no host step in between.  Per stream:
+ *   1. Votes: every good point of the vote source adds 1 to each of its observers (a point held twice votes twice).  voteLastFrame = 0:
+ *      the current frame's mvpMapPoints, i.e. srcPoint[match[i]] for i < nK with match[i] >= 0; voteLastFrame = 1 (IMU initialised, past
+ *      the relocalisation window): mLastFrame.mvpMapPoints, i.e. every srcPoint entry.
+ *   2. The voters that are not bad, in table order (= the std::map's key order), are the first local keyframes; refKF (pKFmax) is the
+ *      first of them with the largest count.
+ *   3. For each voter, while there are at most 80 local keyframes: the first good unmarked keyframe of its covisibles, the first good
+ *      unmarked child, then the parent if unmarked (not tested for isBad()), which ends the loop.
+ *   4. Inertial streams with fewer than 80 local keyframes: up to 20 steps from lastKF along prevKF; an unmarked keyframe is added and the
+ *      walk moves on, a marked one stalls it.
+ *   5. UpdateLocalPoints: the local keyframes in reverse order, each one's slots in slot order; a good point not yet taken is appended.
+ * The caller keeps SetReferenceMapPoints, sets the marks (mnTrackReferenceForFrame) and mpReferenceKF, and NULLs the bad points of the
+ * voting frame (INTEGRATION.md §2).  Precondition: no keyframe or point is marked for this frame at the call.
+ *
+ * Keyframe table: stream b's keyframes are rows [kfStart[b], kfStart[b + 1]) in ascending (uint64_t)KeyFrame* order: every observer of a
+ * srcPoint entry's point, each observer's covisibles, children and parent, and (inertial) the mPrevKF chain of lastKF, at most 20 entries.
+ * Every keyframe index (covKF, childKF, parent, prevKF, obsKF, lastKF, localKF) is relative to the stream's first row; every point index
+ * (slotPoint, srcPoint, localPoint) to its first point row pointStart[b].  covKF / childKF / parent are read for the voters only, prevKF
+ * for the chain only; the others may be empty / -1.  obsKF is read for the points that vote; which of the srcPoint entries vote is decided
+ * by `match`, on the device when the pose step runs there, so give the observations of every srcPoint entry (and put their observers in
+ * the table); other points may have none.
+ * Output rows past nM are zero (localPoint -1); a stream whose local map has more than mcap points gets its true count in nM, no rows
+ * (every row zero, localPoint and lastToLocal -1) and makes the host form return ORB_ERR_CAPACITY naming the stream. */
+typedef struct OrbmUpdateLocalMapBatch {
+    int batch, kcap, mcap, mcapLast;  /* match [batch][kcap]; output slabs [batch][mcap]; srcPoint / lastToLocal [batch][mcapLast] */
+    int nKF, nPoints;                 /* table rows and point rows over the batch (host ints in both forms) */
+    const int32_t* kfStart;           /* [batch + 1] */
+    const uint8_t* kfFlags;           /* [nKF] ORBM_KF_BAD: isBad() */
+    const int32_t* covStart;          /* [nKF + 1] */
+    const int32_t* covKF;             /* [covStart[nKF]] GetBestCovisibilityKeyFrames(10): at most 10 per keyframe, in order */
+    const int32_t* childStart;        /* [nKF + 1] */
+    const int32_t* childKF;           /* [childStart[nKF]] GetChilds(), ascending */
+    const int32_t* parent;            /* [nKF] GetParent(), -1 = NULL */
+    const int32_t* prevKF;            /* [nKF] mPrevKF, -1 = NULL */
+    const int32_t* slotStart;         /* [nKF + 1] */
+    const int32_t* slotPoint;         /* [slotStart[nKF]] the non-NULL slots of GetMapPointMatches(), in slot order */
+    const int32_t* pointStart;        /* [batch + 1] */
+    const uint8_t* pointBad;          /* [nPoints] isBad() */
+    const int32_t* obsStart;          /* [nPoints + 1] */
+    const int32_t* obsKF;             /* [obsStart[nPoints]] the keyframes of GetObservations(): for every point of srcPoint */
+    const float *worldPos, *normal;   /* [nPoints][3] */
+    const float *minDistInv, *maxDistInv, *maxDistance;   /* [nPoints] as OrbmLocalMapBatch */
+    const uint8_t *mpDesc, *hasObs;   /* [nPoints][32], [nPoints] as OrbmLocalMapBatch */
+    const int32_t* nSrc;              /* [batch] entries of the frame's match index space: last-frame slots, or [keyframe features |
+                                         last-frame slots] after TrackReferenceKeyFrame (INTEGRATION.md §2); <= mcapLast */
+    const int32_t* srcPoint;          /* [batch][mcapLast] point of each entry, -1 = NULL */
+    const uint8_t* voteLastFrame;     /* [batch] 0: the frame's match row votes; 1: every srcPoint entry votes */
+    const int32_t* match;             /* [batch][kcap] the frame's matches in the index space (what the pose step wrote), values in [-1, nSrc) */
+    const int32_t* nK;                /* [batch] keypoints of the frame (read for voteLastFrame = 0) */
+    const uint8_t* inertial;          /* [batch] 1: IMU sensor (the temporal walk of step 4) */
+    const int32_t* lastKF;            /* [batch] mCurrentFrame.mpLastKeyFrame, -1 = NULL */
+} OrbmUpdateLocalMapBatch;
+typedef struct OrbmUpdateLocalMapResult {
+    int32_t* localKF;                 /* [nKF] mvpLocalKeyFrames of stream b at rows [kfStart[b], kfStart[b] + nLocalKF[b]), -1 after them */
+    int32_t* nLocalKF;                /* [batch] */
+    int32_t* refKF;                   /* [batch] pKFmax, -1 = none (mpReferenceKF unchanged) */
+    int32_t* localPoint;              /* [batch][mcap] mvpLocalMapPoints */
+    int32_t* nM;                      /* [batch] mvpLocalMapPoints.size() */
+    float *worldPos, *normal;         /* [batch][mcap][3] */
+    float *minDistInv, *maxDistInv, *maxDistance;         /* [batch][mcap] */
+    uint8_t *mpDesc, *hasObs, *bad;   /* [batch][mcap][32], [batch][mcap], [batch][mcap] (0: local points are good) */
+    int32_t* lastToLocal;             /* [batch][mcapLast] local index of srcPoint[j], -1 when NULL, bad or past nSrc */
+} OrbmUpdateLocalMapResult;
+/* Device pointers everywhere; enqueues on `stream`, one launch, and returns without waiting for it.  Its scratch is a device buffer of the
+ * handle's own (grown by the call), shared by every device-form call on the handle: as for the other device forms, the caller orders the
+ * calls on one handle on one stream.  The inputs are trusted as the host form checks them. */
+int orbm_update_local_map_batch_device(orbm_handle* h, const OrbmUpdateLocalMapBatch* in, const OrbmUpdateLocalMapResult* out, void* stream);
+/* HOST pointers (one upload, one launch, one download; no launch when every stream's table is empty).  ORB_ERR_ARG before any launch,
+ * with the outputs and orbm_last_launch_count() unchanged: an index or CSR offset out of range, a CSR not starting at 0 or decreasing,
+ * kfStart[batch] != nKF or pointStart[batch] != nPoints, more than 10 covisibles, children not ascending, nSrc outside [0, mcapLast], nK
+ * outside [0, kcap], a match outside [-1, nSrc), or a null pointer.  ORB_ERR_CAPACITY: a local map larger than mcap (outputs written). */
+int orbm_update_local_map_batch(orbm_handle* h, const OrbmUpdateLocalMapBatch* in, const OrbmUpdateLocalMapResult* out);
 
 /* int ORBmatcher::SearchForInitialization(Frame &F1, Frame &F2, vector<cv::Point2f> &vbPrevMatched, vector<int> &vnMatches12,
  * int windowSize) (include/ORBmatcher.h:74, src/ORBmatcher.cc:648-763): the windowed brute-force search of the monocular

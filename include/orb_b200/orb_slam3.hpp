@@ -223,6 +223,12 @@ public:
     void KeyFrameCullingBatch(const std::vector<OrbmCullingMap>& maps) {
         orb_check(orbm_keyframe_culling_batch(detail::matcher_handle(1, 1, device_), (int)maps.size(), maps.data()), "orbm_keyframe_culling_batch");
     }
+    // Tracking::UpdateLocalMap's UpdateLocalKeyFrames and UpdateLocalPoints for a batch of streams in one launch (orbm_update_local_map_batch).
+    // `out` receives every stream's local keyframes, reference keyframe and local points, and the local map in the slabs of
+    // OrbmLocalMapBatch; the caller replays the marks, mpReferenceKF and the NULLing of the voting frame's bad points (INTEGRATION.md §2).
+    void UpdateLocalMapBatch(const OrbmUpdateLocalMapBatch& in, const OrbmUpdateLocalMapResult& out) {
+        orb_check(orbm_update_local_map_batch(detail::matcher_handle(1, 1, device_), &in, &out), "orbm_update_local_map_batch");
+    }
     // LocalMapping::ProcessNewKeyFrame's map-point loop or the tail of SearchInNeighbors, each followed by KeyFrame::UpdateConnections, for
     // several keyframes of different maps in one launch (orbm_update_connections_batch).  Every item's outputs receive its result; the caller
     // replays it on the host: AddObservation, the point fields, mlpRecentAddedMapPoints, the connection maps and lists, AddChild

@@ -102,6 +102,8 @@ SIGNATURES = {
     'orbm_distinctive_descriptors': (_i, [_vp, _i, _vp, _vp, _vp]),
     'orbm_keyframe_culling_batch': (_i, [_vp, _i, _vp]),
     'orbm_update_connections_batch': (_i, [_vp, _i, _vp]),
+    'orbm_update_local_map_batch_device': (_i, [_vp] * 4),
+    'orbm_update_local_map_batch': (_i, [_vp] * 3),
     'orbm_bf_knn2': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp]),
     'orbm_descriptor_distance': (_i, [_vp, _vp, _vp, _i, _vp]),
     'orbm_last_launch_count': (_i, [_vp]),
@@ -532,6 +534,101 @@ def connections_struct(m):
 
 def _connections_result(out):
     return dict(out, nConnected=int(out['nConnected'][0]), parent=int(out['parent'][0]))
+
+
+#: the arrays of orbm_update_local_map_batch*'s input with their dtypes (OrbmUpdateLocalMapBatch, after its six sizes)
+LOCAL_MAP_ARRAYS = (('kfStart', np.int32), ('kfFlags', np.uint8), ('covStart', np.int32), ('covKF', np.int32), ('childStart', np.int32),
+                    ('childKF', np.int32), ('parent', np.int32), ('prevKF', np.int32), ('slotStart', np.int32), ('slotPoint', np.int32),
+                    ('pointStart', np.int32), ('pointBad', np.uint8), ('obsStart', np.int32), ('obsKF', np.int32), ('worldPos', np.float32),
+                    ('normal', np.float32), ('minDistInv', np.float32), ('maxDistInv', np.float32), ('maxDistance', np.float32),
+                    ('mpDesc', np.uint8), ('hasObs', np.uint8), ('nSrc', np.int32), ('srcPoint', np.int32), ('voteLastFrame', np.uint8),
+                    ('match', np.int32), ('nK', np.int32), ('inertial', np.uint8), ('lastKF', np.int32))
+LOCAL_MAP_SIZES = ('batch', 'kcap', 'mcap', 'mcapLast', 'nKF', 'nPoints')
+#: its outputs: (name, dtype, row shape); rows are 'kf' = [nKF], 'b' = [batch], 'm' = [batch, mcap], 'l' = [batch, mcapLast]
+LOCAL_MAP_OUTPUTS = (('localKF', np.int32, 'kf', ()), ('nLocalKF', np.int32, 'b', ()), ('refKF', np.int32, 'b', ()), ('localPoint', np.int32, 'm', ()),
+                     ('nM', np.int32, 'b', ()), ('worldPos', np.float32, 'm', (3,)), ('normal', np.float32, 'm', (3,)), ('minDistInv', np.float32, 'm', ()),
+                     ('maxDistInv', np.float32, 'm', ()), ('maxDistance', np.float32, 'm', ()), ('mpDesc', np.uint8, 'm', (32,)),
+                     ('hasObs', np.uint8, 'm', ()), ('bad', np.uint8, 'm', ()), ('lastToLocal', np.int32, 'l', ()))
+
+
+class OrbmUpdateLocalMapBatch(C.Structure):
+    """Input of orbm_update_local_map_batch* (include/orb_b200.h)."""
+    _fields_ = [(n, C.c_int) for n in LOCAL_MAP_SIZES] + [(n, C.c_void_p) for n, _ in LOCAL_MAP_ARRAYS]
+
+
+class OrbmUpdateLocalMapResult(C.Structure):
+    """Output of orbm_update_local_map_batch* (include/orb_b200.h)."""
+    _fields_ = [(n, C.c_void_p) for n, _, _, _ in LOCAL_MAP_OUTPUTS]
+
+
+def local_map_batch(items, mcap, kcap=None, mcapLast=None):
+    """The batch dict of orbm_update_local_map_batch from one dict per stream: its keyframe table (kfFlags, parent, prevKF [nk]; covStart /
+    covKF, childStart / childKF, slotStart / slotPoint as CSR), its points (pointBad, minDistInv, maxDistInv, maxDistance, hasObs [np];
+    worldPos, normal [np, 3]; mpDesc [np, 32]; obsStart / obsKF as CSR), its vote source (srcPoint [nSrc], voteLastFrame, match [nK] when
+    voteLastFrame is 0) and inertial / lastKF.  Indices stay stream-local; the CSR offsets become offsets into the concatenated arrays."""
+    B = len(items)
+    kcap = kcap or max([1] + [len(it.get('match', ())) for it in items])
+    mcapLast = mcapLast or max([1] + [len(it['srcPoint']) for it in items])
+    cat = lambda name, dt, shape=(): np.concatenate([np.asarray(it[name], dt).reshape((-1,) + shape) for it in items])   # noqa: E731
+
+    def csr(start, vals):
+        off, starts = 0, [np.zeros(1, np.int32)]
+        for it in items:
+            s = np.asarray(it[start], np.int32)
+            starts.append(s[1:] + off)
+            off += int(s[-1])
+        return np.concatenate(starts).astype(np.int32), cat(vals, np.int32)
+    d = dict(batch=B, kcap=kcap, mcap=mcap, mcapLast=mcapLast)
+    d['kfStart'] = np.concatenate([[0], np.cumsum([len(it['kfFlags']) for it in items])]).astype(np.int32)
+    d['pointStart'] = np.concatenate([[0], np.cumsum([len(it['pointBad']) for it in items])]).astype(np.int32)
+    d['nKF'], d['nPoints'] = int(d['kfStart'][-1]), int(d['pointStart'][-1])
+    for n in ('kfFlags', 'pointBad', 'hasObs'):
+        d[n] = cat(n, np.uint8)
+    for n in ('parent', 'prevKF'):
+        d[n] = cat(n, np.int32)
+    for n in ('minDistInv', 'maxDistInv', 'maxDistance'):
+        d[n] = cat(n, np.float32)
+    d['worldPos'], d['normal'], d['mpDesc'] = cat('worldPos', np.float32, (3,)), cat('normal', np.float32, (3,)), cat('mpDesc', np.uint8, (32,))
+    for start, vals in (('covStart', 'covKF'), ('childStart', 'childKF'), ('slotStart', 'slotPoint'), ('obsStart', 'obsKF')):
+        d[start], d[vals] = csr(start, vals)
+    d['nSrc'] = np.array([len(it['srcPoint']) for it in items], np.int32)
+    d['srcPoint'] = np.full((B, mcapLast), -1, np.int32)
+    d['match'] = np.full((B, kcap), -1, np.int32)
+    d['nK'] = np.zeros(B, np.int32)
+    for b, it in enumerate(items):
+        d['srcPoint'][b, :len(it['srcPoint'])] = it['srcPoint']
+        if it.get('match') is not None:
+            d['match'][b, :len(it['match'])] = it['match']
+            d['nK'][b] = len(it['match'])
+    for n in ('voteLastFrame', 'inertial'):
+        d[n] = np.array([int(it[n]) for it in items], np.uint8)
+    d['lastKF'] = np.array([int(it['lastKF']) for it in items], np.int32)
+    return d
+
+
+def local_map_outputs(d, alloc=None):
+    """Fresh output arrays for batch dict ``d`` (``alloc(shape, dtype)``: numpy zeros by default)."""
+    alloc = alloc or (lambda shape, dt: np.zeros(shape, dt))
+    rows = dict(kf=(d['nKF'],), b=(d['batch'],), m=(d['batch'], d['mcap']), l=(d['batch'], d['mcapLast']))
+    return {n: alloc(rows[r] + sh, dt) for n, dt, r, sh in LOCAL_MAP_OUTPUTS}
+
+
+def local_map_structs(d, out, get):
+    """(OrbmUpdateLocalMapBatch, OrbmUpdateLocalMapResult) over batch dict ``d`` and outputs ``out``; ``get(k)`` gives an array's address."""
+    s = OrbmUpdateLocalMapBatch(*[int(d[n]) for n in LOCAL_MAP_SIZES], *[get(n) for n, _ in LOCAL_MAP_ARRAYS])
+    r = OrbmUpdateLocalMapResult(*[_ptr(out[n]) for n, _, _, _ in LOCAL_MAP_OUTPUTS])
+    return s, r
+
+
+def local_map_split(d, out):
+    """Per stream: dict(localKF (table rows of the stream, in mvpLocalKeyFrames order), refKF, localPoint, nM, lastToLocal [nSrc])."""
+    res = []
+    for b in range(d['batch']):
+        k0, n = int(d['kfStart'][b]), int(out['nLocalKF'][b])
+        nM = int(out['nM'][b])
+        res.append(dict(localKF=out['localKF'][k0:k0 + n].copy(), refKF=int(out['refKF'][b]), nM=nM,
+                        localPoint=out['localPoint'][b, :min(nM, d['mcap'])].copy(), lastToLocal=out['lastToLocal'][b, :int(d['nSrc'][b])].copy()))
+    return res
 
 
 def _c(a, dt):
@@ -1098,6 +1195,28 @@ class ORBmatcher:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_update_connections_batch')
         return [_connections_result(b[1]) for b in built]
+
+    def update_local_map_batch(self, d, out=None):
+        """``Tracking::UpdateLocalMap``'s UpdateLocalKeyFrames and UpdateLocalPoints for ``d['batch']`` streams in one launch
+        (orbm_update_local_map_batch; host numpy).  ``d``: the batch dict of :func:`local_map_batch`.  Returns the outputs of
+        :func:`local_map_outputs` (written into ``out`` when given): the local keyframes and points, and the local map in the slabs
+        ``track_local_map_batch*`` takes (:func:`local_map_split` cuts them per stream).  The caller replays the marks, mpReferenceKF and the
+        NULLing of the voting frame's bad points (INTEGRATION.md §2)."""
+        out = local_map_outputs(d) if out is None else out
+        keep = {n: _c(d[n], dt) for n, dt in LOCAL_MAP_ARRAYS if d.get(n) is not None}
+        s, r = local_map_structs(d, out, lambda n: keep[n].ctypes.data if n in keep else None)
+        rc = lib().orbm_update_local_map_batch(self._h, C.byref(s), C.byref(r))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_update_local_map_batch')
+        return out
+
+    def update_local_map_batch_device(self, d, out, stream=0):
+        """Device form of :meth:`update_local_map_batch`: torch CUDA tensors in ``d`` (the sizes stay ints) and ``out`` (the keys of
+        :func:`local_map_outputs`); enqueues on ``stream``."""
+        s, r = local_map_structs(d, out, lambda n: d[n].data_ptr() if d.get(n) is not None else None)
+        rc = lib().orbm_update_local_map_batch_device(self._h, C.byref(s), C.byref(r), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_update_local_map_batch_device')
 
     def ComputeDistinctiveDescriptors(self, obs_list):
         """``MapPoint::ComputeDistinctiveDescriptors`` for a list of map points (each an [n, 32] u8 array of observed descriptors): index of the chosen row."""

@@ -1293,6 +1293,7 @@ struct Matcher {
     int* d_status = nullptr;
     int numSMs = 132;
     uint8_t* d_track = nullptr;                          // scratch of the batched tracking calls, allocated by their first call (track_scratch)
+    orbm::DeviceScratch ulm;                             // scratch of orbm_update_local_map_batch_device, grown by its calls
     Staging staging;                                     // the single-call host entry points' operands
     uint8_t* d_batch = nullptr; size_t batchBytes = 0;   // device staging of search_last_frame_batch_host (copied straight from the caller)
     int launches = 0;
@@ -1302,7 +1303,7 @@ struct Matcher {
 
     ~Matcher() {
         cudaSetDevice(device);
-        void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_batch, d_track};
+        void* ptrs[] = {d_query, d_resultIdx, d_resultDist, d_status, d_batch, d_track, ulm.ptr};
         for (void* p : ptrs) if (p) cudaFree(p);
         if (h_route) cudaFreeHost(h_route);
         if (evRoute) cudaEventDestroy(evRoute);
@@ -1542,7 +1543,7 @@ using namespace orbm;
 
 struct orbm_handle { Matcher m; };
 
-MatcherContext orbm::matcher_context(orbm_handle* h) { return {&h->m.staging, h->m.stream, h->m.device, &h->m.launches}; }
+MatcherContext orbm::matcher_context(orbm_handle* h) { return {&h->m.staging, h->m.stream, h->m.device, &h->m.launches, &h->m.ulm}; }
 
 // ---- the host forms of the batched tracking calls (below): what they share about the current frame ----
 // One stream's current frame: nK in [0, kcap] and every keypoint octave in [0, nlevels).
