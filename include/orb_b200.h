@@ -824,6 +824,66 @@ int lba_last_helpers(const lba_handle* h);
  * (back-substitution + update + residuals), and last a count instead of a time: the chunks helper clusters served for problem i. */
 int lba_get_phase_ns(const lba_handle* h, int i, double* ns10);
 
+/* void Optimizer::LocalBundleAdjustment(KeyFrame* pKF, bool* pbStopFlag, Map* pMap, int& num_fixedKF, int& num_OptKF, int& num_MPs,
+ * int& num_edges) (src/Optimizer.cc:1116-1498) as a whole, for a batch of maps: the graph walk (:1125-1403), the solve above, the
+ * outlier test and the EraseMapPointMatch / EraseObservation cascade (:1417-1460), and the write-back (:1464-1497).  One map per item,
+ * at most one keyframe per map, and the maps share no keyframe and no point.  Monocular observations only: the table has no field for
+ * right-camera / stereo observations, so it describes mono maps and mono-inertial maps before IMU initialisation (LocalMapping.cc:129-156).
+ * Everything is read once at the call.  Keyframes are table indices, points point indices; std::map<KeyFrame*, ...> order is the caller's
+ * key order, in which every point's observations are listed.
+ *   keyframe table [nKF]: entry 0 is pKF, then its GetVectorCovisibleKeyFrames() and every observer of the points in their slots.
+ *     mnId, kfFlags (ORBM_KF_BAD: isBad(), ORBM_KF_OTHER_MAP: GetMap() != pKF->GetMap(), ORBM_KF_INIT: mnId == pMap->GetInitKFid()),
+ *     pose7 = GetPose() as (w, x, y, z, tx, ty, tz), cameraCenter = GetCameraCenter(), cam4 = fx, fy, cx, cy.
+ *   cov [nCov]: pKF->GetVectorCovisibleKeyFrames() in order (bad and other-map entries included: the walk filters them).
+ *   slots of the candidate local keyframes, candidate c = 0 for pKF and 1 + i for cov[i]: slotStart [nCov + 2], slotPoint = the point of
+ *     GetMapPointMatches()[s], -1 for NULL.
+ *   points [nPoints]: pointId = mnId, pointFlags (ORBM_KF_BAD: isBad(), ORBM_KF_OTHER_MAP: GetMap() != pKF->GetMap()), worldPos = GetWorldPos(),
+ *     refKF = mpRefKF; GetObservations() as CSR obsStart [nPoints + 1] / obsKF / obsIdx, with obsPt = mvKeysUn[idx].pt and obsOctave = .octave.
+ *   invLevelSigma2 / scaleFactors [nlevels]: the map's extractor tables; inertial = pMap->IsInertial() (setUserLambdaInit(100)); stopFlag =
+ *     pbStopFlag, one byte (may be NULL), read after the walk (:1406) and polled by the solver.
+ * Outputs (host pointers):
+ *   status: LBA_LOCAL_RAN, LBA_LOCAL_NO_FIXED (num_fixedKF == 0: the reference returns after the walk) or LBA_LOCAL_STOPPED (*pbStopFlag at
+ *     :1406: nothing is erased or written back); counts = num_fixedKF, num_OptKF, num_MPs, num_edges (the last three 0 for NO_FIXED, which
+ *     returns before assigning them); nLists = |lLocalKeyFrames|, |lFixedCameras|, |lLocalMapPoints|.
+ *   localKF [nKF], fixedKF [nKF], localPoint [nPoints]: lLocalKeyFrames, lFixedCameras, lLocalMapPoints in the reference's order.
+ *   obsFlag [obsStart[nPoints]]: LBA_OBS_NO_EDGE, LBA_OBS_KEPT or LBA_OBS_ERASED (chi2 > 5.991 or depth not positive); vToErase is the
+ *     ERASED observations of lLocalMapPoints in list order, each point's in key order.
+ *   per local keyframe i (list order): kfPose7 [nKF][7] = the float pose SetPose receives, kfCenter [nKF][3] = its new GetCameraCenter().
+ *   per local point i (list order): pointPos [nPoints][3] = SetWorldPos' argument, pointBad = bad after the cascade, pointRefKF = mpRefKF
+ *     after it (-1 once no observation remains), normal [nPoints][3] / minDistance / maxDistance as UpdateNormalAndDepth leaves them
+ *     (0 for a bad point, which it leaves unchanged).
+ *   lmStats [5]: iterations, trials, lambda, chi2, initial chi2 of LbaResult (iterations -1 when nothing was optimised).
+ *   optional (may be NULL): optPose [nKF][7] / optPoint [nPoints][3], the solver's double estimates per local keyframe / point in list order;
+ *     edgeChi2 / edgeDepthPositive [obsStart[nPoints]] per observation with an edge.
+ * Errors: ORB_ERR_ARG for an index, octave or CSR offset out of range, a CSR that does not start at 0 or decreases, repeated keyframe /
+ * point ids, a keyframe listed twice among a point's observations, or null arrays a map needs; ORB_ERR_CAPACITY when nMaps > max_batch or a map's built problem exceeds max_poses / max_points /
+ * max_edges.  The message names the map.  Launches (lba_local_last_launches): walk, fill, structure, solver and finish whatever nMaps
+ * when any map reaches the solver, else walk and finish.  One staging upload, one copy of the built sizes back, three small tables
+ * (slot records, fill sources, solve results) to the device, one download. */
+enum { LBA_LOCAL_RAN = 0, LBA_LOCAL_NO_FIXED = 1, LBA_LOCAL_STOPPED = 2 };
+enum { LBA_OBS_NO_EDGE = 0, LBA_OBS_KEPT = 1, LBA_OBS_ERASED = 2 };
+typedef struct LbaLocalMap {
+    int32_t nKF;
+    const uint64_t* mnId; const uint8_t* kfFlags; const float* pose7; const float* cameraCenter; const float* cam4;
+    int32_t nCov;
+    const int32_t* cov; const int32_t* slotStart; const int32_t* slotPoint;
+    int32_t nPoints;
+    const uint64_t* pointId; const uint8_t* pointFlags; const float* worldPos; const int32_t* refKF;
+    const int32_t* obsStart; const int32_t* obsKF; const int32_t* obsIdx; const float* obsPt; const int32_t* obsOctave;
+    int32_t nlevels;
+    const float* invLevelSigma2; const float* scaleFactors;
+    int32_t inertial;
+    const volatile uint8_t* stopFlag;
+    int32_t* status; int32_t* counts; int32_t* nLists;
+    int32_t* localKF; int32_t* fixedKF; int32_t* localPoint; uint8_t* obsFlag;
+    float* kfPose7; float* kfCenter;
+    float* pointPos; uint8_t* pointBad; int32_t* pointRefKF; float* normal; float* minDistance; float* maxDistance;
+    double* lmStats;
+    double* optPose; double* optPoint; double* edgeChi2; uint8_t* edgeDepthPositive;
+} LbaLocalMap;
+int lba_local_bundle_adjustment_batch(lba_handle* h, int nMaps, const LbaLocalMap* maps);
+int lba_local_last_launches(const lba_handle* h);
+
 /* ------------------------------------------------------------------------------------------
  * int Optimizer::PoseOptimization(Frame* pFrame) (reference include/Optimizer.h:62, src/Optimizer.cc:814-1114), monocular
  * branch, for `count` frames at once (one CTA per frame).  Per frame f (slots of `cap` entries, N[f] used):

@@ -303,6 +303,12 @@ public:
         orb_check(lba_solve(detail::lba_handle_for(graph.nPoses, graph.nPoints > 0 ? graph.nPoints : 1, graph.nEdges > 0 ? graph.nEdges : 1, device),
                             &graph, &out), "lba_solve");
     }
+    // The same function as a whole, walk, erase cascade and write-back included, for a batch of maps (one keyframe each): each LbaLocalMap
+    // is the flattened map and receives the record the host replays (include/orb_b200.h, INTEGRATION.md §3).  h is sized for the largest
+    // built problem and for nMaps (lba_create_batch).
+    static void LocalBundleAdjustmentBatch(lba_handle* h, int nMaps, const LbaLocalMap* maps) {
+        orb_check(lba_local_bundle_adjustment_batch(h, nMaps, maps), "lba_local_bundle_adjustment_batch");
+    }
     // int static PoseOptimization(Frame* pFrame)  (src/Optimizer.cc:814-1113, monocular branch): the caller flattens the frame's map
     // point associations (:862-905); returns nInitialCorrespondences - nBad, writes the pose and the outlier flags.
     static int PoseOptimization(int N, const double pose7[7], const float cam4[4], const double* Xw, const double* obs, const float* invSigma2,

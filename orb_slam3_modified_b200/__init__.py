@@ -121,6 +121,8 @@ SIGNATURES = {
     'lba_last_helpers': (_i, [_vp]),
     'lba_set_helpers': (_i, [_vp, _i]),
     'lba_get_phase_ns': (_i, [_vp, _i, _vp]),
+    'lba_local_bundle_adjustment_batch': (_i, [_vp, _i, _vp]),
+    'lba_local_last_launches': (_i, [_vp]),
     'pose_optimization_batch': (_i, [_i, _i] + [_vp] * 6 + [_d] + [_vp] * 3 + [_i]),
     'imu_preintegrate_batch': (_i, [_i, _vp, _i] + [_vp] * 6 + [_i]),
     'imu_information_batch': (_i, [_i] + [_vp] * 4 + [_i]),
@@ -1263,10 +1265,79 @@ class _LbaResult(C.Structure):
                 ('initialChi2', C.c_double), ('gpuLaunches', C.c_int)]
 
 
+#: lba_local_bundle_adjustment_batch's map statuses and observation flags (LBA_LOCAL_*, LBA_OBS_*; include/orb_b200.h)
+LBA_LOCAL_RAN, LBA_LOCAL_NO_FIXED, LBA_LOCAL_STOPPED = 0, 1, 2
+LBA_OBS_NO_EDGE, LBA_OBS_KEPT, LBA_OBS_ERASED = 0, 1, 2
+#: the input arrays of one LbaLocalMap, with their dtypes
+LOCAL_BA_ARRAYS = (('mnId', np.uint64), ('kfFlags', np.uint8), ('pose7', np.float32), ('cameraCenter', np.float32), ('cam4', np.float32),
+                   ('cov', np.int32), ('slotStart', np.int32), ('slotPoint', np.int32), ('pointId', np.uint64), ('pointFlags', np.uint8),
+                   ('worldPos', np.float32), ('refKF', np.int32), ('obsStart', np.int32), ('obsKF', np.int32), ('obsIdx', np.int32),
+                   ('obsPt', np.float32), ('obsOctave', np.int32), ('invLevelSigma2', np.float32), ('scaleFactors', np.float32))
+#: its outputs: (name, dtype, rows, row shape); rows 'kf' = [nKF], 'pt' = [nPoints], 'obs' = [obsStart[-1]], or a fixed count
+LOCAL_BA_OUTPUTS = (('counts', np.int32, 4, ()), ('nLists', np.int32, 3, ()), ('localKF', np.int32, 'kf', ()), ('fixedKF', np.int32, 'kf', ()),
+                    ('localPoint', np.int32, 'pt', ()), ('obsFlag', np.uint8, 'obs', ()), ('kfPose7', np.float32, 'kf', (7,)),
+                    ('kfCenter', np.float32, 'kf', (3,)), ('pointPos', np.float32, 'pt', (3,)), ('pointBad', np.uint8, 'pt', ()),
+                    ('pointRefKF', np.int32, 'pt', ()), ('normal', np.float32, 'pt', (3,)), ('minDistance', np.float32, 'pt', ()),
+                    ('maxDistance', np.float32, 'pt', ()), ('lmStats', np.float64, 5, ()))
+#: the optional outputs (the solver's own results)
+LOCAL_BA_DEBUG = (('optPose', np.float64, 'kf', (7,)), ('optPoint', np.float64, 'pt', (3,)), ('edgeChi2', np.float64, 'obs', ()),
+                  ('edgeDepthPositive', np.uint8, 'obs', ()))
+
+
+class LbaLocalMap(C.Structure):
+    """One map of lba_local_bundle_adjustment_batch (include/orb_b200.h)."""
+    _fields_ = [('nKF', C.c_int)] + [(n, C.c_void_p) for n in ('mnId', 'kfFlags', 'pose7', 'cameraCenter', 'cam4')] + [('nCov', C.c_int)] + \
+               [(n, C.c_void_p) for n in ('cov', 'slotStart', 'slotPoint')] + [('nPoints', C.c_int)] + \
+               [(n, C.c_void_p) for n in ('pointId', 'pointFlags', 'worldPos', 'refKF', 'obsStart', 'obsKF', 'obsIdx', 'obsPt', 'obsOctave')] + \
+               [('nlevels', C.c_int), ('invLevelSigma2', C.c_void_p), ('scaleFactors', C.c_void_p), ('inertial', C.c_int), ('stopFlag', C.c_void_p),
+                ('status', C.c_void_p)] + [(n, C.c_void_p) for n, _, _, _ in LOCAL_BA_OUTPUTS] + \
+               [(n, C.c_void_p) for n, _, _, _ in LOCAL_BA_DEBUG]
+
+
+def local_ba_struct(m, debug=False, given=None):
+    """LbaLocalMap over map dict `m` (keys LOCAL_BA_ARRAYS, 'inertial' and optionally 'stop' = a one-byte uint8 array) with fresh outputs:
+    (struct, out dict, arrays to keep alive).  debug: also the optional outputs.  given: a dict of LOCAL_BA_DEBUG arrays to point them at
+    instead (the CPU oracle reads them as the optimiser's results)."""
+    a = {n: _c(m[n] if m.get(n) is not None else np.zeros(0), dt) for n, dt in LOCAL_BA_ARRAYS}
+    nK, nP, nC = len(a['kfFlags']), len(a['pointFlags']), len(a['cov'])
+    nO = int(a['obsStart'][-1]) if nP else 0
+    rows = dict(kf=nK, pt=nP, obs=nO)
+    out = {n: np.zeros((r if isinstance(r, int) else rows[r],) + sh, dt) for n, dt, r, sh in LOCAL_BA_OUTPUTS}
+    out['status'] = np.zeros(1, np.int32)
+    if given is not None:
+        out.update({n: _c(given[n], dt) for n, dt, _, _ in LOCAL_BA_DEBUG})
+    elif debug:
+        out.update({n: np.zeros((rows[r],) + sh, dt) for n, dt, r, sh in LOCAL_BA_DEBUG})
+    stop = m.get('stop')
+    s = LbaLocalMap(nK, *[_ptr(a[n]) for n in ('mnId', 'kfFlags', 'pose7', 'cameraCenter', 'cam4')], nC,
+                    *[_ptr(a[n]) for n in ('cov', 'slotStart', 'slotPoint')], nP,
+                    *[_ptr(a[n]) for n in ('pointId', 'pointFlags', 'worldPos', 'refKF', 'obsStart', 'obsKF', 'obsIdx', 'obsPt', 'obsOctave')],
+                    len(a['scaleFactors']), _ptr(a['invLevelSigma2']), _ptr(a['scaleFactors']), int(m.get('inertial', 0)), _ptr(stop),
+                    _ptr(out['status']), *[_ptr(out[n]) for n, _, _, _ in LOCAL_BA_OUTPUTS], *[_ptr(out.get(n)) for n, _, _, _ in LOCAL_BA_DEBUG])
+    a['stop'] = stop
+    return s, out, a
+
+
+def local_ba_result(out):
+    """The output dict with the scalars unpacked and the lists cut to their lengths."""
+    nLoc, nFix, nPt = (int(v) for v in out['nLists'])
+    r = dict(out, status=int(out['status'][0]), num_fixedKF=int(out['counts'][0]), num_OptKF=int(out['counts'][1]), num_MPs=int(out['counts'][2]),
+             num_edges=int(out['counts'][3]))
+    r['localKF'], r['fixedKF'], r['localPoint'] = out['localKF'][:nLoc].copy(), out['fixedKF'][:nFix].copy(), out['localPoint'][:nPt].copy()
+    for n in ('kfPose7', 'kfCenter', 'optPose'):
+        if n in r:
+            r[n] = out[n][:nLoc].copy()
+    for n in ('pointPos', 'pointBad', 'pointRefKF', 'normal', 'minDistance', 'maxDistance', 'optPoint'):
+        if n in r:
+            r[n] = out[n][:nPt].copy()
+    return r
+
+
 class Optimizer:
-    """Mirror of the static ``ORB_SLAM3::Optimizer`` functions on the hot path.  The pointer-graph walk of
-    ``LocalBundleAdjustment`` (src/Optimizer.cc:1125-1403) stays with the caller; this object runs the numeric core
-    on flat arrays (``synth.lba_problem`` has the layout) and returns what the write-back / outlier test reads."""
+    """Mirror of the static ``ORB_SLAM3::Optimizer`` functions on the hot path.  ``LocalBundleAdjustment`` runs the numeric core
+    on flat arrays (``synth.lba_problem`` has the layout) and returns what the write-back / outlier test reads, the caller keeping the
+    pointer-graph walk (src/Optimizer.cc:1125-1403); ``local_bundle_adjustment_batch`` runs the whole function, walk, erase cascade and
+    write-back included, from flattened maps and returns the record the caller replays."""
 
     def __init__(self, max_poses=64, max_points=8192, max_edges=65536, max_batch=1, device=0):
         L = lib()
@@ -1349,6 +1420,19 @@ class Optimizer:
         rc = lib().lba_set_helpers(self._h, clusters)
         if rc != ORB_OK:
             raise OrbError(rc, 'lba_set_helpers')
+
+    def local_bundle_adjustment_batch(self, maps, debug=False):
+        """``Optimizer::LocalBundleAdjustment`` as a whole -- walk, solve, erase cascade, write-back -- for one map per item (dicts as
+        ``local_ba_struct`` reads them), in one call.  Returns one ``local_ba_result`` dict per map; debug adds the solver's own results."""
+        packs = [local_ba_struct(m, debug=debug) for m in maps]
+        arr = (LbaLocalMap * max(1, len(maps)))(*[p[0] for p in packs])
+        rc = lib().lba_local_bundle_adjustment_batch(self._h, len(maps), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'lba_local_bundle_adjustment_batch')
+        return [local_ba_result(p[1]) for p in packs]
+
+    def local_last_launches(self):
+        return lib().lba_local_last_launches(self._h)
 
     def LocalBundleAdjustment(self, prob, iterations=10, user_lambda_init=0.0, stop_flag=None):
         keep = dict(poses=_c(prob['poses'], np.float64), fixed=_c(prob['fixed'], np.uint8), cam=_c(prob['cam'], np.float32),

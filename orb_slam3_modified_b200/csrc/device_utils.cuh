@@ -40,14 +40,18 @@ inline int require_sm90(int major, int minor) {
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of the (function, device) pair, not of a handle: several handles of
 // different sizes share it.  Keep a process-wide monotonic maximum per kernel and device and only ever raise it, so that a
-// smaller handle created later can never lower the limit under a larger one (the launch would fail with invalid-value).
+// smaller handle created later can never lower the limit under a larger one (the launch would fail with invalid-value).  Without the
+// opt-in, static + dynamic shared memory must stay within 48 KB: the kernel's static shared memory counts towards that bound.
 template <class Kernel>
 inline int ensure_dynamic_smem(Kernel* kernel, size_t bytes, int device) {
     static std::mutex mu;
     static std::map<std::pair<const void*, int>, size_t> current;
     std::lock_guard<std::mutex> lock(mu);
     size_t& cur = current[std::make_pair((const void*)kernel, device)];
-    if (bytes <= cur || bytes <= 48 * 1024) return 0;
+    if (bytes <= cur) return 0;
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) { set_error("cudaFuncGetAttributes failed"); return ORB_ERR_CUDA; }
+    if (bytes + fa.sharedSizeBytes <= 48 * 1024) return 0;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute(MaxDynamicSharedMemorySize): ") + cudaGetErrorString(e)); return ORB_ERR_CUDA; }
     cur = bytes;

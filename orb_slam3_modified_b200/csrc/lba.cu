@@ -36,6 +36,8 @@
 #include "host_affinity.h"
 #include "device_utils.cuh"
 #include "inertial_dev.cuh"
+#include "local_ba.h"
+#include "staging.h"
 
 using orbx::set_error;
 
@@ -1395,6 +1397,30 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     if (tid == 0) { D.nChunks = nChunks; status[blockIdx.x] = 0; }
 }
 
+// A graph built on the device (csrc/local_ba.cu) copied into its slot's uploaded block, as pack() copies a caller's graph: one CTA
+// per slot; hidx / freePose from the fixed flags in pose order.
+__global__ void __launch_bounds__(BT) lba_fill_kernel(Dev* probs, const FillSrc* src) {
+    const Dev& D = probs[blockIdx.x];
+    const FillSrc& F = src[blockIdx.x];
+    const int tid = threadIdx.x;
+    for (int i = tid; i < 7 * D.nP; i += BT) const_cast<double*>(D.initPoses)[i] = F.poses[i];
+    for (int i = tid; i < 4 * D.nP; i += BT) const_cast<float*>(D.cam)[i] = F.cam[i];
+    for (int i = tid; i < 3 * D.nL; i += BT) const_cast<double*>(D.initPts)[i] = F.points[i];
+    for (int e = tid; e < D.nE; e += BT) {
+        const_cast<int*>(D.rawEdgePoint)[e] = F.edgePoint[e]; const_cast<int*>(D.rawEdgePose)[e] = F.edgePose[e];
+        const_cast<double*>(D.rawObs)[2 * e] = F.obs[2 * e]; const_cast<double*>(D.rawObs)[2 * e + 1] = F.obs[2 * e + 1];
+        const_cast<float*>(D.rawInvSigma2)[e] = F.invSigma2[e];
+    }
+    if (tid == 0) {
+        int nF = 0;
+        for (int i = 0; i < D.nP; ++i) {
+            const int h = F.fixed[i] ? -1 : nF++;
+            const_cast<int*>(D.hidx)[i] = h;
+            if (h >= 0) const_cast<int*>(D.freePose)[h] = i;
+        }
+    }
+}
+
 // =============================================================================================
 // host side
 // =============================================================================================
@@ -1416,6 +1442,8 @@ struct Solver {
     bool ranOnce = false;
     int nLoaded = 0, launches = 0, numSMs = 132;
     unsigned long long* d_finished = nullptr;        // problems finished in the running launch (helper CTAs leave when it reaches the batch)
+    orbx::Staging stage;                             // lba_local_bundle_adjustment_batch's inputs and outputs (csrc/local_ba.cu)
+    int localLaunches = 0;
     ~Solver() {
         cudaSetDevice(device);
         if (d_finished) cudaFree(d_finished);
@@ -1456,6 +1484,7 @@ struct Solver {
         CK(cudaGetDeviceProperties(&prop, device));
         if (orbx::require_sm90(prop.major, prop.minor)) return ORB_ERR_CUDA;
         numSMs = prop.multiProcessorCount;
+        stage.device = device;
         perProblem = need(maxP, maxL, maxE);
         arenaBytes = perProblem * (size_t)maxBatch;
         CK(cudaMalloc(&d_arena, arenaBytes));
@@ -1477,24 +1506,18 @@ struct Solver {
         return ORB_OK;
     }
 
-    // Lays one problem out in slot `slot` of the arena and copies the caller's graph into the pinned mirror; the index
-    // structures are derived on the device (lba_build_structure_kernel).
-    int pack(int slot, const LbaProblem* P) {
-        const int nP = P->nPoses, nL = P->nPoints, nE = P->nEdges;
-        if (nP < 1 || nL < 0 || nE < 0 || nP > maxP || nL > maxL || nE > maxE || !P->poses || !P->poseFixed || !P->cam ||
-            (nL && !P->points) || (nE && (!P->edgePoint || !P->edgePose || !P->obs || !P->invSigma2))) {
-            set_error("lba: problem larger than the handle or null arrays"); return ORB_ERR_ARG;
-        }
-        std::vector<int> hidx(nP, -1), freePose;
-        for (int i = 0; i < nP; ++i) if (!P->poseFixed[i]) { hidx[i] = (int)freePose.size(); freePose.push_back(i); }
-        const int nF = (int)freePose.size(), n = 6 * nF;
-        if (nF + nL == 0) { set_error("lba: 0 vertices to optimize"); return ORB_ERR_ARG; }
+    // Where a slot's uploaded block keeps the caller's graph (arena offsets)
+    struct UpBlock { size_t poses, pts, cam, hidx, freePose, ePt, ePose, obs, isg; };
+
+    // Lays slot `slot` of the arena out for a problem of the given sizes: the device views of every piece in h_probs[slot], the
+    // download layout in packed[slot] and the uploaded block in U.  The problem's scalars are left to the caller.
+    int layout(int slot, int nP, int nL, int nE, int nF, UpBlock& U) {
+        const int n = 6 * nF;
         const int nOff = nF * (nF - 1) / 2, nTasks = nF + nOff;
         const size_t pc = pairCapOf(nP, nE), cc = chunkCapOf(nP, nE);
         const size_t base = perProblem * (size_t)slot;
         size_t off = base;
         auto carve = [&](size_t bytes) { size_t o = off; off += al(bytes); return o; };
-        auto put = [&](size_t o, const void* src, size_t bytes) { if (bytes) memcpy(h_arena + o, src, bytes); };
         Dev& D = h_probs[slot]; memset(&D, 0, sizeof(D));
         Packed& K = packed[slot];
         K.nP = nP; K.nL = nL; K.nE = nE; K.nF = nF;
@@ -1507,16 +1530,15 @@ struct Solver {
         K.statsOff = carve(512); D.stats = (double*)(d_arena + K.statsOff);
         // --- uploaded block: the caller's graph ---
         const size_t upBase = off;
-        size_t o;
-        o = carve(56 * (size_t)nP); put(o, P->poses, 56 * (size_t)nP); D.initPoses = (const double*)(d_arena + o);
-        o = carve(24 * (size_t)nL); put(o, P->points, 24 * (size_t)nL); D.initPts = (const double*)(d_arena + o);
-        o = carve(16 * (size_t)nP); put(o, P->cam, 16 * (size_t)nP); D.cam = (const float*)(d_arena + o);
-        o = carve(4 * (size_t)nP); put(o, hidx.data(), 4 * (size_t)nP); D.hidx = (const int*)(d_arena + o);
-        o = carve(4 * (size_t)std::max(nF, 1)); put(o, freePose.data(), 4 * (size_t)nF); D.freePose = (const int*)(d_arena + o);
-        o = carve(4 * (size_t)nE); put(o, P->edgePoint, 4 * (size_t)nE); D.rawEdgePoint = (const int*)(d_arena + o);
-        o = carve(4 * (size_t)nE); put(o, P->edgePose, 4 * (size_t)nE); D.rawEdgePose = (const int*)(d_arena + o);
-        o = carve(16 * (size_t)nE); put(o, P->obs, 16 * (size_t)nE); D.rawObs = (const double*)(d_arena + o);
-        o = carve(4 * (size_t)nE); put(o, P->invSigma2, 4 * (size_t)nE); D.rawInvSigma2 = (const float*)(d_arena + o);
+        U.poses = carve(56 * (size_t)nP); D.initPoses = (const double*)(d_arena + U.poses);
+        U.pts = carve(24 * (size_t)nL); D.initPts = (const double*)(d_arena + U.pts);
+        U.cam = carve(16 * (size_t)nP); D.cam = (const float*)(d_arena + U.cam);
+        U.hidx = carve(4 * (size_t)nP); D.hidx = (const int*)(d_arena + U.hidx);
+        U.freePose = carve(4 * (size_t)std::max(nF, 1)); D.freePose = (const int*)(d_arena + U.freePose);
+        U.ePt = carve(4 * (size_t)nE); D.rawEdgePoint = (const int*)(d_arena + U.ePt);
+        U.ePose = carve(4 * (size_t)nE); D.rawEdgePose = (const int*)(d_arena + U.ePose);
+        U.obs = carve(16 * (size_t)nE); D.rawObs = (const double*)(d_arena + U.obs);
+        U.isg = carve(4 * (size_t)nE); D.rawInvSigma2 = (const float*)(d_arena + U.isg);
         uploadOff[slot] = upBase; uploadBytes[slot] = off - upBase;
         // --- derived on the device ---
         D.ePt = (const int*)(d_arena + carve(4 * (size_t)nE)); D.ePose = (const int*)(d_arena + carve(4 * (size_t)nE));
@@ -1546,6 +1568,29 @@ struct Solver {
         D.job = (Job*)(d_arena + carve(sizeof(Job))); D.pcm = (double*)(d_arena + carve(8 * PC * (size_t)nP));
         if (cc + ((size_t)nL + PCH - 1) / PCH >= ((size_t)1 << 23)) { set_error("lba: more chunks in one phase than the claim word counts"); return ORB_ERR_CAPACITY; }
         if (off - base > perProblem) { set_error("lba: arena too small (internal sizing error)"); return ORB_ERR_CAPACITY; }
+        return ORB_OK;
+    }
+
+    // Lays one problem out in slot `slot` of the arena and copies the caller's graph into the pinned mirror; the index
+    // structures are derived on the device (lba_build_structure_kernel).
+    int pack(int slot, const LbaProblem* P) {
+        const int nP = P->nPoses, nL = P->nPoints, nE = P->nEdges;
+        if (nP < 1 || nL < 0 || nE < 0 || nP > maxP || nL > maxL || nE > maxE || !P->poses || !P->poseFixed || !P->cam ||
+            (nL && !P->points) || (nE && (!P->edgePoint || !P->edgePose || !P->obs || !P->invSigma2))) {
+            set_error("lba: problem larger than the handle or null arrays"); return ORB_ERR_ARG;
+        }
+        std::vector<int> hidx(nP, -1), freePose;
+        for (int i = 0; i < nP; ++i) if (!P->poseFixed[i]) { hidx[i] = (int)freePose.size(); freePose.push_back(i); }
+        const int nF = (int)freePose.size();
+        if (nF + nL == 0) { set_error("lba: 0 vertices to optimize"); return ORB_ERR_ARG; }
+        UpBlock U;
+        if (int rc = layout(slot, nP, nL, nE, nF, U)) return rc;
+        auto put = [&](size_t o, const void* src, size_t bytes) { if (bytes) memcpy(h_arena + o, src, bytes); };
+        put(U.poses, P->poses, 56 * (size_t)nP); put(U.pts, P->points, 24 * (size_t)nL); put(U.cam, P->cam, 16 * (size_t)nP);
+        put(U.hidx, hidx.data(), 4 * (size_t)nP); put(U.freePose, freePose.data(), 4 * (size_t)nF);
+        put(U.ePt, P->edgePoint, 4 * (size_t)nE); put(U.ePose, P->edgePose, 4 * (size_t)nE); put(U.obs, P->obs, 16 * (size_t)nE);
+        put(U.isg, P->invSigma2, 4 * (size_t)nE);
+        Dev& D = h_probs[slot];
         D.delta = P->huberDelta; D.dsqr = P->huberDelta * P->huberDelta; D.userLambdaInit = P->userLambdaInit; D.iterations = P->iterations;
         return ORB_OK;
     }
@@ -1588,6 +1633,12 @@ struct Solver {
         lba_build_structure_kernel<<<count, BT, 0, st>>>(d_probs, d_status);     // BlockSolver::buildStructure, one CTA per problem
         CK(cudaGetLastError());
         CK(orbx::wait_stream_blocking(st, evWait));   // the resident copy must be complete before a run on any other stream
+        if (int rc = check_structure(count)) return rc;
+        nLoaded = count;
+        return ORB_OK;
+    }
+    // the status words lba_build_structure_kernel left, once its stream has been synchronised
+    int check_structure(int count) {
         for (int i = 0; i < count; ++i) {
             if (h_status[i] == 0) continue;
             nLoaded = 0;
@@ -1595,7 +1646,47 @@ struct Solver {
             if (h_status[i] == 2) { set_error("lba: duplicate (point, keyframe) observation"); return ORB_ERR_ARG; }
             set_error("lba: pair / chunk list larger than sized"); return ORB_ERR_CAPACITY;
         }
+        return ORB_OK;
+    }
+    // The device form of upload for graphs built on the device (csrc/local_ba.cu): lays every slot out from its sizes, copies the
+    // graphs in with lba_fill_kernel and enqueues lba_build_structure_kernel on st.  Its status words are read by check_structure
+    // once the caller has synchronised st.
+    int load_device(int count, const int4* sizes, const double* userLambdaInit, const FillSrc* dFill) {
+        nLoaded = 0;
+        uploadBytes.assign(maxBatch, 0); uploadOff.assign(maxBatch, 0);
+        CK(cudaSetDevice(device));
+        if (ranOnce) CK(cudaStreamWaitEvent(st, evRun, 0));
+        for (int i = 0; i < count; ++i) {
+            UpBlock U;
+            if (int rc = layout(i, sizes[i].x, sizes[i].y, sizes[i].z, sizes[i].w, U)) return rc;
+            Dev& D = h_probs[i];
+            D.delta = huber_mono(); D.dsqr = D.delta * D.delta; D.userLambdaInit = userLambdaInit[i]; D.iterations = 10;
+        }
+        CK(cudaMemcpyAsync(d_probs, h_probs.data(), sizeof(Dev) * count, cudaMemcpyHostToDevice, st));
+        lba_fill_kernel<<<count, BT, 0, st>>>(d_probs, dFill);
+        CK(cudaGetLastError());
+        for (int i = 0; i < count; ++i) h_status[i] = -1;
+        lba_build_structure_kernel<<<count, BT, 0, st>>>(d_probs, d_status);
+        CK(cudaGetLastError());
         nLoaded = count;
+        return ORB_OK;
+    }
+    // run on st, forwarding the callers' stop flags (SparseOptimizer::terminate() polls *pbStopFlag) while the kernel runs
+    int run_forwarding(const volatile uint8_t* const* flags) {
+        const int count = nLoaded;
+        for (int i = 0; i < count; ++i) h_stop[i] = (flags[i] && *flags[i]) ? 1 : 0;
+        if (int rc = run(st)) return rc;
+        bool anyFlag = false;
+        for (int i = 0; i < count; ++i) anyFlag = anyFlag || flags[i];
+        if (anyFlag) {
+            CK(cudaEventRecord(evDone, st));
+            while (cudaEventQuery(evDone) == cudaErrorNotReady) {
+                for (int i = 0; i < count; ++i)
+                    if (flags[i] && *flags[i]) h_stop[i] = 1;
+                std::this_thread::yield();
+            }
+        }
+        CK(cudaGetLastError());
         return ORB_OK;
     }
     // (re)start from the uploaded initial estimates and run the whole LM loop for every loaded problem
@@ -1743,23 +1834,36 @@ int lba_solve_batch(lba_handle* h, int count, const LbaProblem* problems, LbaRes
     Solver& S = h->s;
     int rc = S.upload(count, problems);
     if (rc) return rc;
-    for (int i = 0; i < count; ++i) S.h_stop[i] = (problems[i].stopFlag && *problems[i].stopFlag) ? 1 : 0;
-    rc = S.run(S.st);
-    if (rc) return rc;
-    bool anyFlag = false;
-    for (int i = 0; i < count; ++i) anyFlag = anyFlag || problems[i].stopFlag;
-    if (anyFlag) {
-        CK(cudaEventRecord(S.evDone, S.st));
-        // forward the callers' stop flags (SparseOptimizer::terminate() polls *pbStopFlag) while the kernel runs
-        while (cudaEventQuery(S.evDone) == cudaErrorNotReady) {
-            for (int i = 0; i < count; ++i)
-                if (problems[i].stopFlag && *problems[i].stopFlag) S.h_stop[i] = 1;
-            std::this_thread::yield();
-        }
-    }
-    CK(cudaGetLastError());
+    std::vector<const volatile uint8_t*> flags(count);
+    for (int i = 0; i < count; ++i) flags[i] = problems[i].stopFlag;
+    if ((rc = S.run_forwarding(flags.data()))) return rc;
     return S.download(count, results, S.st);
 }
 int lba_solve(lba_handle* h, const LbaProblem* problem, LbaResult* result) { return lba_solve_batch(h, 1, problem, result); }
+int lba_local_last_launches(const lba_handle* h) { return h ? h->s.localLaunches : ORB_ERR_ARG; }
 
 }  // extern "C"
+
+namespace lba {
+cudaStream_t solver_stream(lba_handle* h) { return h->s.st; }
+orbx::Staging& solver_staging(lba_handle* h) { return h->s.stage; }
+void solver_limits(const lba_handle* h, int* maxP, int* maxL, int* maxE, int* maxBatch) {
+    *maxP = h->s.maxP; *maxL = h->s.maxL; *maxE = h->s.maxE; *maxBatch = h->s.maxBatch;
+}
+int solver_load_device(lba_handle* h, int count, const int4* sizes, const double* userLambdaInit, const FillSrc* dFill, SlotOut* out) {
+    Solver& S = h->s;
+    if (int rc = S.load_device(count, sizes, userLambdaInit, dFill)) return rc;
+    for (int i = 0; i < count; ++i) {
+        const Dev& D = S.h_probs[i];
+        out[i] = SlotOut{D.poses, D.pts, D.outChi2, D.outDepthPos, D.stats};
+    }
+    return ORB_OK;
+}
+int solver_run(lba_handle* h, const volatile uint8_t* const* flags) { return h->s.run_forwarding(flags); }
+int solver_check_structure(lba_handle* h, int count) {
+    Solver& S = h->s;
+    CK(orbx::wait_stream_blocking(S.st, S.evWait));
+    return S.check_structure(count);
+}
+void solver_set_local_launches(lba_handle* h, int n) { h->s.localLaunches = n; }
+}  // namespace lba

@@ -9,10 +9,7 @@
 //   3. KFcounter in shared memory (in the counter output beyond UC_SMEM_KF keyframes), atomics over (slot, observation);
 //   4. the selection (th = 15, else the first strict maximum in key order), the ordered list by rank over (weight, key), the parent;
 //   5. warp per AddConnection target: its new weight map re-sorted by (weight, key) without bad keyframes, unless the weight is equal.
-//
-// Float rules (the oracle evaluates the same expressions with -ffp-contract=off): |v| = sqrtf((x*x + y*y) + z*z), every operation
-// rounded; the normal is the running sum of v / |v| element-wise from zero in key order, then / (float)n; mfMaxDistance = dist *
-// scaleFactors[level], mfMinDistance = mfMaxDistance / scaleFactors[nlevels - 1].
+// UpdateNormalAndDepth's float rules are normal_depth.cuh's.
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <stdint.h>
@@ -24,11 +21,13 @@
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
 #include "matcher_context.h"
+#include "normal_depth.cuh"
 #include "staging.h"
 
 namespace orbm {
 
 using orbx::distinctive_best;
+using orbx::update_normal_and_depth;
 using orbx::set_error;
 
 constexpr int UC_NT = 256;
@@ -49,10 +48,6 @@ struct UcItem {
     int* rows;               // [obsStart[nPoints] + nPoints] per point from obsStart[p] + p: its descriptor rows (observation, -1 = new)
     int* cand;               // [nKF] the keyframes of vPairs
 };
-
-__device__ __forceinline__ float norm3(float x, float y, float z) {
-    return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
-}
 
 // (w1, key1) > (w2, key2): the order of the ordered lists (sort ascending by pair<int, KeyFrame*>, then push_front)
 __device__ __forceinline__ bool heavier(int w1, unsigned long long k1, int w2, unsigned long long k2) { return w1 > w2 || (w1 == w2 && k1 > k2); }
@@ -109,30 +104,19 @@ __global__ void __launch_bounds__(UC_NT) update_connections_kernel(const UcItem*
         int* rows = I.rows + o0 + p;
         int nRows = 0;
         if (lane == 0) {
-            const float px = I.pos[3 * p], py = I.pos[3 * p + 1], pz = I.pos[3 * p + 2];
-            const int ref = I.refKF[p];
             const unsigned long long newKey = I.order[0];
-            float nx = 0.f, ny = 0.f, nz = 0.f;
-            int n = 0, level = 0;
             bool pending = ns >= 0;
-            for (int o = o0; o <= o1; ++o) {
-                int k, oct, row;
-                if (pending && (o == o1 || I.order[I.obsKF[o]] > newKey)) { k = 0; oct = I.slotOctave[ns]; row = -1; pending = false; --o; }
-                else if (o == o1) break;
-                else { k = I.obsKF[o]; oct = I.obsOctave[o]; row = o; }
-                const float vx = __fsub_rn(px, I.Ow[3 * k]), vy = __fsub_rn(py, I.Ow[3 * k + 1]), vz = __fsub_rn(pz, I.Ow[3 * k + 2]);
-                const float d = norm3(vx, vy, vz);
-                nx = __fadd_rn(nx, __fdiv_rn(vx, d)); ny = __fadd_rn(ny, __fdiv_rn(vy, d)); nz = __fadd_rn(nz, __fdiv_rn(vz, d));
-                ++n;
-                if (k == ref) level = oct;
+            int o = o0;
+            // the observations in key order with the new one inserted at its key; the descriptor rows of the good observers on the way
+            auto next = [&](int& k, int& oct) {
+                int row;
+                if (pending && (o == o1 || I.order[I.obsKF[o]] > newKey)) { k = 0; oct = I.slotOctave[ns]; row = -1; pending = false; }
+                else if (o == o1) return false;
+                else { k = I.obsKF[o]; oct = I.obsOctave[o]; row = o; ++o; }
                 if (!(I.kfFlags[k] & ORBM_KF_BAD)) rows[nRows++] = row;
-            }
-            const float fn = (float)n;
-            I.normal[3 * p] = __fdiv_rn(nx, fn); I.normal[3 * p + 1] = __fdiv_rn(ny, fn); I.normal[3 * p + 2] = __fdiv_rn(nz, fn);
-            const float dist = norm3(__fsub_rn(px, I.Ow[3 * ref]), __fsub_rn(py, I.Ow[3 * ref + 1]), __fsub_rn(pz, I.Ow[3 * ref + 2]));
-            const float dmax = __fmul_rn(dist, I.scaleFactors[level]);
-            I.maxDistance[p] = dmax;
-            I.minDistance[p] = __fdiv_rn(dmax, I.scaleFactors[I.nlevels - 1]);
+                return true;
+            };
+            update_normal_and_depth(I.pos + 3 * p, I.Ow, I.refKF[p], I.scaleFactors, I.nlevels, next, I.normal + 3 * p, I.minDistance + p, I.maxDistance + p);
         }
         nRows = __shfl_sync(0xffffffffu, nRows, 0);
         __syncwarp();
