@@ -263,13 +263,14 @@ struct Extractor {
                     t.z = (short)cvRoundF((1.f - fy) * 2048); t.w = (short)cvRoundF(fy * 2048);
                     ytab.push_back(t);
                 }
-                // TMA box that covers the sources of any 128 x 8 destination tile (start column aligned down to 16 bytes)
+                // TMA box that covers the sources of any PYR_TILE_W x PYR_TILE_H destination tile (start column aligned down to 16 bytes)
                 int bw = 16, bh = 2;
-                for (int dx0 = 0; dx0 < G.w; dx0 += 128) {
-                    const int first = xtab[G.xtabOff + dx0].x & ~15, last = xtab[G.xtabOff + std::min(dx0 + 127, G.w - 1)].y;
+                for (int dx0 = 0; dx0 < G.w; dx0 += PYR_TILE_W) {
+                    const int first = xtab[G.xtabOff + dx0].x & ~15, last = xtab[G.xtabOff + std::min(dx0 + PYR_TILE_W - 1, G.w - 1)].y;
                     bw = std::max(bw, last - first + 1);
                 }
-                for (int dy0 = 0; dy0 < G.h; dy0 += 8) bh = std::max(bh, ytab[G.ytabOff + std::min(dy0 + 7, G.h - 1)].y - ytab[G.ytabOff + dy0].x + 1);
+                for (int dy0 = 0; dy0 < G.h; dy0 += PYR_TILE_H)
+                    bh = std::max(bh, ytab[G.ytabOff + std::min(dy0 + PYR_TILE_H - 1, G.h - 1)].y - ytab[G.ytabOff + dy0].x + 1);
                 G.pyrBoxW = (int)alignUp(bw, 16); G.pyrBoxH = bh;
             }
         }
@@ -419,11 +420,13 @@ struct Extractor {
         if (profiling) CK(cudaEventRecord(evStage[0], st));
         // pyramid: levels depend on each other
         for (int l = 1; l < nlevels; ++l) {
-            dim3 blk(32, 8), grd((Q.lv[l].w + 127) / 128, (Q.lv[l].h + 7) / 8, batch);
             CUtensorMap srcMap;
-            bool tma = Q.lv[l].pyrBoxW > 0 && !Q.lv[l].area2x && Q.lv[l].pyrBoxW <= 256 && Q.lv[l].pyrBoxH <= 256;
+            bool tma = Q.lv[l].pyrBoxW > 0 && !Q.lv[l].area2x && Q.lv[l].pyrBoxW <= 256 && Q.lv[l].pyrBoxH <= 256 &&
+                       Q.lv[l].pyrBoxW * Q.lv[l].pyrBoxH <= 48 * 1024;   // default dynamic shared-memory limit
             if (tma && l == 1) tma = encode_plane_map(&srcMap, Q.lv0, Q.lv[0].w, Q.lv[0].h, batch, Q.lv0Pitch, Q.lv0FrameStride, Q.lv[1].pyrBoxW, Q.lv[1].pyrBoxH);
             else if (tma) srcMap = pyrMaps.lv[l];
+            const int tileH = tma ? PYR_TILE_H : 8;   // pyr_resize_kernel: one destination row per thread
+            dim3 blk(32, 8), grd((Q.lv[l].w + PYR_TILE_W - 1) / PYR_TILE_W, (Q.lv[l].h + tileH - 1) / tileH, batch);
             if (tma) pyr_resize_tma_kernel<<<grd, blk, (size_t)Q.lv[l].pyrBoxW * Q.lv[l].pyrBoxH, st>>>(Q, l, srcMap);
             else pyr_resize_kernel<<<grd, blk, 0, st>>>(Q, l);     // exact 2x decimation (INTER_AREA promotion) or a box TMA cannot express
             ++launches;

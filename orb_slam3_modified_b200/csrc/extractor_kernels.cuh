@@ -101,9 +101,17 @@ __global__ void __launch_bounds__(256) pyr_resize_kernel(ExtractParams P, int l)
 // Output: per cell a count and a row-major (y, x) list of packed (x+offX, y+offY, score).
 // ------------------------------------------------------------------------------------------
 // Threads per (block, frame) CTA: 64 per cell of a 2 x 2 block.  Measured per 240 frames of 640x480 on an H100 80GB HBM3 at 700 W:
-// 0.914 ms, against 1.05 ms for the former 64-thread CTA per cell.  ptxas: 63 registers, no spills; ~28 KB of dynamic shared memory
-// at 640x480, so registers cap an SM at 4 CTAs (32 warps).  Capping the kernel at 48 registers for 5 CTAs measured 0.92 ms.
+// 0.88 ms with the quick test's row runs of 6 (0.92 ms with a thread per quad, 1.05 ms for the former 64-thread CTA per cell).
+// ptxas: 64 registers (the launch bound asks for 4 CTAs per SM; unbounded, the row window takes 94), no spills; ~28 KB of dynamic
+// shared memory at 640x480, so registers cap an SM at 4 CTAs (32 warps).  Capping the per-quad form at 48 registers for 5 CTAs measured 0.92 ms.
 constexpr int FAST_NT = 256;
+// Interior rows per thread in the quick test (phase 1): a run's candidates travel as one 32-bit mask, 4 pixels per row.  Measured per
+// 240 frames as above: runs of 4 / 6 / 8 rows 0.890 / 0.873 / 0.891 ms (at 6, the 18 quads x 13 runs of a level-0 block fill 234 of
+// the 256 threads in one pass).
+#ifndef FAST_RUN
+#define FAST_RUN 6
+#endif
+static_assert(FAST_RUN >= 1 && FAST_RUN <= 8, "a run's candidate mask is 4 * FAST_RUN bits of one word");
 
 __device__ __forceinline__ int fast_score_at(const uint8_t* t, const int* off) {
     // d_k = v - p_k (darker ring), e_k = p_k - v (brighter ring) for the 16 ring pixels.
@@ -161,7 +169,7 @@ __device__ __forceinline__ uint32_t fast_col_mask(int w, int x0, int x1) {
     return (hi >= 32 ? 0xFFFFFFFFu : (1u << hi) - 1u) & (0xFFFFFFFFu << lo);
 }
 
-__global__ void __launch_bounds__(FAST_NT) fast_cells_kernel(ExtractParams P, const __grid_constant__ CUtensorMap map0, const CUtensorMap* __restrict__ maps) {
+__global__ void __launch_bounds__(FAST_NT, 4) fast_cells_kernel(ExtractParams P, const __grid_constant__ CUtensorMap map0, const CUtensorMap* __restrict__ maps) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_bar;
     __shared__ int s_nCand, s_warp[33];
@@ -214,68 +222,74 @@ __global__ void __launch_bounds__(FAST_NT) fast_cells_kernel(ExtractParams P, co
     mbar_wait(&s_bar, 0);
 
     // phase 1: cheap rejection (any 9-arc contains ring pixel k or k+8 for every k) + compaction of the survivors.
-    // One thread tests four horizontally adjacent pixels; pixels travel in pairs as 2 x 16-bit lanes so that one
-    // VIADD.16x2 / LOP3 serves two pixels: with NLO = T - v and NHI1 = -(v + T + 1) per lane,
+    // One thread owns a run of FAST_RUN interior rows of one quad column (four horizontally adjacent pixels).  It walks the run
+    // down a sliding window of tile rows: every tile row of the run (and its 3-row ring margins) is loaded and funnel-shifted once,
+    // into the five 4-pixel windows the ring reads from it, instead of once per quad that reads it.  Rows y +- 1 are never read.
+    // Pixels travel in pairs as 2 x 16-bit lanes so that one VIADD.16x2 / LOP3 serves two pixels: with NLO = T - v and
+    // NHI1 = -(v + T + 1) per lane,
     //   p < v - T  <=>  sign(p + NLO) set,      p > v + T  <=>  sign(p + NHI1) clear.
     const int th = P.minTh;
     {
-        const int nq = (iw + 3) >> 2, nQ = nq * ih;
+        const int nq = (iw + 3) >> 2, nI = nq * ((ih + FAST_RUN - 1) / FAST_RUN);
         const unsigned qmagic = 0xFFFFFFFFu / (unsigned)nq + 1u;
         const uint32_t TT = (uint32_t)th * 0x10001u, TT1 = (uint32_t)(th + 1) * 0x10001u;
         const int shC = ((xoff) & 3) * 8;            // byte phase of column (4q + xoff) inside an aligned word
-        for (int base = 0; base < nQ; base += FAST_NT) {
-            const int qi = base + tid;
-            uint32_t c01 = 0, c23 = 0;
-            int y = 0, q = 0;
-            if (qi < nQ) {
-                y = (int)__umulhi((unsigned)qi, qmagic); q = qi - y * nq;
-                // aligned word address of tile byte (row y+3, column 4q + xoff) = first of the 10 bytes c0-3 .. c0+6, c0 = 4q + 3 + xoff
-                const uint32_t* rc = reinterpret_cast<const uint32_t*>(tileBase + (y + 3) * tp + ((4 * q + xoff) & ~3));
-                const int tpw = tp >> 2;
-                // three 4-byte windows per row: bytes [c0-3, c0], [c0+1, c0+4], [c0+5, c0+8]
-#define ORBX_WIN3(r, A, B, C) { const uint32_t w0 = (r)[0], w1 = (r)[1], w2 = (r)[2], w3 = (r)[3]; \
-                                A = __funnelshift_r(w0, w1, shC); B = __funnelshift_r(w1, w2, shC); C = __funnelshift_r(w2, w3, shC); }
-                uint32_t A0, B0, C0, Au, Bu, Cu, Ad, Bd, Cd;
-                ORBX_WIN3(rc, A0, B0, C0);                         // centre row
-                ORBX_WIN3(rc + 2 * tpw, Au, Bu, Cu);               // row +2
-                ORBX_WIN3(rc - 2 * tpw, Ad, Bd, Cd);               // row -2
-                uint32_t t3a, t3b;                                 // rows +-3: bytes c0 .. c0+3 = window offset 3..6
-                { const uint32_t* r3 = rc + 3 * tpw; const uint32_t w0 = r3[0], w1 = r3[1], w2 = r3[2];
-                  t3a = __funnelshift_r(__funnelshift_r(w0, w1, shC), __funnelshift_r(w1, w2, shC), 24); }
-                { const uint32_t* r3 = rc - 3 * tpw; const uint32_t w0 = r3[0], w1 = r3[1], w2 = r3[2];
-                  t3b = __funnelshift_r(__funnelshift_r(w0, w1, shC), __funnelshift_r(w1, w2, shC), 24); }
-#undef ORBX_WIN3
-                // window byte offsets (relative to c0-3): centre = 3..6, p12 (x-3) = 0..3, p4 (x+3) = 6..9, x-2 = 1..4, x+2 = 5..8
-                const uint32_t ctr = __funnelshift_r(A0, B0, 24);                 // bytes c0 .. c0+3
-                const uint32_t p12 = A0;                                           // bytes c0-3 .. c0
-                const uint32_t p4 = __funnelshift_r(B0, C0, 16);                  // bytes c0+3 .. c0+6
-                const uint32_t p2 = __funnelshift_r(Bu, Cu, 8), p14 = __funnelshift_r(Au, Bu, 8);    // row +2: x+2 (5..8), x-2 (1..4)
-                const uint32_t p6 = __funnelshift_r(Bd, Cd, 8), p10 = __funnelshift_r(Ad, Bd, 8);    // row -2: x+2, x-2
-                const uint32_t p0 = t3a, p8 = t3b;
+        const int tpw = tp >> 2;
+        for (int base = 0; base < nI; base += FAST_NT) {
+            // consecutive lanes take consecutive quads of one run, so the lanes of a run read consecutive words of a tile row
+            const int it = base + tid;
+            uint32_t cand = 0;                       // bit 4k + i: pixel (y0 + k, 4q + i) survives
+            int y0 = 0, q = 0;
+            if (it < nI) {
+                const int j = (int)__umulhi((unsigned)it, qmagic);
+                q = it - j * nq; y0 = j * FAST_RUN;
+                // aligned word of tile byte (row 0, column 4q + xoff) = first of the 10 bytes c0-3 .. c0+6, c0 = 4q + 3 + xoff
+                const uint32_t* col = reinterpret_cast<const uint32_t*>(tileBase + ((4 * q + xoff) & ~3));
+                // window byte offsets (relative to c0-3) of tile row y0 + r: x..x+3 = 3..6, x-3 = 0..3, x+3 = 6..9, x-2 = 1..4, x+2 = 5..8
+                uint32_t M[FAST_RUN + 6], L0[FAST_RUN + 6], R6[FAST_RUN + 6], L1[FAST_RUN + 6], R5[FAST_RUN + 6];
 #define ORBX_LO(w) __byte_perm((w), 0u, 0x4140)   /* bytes 0,1 -> two 16-bit lanes */
 #define ORBX_HI(w) __byte_perm((w), 0u, 0x4342)   /* bytes 2,3 */
-                const uint32_t V01 = ORBX_LO(ctr), V23 = ORBX_HI(ctr);
-                const uint32_t NLO01 = __vsub2(TT, V01), NLO23 = __vsub2(TT, V23);                 // T - v
-                const uint32_t NHI01 = __vsub2(0u, __vadd2(V01, TT1)), NHI23 = __vsub2(0u, __vadd2(V23, TT1));   // -(v + T + 1)
-                uint32_t dk01 = 0xFFFFFFFFu, dk23 = 0xFFFFFFFFu, br01 = 0u, br23 = 0u;
+#pragma unroll
+                for (int r = 0; r < FAST_RUN + 6; ++r) {
+                    // the last run of a block may stop short: its rows past the window's last tile row (ih + 5) are clamped and
+                    // the pixels they feed are dropped below
+                    const uint32_t* rw = col + min(y0 + r, ih + 5) * tpw;
+                    const uint32_t w0 = rw[0], w1 = rw[1], w2 = rw[2];
+                    const uint32_t A = __funnelshift_r(w0, w1, shC), B = __funnelshift_r(w1, w2, shC);
+                    M[r] = __funnelshift_r(A, B, 24); L0[r] = A; L1[r] = __funnelshift_r(A, B, 8);
+                    if (r > 0 && r < FAST_RUN + 5) {     // the first and last rows only serve as ring rows +-3 (M)
+                        const uint32_t C = __funnelshift_r(w2, rw[3], shC);
+                        R6[r] = __funnelshift_r(B, C, 16); R5[r] = __funnelshift_r(B, C, 8);
+                    }
+                    if (r < 6) continue;
+                    // interior row y0 + k: centre = tile row k + 3, ring rows k + 1, k + 5 (x +- 2) and k, k + 6 (x)
+                    const int k = r - 6;
+                    const uint32_t p0 = M[k + 6], p8 = M[k], p4 = R6[k + 3], p12 = L0[k + 3];
+                    const uint32_t p2 = R5[k + 5], p14 = L1[k + 5], p6 = R5[k + 1], p10 = L1[k + 1];
+                    const uint32_t V01 = ORBX_LO(M[k + 3]), V23 = ORBX_HI(M[k + 3]);
+                    const uint32_t NLO01 = __vsub2(TT, V01), NLO23 = __vsub2(TT, V23);                 // T - v
+                    const uint32_t NHI01 = __vsub2(0u, __vadd2(V01, TT1)), NHI23 = __vsub2(0u, __vadd2(V23, TT1));   // -(v + T + 1)
+                    uint32_t dk01 = 0xFFFFFFFFu, dk23 = 0xFFFFFFFFu, br01 = 0u, br23 = 0u;
 #define ORBX_OPP(pa, pb) { \
                     const uint32_t a01 = ORBX_LO(pa), a23 = ORBX_HI(pa), b01 = ORBX_LO(pb), b23 = ORBX_HI(pb); \
                     dk01 &= __vadd2(a01, NLO01) | __vadd2(b01, NLO01); dk23 &= __vadd2(a23, NLO23) | __vadd2(b23, NLO23); \
                     br01 |= __vadd2(a01, NHI01) & __vadd2(b01, NHI01); br23 |= __vadd2(a23, NHI23) & __vadd2(b23, NHI23); }
-                ORBX_OPP(p0, p8); ORBX_OPP(p4, p12); ORBX_OPP(p2, p10); ORBX_OPP(p6, p14);
+                    ORBX_OPP(p0, p8); ORBX_OPP(p4, p12); ORBX_OPP(p2, p10); ORBX_OPP(p6, p14);
 #undef ORBX_OPP
+                    const uint32_t c01 = dk01 | ~br01, c23 = dk23 | ~br23;
+                    cand |= (((c01 >> 15) & 1u) | ((c01 >> 30) & 2u) | ((c23 >> 13) & 4u) | ((c23 >> 28) & 8u)) << (4 * k);
+                    // the score map needs no clearing pass: every quad writes 0 here and phase 2 overwrites its corners
+                    if (y0 + k < ih) *reinterpret_cast<uint32_t*>(score + (y0 + k + 1) * sp + 4 * q + 4) = 0u;
+                }
 #undef ORBX_LO
 #undef ORBX_HI
-                c01 = (dk01 | ~br01) & 0x80008000u;
-                c23 = (dk23 | ~br23) & 0x80008000u;
-                const int xr = iw - 4 * q;     // pixels of this quad inside the interior
-                if (xr < 4) { c23 = xr <= 2 ? 0u : (c23 & 0x8000u); if (xr < 2) c01 &= 0x8000u; }
-                // the score map needs no clearing pass: every quad writes 0 here and phase 2 overwrites its corners
-                *reinterpret_cast<uint32_t*>(score + (y + 1) * sp + 4 * q + 4) = 0u;
+                const int xr = iw - 4 * q, yr = ih - y0;     // pixels of this quad inside the interior, rows of this run inside it
+                if (xr < 4) cand &= ((1u << xr) - 1u) * 0x11111111u;
+                if (yr < FAST_RUN) cand &= (1u << (4 * yr)) - 1u;
             }
-            // compaction: up to four candidates per lane, in (y, x) packed form
-            const int n4 = ((c01 >> 15) & 1) + (c01 >> 31) + ((c23 >> 15) & 1) + (c23 >> 31);
-            int incl = n4;
+            // compaction: up to 4 * FAST_RUN candidates per lane, in (y, x) packed form
+            const int n = __popc(cand);
+            int incl = n;
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
             const int wtot = __shfl_sync(0xffffffffu, incl, 31);
@@ -283,12 +297,12 @@ __global__ void __launch_bounds__(FAST_NT) fast_cells_kernel(ExtractParams P, co
                 int wbase = 0;
                 if (lane == 31) wbase = atomicAdd(&s_nCand, wtot);
                 wbase = __shfl_sync(0xffffffffu, wbase, 31);
-                int o = wbase + incl - n4;
-                const int yx = (y << 8) | (4 * q);
-                if (c01 & 0x8000u) list[o++] = (uint16_t)yx;
-                if (c01 & 0x80000000u) list[o++] = (uint16_t)(yx + 1);
-                if (c23 & 0x8000u) list[o++] = (uint16_t)(yx + 2);
-                if (c23 & 0x80000000u) list[o++] = (uint16_t)(yx + 3);
+                int o = wbase + incl - n;
+                const int yx = (y0 << 8) | (4 * q);
+                for (uint32_t m = cand; m; m &= m - 1) {
+                    const int b = __ffs(m) - 1;
+                    list[o++] = (uint16_t)(yx + ((b >> 2) << 8) + (b & 3));
+                }
             }
         }
     }
@@ -372,11 +386,19 @@ __global__ void __launch_bounds__(FAST_NT) fast_cells_kernel(ExtractParams P, co
 
 
 // ------------------------------------------------------------------------------------------
-// K1 (TMA form): pyramid level l from level l-1 with the source rows of a 128 x 8 destination tile staged into shared memory by ONE
-// TMA bulk-tensor load (box pyrBoxW x pyrBoxH of level l-1, start aligned to 16 bytes); the fixed-point bilinear taps then read
+// K1 (TMA form): pyramid level l from level l-1 with the source rows of a 128 x PYR_TILE_H destination tile staged into shared memory by
+// ONE TMA bulk-tensor load (box pyrBoxW x pyrBoxH of level l-1, start aligned to 16 bytes); the fixed-point bilinear taps then read
 // shared memory instead of gathering bytes from global memory.  Same integer arithmetic as pyr_resize_kernel (cv::resize INTER_LINEAR).
+// A thread produces 4 columns of PYR_TILE_H / 8 consecutive rows, so one load feeds many output rows and the column taps are read once.
 // ------------------------------------------------------------------------------------------
-constexpr int PYR_TILE_W = 128, PYR_TILE_H = 8;
+// The 7 levels of 240 frames of 640x480 on an H100 80GB HBM3 at 700 W: 0.44 ms with 128 x 8 tiles; 0.38 / 0.34 / 0.33 ms with
+// tiles 16 / 32 / 64 rows tall and strided rows per warp; 0.29 / 0.26 ms at 32 / 64 rows with consecutive rows and the taps reuse.
+// At 64 rows a box is at most ~122 rows (256 bytes wide caps the scale below 2), so it stays under 32 KB of shared memory.
+constexpr int PYR_TILE_W = 128;
+#ifndef PYR_TILE_H
+#define PYR_TILE_H 64
+#endif
+static_assert(PYR_TILE_H % 8 == 0, "a CTA is 32 x 8 threads");
 __global__ void __launch_bounds__(256) pyr_resize_tma_kernel(ExtractParams P, int l, const __grid_constant__ CUtensorMap srcMap) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_bar;
@@ -392,28 +414,41 @@ __global__ void __launch_bounds__(256) pyr_resize_tma_kernel(ExtractParams P, in
         tma_load_3d(smem_raw, &srcMap, cx0, ry0, f, &s_bar);
     }
     __syncthreads();
-    mbar_wait(&s_bar, 0);
-    const int dy = dyT + threadIdx.y;
     const int dx0 = dxT + threadIdx.x * 4;
-    if (dy >= G.h || dx0 >= G.w) return;
-    const short4 yt = P.ytab[G.ytabOff + dy];  // {sy0, sy1, b0, b1}
-    const uint8_t* r0 = smem_raw + (yt.x - ry0) * G.pyrBoxW - cx0;
-    const uint8_t* r1 = smem_raw + (yt.y - ry0) * G.pyrBoxW - cx0;
-    const int b0 = yt.z, b1 = yt.w;
-    uint32_t out = 0;
+    if (dx0 >= G.w) return;
+    short4 xt[4];                                                          // {sx0, sx1, a0, a1}, shared by the thread's rows
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int dx = dx0 + k;
-        if (dx < G.w) {
-            const short4 xt = __ldg(&P.xtab[G.xtabOff + dx]);  // {sx0, sx1, a0, a1}
-            const int s0 = r0[xt.x] * xt.z + r0[xt.y] * xt.w;
-            const int s1 = r1[xt.x] * xt.z + r1[xt.y] * xt.w;
-            const int v = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
-            out |= (uint32_t)(v & 0xFF) << (8 * k);
+    for (int k = 0; k < 4; ++k) xt[k] = __ldg(&P.xtab[G.xtabOff + min(dx0 + k, G.w - 1)]);
+    mbar_wait(&s_bar, 0);
+    uint8_t* dst = P.pyr + (size_t)f * P.pyrFrameStride + G.planeOff + dx0;
+    // a warp owns PYR_TILE_H / 8 consecutive destination rows: where a row's upper source row is the previous row's lower one, its
+    // horizontal taps are taken over instead of gathered again (most rows when downscaling by less than 2)
+    int s0[4], s1[4], prevY1 = -1;
+#pragma unroll
+    for (int i = 0; i < PYR_TILE_H / 8; ++i) {
+        const int dy = dyT + threadIdx.y * (PYR_TILE_H / 8) + i;
+        if (dy >= G.h) break;
+        const short4 yt = P.ytab[G.ytabOff + dy];  // {sy0, sy1, b0, b1}
+        const uint8_t* r0 = smem_raw + (yt.x - ry0) * G.pyrBoxW - cx0;
+        const uint8_t* r1 = smem_raw + (yt.y - ry0) * G.pyrBoxW - cx0;
+        const bool reuse = yt.x == prevY1;
+        prevY1 = yt.y;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if (reuse) s0[k] = s1[k];
+            else s0[k] = r0[xt[k].x] * xt[k].z + r0[xt[k].y] * xt[k].w;
+            s1[k] = r1[xt[k].x] * xt[k].z + r1[xt[k].y] * xt[k].w;
         }
+        const int b0 = yt.z, b1 = yt.w;
+        uint32_t out = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (dx0 + k < G.w) {
+                const int v = (((b0 * (s0[k] >> 4)) >> 16) + ((b1 * (s1[k] >> 4)) >> 16) + 2) >> 2;
+                out |= (uint32_t)(v & 0xFF) << (8 * k);
+            }
+        *reinterpret_cast<uint32_t*>(dst + (size_t)dy * G.pitch) = out;   // pitch is a multiple of 32: in-bounds even for the tail
     }
-    uint8_t* dst = P.pyr + (size_t)f * P.pyrFrameStride + G.planeOff + (size_t)dy * G.pitch;
-    *reinterpret_cast<uint32_t*>(dst + dx0) = out;   // pitch is a multiple of 32: in-bounds even for the tail
 }
 
 // ------------------------------------------------------------------------------------------

@@ -26,7 +26,7 @@ struct LevelGeom {
     uint32_t xtabOff, ytabOff;        // resize coefficient tables (entries, not bytes)
     int blurTileBase, blurTilesX, blurTilesY;   // flattened tile index range of the blur launch
     int fastBoxW, fastBoxH;   // TMA box of the FAST cell ROI: width (multiple of 16 bytes) x height
-    int pyrBoxW, pyrBoxH;     // TMA box (in level l-1) that covers the sources of one 128 x 8 destination tile of this level
+    int pyrBoxW, pyrBoxH;     // TMA box (in level l-1) that covers the sources of one PYR_TILE_W x PYR_TILE_H destination tile of this level
 };
 
 // One active FAST cell (cells skipped by the reference's `continue`s are not listed).
