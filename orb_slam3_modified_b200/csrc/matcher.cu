@@ -326,7 +326,21 @@ __device__ void build_frame_smem(const FrameSmem& S, const OrbKeyPoint* kps, con
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
+// Phase stamps of match_frame_kernel (build with -DMF_PHASES, read by tools/match_phases.py through orbm_match_phases): thread 0 of
+// every CTA adds the clock64() spans between the kernel's barriers.  [0] grid build, [1] pass 1 (to the cluster barrier), both summed
+// over all CTAs; [2] pass 2, [3] outcome / histogram, summed over the CTAs 0; [4] pass-2 sweeps, [5] map points queued for a rescan,
+// [6] CTAs, [7] frames.
+#ifdef MF_PHASES
+__device__ unsigned long long mf_phase[8];
+#define MF_STAMP(t) long long t = 0; if (tid == 0) t = clock64()
+#define MF_ADD(k, v) if (tid == 0) atomicAdd(&mf_phase[k], (unsigned long long)(v))
+#else
+#define MF_STAMP(t)
+#define MF_ADD(k, v)
+#endif
+
+// 64 registers: two 512-thread CTAs per SM when the frame's shared memory allows it (frame_smem_bytes <= 100 KB).
+__global__ void __launch_bounds__(MF_NT, 2) match_frame_kernel(MatchParams P) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     __shared__ int s_warp[33];
     __shared__ int s_changed, s_nq, s_nAcc, s_nRemoved, s_ind[3];
@@ -334,6 +348,7 @@ __global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
     const int C = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
     const int f = blockIdx.x / C, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (P.active && !P.active[f]) return;          // the whole cluster of an inactive stream leaves before its first cluster barrier
+    MF_STAMP(t0);
     const int K = min(P.nK[f], P.kcap), M = min(P.nM[f], P.mcap);
     const FrameSmem S = carve_frame_smem(smem_raw, P.ks, P.ms, P.descInSmem != 0);
     const OrbKeyPoint* kps = P.kps + (size_t)f * P.kcap;
@@ -349,29 +364,48 @@ __global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
             if (match[i] >= 0 && claimed[i]) atomicOr(&S.initBits[i >> 5], 1u << (i & 31));
         __syncthreads();
     }
+    MF_STAMP(t1);
 
     // ---- pass 1: this CTA's share of the map points, warp per map point ----
+    // The warp's map points are i = first + j * stride.  They are taken 32 at a time: lane j makes the query of the j-th point and
+    // prefetches its descriptor into L1, so the dependent loads of make_query (valid, then pose / position / octave) are in flight
+    // for 32 points at once; the warp then scans the points in order with the query broadcast from lane j.  Holding the descriptors
+    // in registers instead measured no faster and spills at the 64-register bound.
     auto notInit = [&](int idx) { return !((S.initBits[idx >> 5] >> (idx & 31)) & 1u); };
-    for (int i = rank * (MF_NT / 32) + wid; i < M; i += C * (MF_NT / 32)) {
-        const size_t o = (size_t)f * P.mcap + i;
-        float u = 0, v = 0, r = 0; int minL = 0, maxL = 0;
-        const bool ok = make_query(P, f, i, u, v, r, minL, maxL);
-        int4 ri = make_int4(-1, -1, -1, -1), rd = make_int4(256, 256, 256, 256);
-        if (ok) {
-            uint32_t mpd[8];
-            load_mp_desc(P, f, i, mpd);
-            const TopK<4> t = scan_candidates<4>(P, S, f, u, v, r, minL, maxL, mpd, notInit);
-            ri = make_int4(t.i[0], t.i[1], t.i[2], t.i[3]);
-            rd = make_int4(t.i[0] >= 0 ? (int)(t.k[0] >> 40) : 256, t.i[1] >= 0 ? (int)(t.k[1] >> 40) : 256,
-                           t.i[2] >= 0 ? (int)(t.k[2] >> 40) : 256, t.i[3] >= 0 ? (int)(t.k[3] >> 40) : 256);
+    const int stride = C * (MF_NT / 32);
+    for (int first = rank * (MF_NT / 32) + wid; first < M; first += 32 * stride) {
+        const int il = first + lane * stride;
+        float qu = 0, qv = 0, qr = 0; int minL = 0, maxL = 0;
+        bool qok = false;
+        if (il < M) {
+            const size_t o = (size_t)f * P.mcap + il;
+            qok = make_query(P, f, il, qu, qv, qr, minL, maxL);
+            if (qok) asm volatile("prefetch.global.L1 [%0];" :: "l"(P.mpDesc + o * 32));
+            P.query[o] = make_float4(qu, qv, qr, __int_as_float((minL + 1) | ((maxL + 1) << 8) | ((qok ? 1 : 0) << 16)));
         }
-        if (lane == 0) {
-            P.resultIdx[o] = ri; P.resultDist[o] = rd;
-            P.query[o] = make_float4(u, v, r, __int_as_float((minL + 1) | ((maxL + 1) << 8) | ((ok ? 1 : 0) << 16)));
+        const unsigned okMask = __ballot_sync(0xffffffffu, qok);
+        const int levels = (minL + 1) | ((maxL + 1) << 8);
+        const int n = min(32, (M - first + stride - 1) / stride);
+        for (int j = 0; j < n; ++j) {
+            const size_t o = (size_t)f * P.mcap + first + j * stride;
+            int4 ri = make_int4(-1, -1, -1, -1), rd = make_int4(256, 256, 256, 256);
+            if ((okMask >> j) & 1u) {
+                const float u = __shfl_sync(0xffffffffu, qu, j), v = __shfl_sync(0xffffffffu, qv, j), r = __shfl_sync(0xffffffffu, qr, j);
+                const int lv = __shfl_sync(0xffffffffu, levels, j);
+                uint32_t mpd[8];
+                load_mp_desc(P, f, first + j * stride, mpd);
+                const TopK<4> t = scan_candidates<4>(P, S, f, u, v, r, (lv & 0xff) - 1, (lv >> 8) - 1, mpd, notInit);
+                ri = make_int4(t.i[0], t.i[1], t.i[2], t.i[3]);
+                rd = make_int4(t.i[0] >= 0 ? (int)(t.k[0] >> 40) : 256, t.i[1] >= 0 ? (int)(t.k[1] >> 40) : 256,
+                               t.i[2] >= 0 ? (int)(t.k[2] >> 40) : 256, t.i[3] >= 0 ? (int)(t.k[3] >> 40) : 256);
+            }
+            if (lane == 0) { P.resultIdx[o] = ri; P.resultDist[o] = rd; }
         }
     }
     if (C > 1) { __threadfence(); cluster.sync(); }     // the lists of all CTAs are visible to CTA 0
     else __syncthreads();
+    MF_STAMP(t2);
+    MF_ADD(0, t1 - t0); MF_ADD(1, t2 - t1); MF_ADD(6, 1);
     if (rank != 0) return;
 
     // ---- pass 2 (CTA 0): fixed-point resolution of the sequential claim rule ----
@@ -420,6 +454,7 @@ __global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
         __syncthreads();
         // B. warp per queued map point: exact rescan against the current claims
         const int nq = s_nq;
+        MF_ADD(4, 1); MF_ADD(5, nq);
         for (int q = wid; q < nq; q += MF_NT / 32) {
             const int i = S.queue[q];
             const float4 qq = P.query[(size_t)f * P.mcap + i];
@@ -445,6 +480,8 @@ __global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
         }
         __syncthreads();
     }
+    MF_STAMP(t3);
+    MF_ADD(2, t3 - t2); MF_ADD(7, 1);
 
     // ---- outcome: nmatches++ per accepted map point (:1762-1776), rotation histogram, ComputeThreeMaxima (:2012-2053) ----
     const bool hist = P.mode == 1 && P.checkOri;
@@ -502,6 +539,8 @@ __global__ void __launch_bounds__(MF_NT) match_frame_kernel(MatchParams P) {
     }
     if (reset) for (int c = K + tid; c < P.kcap; c += MF_NT) { match[c] = -1; claimed[c] = 0; }
     if (tid == 0) P.nmatches[f] = s_nAcc - s_nRemoved;
+    MF_STAMP(t4);
+    MF_ADD(3, t4 - t3);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1342,20 +1381,36 @@ struct Matcher {
         if (sm > limit) { set_error("frame too large for the matcher's shared-memory grid (keypoints + map points)"); return ORB_ERR_CAPACITY; }
         int rc = ensure_dynamic_smem(match_frame_kernel, sm, device);
         if (rc) return rc;
-        // cluster size: as many CTAs per frame as keeps the whole call resident at once (pass 1 is spread over the cluster)
-        int C = 1;
-        while (C < 8 && (long)P.batch * (C * 2) <= (long)numSMs * (sm > 100 * 1024 ? 1 : 2)) C *= 2;
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)(P.batch * C)); cfg.blockDim = dim3(MF_NT); cfg.dynamicSmemBytes = sm; cfg.stream = st;
+        cfg.blockDim = dim3(MF_NT); cfg.dynamicSmemBytes = sm; cfg.stream = st;
         cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
+        // cluster size: the largest (up to 8) for which every frame's cluster is resident at once (pass 1 is spread over the
+        // cluster; a second wave would double the call's time).  Asked from the occupancy calculator, which counts registers, shared
+        // memory and the GPCs clusters cannot straddle; the answer depends only on (batch, shared memory), so it is kept.
+        if (P.batch != occBatch || sm != occSmem) {
+            occC = 1;
+            for (int cand = 8; cand > 1; --cand) {
+                if ((long)P.batch * cand > 2L * numSMs) continue;
+                at[0].val.clusterDim.x = cand;
+                cfg.gridDim = dim3((unsigned)(P.batch * cand));
+                int nClusters = 0;
+                if (cudaOccupancyMaxActiveClusters(&nClusters, match_frame_kernel, &cfg) == cudaSuccess && nClusters >= P.batch) { occC = cand; break; }
+            }
+            (void)cudaGetLastError();
+            occBatch = P.batch; occSmem = sm;
+        }
+        const int C = occC;
+        at[0].val.clusterDim.x = C;
+        cfg.gridDim = dim3((unsigned)(P.batch * C));
         CK(cudaLaunchKernelEx(&cfg, match_frame_kernel, P));
         launches = 1;
         lastCluster = C;
         return ORB_OK;
     }
     int lastCluster = 1;
+    int occBatch = -1, occC = 1; size_t occSmem = 0;   // run's cluster size for the last (batch, shared memory) it was asked for
 
     // The batched tracking calls' scratch, sized for max_batch x max_keypoints / max_mappoints: PoseOptimization's gathered edges
     // ([B][kcap]), the frustum stage's per-point fields and flags ([B][mcap]) and the motion-model step's nInliers ([B]).  The
@@ -1593,6 +1648,18 @@ int orbm_create(orbm_handle** out, int max_batch, int max_keypoints, int max_map
 
 void orbm_destroy(orbm_handle* h) { delete h; }
 int orbm_last_launch_count(const orbm_handle* h) { return h ? h->m.launches : ORB_ERR_ARG; }
+#ifdef MF_PHASES
+// out[8]: match_frame_kernel's phase counters (mf_phase) since the last call, which zeroes them; returns the last call's cluster size.
+int orbm_match_phases(const orbm_handle* h, unsigned long long* out) {
+    if (!h || !out) return ORB_ERR_ARG;
+    CK(cudaSetDevice(h->m.device));
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpyFromSymbol(out, orbm::mf_phase, sizeof(orbm::mf_phase)));
+    const unsigned long long zero[8] = {};
+    CK(cudaMemcpyToSymbol(orbm::mf_phase, zero, sizeof(zero)));
+    return h->m.lastCluster;
+}
+#endif
 
 static bool frame_ok(const Matcher& m, const OrbmFrame* fr) {
     if (!fr || fr->K < 0 || fr->K > m.kcap || !fr->scaleFactors || fr->nlevels < 1 || !(fr->maxX > fr->minX) || !(fr->maxY > fr->minY)) {
