@@ -65,15 +65,20 @@ struct Dev {
     Job* job;
     double* pcm;                      // nP x PC: the pose cache of the open phase, for helper CTAs
     double *poses, *posesB, *pts, *ptsB;        // nP x 7, nL x 3: estimate / second buffer (trial state; the two swap when a step is accepted)
+    double* outPts;                             // nL x 3: the final point estimates in the caller's point order
     const double *initPoses, *initPts;          // the uploaded initial estimates (a run always restarts from them)
     // the caller's graph as uploaded (caller's edge order); lba_build_structure_kernel derives everything below from it
     const int *rawEdgePoint, *rawEdgePose; const double* rawObs; const float* rawInvSigma2;
     int *bCnt, *bCursor, *bTmp, *bEid, *bTaskLen, *bItemStart;   // build scratch: nL + 1, nL + 1, nE, nF x nL, nTasks, nTasks
+    unsigned long long* bKey;         // build scratch: the point sort's keys, nL rounded up to a power of two
     int pairCap, chunkCap;
     const float* cam;                 // nP x 4
     const int* hidx;                  // nP: Hessian block index or -1
     const int* freePose;              // nF: pose index of Hessian block
-    // edges in INTERNAL order = sorted by point (the edges of a point are contiguous)
+    // INTERNAL point order: every per-point array of the LM kernel (pts / ptsB, Hll, bl, PT) and every point index below is a
+    // rank in it; lba_build_structure_kernel sorts the points by their observing free poses (see there)
+    const int* ptOrig;                // nL: caller's index of the point at internal rank r
+    // edges in INTERNAL order = sorted by point rank (the edges of a point are contiguous)
     const int *ePt, *ePose;           // nE
     const int* eH;                    // nE: Hessian block of the edge's pose (hidx[ePose]) or -1
     const int* eOrig;                 // nE: caller's edge index
@@ -939,8 +944,11 @@ __device__ void phase_finalize(const Dev& D, const Ctx& c, const double* pts) {
         double r[3]; qrot(P, pts + 3 * (size_t)D.ePt[e], r);
         D.outDepthPos[o] = r[2] + P[6] > 0.0;
     }
-    // the estimate ends in whichever buffer was current last; the caller reads D.poses / D.pts
-    if (pts != D.pts) for (int i = c.wid(); i < 3 * D.nL; i += nw) D.pts[i] = pts[i];
+    // the estimate ends in whichever buffer was current last; the caller reads D.poses and D.outPts, in its own point order
+    for (int i = c.wid(); i < 3 * D.nL; i += nw) {
+        const int r = i / 3;
+        D.outPts[3 * (size_t)D.ptOrig[r] + (i - 3 * r)] = pts[i];
+    }
 }
 
 // =============================================================================================
@@ -1112,7 +1120,10 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
         for (int k = 0; k < 7; ++k) T[k] = D.initPoses[7 * (size_t)i + k];
         qnormalize(T);                                              // SE3Quat(q, t) constructor
     }
-    for (int i = c.wid(); i < 3 * D.nL; i += nw) D.pts[i] = D.initPts[i];
+    for (int i = c.wid(); i < 3 * D.nL; i += nw) {
+        const int r = i / 3;
+        D.pts[i] = D.initPts[3 * (size_t)D.ptOrig[r] + (i - 3 * r)];
+    }
     for (int i = c.wid(); i < 2 * D.nE; i += nw) D.err[i] = 0.0;
     for (int i = c.wid(); i < D.n; i += nw) D.x[i] = 0.0;
     int flag;
@@ -1219,10 +1230,15 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
 
 // =============================================================================================
 // BlockSolver::buildStructure (block_solver.hpp:143-295) on the device: one CTA per problem turns the caller's edge list
-// into the index structures of the LM kernel -- edges sorted by point (stable), the (free pose, point) -> edge table, the
-// per-pose edge lists (the pose-major edge order), the pair list of every off-diagonal Schur block in pose-major indices, and
-// the chunked work list.  Only the raw graph (28 B per edge) crosses PCIe; the derived lists (~2.3 MB per 40k-edge problem) never exist on the host.
-// Every list is in a deterministic order (by point, ties by the caller's edge index).
+// into the index structures of the LM kernel -- the internal point order, edges sorted by point (stable), the (free pose, point)
+// -> edge table, the per-pose edge lists (the pose-major edge order), the pair list of every off-diagonal Schur block in
+// pose-major indices, and the chunked work list.  Only the raw graph (28 B per edge) crosses PCIe; the derived lists (~2.3 MB per
+// 40k-edge problem) never exist on the host.
+// The internal point order sorts the points by the ascending list of their observing free poses (the first four, points seen
+// only by fixed poses last), ties by the caller's index.  Points with the same observers are then neighbours, so the points a
+// pose pair shares form a few long runs, and the lanes of a Schur chunk read neighbouring point records and pose-major entries
+// instead of lines scattered over the caller's order.  Every list is in a deterministic order (by point rank, ties by the
+// caller's edge index).
 // status: 0 ok, 1 edge index out of range, 2 duplicate (point, keyframe) observation, 3 pair list larger than sized.
 // =============================================================================================
 constexpr int BT = 1024;
@@ -1245,6 +1261,34 @@ __device__ __forceinline__ int bt_excl_scan(int v, int* sm, int& total) {   // e
     __syncthreads();
     return base + inc - v;
 }
+// Ascending bitonic sort of key[n2] (global memory, n2 a power of two), all threads of the CTA.  The stages whose stride is below
+// the tile of 2 BT keys run on that tile in shared memory, so only strides of 2 BT and more cost a pass over global memory.
+constexpr int SORT_TILE = 2 * BT;
+__device__ __forceinline__ void bitonic_pair(unsigned long long* k, int base, int k2, int j, int pr) {   // pair pr of stage k2, stride j
+    const int lo = 2 * pr - (pr & (j - 1)), hi = lo + j;
+    const unsigned long long a = k[lo], b = k[hi];
+    if ((a > b) == (((base + lo) & k2) == 0)) { k[lo] = b; k[hi] = a; }
+}
+__device__ void bitonic_sort_keys(unsigned long long* key, int n2, unsigned long long* tile) {
+    const int T = min(n2, SORT_TILE), tid = threadIdx.x;
+    for (int k2 = T; k2 <= n2; k2 <<= 1) {
+        for (int j = k2 >> 1; j >= T; j >>= 1) {
+            for (int pr = tid; pr < n2 / 2; pr += BT) bitonic_pair(key, 0, k2, j, pr);
+            __syncthreads();
+        }
+        for (int t0 = 0; t0 < n2; t0 += T) {
+            for (int i = tid; i < T; i += BT) tile[i] = key[t0 + i];
+            __syncthreads();
+            for (int s2 = k2 == T ? 2 : k2; s2 <= k2; s2 <<= 1)      // the first round sorts every tile whole
+                for (int j = min(s2, T) >> 1; j > 0; j >>= 1) {
+                    if (tid < T / 2) bitonic_pair(tile, t0, s2, j, tid);
+                    __syncthreads();
+                }
+            for (int i = tid; i < T; i += BT) key[t0 + i] = tile[i];
+            __syncthreads();
+        }
+    }
+}
 __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int* status) {
     Dev& D = probs[blockIdx.x];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1252,7 +1296,8 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     const int nOff = nF * (nF - 1) / 2, nTasks = nF + nOff;
     __shared__ int s_sm[32];
     __shared__ int s_err;
-    int* ptStart = const_cast<int*>(D.ptStart);
+    __shared__ unsigned long long s_tile[SORT_TILE];
+    int* ptStart = const_cast<int*>(D.ptStart); int* ptOrig = const_cast<int*>(D.ptOrig);
     int* ePt = const_cast<int*>(D.ePt); int* ePose = const_cast<int*>(D.ePose); int* eH = const_cast<int*>(D.eH); int* eOrig = const_cast<int*>(D.eOrig);
     double* obs = const_cast<double*>(D.obs); float* is2 = const_cast<float*>(D.invSigma2);
     int* poseEdges = const_cast<int*>(D.poseEdges); int* poseEdgePt = const_cast<int*>(D.poseEdgePt);
@@ -1262,7 +1307,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     for (int i = tid; i <= nL; i += BT) D.bCnt[i] = 0;
     for (size_t i = tid; i < (size_t)nF * nL; i += BT) D.bEid[i] = -1;
     __syncthreads();
-    // 1. edges per point
+    // 1. edges per point (bCnt, by the caller's point index p)
     for (int e = tid; e < nE; e += BT) {
         const int p = D.rawEdgePoint[e], c = D.rawEdgePose[e];
         if (p < 0 || p >= nL || c < 0 || c >= nP) s_err = 1;
@@ -1270,7 +1315,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     }
     __syncthreads();
     if (s_err) { if (tid == 0) status[blockIdx.x] = s_err; return; }
-    // 2. ptStart = exclusive scan
+    // 2. where every point's edges start in the caller's point order (exclusive scan, into the cursors of step 3)
     {
         int carry = 0;
         for (int b0 = 0; b0 < nL; b0 += BT) {
@@ -1278,38 +1323,81 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
             const int v = i < nL ? D.bCnt[i] : 0;
             int total;
             const int ex = bt_excl_scan(v, s_sm, total);
-            if (i < nL) { ptStart[i] = carry + ex; D.bCursor[i] = carry + ex; }
+            if (i < nL) D.bCursor[i] = carry + ex;
+            carry += total;
+        }
+    }
+    __syncthreads();
+    // 3. group by point (arbitrary order), then order every point's slice by the caller's edge index; afterwards bCursor[p] is the
+    //    end of point p's slice of bTmp.  The point's sort key: its four lowest observing free poses (Hessian blocks) in
+    //    ascending order, in `sb` bits each, then the caller's index in `ib` bits, so that every key is distinct (the order is
+    //    that of 16-bit pose fields with ties broken by the caller's index whenever nF < 2^sb - 1, i.e. for every problem whose
+    //    pose caches fit in shared memory; beyond that the poses share the top field value, which still leaves a valid order).
+    //    A missing observer is the all-ones field value: fewer free observers sort after more, fixed-only points last.
+    for (int e = tid; e < nE; e += BT) D.bTmp[atomicAdd(&D.bCursor[D.rawEdgePoint[e]], 1)] = e;
+    __syncthreads();
+    const int n2 = nL > 1 ? 1 << (32 - __clz(nL - 1)) : 1;
+    {
+        const int ib = 32 - __clz(nL), sb = (64 - ib) / 4;        // 2^ib > nL: no real key is all ones, the padding's value
+        const unsigned none = (1u << sb) - 1;
+        for (int p = tid; p < n2; p += BT) {
+            unsigned long long key = ~0ull;
+            if (p < nL) {
+                const int b = D.bCursor[p], a = b - D.bCnt[p];
+                for (int i = a + 1; i < b; ++i) {
+                    const int v = D.bTmp[i];
+                    int j = i - 1;
+                    while (j >= a && D.bTmp[j] > v) { D.bTmp[j + 1] = D.bTmp[j]; --j; }
+                    D.bTmp[j + 1] = v;
+                }
+                unsigned s[4] = {none, none, none, none};
+                for (int i = a; i < b; ++i) {
+                    const int h = D.hidx[D.rawEdgePose[D.bTmp[i]]];
+                    unsigned v = h < 0 ? none : min((unsigned)h, none - 1);
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) { const unsigned lo = min(s[q], v); v = max(s[q], v); s[q] = lo; }
+                }
+                key = (unsigned long long)p;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) key |= (unsigned long long)s[q] << (ib + (3 - q) * sb);
+            }
+            D.bKey[p] = key;
+        }
+    }
+    __syncthreads();
+    if (nL > 0) bitonic_sort_keys(D.bKey, n2, s_tile);
+    for (int r = tid; r < nL; r += BT) ptOrig[r] = (int)(D.bKey[r] & ((1ull << (32 - __clz(nL))) - 1));
+    __syncthreads();
+    // 4. ptStart over the internal order, then every point's edges in their slots: internal edge id = ptStart[rank] + position in
+    //    the point's caller-ordered slice (a stable sort of the edges by point rank)
+    {
+        int carry = 0;
+        for (int b0 = 0; b0 < nL; b0 += BT) {
+            const int r = b0 + tid;
+            const int v = r < nL ? D.bCnt[ptOrig[r]] : 0;
+            int total;
+            const int ex = bt_excl_scan(v, s_sm, total);
+            if (r < nL) ptStart[r] = carry + ex;
             carry += total;
         }
         if (tid == 0) ptStart[nL] = carry;
     }
     __syncthreads();
-    // 3. group by point (arbitrary order), then order every point's slice by the caller's edge index (stable sort by point)
-    for (int e = tid; e < nE; e += BT) D.bTmp[atomicAdd(&D.bCursor[D.rawEdgePoint[e]], 1)] = e;
-    __syncthreads();
-    for (int p = tid; p < nL; p += BT) {
-        const int a = ptStart[p], b = ptStart[p + 1];
-        for (int i = a + 1; i < b; ++i) {
-            const int v = D.bTmp[i];
-            int j = i - 1;
-            while (j >= a && D.bTmp[j] > v) { D.bTmp[j + 1] = D.bTmp[j]; --j; }
-            D.bTmp[j + 1] = v;
-        }
-    }
-    __syncthreads();
-    for (int p = tid; p < nL; p += BT)
-        for (int k = ptStart[p]; k < ptStart[p + 1]; ++k) {
-            const int e = D.bTmp[k], c = D.rawEdgePose[e];
-            ePt[k] = p; ePose[k] = c; eOrig[k] = e;
+    for (int r = tid; r < nL; r += BT) {
+        const int p = ptOrig[r], n = D.bCnt[p], a = D.bCursor[p] - n, k0 = ptStart[r];
+        for (int i = 0; i < n; ++i) {
+            const int e = D.bTmp[a + i], c = D.rawEdgePose[e], k = k0 + i;
+            ePt[k] = r; ePose[k] = c; eOrig[k] = e;
             obs[2 * (size_t)k] = D.rawObs[2 * (size_t)e]; obs[2 * (size_t)k + 1] = D.rawObs[2 * (size_t)e + 1];
             is2[k] = D.rawInvSigma2[e];
             const int h = D.hidx[c];
             eH[k] = h;
-            if (h >= 0 && atomicCAS(&D.bEid[(size_t)h * nL + p], -1, k) != -1) s_err = 2;
+            if (h >= 0 && atomicCAS(&D.bEid[(size_t)h * nL + r], -1, k) != -1) s_err = 2;
         }
+    }
     __syncthreads();
     if (s_err) { if (tid == 0) status[blockIdx.x] = s_err; return; }
-    // 4. items per task: edges of a free pose / points shared by a pair of free poses; warp per task, ballot over points
+    // 5. items per task: edges of a free pose / points shared by a pair of free poses; warp per task, ballot over points
     auto taskRows = [&](int t, const int*& r1, const int*& r2) {
         if (t < nF) { r1 = D.bEid + (size_t)t * nL; r2 = r1; return; }
         int i1 = 0, rem = t - nF;
@@ -1329,7 +1417,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
         if (lane == 0) D.bTaskLen[t] = cnt;
     }
     __syncthreads();
-    // 5. where every task's items and chunks start (pose lists and pair lists are separate arrays)
+    // 6. where every task's items and chunks start (pose lists and pair lists are separate arrays)
     int nChunks = 0;
     {
         int carry = 0, tot;
@@ -1360,8 +1448,8 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     }
     __syncthreads();
     if (s_err) { if (tid == 0) status[blockIdx.x] = s_err; return; }
-    // 6. the lists themselves (ascending point = ascending internal edge id) and the chunk headers; the pose lists first: the
-    //    position of an edge in them is its pose-major index (kept in bTmp, free since step 3), and the pair lists hold those
+    // 7. the lists themselves (ascending point rank = ascending internal edge id) and the chunk headers; the pose lists first: the
+    //    position of an edge in them is its pose-major index (kept in bTmp, free since step 4), and the pair lists hold those
     for (int pass = 0; pass < 2; ++pass) {
         for (int t = (pass ? nF : 0) + warp; t < (pass ? nTasks : nF); t += BT / 32) {
             const int *r1, *r2;
@@ -1461,16 +1549,18 @@ struct Solver {
     static size_t outBlock(size_t nP, size_t nL, size_t nE) { return al(56 * nP) + al(24 * nL) + al(8 * nE) + al(nE) + al(512); }
     static size_t pairCapOf(size_t nP, size_t nE) { return nE * (nP > 1 ? nP - 1 : 1) / 2 + 1; }
     static size_t chunkCapOf(size_t nP, size_t nE) { return nP + nP * nP / 2 + 2 + (nE + pairCapOf(nP, nE)) / SCH + 1; }
+    static size_t pow2Of(size_t n) { size_t p = 1; while (p < n) p <<= 1; return p; }
     static size_t need(size_t nP, size_t nL, size_t nE) {
         const size_t n = 6 * nP, pc = pairCapOf(nP, nE), cc = chunkCapOf(nP, nE), tasks = nP + nP * nP / 2 + 2;
         size_t b = outBlock(nP, nL, nE);                                          // poses, pts, chi2, depth flags, stats (downloaded in one copy)
         b += al(56 * nP) + al(24 * nL) + al(16 * nP) + 2 * al(4 * nP);            // uploaded: initial estimates, cam, hidx, freePose
         b += 2 * al(4 * nE) + al(16 * nE) + al(4 * nE);                           // uploaded: the caller's edges (point, pose, obs, invSigma2)
+        b += al(4 * nL);                                                          // internal point order
         b += 4 * al(4 * nE) + al(16 * nE) + al(4 * nE) + al(4 * (nL + 1));        // edges sorted by point: ePt, ePose, eH, eOrig, obs, invSigma2; ptStart
         b += 2 * al(4 * nE) + al(8 * pc) + al(4 * pc);                            // poseEdges, poseEdgePt, pairs, pairPt
         b += al(16 * cc) + al(4 * (tasks + 1));                                   // chunk headers, task chunk starts
-        b += 2 * al(4 * (nL + 1)) + al(4 * nE) + al(4 * nP * nL) + 2 * al(4 * tasks);   // structure-build scratch
-        b += al(56 * nP) + al(24 * nL);                                           // second state buffers
+        b += 2 * al(4 * (nL + 1)) + al(4 * nE) + al(4 * nP * nL) + 2 * al(4 * tasks) + al(8 * pow2Of(nL));   // structure-build scratch
+        b += al(24 * nL) + al(56 * nP) + al(24 * nL);                             // point state, second state buffers
         b += al(16 * nE) + 3 * al(32 * nE);                                       // err, edge factors x 2, pose-major copy
         b += al(288 * nP) + al(48 * nP) + al(48 * nL) + al(72 * nL) + al(24 * nL);   // Hpp, bp, Hll, PT, bl
         b += al(8 * 42 * cc) + al(8 * 28 * (nP + nE / SCH + 1));                  // Spart, Ppart
@@ -1524,7 +1614,7 @@ struct Solver {
         D.nP = nP; D.nL = nL; D.nE = nE; D.nF = nF; D.n = n; D.pairCap = (int)pc; D.chunkCap = (int)cc;
         // --- output block: fixed layout (sized by the handle's maxima) so that one strided copy downloads every problem ---
         K.posesOff = carve(56 * (size_t)maxP); D.poses = (double*)(d_arena + K.posesOff);
-        K.ptsOff = carve(24 * (size_t)maxL); D.pts = (double*)(d_arena + K.ptsOff);
+        K.ptsOff = carve(24 * (size_t)maxL); D.outPts = (double*)(d_arena + K.ptsOff);
         K.chi2Off = carve(8 * (size_t)maxE); D.outChi2 = (double*)(d_arena + K.chi2Off);
         K.dposOff = carve((size_t)maxE); D.outDepthPos = (uint8_t*)(d_arena + K.dposOff);
         K.statsOff = carve(512); D.stats = (double*)(d_arena + K.statsOff);
@@ -1541,6 +1631,7 @@ struct Solver {
         U.isg = carve(4 * (size_t)nE); D.rawInvSigma2 = (const float*)(d_arena + U.isg);
         uploadOff[slot] = upBase; uploadBytes[slot] = off - upBase;
         // --- derived on the device ---
+        D.ptOrig = (const int*)(d_arena + carve(4 * (size_t)nL));
         D.ePt = (const int*)(d_arena + carve(4 * (size_t)nE)); D.ePose = (const int*)(d_arena + carve(4 * (size_t)nE));
         D.eH = (const int*)(d_arena + carve(4 * (size_t)nE)); D.eOrig = (const int*)(d_arena + carve(4 * (size_t)nE));
         D.obs = (const double*)(d_arena + carve(16 * (size_t)nE)); D.invSigma2 = (const float*)(d_arena + carve(4 * (size_t)nE));
@@ -1551,7 +1642,9 @@ struct Solver {
         D.bCnt = (int*)(d_arena + carve(4 * (size_t)(nL + 1))); D.bCursor = (int*)(d_arena + carve(4 * (size_t)(nL + 1)));
         D.bTmp = (int*)(d_arena + carve(4 * (size_t)nE)); D.bEid = (int*)(d_arena + carve(4 * (size_t)std::max(nF, 1) * (size_t)std::max(nL, 1)));
         D.bTaskLen = (int*)(d_arena + carve(4 * (size_t)std::max(nTasks, 1))); D.bItemStart = (int*)(d_arena + carve(4 * (size_t)std::max(nTasks, 1)));
+        D.bKey = (unsigned long long*)(d_arena + carve(8 * pow2Of(nL)));
         // --- state / scratch of the LM kernel ---
+        D.pts = (double*)(d_arena + carve(24 * (size_t)nL));
         D.posesB = (double*)(d_arena + carve(56 * (size_t)nP));
         D.ptsB = (double*)(d_arena + carve(24 * (size_t)nL));
         D.err = (double*)(d_arena + carve(16 * (size_t)nE));
@@ -1855,7 +1948,7 @@ int solver_load_device(lba_handle* h, int count, const int4* sizes, const double
     if (int rc = S.load_device(count, sizes, userLambdaInit, dFill)) return rc;
     for (int i = 0; i < count; ++i) {
         const Dev& D = S.h_probs[i];
-        out[i] = SlotOut{D.poses, D.pts, D.outChi2, D.outDepthPos, D.stats};
+        out[i] = SlotOut{D.poses, D.outPts, D.outChi2, D.outDepthPos, D.stats};
     }
     return ORB_OK;
 }
