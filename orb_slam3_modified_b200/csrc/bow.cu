@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(BA_NT) bow_assemble_kernel(Voc V, int cap, int
     bitonic_sort(s_keys, n2);
     for (int i = tid; i < n2; i += BA_NT) s_flag[i] = i < kept && (i == 0 || (s_keys[i] >> 32) != (s_keys[i - 1] >> 32));
     __syncthreads();
-    const int nw = orbx::block_excl_scan(s_flag, n2, s_warp);           // s_flag[i] = output slot of the run starting at i (for heads)
+    const int nw = orbx::block_prefix<BA_NT>(n2, s_flag, s_warp, [&](int i) { return s_flag[i]; });   // s_flag[i] = output slot of the run starting at i (for heads)
     for (int i = tid; i < kept; i += BA_NT) {
         const unsigned word = (unsigned)(s_keys[i] >> 32);
         if (i == 0 || word != (unsigned)(s_keys[i - 1] >> 32)) {

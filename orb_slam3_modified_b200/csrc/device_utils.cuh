@@ -58,40 +58,45 @@ inline int ensure_dynamic_smem(Kernel* kernel, size_t bytes, int device) {
     return 0;
 }
 
-// ------------------------------------------------------------------------------------------
-// block-wide exclusive scan of an int array living in shared memory (in place).
-// Returns the total.  `warpTmp` needs 33 ints.  All threads of the block must call.
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ int block_excl_scan(int* data, int m, int* warpTmp) {
-    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, wid = tid >> 5, nw = nt >> 5;
-    int carry = 0;
-    for (int base = 0; base < m; base += nt) {
-        const int i = base + tid;
-        const int v = i < m ? data[i] : 0;
-        int inc = v;
+// Exclusive scan of one int per thread over a CTA of NT threads; `total` gets the CTA's sum.  `sm` needs 33 ints and is free again
+// on return.  All threads of the block must call.
+template <int NT> __device__ __forceinline__ int block_scan_excl(int v, int* sm, int& total) {
+    static_assert(NT % 32 == 0 && NT <= 1024, "NT must be whole warps, at most 1024 threads");
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int inc = v;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            int t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) warpTmp[wid] = inc;
-        __syncthreads();
-        if (wid == 0) {
-            int w = lane < nw ? warpTmp[lane] : 0;
-            int winc = w;
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+    if (lane == 31) sm[w] = inc;
+    __syncthreads();
+    if (w == 0) {
+        const int x = lane < NT / 32 ? sm[lane] : 0;
+        int y = x;
 #pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                int t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
-            warpTmp[lane] = winc - w;       // exclusive warp offsets
-            if (lane == 31) warpTmp[32] = winc;  // tile total
-        }
-        __syncthreads();
-        if (i < m) data[i] = carry + warpTmp[wid] + inc - v;
-        carry += warpTmp[32];
-        __syncthreads();
+        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, y, o); if (lane >= o) y += t; }
+        sm[lane] = y - x;
+        if (lane == 31) sm[32] = y;
     }
+    __syncthreads();
+    const int r = sm[w] + inc - v;
+    total = sm[32];
+    __syncthreads();
+    return r;
+}
+
+// Exclusive prefix of count(i) over i in [0, n), n >= 0, into out[0, n); returns the total and does not write out[n].  count(i) may read out[i]
+// (an in-place scan): each thread reads its element before the tile's barriers and writes it after.  `sm` needs 33 ints.  All threads
+// of the block must call; on return `out` is visible to all of them.
+template <int NT, class Count> __device__ __forceinline__ int block_prefix(int n, int* out, int* sm, Count count) {
+    int carry = 0;
+    // An unsigned tile base: with a signed one the compiler unrolls this loop, and quadtree_orient_kernel spills more
+    for (unsigned b = 0; b < (unsigned)n; b += NT) {
+        const int i = (int)(b + threadIdx.x);
+        int tot;
+        const int r = block_scan_excl<NT>(i < n ? count(i) : 0, sm, tot);
+        if (i < n) out[i] = carry + r;
+        carry += tot;
+    }
+    __syncthreads();
     return carry;
 }
 // Ordered sum of one double per thread over a CTA of NT threads: an xor butterfly in each warp, then the warp sums in warp order, so the

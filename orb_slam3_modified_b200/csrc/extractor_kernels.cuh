@@ -363,7 +363,7 @@ __global__ void __launch_bounds__(FAST_NT, 4) fast_cells_kernel(ExtractParams P,
         rowOff[e] = cnt;
     }
     __syncthreads();
-    const int total = block_excl_scan(rowOff, nE, s_warp);
+    const int total = block_prefix<FAST_NT>(nE, rowOff, s_warp, [&](int e) { return rowOff[e]; });
     for (int e = tid; e < nE; e += FAST_NT) {
         int k = 0;
         while (e >= s_rowBase[k + 1]) ++k;
@@ -557,7 +557,7 @@ __global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams
     const int* cellCount = P.cellCount + (size_t)f * P.cellCountStride + G.cellBase;
     for (int c = tid; c < G.nCells; c += QT_NT) cellOff[c] = cellCount[c];
     __syncthreads();
-    const int n = block_excl_scan(cellOff, G.nCells, s_warp);
+    const int n = block_prefix<QT_NT>(G.nCells, cellOff, s_warp, [&](int c) { return cellOff[c]; });
     {
         const uint32_t* lists = P.cellList + (size_t)f * P.cellListStride;
         const int wid = tid >> 5, lane = tid & 31;
@@ -587,7 +587,7 @@ __global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams
     // erase empty roots, keep order
     for (int i = tid; i < G.nIni; i += QT_NT) S.scanA[i] = S.cnt[0][i] > 0;
     __syncthreads();
-    int m = block_excl_scan(S.scanA, G.nIni, s_warp);
+    int m = block_prefix<QT_NT>(G.nIni, S.scanA, s_warp, [&](int i) { return S.scanA[i]; });
     for (int i = tid; i < G.nIni; i += QT_NT) {
         S.keepPos[i] = S.cnt[0][i] > 0 ? S.scanA[i] : -1;
         if (S.cnt[0][i] > 0) { S.bnd[1][S.scanA[i]] = S.bnd[0][i]; S.cnt[1][S.scanA[i]] = S.cnt[0][i]; }
@@ -610,7 +610,7 @@ __global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams
         if (!careful) {
             for (int s = tid; s < m; s += QT_NT) S.scanA[s] = cntC[s] > 1;
             __syncthreads();
-            P0 = block_excl_scan(S.scanA, m, s_warp);
+            P0 = block_prefix<QT_NT>(m, S.scanA, s_warp, [&](int s) { return S.scanA[s]; });
             for (int s = tid; s < m; s += QT_NT) {
                 if (cntC[s] > 1) { S.proc[s] = S.scanA[s]; S.procNode[S.scanA[s]] = s; }
                 else S.proc[s] = -1;
@@ -650,7 +650,7 @@ __global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams
         }
         __syncthreads();
         // exclusive scan of k -> scanA; keep k in childPos scratch? recompute instead
-        const int totalK = block_excl_scan(S.scanA, P0, s_warp);
+        const int totalK = block_prefix<QT_NT>(P0, S.scanA, s_warp, [&](int pi) { return S.scanA[pi]; });
         if (careful) {
             if (tid == 0) s_P = P0;
             __syncthreads();
@@ -693,7 +693,7 @@ __global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams
         // --- F. unsplit nodes keep their order behind the new blocks ---
         for (int s = tid; s < m; s += QT_NT) S.keepPos[s] = S.proc[s] < 0;
         __syncthreads();
-        const int nKeep = block_excl_scan(S.keepPos, m, s_warp);
+        const int nKeep = block_prefix<QT_NT>(m, S.keepPos, s_warp, [&](int s) { return S.keepPos[s]; });
         for (int s = tid; s < m; s += QT_NT) {
             if (S.proc[s] < 0) {
                 const int pos = totalChildren + S.keepPos[s];
@@ -704,7 +704,7 @@ __global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams
         // --- new expandable list in creation order (processing order, n1..n4) (:634-668) ---
         for (int i = tid; i < 4 * Pn; i += QT_NT) S.scanA[i] = S.childCnt[i] > 1;
         __syncthreads();
-        const int qNew = block_excl_scan(S.scanA, 4 * Pn, s_warp);
+        const int qNew = block_prefix<QT_NT>(4 * Pn, S.scanA, s_warp, [&](int i) { return S.scanA[i]; });
         for (int i = tid; i < 4 * Pn; i += QT_NT) {
             if (S.childCnt[i] > 1) {
                 QtSort e; e.size = S.childCnt[i]; e.node = S.childPos[i]; e.ulx = bndN[e.node].ulx;
@@ -941,7 +941,7 @@ __global__ void __launch_bounds__(AS_NT) assemble_kernel(ExtractParams P) {
     int* s_scan = s_flags + P.selStride;
     for (int e = tid; e < K; e += AS_NT) s_scan[e] = s_flags[e];
     __syncthreads();
-    const int nLap = block_excl_scan(s_scan, K, s_warp);
+    const int nLap = block_prefix<AS_NT>(K, s_scan, s_warp, [&](int e) { return s_scan[e]; });
     int* dstIndex = P.dstIndex + (size_t)f * P.selStride;
     OrbKeyPoint* out = reinterpret_cast<OrbKeyPoint*>(P.outKp) + (size_t)f * P.outCap;
     const bool fits = K <= P.outCap;

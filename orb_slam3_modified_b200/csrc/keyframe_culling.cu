@@ -24,6 +24,7 @@
 namespace orbm {
 
 using orbx::set_error;
+using orbx::csr_ok;
 
 constexpr int KFC_NT = 256;
 constexpr int KFC_ND = 21;
@@ -149,12 +150,6 @@ __global__ void __launch_bounds__(KFC_NT) keyframe_culling_kernel(const KfcMap* 
 using namespace orbm;
 
 namespace {
-
-bool csr_ok(int n, const int32_t* start) {
-    if (start[0] != 0) return false;
-    for (int i = 0; i < n; ++i) if (start[i + 1] < start[i]) return false;
-    return true;
-}
 
 // ORB_ERR_ARG with a message naming the map, or ORB_OK.
 int check_map(const OrbmCullingMap& m, int j) {

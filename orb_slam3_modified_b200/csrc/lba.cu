@@ -44,6 +44,7 @@ using orbx::set_error;
 namespace lba {
 
 using namespace g2o;
+using orbx::block_prefix;
 using orbx::block_sum;
 
 // The open data-parallel phase of one problem, in global memory: CTA 0 of the problem's cluster opens a phase, and the owner CTAs
@@ -1242,25 +1243,6 @@ __global__ void __launch_bounds__(NT, LBA_MINB) lba_cluster_kernel(const Dev* __
 // status: 0 ok, 1 edge index out of range, 2 duplicate (point, keyframe) observation, 3 pair list larger than sized.
 // =============================================================================================
 constexpr int BT = 1024;
-__device__ __forceinline__ int bt_excl_scan(int v, int* sm, int& total) {   // exclusive scan of one int per thread over the CTA
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-    if (lane == 31) sm[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        int x = sm[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += t; }
-        sm[lane] = x;
-    }
-    __syncthreads();
-    const int base = w ? sm[w - 1] : 0;
-    total = sm[31];
-    __syncthreads();
-    return base + inc - v;
-}
 // Ascending bitonic sort of key[n2] (global memory, n2 a power of two), all threads of the CTA.  The stages whose stride is below
 // the tile of 2 BT keys run on that tile in shared memory, so only strides of 2 BT and more cost a pass over global memory.
 constexpr int SORT_TILE = 2 * BT;
@@ -1294,7 +1276,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nL = D.nL, nE = D.nE, nF = D.nF, nP = D.nP;
     const int nOff = nF * (nF - 1) / 2, nTasks = nF + nOff;
-    __shared__ int s_sm[32];
+    __shared__ int s_sm[33];
     __shared__ int s_err;
     __shared__ unsigned long long s_tile[SORT_TILE];
     int* ptStart = const_cast<int*>(D.ptStart); int* ptOrig = const_cast<int*>(D.ptOrig);
@@ -1316,18 +1298,7 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     __syncthreads();
     if (s_err) { if (tid == 0) status[blockIdx.x] = s_err; return; }
     // 2. where every point's edges start in the caller's point order (exclusive scan, into the cursors of step 3)
-    {
-        int carry = 0;
-        for (int b0 = 0; b0 < nL; b0 += BT) {
-            const int i = b0 + tid;
-            const int v = i < nL ? D.bCnt[i] : 0;
-            int total;
-            const int ex = bt_excl_scan(v, s_sm, total);
-            if (i < nL) D.bCursor[i] = carry + ex;
-            carry += total;
-        }
-    }
-    __syncthreads();
+    block_prefix<BT>(nL, D.bCursor, s_sm, [&](int i) { return D.bCnt[i]; });
     // 3. group by point (arbitrary order), then order every point's slice by the caller's edge index; afterwards bCursor[p] is the
     //    end of point p's slice of bTmp.  The point's sort key: its four lowest observing free poses (Hessian blocks) in
     //    ascending order, in `sb` bits each, then the caller's index in `ib` bits, so that every key is distinct (the order is
@@ -1370,19 +1341,8 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     __syncthreads();
     // 4. ptStart over the internal order, then every point's edges in their slots: internal edge id = ptStart[rank] + position in
     //    the point's caller-ordered slice (a stable sort of the edges by point rank)
-    {
-        int carry = 0;
-        for (int b0 = 0; b0 < nL; b0 += BT) {
-            const int r = b0 + tid;
-            const int v = r < nL ? D.bCnt[ptOrig[r]] : 0;
-            int total;
-            const int ex = bt_excl_scan(v, s_sm, total);
-            if (r < nL) ptStart[r] = carry + ex;
-            carry += total;
-        }
-        if (tid == 0) ptStart[nL] = carry;
-    }
-    __syncthreads();
+    const int ptEnd = block_prefix<BT>(nL, ptStart, s_sm, [&](int r) { return D.bCnt[ptOrig[r]]; });
+    if (tid == 0) ptStart[nL] = ptEnd;
     for (int r = tid; r < nL; r += BT) {
         const int p = ptOrig[r], n = D.bCnt[p], a = D.bCursor[p] - n, k0 = ptStart[r];
         for (int i = 0; i < n; ++i) {
@@ -1418,34 +1378,12 @@ __global__ void __launch_bounds__(BT) lba_build_structure_kernel(Dev* probs, int
     }
     __syncthreads();
     // 6. where every task's items and chunks start (pose lists and pair lists are separate arrays)
-    int nChunks = 0;
-    {
-        int carry = 0, tot;
-        for (int b0 = 0; b0 < nF; b0 += BT) {                  // pose lists
-            const int t = b0 + tid;
-            const int ex = bt_excl_scan(t < nF ? D.bTaskLen[t] : 0, s_sm, tot);
-            if (t < nF) D.bItemStart[t] = carry + ex;
-            carry += tot;
-        }
-        carry = 0;
-        for (int b0 = nF; b0 < nTasks; b0 += BT) {             // pair lists
-            const int t = b0 + tid;
-            const int ex = bt_excl_scan(t < nTasks ? D.bTaskLen[t] : 0, s_sm, tot);
-            if (t < nTasks) D.bItemStart[t] = carry + ex;
-            carry += tot;
-        }
-        if (carry > D.pairCap) s_err = 3;
-        carry = 0;
-        for (int b0 = 0; b0 < nTasks; b0 += BT) {              // chunks
-            const int t = b0 + tid;
-            const int ex = bt_excl_scan(t < nTasks ? (D.bTaskLen[t] + SCH - 1) / SCH : 0, s_sm, tot);
-            if (t < nTasks) taskChunkStart[t] = carry + ex;
-            carry += tot;
-        }
-        nChunks = carry;
-        if (tid == 0) taskChunkStart[nTasks] = nChunks;
-        if (nChunks > D.chunkCap) s_err = 3;
-    }
+    block_prefix<BT>(nF, D.bItemStart, s_sm, [&](int t) { return D.bTaskLen[t]; });
+    const int nPairItems = block_prefix<BT>(nOff, D.bItemStart + nF, s_sm, [&](int i) { return D.bTaskLen[nF + i]; });
+    if (nPairItems > D.pairCap) s_err = 3;
+    const int nChunks = block_prefix<BT>(nTasks, taskChunkStart, s_sm, [&](int t) { return (D.bTaskLen[t] + SCH - 1) / SCH; });
+    if (tid == 0) taskChunkStart[nTasks] = nChunks;
+    if (nChunks > D.chunkCap) s_err = 3;
     __syncthreads();
     if (s_err) { if (tid == 0) status[blockIdx.x] = s_err; return; }
     // 7. the lists themselves (ascending point rank = ascending internal edge id) and the chunk headers; the pose lists first: the

@@ -26,6 +26,8 @@
 namespace lba_local {
 
 using orbx::set_error;
+using orbx::csr_ok;
+using orbx::all_distinct;
 
 constexpr int WT = 512;
 constexpr unsigned char KF_SKIP = ORBM_KF_BAD | ORBM_KF_OTHER_MAP;   // isBad() || GetMap() != pCurrentMap
@@ -58,29 +60,6 @@ struct Map {
 // What the finish kernel reads of the solve: status (LBA_LOCAL_*), solved (0: nothing was optimised), the slot's results.
 struct Solve { int status, solved; lba::SlotOut r; };
 
-// exclusive scan of one int per thread over the CTA; `total` gets the sum.  sm: 33 ints.  All threads.
-__device__ __forceinline__ int scan_excl(int v, int* sm, int& total) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-    if (lane == 31) sm[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        const int x = lane < WT / 32 ? sm[lane] : 0;
-        int y = x;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, y, o); if (lane >= o) y += t; }
-        sm[lane] = y - x;
-        if (lane == 31) sm[32] = y;
-    }
-    __syncthreads();
-    const int r = sm[w] + inc - v;
-    total = sm[32];
-    __syncthreads();
-    return r;
-}
-
 // the segment r of base [0..R] (ascending, base[0] = 0, base[R] > q) with base[r] <= q < base[r + 1]
 __device__ __forceinline__ int segment(const int* base, int R, int q) {
     int lo = 0, hi = R;
@@ -96,26 +75,11 @@ __device__ int compact(int Q, int* sm, Flag flag, Emit emit) {
         const int q = b + (int)threadIdx.x;
         const bool f = q < Q && flag(q);
         int tot;
-        const int r = scan_excl(f ? 1 : 0, sm, tot);
+        const int r = orbx::block_scan_excl<WT>(f ? 1 : 0, sm, tot);
         if (f) emit(q, carry + r);
         carry += tot;
     }
     return carry;
-}
-
-// exclusive prefix of count(i) over i in [0, n) into base [n + 1].  All threads.
-template <class Count>
-__device__ void prefix(int n, int* base, int* sm, Count count) {
-    int carry = 0;
-    for (int b = 0; b < n; b += WT) {
-        const int i = b + (int)threadIdx.x;
-        int tot;
-        const int r = scan_excl(i < n ? count(i) : 0, sm, tot);
-        if (i < n) base[i] = carry + r;
-        carry += tot;
-    }
-    if (threadIdx.x == 0) base[n] = carry;
-    __syncthreads();
 }
 
 // ascending bitonic sort of key / val [n2], n2 a power of two, in global memory.  All threads.
@@ -161,8 +125,8 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     __syncthreads();
     const int nLocal = s_nLocal;
     // lLocalMapPoints: first appearance over the local keyframes' slots, bad and other-map points skipped
-    prefix(nLocal, M.locBase, sm, [&](int r) { const int c = M.locCand[r]; return M.slotStart[c + 1] - M.slotStart[c]; });
-    const int Qs = M.locBase[nLocal];
+    const int Qs = orbx::block_prefix<WT>(nLocal, M.locBase, sm, [&](int r) { const int c = M.locCand[r]; return M.slotStart[c + 1] - M.slotStart[c]; });
+    if (tid == 0) M.locBase[nLocal] = Qs;
     auto slotPt = [&](int q) {
         const int r = segment(M.locBase, nLocal, q);
         const int p = M.slotPoint[M.slotStart[M.locCand[r]] + q - M.locBase[r]];
@@ -174,8 +138,8 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
                            [&](int q, int r) { M.localPoint[r] = slotPt(q); });
     __syncthreads();
     // lFixedCameras: first appearance over (local point, observation) of the unmarked observers, kept when good and in the current map
-    prefix(nL, M.lpBase, sm, [&](int r) { const int p = M.localPoint[r]; return M.obsStart[p + 1] - M.obsStart[p]; });
-    const int Qo = M.lpBase[nL];
+    const int Qo = orbx::block_prefix<WT>(nL, M.lpBase, sm, [&](int r) { const int p = M.localPoint[r]; return M.obsStart[p + 1] - M.obsStart[p]; });
+    if (tid == 0) M.lpBase[nL] = Qo;
     auto obsAt = [&](int q) { const int r = segment(M.lpBase, nL, q); return M.obsStart[M.localPoint[r]] + q - M.lpBase[r]; };
     for (int q = tid; q < Qo; q += WT) {
         const int k = M.obsKF[obsAt(q)];
@@ -238,7 +202,7 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     int nFree = 0;
     for (int v = tid; v < nP; v += WT) nFree += !M.bFixed[v];
     int nF;
-    scan_excl(nFree, sm, nF);
+    orbx::block_scan_excl<WT>(nFree, sm, nF);
     if (tid == 0) {
         M.sizes[0] = 0; M.sizes[1] = nP; M.sizes[2] = nL; M.sizes[3] = nE; M.sizes[4] = nF;
         M.counts[0] = numFixed; M.counts[1] = nLocal; M.counts[2] = nL; M.counts[3] = nE;
@@ -342,12 +306,6 @@ __global__ void __launch_bounds__(WT) local_ba_finish_kernel(const Map* __restri
     }
 }
 
-bool csr_ok(int n, const int32_t* start) {
-    if (start[0] != 0) return false;
-    for (int i = 0; i < n; ++i) if (start[i + 1] < start[i]) return false;
-    return true;
-}
-
 // ORB_ERR_ARG with a message naming the map, or ORB_OK
 int check_map(const LbaLocalMap& m, int j) {
     auto bad = [j](const std::string& what) { set_error("lba_local_bundle_adjustment_batch: map " + std::to_string(j) + ": " + what); return ORB_ERR_ARG; };
@@ -360,9 +318,7 @@ int check_map(const LbaLocalMap& m, int j) {
                           !m.pointRefKF || !m.normal || !m.minDistance || !m.maxDistance)) return bad("a point array is null");
     if ((m.edgeChi2 == nullptr) != (m.edgeDepthPositive == nullptr)) return bad("edgeChi2 and edgeDepthPositive go together");
     if (m.kfFlags[0] & ORBM_KF_OTHER_MAP) return bad("pKF (entry 0) cannot be of another map");
-    std::vector<uint64_t> ids(m.mnId, m.mnId + m.nKF);
-    std::sort(ids.begin(), ids.end());
-    if (std::adjacent_find(ids.begin(), ids.end()) != ids.end()) return bad("keyframe mnIds repeat");
+    if (!all_distinct(m.mnId, m.nKF)) return bad("keyframe mnIds repeat");
     std::vector<char> seen(m.nKF, 0);
     seen[0] = 1;
     for (int i = 0; i < m.nCov; ++i) {
@@ -376,9 +332,7 @@ int check_map(const LbaLocalMap& m, int j) {
     for (int s = 0; s < nSlots; ++s)
         if (m.slotPoint[s] < -1 || m.slotPoint[s] >= m.nPoints) return bad("slotPoint out of range");
     if (m.nPoints > 0) {
-        std::vector<uint64_t> pid(m.pointId, m.pointId + m.nPoints);
-        std::sort(pid.begin(), pid.end());
-        if (std::adjacent_find(pid.begin(), pid.end()) != pid.end()) return bad("point mnIds repeat");
+        if (!all_distinct(m.pointId, m.nPoints)) return bad("point mnIds repeat");
         if (!csr_ok(m.nPoints, m.obsStart)) return bad("obsStart must start at 0 and not decrease");
         const int nObs = m.obsStart[m.nPoints];
         if (nObs > 0 && (!m.obsKF || !m.obsIdx || !m.obsPt || !m.obsOctave || !m.obsFlag)) return bad("an observation array is null");

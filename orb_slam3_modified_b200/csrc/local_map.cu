@@ -23,6 +23,7 @@
 namespace orbm {
 
 using orbx::set_error;
+using orbx::csr_ok;
 
 constexpr int ULM_NT = 256;
 constexpr int ULM_MAX_LOCAL_KF = 80;    // if(mvpLocalKeyFrames.size()>80) break;  /  mvpLocalKeyFrames.size()<80
@@ -36,20 +37,6 @@ struct UlmArgs {
     uint8_t* mark;       // [nKF] mnTrackReferenceForFrame == mCurrentFrame.mnId
     int* key;            // [nPoints] first occurrence in UpdateLocalPoints' order (INT_MAX: none), then -2 - the point's local index
 };
-
-// Exclusive count of the threads before this one with `flag` set, over the CTA; the CTA's total in *total.  All threads call.
-__device__ __forceinline__ int flag_scan(bool flag, int* s_warp, int* total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const unsigned ball = __ballot_sync(0xffffffffu, flag);
-    if (lane == 0) s_warp[warp] = __popc(ball);
-    __syncthreads();
-    int before = 0, sum = 0;
-#pragma unroll
-    for (int w = 0; w < ULM_NT / 32; ++w) { const int c = s_warp[w]; before += w < warp ? c : 0; sum += c; }
-    __syncthreads();
-    *total = sum;
-    return before + __popc(ball & ((1u << lane) - 1u));
-}
 
 // Warp 0: appends the first keyframe of list[0, n) that is not bad and not marked, if any (the covisibles' and the children's loops, each
 // of which pushes one keyframe and breaks).  Returns whether it pushed.
@@ -75,7 +62,7 @@ __device__ __forceinline__ bool push_first(const int* list, int n, const uint8_t
 __global__ void __launch_bounds__(ULM_NT) update_local_map_kernel(const UlmArgs A) {
     const OrbmUpdateLocalMapBatch& I = A.in;
     const OrbmUpdateLocalMapResult& O = A.out;
-    __shared__ int s_warp[ULM_NT / 32], s_bestC[ULM_NT / 32], s_bestK[ULM_NT / 32];
+    __shared__ int s_warp[33], s_bestC[ULM_NT / 32], s_bestK[ULM_NT / 32];
     __shared__ int s_nLocal, s_ref;
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int k0 = I.kfStart[b], nk = I.kfStart[b + 1] - k0, p0 = I.pointStart[b], np = I.pointStart[b + 1] - p0;
@@ -113,7 +100,7 @@ __global__ void __launch_bounds__(ULM_NT) update_local_map_kernel(const UlmArgs 
         const int c = k < nk ? counter[k] : 0;
         const bool voter = c > 0 && !(flags[k] & ORBM_KF_BAD);
         int total;
-        const int pos = flag_scan(voter, s_warp, &total);
+        const int pos = orbx::block_scan_excl<ULM_NT>(voter ? 1 : 0, s_warp, total);
         if (voter) {
             localKF[nL + pos] = k;
             mark[k] = 1;
@@ -193,7 +180,7 @@ __global__ void __launch_bounds__(ULM_NT) update_local_map_kernel(const UlmArgs 
             bool first = false;
             if (s < n) { p = I.slotPoint[s0 + s]; first = !pointBad[p] && key[p] == off + s; }
             int total;
-            const int pos = flag_scan(first, s_warp, &total);
+            const int pos = orbx::block_scan_excl<ULM_NT>(first ? 1 : 0, s_warp, total);
             if (first) key[p] = -2 - (nM + pos);       // read by no later occurrence as a match: keys are >= 0
             nM += total;
         }
@@ -261,13 +248,6 @@ int ulm_shape(const OrbmUpdateLocalMapBatch* in, const OrbmUpdateLocalMapResult*
         !out->maxDistance || !out->mpDesc || !out->hasObs || !out->bad || !out->lastToLocal)
         return bad("an output is null");
     return ORB_OK;
-}
-
-// CSR offsets [n + 1] starting at 0 and not decreasing.
-bool csr_ok(int n, const int32_t* start) {
-    if (start[0] != 0) return false;
-    for (int i = 0; i < n; ++i) if (start[i + 1] < start[i]) return false;
-    return true;
 }
 
 // The host form's data checks, before anything is staged.

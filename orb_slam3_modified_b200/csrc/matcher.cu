@@ -304,7 +304,7 @@ __device__ void build_frame_smem(const FrameSmem& S, const OrbKeyPoint* kps, con
         for (int i = tid; i < 2 * K; i += MF_NT) dst[i] = __ldg(src + i);
     }
     __syncthreads();
-    const int total = block_excl_scan(S.cnt, GRID_CELLS, s_warp);
+    const int total = block_prefix<MF_NT>(GRID_CELLS, S.cnt, s_warp, [&](int c) { return S.cnt[c]; });
     for (int c = tid; c < GRID_CELLS; c += MF_NT) S.cellStart[c] = (uint16_t)S.cnt[c];
     if (tid == 0) S.cellStart[GRID_CELLS] = (uint16_t)total;
     __syncthreads();
@@ -1227,9 +1227,9 @@ __global__ void __launch_bounds__(NP_NT) new_points_kernel(NewPointsParams P) {
 // One CTA per item: winner[idx1] = first neighbour that created idx1's point; then per neighbour, in order, the counts and the records
 // compacted in idx1 order (thread t owns a contiguous run of idx1, a block scan gives each run its place).
 __global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsParams P) {
-    __shared__ int s_scan[NPC_NT / 32], s_msum[NPC_NT / 32];
+    __shared__ int s_warp[33];
     const NpItem& I = P.items[blockIdx.x];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, N1 = P.tri[blockIdx.x].N1, K = I.nKF2;
+    const int tid = threadIdx.x, N1 = P.tri[blockIdx.x].N1, K = I.nKF2;
     const int* matches12 = P.matches12 + I.slot0;
     const uint8_t* reason = P.reason + I.slot0;
     const OrbmNewPoint* recs = P.recs + I.slot0;
@@ -1249,28 +1249,12 @@ __global__ void __launch_bounds__(NPC_NT) new_points_commit_kernel(NewPointsPara
             c += w == k;
             mt += matches12[(size_t)k * N1 + i] >= 0 && (w < 0 || w >= k);     // the reference's search skips idx1 once an earlier k made its point
         }
-        int incl = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-        const int msum = __reduce_add_sync(0xffffffffu, mt);
-        if (lane == 31) s_scan[wid] = incl;
-        if (lane == 0) s_msum[wid] = msum;
-        __syncthreads();
-        if (wid == 0) {
-            int v = s_scan[lane], m = s_msum[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
-            m = __reduce_add_sync(0xffffffffu, m);
-            s_scan[lane] = v;                                   // inclusive over warps
-            if (lane == 0) s_msum[0] = m;
-        }
-        __syncthreads();
-        int pos = base + (wid ? s_scan[wid - 1] : 0) + incl - c;
+        int created, matched;
+        int pos = base + block_scan_excl<NPC_NT>(c, s_warp, created);
+        block_scan_excl<NPC_NT>(mt, s_warp, matched);
         for (int i = i0; i < i1; ++i) if (winner[i] == k) I.out[pos++] = recs[(size_t)k * N1 + i];
-        const int created = s_scan[NPC_NT / 32 - 1];
-        if (tid == 0) { I.counts[1 + k] = s_msum[0]; I.counts[1 + K + k] = created; }
+        if (tid == 0) { I.counts[1 + k] = matched; I.counts[1 + K + k] = created; }
         base += created;
-        __syncthreads();
     }
     if (tid == 0) I.counts[0] = base;
 }

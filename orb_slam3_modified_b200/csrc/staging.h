@@ -114,6 +114,18 @@ inline int check_row_counts(const char* where, const int32_t* N, int count, int 
         if (N[f] < 0 || N[f] > cap) { set_error(std::string(where) + ": N[f] outside [0, cap]"); return ORB_ERR_ARG; }
     return ORB_OK;
 }
+// CSR offsets start[0, n] that start at 0 and do not decrease.
+inline bool csr_ok(int n, const int32_t* start) {
+    if (start[0] != 0) return false;
+    for (int i = 0; i < n; ++i) if (start[i + 1] < start[i]) return false;
+    return true;
+}
+// No key of keys[0, n) repeats.
+inline bool all_distinct(const uint64_t* keys, int n) {
+    std::vector<uint64_t> s(keys, keys + n);
+    std::sort(s.begin(), s.end());
+    return std::adjacent_find(s.begin(), s.end()) == s.end();
+}
 // The kernels write the slots [0, N[f]) of an output row only and download copies the whole row, so the slots past N[f] would carry
 // whatever the staging buffer last held there: they are set to 0 after download.
 inline void zero_row_tails(uint8_t* rows, const int32_t* N, int count, int cap) {

@@ -29,6 +29,8 @@ namespace orbm {
 using orbx::distinctive_best;
 using orbx::update_normal_and_depth;
 using orbx::set_error;
+using orbx::csr_ok;
+using orbx::all_distinct;
 
 constexpr int UC_NT = 256;
 constexpr int UC_TH = 15;
@@ -201,12 +203,6 @@ using namespace orbm;
 
 namespace {
 
-bool csr_ok(int n, const int32_t* start) {
-    if (start[0] != 0) return false;
-    for (int i = 0; i < n; ++i) if (start[i + 1] < start[i]) return false;
-    return true;
-}
-
 // ORB_ERR_ARG / ORB_ERR_CAPACITY with a message naming the item, or ORB_OK.
 int check_item(const OrbmConnectionsItem& it, int j) {
     auto fail = [j](int rc, const char* what) { set_error("orbm_update_connections_batch: item " + std::to_string(j) + ": " + what); return rc; };
@@ -218,9 +214,7 @@ int check_item(const OrbmConnectionsItem& it, int j) {
     if (it.nSlots > 0 && (!it.slotPoint || !it.slotOctave || !it.slotDesc || !it.slotStatus)) return bad("a slot array is null");
     if (it.nPoints > 0 && (!it.pointBad || !it.pointPos || !it.pointRefKF || !it.obsStart || !it.pointUpdated || !it.normal || !it.minDistance ||
                            !it.maxDistance || !it.descKF || !it.descIdx)) return bad("a point array is null");
-    std::vector<uint64_t> keys(it.order, it.order + it.nKF);
-    std::sort(keys.begin(), keys.end());
-    if (std::adjacent_find(keys.begin(), keys.end()) != keys.end()) return bad("order keys are not distinct");
+    if (!all_distinct(it.order, it.nKF)) return bad("order keys are not distinct");
     if (!csr_ok(it.nKF, it.connStart)) return bad("connStart must start at 0 and not decrease");
     const int nConn = it.connStart[it.nKF];
     if (!it.nbrKF || !it.nbrWeight) return bad("nbrKF / nbrWeight is null");
