@@ -996,6 +996,66 @@ typedef struct LocalInertialBAResult {
 } LocalInertialBAResult;
 int local_inertial_ba_batch(int count, const LocalInertialBAProblem* problems, const LocalInertialBAResult* results, int32_t* iterationsOut, int device);
 
+/* void Optimizer::LocalInertialBA(KeyFrame* pKF, bool* pbStopFlag, Map* pMap, int&, int&, int&, int&, bool bLarge, bool bRecInit)
+ * (src/Optimizer.cc:2383-2958, monocular observations) as a whole, for a batch of maps: the window / point / fixed-keyframe walk
+ * (:2385-2478), the edge walk (:2593-2763), the solve of local_inertial_ba_batch, the EraseMapPointMatch / EraseObservation cascade
+ * (:2848-2902) and the write-back (:2905-2957).  One map per item, at most one keyframe per map, the maps share no keyframe and no point,
+ * and no keyframe or point carries a mark (mnBALocalForKF / mnBAFixedForKF) equal to pKF->mnId at the call.  Keyframes are table indices,
+ * points point indices; std::map<KeyFrame*, ...> order is the caller's key order, in which every point's observations are listed.
+ *   keyframe table [nKF]: entry 0 is pKF, then its mPrevKF chain (at least Nd + 1 links where they exist) and every observer of the points
+ *     in the slots of the chain's first Nd keyframes.  kfFlags: ORBM_KF_BAD (isBad()), ORBM_KF_OTHER_MAP (GetMap() != pKF->GetMap()),
+ *     ORBM_KF_IMU (bImu), ORBM_KF_PREINT (mpImuPreintegrated != NULL); prevKF = mPrevKF as a table index (-1 = NULL);
+ *     state21 = GetImuRotation | GetImuPosition | GetVelocity | GetGyroBias | GetAccBias, tcw12 = GetRotation | GetTranslation,
+ *     cameraCenter = GetCameraCenter(), cam4 = fx fy cx cy; preint [nKF][IMU_PREINT_FLOATS] = mpImuPreintegrated (rows read where
+ *     ORBM_KF_PREINT; may be NULL when no entry has it); extrinsics24 as local_inertial_ba_batch takes it.
+ *   slots [nKF + 1] CSR: slotPoint = the point of GetMapPointMatches()[s], -1 for NULL (only the window candidates' slots are read).
+ *   points [nPoints]: pointFlags (ORBM_KF_BAD: isBad()), worldPos, trackDepth = mTrackDepth, refKF = mpRefKF; GetObservations() as CSR
+ *     obsStart [nPoints + 1] / obsKF / obsIdx with obsPt = mvKeysUn[idx].pt and obsOctave = .octave (Pinhole: uncertainty2 = 1).
+ *   keyFramesInMap = pMap->KeyFramesInMap(); bLarge, bRecInit as the reference takes them.
+ * Outputs (host pointers):
+ *   status: LIBA_LOCAL_RAN or LIBA_LOCAL_FAILED ("FAIL LOCAL-INERTIAL BA": nothing is erased or written back, and the marks stay set);
+ *   nLists [4] = N, |lFixedKeyFrames|, |lLocalMapPoints|, mono edges.
+ *   optKF [nKF] = vpOptimizableKFs (newest first), fixedKF [nKF] = lFixedKeyFrames, localPoint [nPoints] = lLocalMapPoints, all in the
+ *     reference's order; ieLinked [nKF]: window keyframe i got its inertial edge (and its preintegration SetNewBias(mPrevKF->GetImuBias())).
+ *   obsFlag [obsStart[nPoints]]: LBA_OBS_NO_EDGE, LBA_OBS_KEPT or LBA_OBS_ERASED; vToErase is the ERASED observations of localPoint in
+ *     list order, each point's in key order (none on FAILED).
+ *   per window keyframe i: kfPose7 [nKF][7] = the SE3f SetPose receives, kfCenter [nKF][3] = its GetCameraCenter(), kfVelocity [nKF][3],
+ *     kfBias6 [nKF][6] = IMU::Bias (bax, bay, baz, bwx, bwy, bwz).
+ *   per local point i: pointPos [nPoints][3], pointBad, pointRefKF, normal [nPoints][3] / minDistance / maxDistance as in
+ *     lba_local_bundle_adjustment_batch.  Every per-keyframe and per-point value is 0 on FAILED (pointRefKF -1).
+ *   stats8 as LocalInertialBAResult.stats8.
+ *   optional (all four or none): optState21 [nKF][21] / optTcw12 [nKF][12] = the solver's doubles per problem keyframe (window, then
+ *     lFixedKeyFrames), optPoint [nPoints][3] per local point, edgeChi2 [obsStart[nPoints]] per observation with an edge (0 elsewhere);
+ *     the first three are 0 on FAILED.
+ * Errors, before the device is touched: ORB_ERR_ARG naming the map for an index, octave or CSR offset out of range, a keyframe that
+ * observes a point twice, an mpRefKF of a good point that is not among its observers, pKF of another map or without mPrevKF, a window
+ * keyframe without ORBM_KF_IMU, an mPrevKF chain that revisits a keyframe within Nd + 1 steps, or a null array a map needs.  Then
+ * ORB_ERR_CUDA without a usable device.  Three launches whatever nMaps (walk, solver, finish; local_inertial_ba_map_last_launches), one
+ * staging upload and one download, no host synchronisation in between.  Like local_inertial_ba_batch it uses the thread's staging on device. */
+enum { ORBM_KF_IMU = 16, ORBM_KF_PREINT = 32 };
+enum { LIBA_LOCAL_RAN = 0, LIBA_LOCAL_FAILED = 1 };
+typedef struct LocalInertialBAMap {
+    int32_t nKF;
+    const uint8_t* kfFlags; const int32_t* prevKF;
+    const float* state21; const float* tcw12; const float* cameraCenter; const float* cam4;
+    const float* preint; const double* extrinsics24;
+    const int32_t* slotStart; const int32_t* slotPoint;
+    int32_t nPoints;
+    const uint8_t* pointFlags; const float* worldPos; const float* trackDepth; const int32_t* refKF;
+    const int32_t* obsStart; const int32_t* obsKF; const int32_t* obsIdx; const float* obsPt; const int32_t* obsOctave;
+    int32_t nlevels;
+    const float* invLevelSigma2; const float* scaleFactors;
+    int32_t keyFramesInMap; int32_t bLarge; int32_t bRecInit;
+    int32_t* status; int32_t* nLists;
+    int32_t* optKF; int32_t* fixedKF; int32_t* localPoint; uint8_t* ieLinked; uint8_t* obsFlag;
+    float* kfPose7; float* kfCenter; float* kfVelocity; float* kfBias6;
+    float* pointPos; uint8_t* pointBad; int32_t* pointRefKF; float* normal; float* minDistance; float* maxDistance;
+    double* stats8;
+    double* optState21; double* optTcw12; double* optPoint; double* edgeChi2;
+} LocalInertialBAMap;
+int local_inertial_ba_map_batch(int nMaps, const LocalInertialBAMap* maps, int device);
+int local_inertial_ba_map_last_launches(void);
+
 /* ------------------------------------------------------------------------------------------
  * DBoW2 transform (SURVEY.md 8f rank 3): Frame::ComputeBoW / KeyFrame::ComputeBoW (reference src/Frame.cc:738-745) call
  * ORBVocabulary::transform(vCurrentDesc, mBowVec, mFeatVec, 4) = DBoW2::TemplatedVocabulary<FORB::TDescriptor, FORB>::transform

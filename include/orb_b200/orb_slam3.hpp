@@ -341,6 +341,12 @@ public:
         orb_check(local_inertial_ba_batch(1, &graph, &r, nullptr, device), "local_inertial_ba_batch");
         return r.stats8[2] == 0.0;
     }
+    // The same function as a whole -- window walk, solve, erase cascade and write-back -- for a batch of maps (one keyframe each): each
+    // LocalInertialBAMap is the flattened map and receives the record the host replays (include/orb_b200.h, INTEGRATION.md §3).  Like
+    // LocalInertialBA it needs no handle; the staging is the calling thread's.
+    static void LocalInertialBABatch(int nMaps, const LocalInertialBAMap* maps, int device = 0) {
+        orb_check(local_inertial_ba_map_batch(nMaps, maps, device), "local_inertial_ba_map_batch");
+    }
 };
 
 }  // namespace ORB_SLAM3

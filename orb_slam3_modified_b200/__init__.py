@@ -131,6 +131,8 @@ SIGNATURES = {
     'pose_inertial_optimization_last_kf_batch': (_i, [_i, _i] + [_vp] * 10 + [_i, _vp, _vp, _vp, _i]),
     'pose_inertial_optimization_last_frame_batch': (_i, [_i, _i] + [_vp] * 13 + [_i, _vp, _vp, _vp, _i]),
     'local_inertial_ba_batch': (_i, [_i, _vp, _vp, _vp, _i]),
+    'local_inertial_ba_map_batch': (_i, [_i, _vp, _i]),
+    'local_inertial_ba_map_last_launches': (_i, []),
     # ORBVocabulary
     'orbv_create': (_i, [_out, _vp, _i]),
     'orbv_destroy': (None, [_vp]),
@@ -1434,6 +1436,23 @@ class Optimizer:
     def local_last_launches(self):
         return lib().lba_local_last_launches(self._h)
 
+    @staticmethod
+    def local_inertial_ba_map_batch(maps, debug=False, device=0):
+        """``Optimizer::LocalInertialBA`` as a whole -- window walk, solve, erase cascade, write-back -- for one map per item (dicts as
+        ``liba_map_struct`` reads them), in one call on `device`; like ``LocalInertialBA`` it needs no handle.  Returns one
+        ``liba_map_result`` dict per map; debug adds the solver's own results."""
+        packs = [liba_map_struct(m, debug=debug) for m in maps]
+        arr = (LocalInertialBAMap * max(1, len(maps)))(*[p[0] for p in packs])
+        rc = lib().local_inertial_ba_map_batch(len(maps), arr, device)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'local_inertial_ba_map_batch')
+        return [liba_map_result(p[1]) for p in packs]
+
+    @staticmethod
+    def local_inertial_ba_map_last_launches():
+        """Launches of this thread's last local_inertial_ba_map_batch call."""
+        return lib().local_inertial_ba_map_last_launches()
+
     def LocalBundleAdjustment(self, prob, iterations=10, user_lambda_init=0.0, stop_flag=None):
         keep = dict(poses=_c(prob['poses'], np.float64), fixed=_c(prob['fixed'], np.uint8), cam=_c(prob['cam'], np.float32),
                     points=_c(prob['points'], np.float64), ep=_c(prob['edge_point'], np.int32), ek=_c(prob['edge_pose'], np.int32),
@@ -1635,6 +1654,73 @@ def LocalInertialBA(probs, device=0):
     if rc != ORB_OK:
         raise OrbError(rc, 'local_inertial_ba_batch')
     return _liba_finish(outs, iters)
+
+
+#: local_inertial_ba_map_batch's keyframe flags (besides KF_BAD / KF_OTHER_MAP) and map statuses (include/orb_b200.h)
+KF_IMU, KF_PREINT = 16, 32
+LIBA_LOCAL_RAN, LIBA_LOCAL_FAILED = 0, 1
+#: the input arrays of one LocalInertialBAMap, with their dtypes
+LIBA_MAP_ARRAYS = (('kfFlags', np.uint8), ('prevKF', np.int32), ('state21', np.float32), ('tcw12', np.float32), ('cameraCenter', np.float32),
+                   ('cam4', np.float32), ('preint', np.float32), ('extrinsics24', np.float64), ('slotStart', np.int32), ('slotPoint', np.int32),
+                   ('pointFlags', np.uint8), ('worldPos', np.float32), ('trackDepth', np.float32), ('refKF', np.int32), ('obsStart', np.int32),
+                   ('obsKF', np.int32), ('obsIdx', np.int32), ('obsPt', np.float32), ('obsOctave', np.int32), ('invLevelSigma2', np.float32),
+                   ('scaleFactors', np.float32))
+#: its outputs: (name, dtype, rows, row shape); rows 'kf' = [nKF], 'pt' = [nPoints], 'obs' = [obsStart[-1]], or a fixed count
+LIBA_MAP_OUTPUTS = (('nLists', np.int32, 4, ()), ('optKF', np.int32, 'kf', ()), ('fixedKF', np.int32, 'kf', ()), ('localPoint', np.int32, 'pt', ()),
+                    ('ieLinked', np.uint8, 'kf', ()), ('obsFlag', np.uint8, 'obs', ()), ('kfPose7', np.float32, 'kf', (7,)),
+                    ('kfCenter', np.float32, 'kf', (3,)), ('kfVelocity', np.float32, 'kf', (3,)), ('kfBias6', np.float32, 'kf', (6,)),
+                    ('pointPos', np.float32, 'pt', (3,)), ('pointBad', np.uint8, 'pt', ()), ('pointRefKF', np.int32, 'pt', ()),
+                    ('normal', np.float32, 'pt', (3,)), ('minDistance', np.float32, 'pt', ()), ('maxDistance', np.float32, 'pt', ()),
+                    ('stats8', np.float64, 8, ()))
+#: the optional outputs (the solver's own results)
+LIBA_MAP_DEBUG = (('optState21', np.float64, 'kf', (21,)), ('optTcw12', np.float64, 'kf', (12,)), ('optPoint', np.float64, 'pt', (3,)),
+                  ('edgeChi2', np.float64, 'obs', ()))
+
+
+class LocalInertialBAMap(C.Structure):
+    """One map of local_inertial_ba_map_batch (include/orb_b200.h)."""
+    _fields_ = [('nKF', C.c_int32)] + [(n, C.c_void_p) for n, _ in LIBA_MAP_ARRAYS[:10]] + [('nPoints', C.c_int32)] + \
+               [(n, C.c_void_p) for n, _ in LIBA_MAP_ARRAYS[10:19]] + [('nlevels', C.c_int32)] + [(n, C.c_void_p) for n, _ in LIBA_MAP_ARRAYS[19:]] + \
+               [('keyFramesInMap', C.c_int32), ('bLarge', C.c_int32), ('bRecInit', C.c_int32), ('status', C.c_void_p)] + \
+               [(n, C.c_void_p) for n, _, _, _ in LIBA_MAP_OUTPUTS + LIBA_MAP_DEBUG]
+
+
+def liba_map_struct(m, debug=False, given=None):
+    """LocalInertialBAMap over map dict `m` (keys LIBA_MAP_ARRAYS, 'keyFramesInMap', 'bLarge', 'bRecInit') with fresh outputs: (struct, out
+    dict, arrays to keep alive).  debug: also the optional outputs.  given: a dict of LIBA_MAP_DEBUG arrays and 'stats8' to point them at
+    instead (the CPU oracle finishes from them)."""
+    a = {n: _c(m[n] if m.get(n) is not None else np.zeros(0), dt) for n, dt in LIBA_MAP_ARRAYS}
+    nK, nP = len(a['kfFlags']), len(a['pointFlags'])
+    nO = int(a['obsStart'][-1]) if nP else 0
+    rows = dict(kf=nK, pt=nP, obs=nO)
+    out = {n: np.zeros((r if isinstance(r, int) else rows[r],) + sh, dt) for n, dt, r, sh in LIBA_MAP_OUTPUTS}
+    out['status'] = np.zeros(1, np.int32)
+    if given is not None:
+        out.update({n: _c(given[n], dt).copy() for n, dt, _, _ in LIBA_MAP_DEBUG + (('stats8', np.float64, 8, ()),)})
+    elif debug:
+        out.update({n: np.zeros((rows[r],) + sh, dt) for n, dt, r, sh in LIBA_MAP_DEBUG})
+    p = lambda n: _ptr(a[n])
+    s = LocalInertialBAMap(nK, *[p(n) for n, _ in LIBA_MAP_ARRAYS[:10]], nP, *[p(n) for n, _ in LIBA_MAP_ARRAYS[10:19]], len(a['scaleFactors']),
+                           *[p(n) for n, _ in LIBA_MAP_ARRAYS[19:]], int(m['keyFramesInMap']), int(m.get('bLarge', 0)), int(m.get('bRecInit', 0)),
+                           _ptr(out['status']), *[_ptr(out.get(n)) for n, _, _, _ in LIBA_MAP_OUTPUTS + LIBA_MAP_DEBUG])
+    return s, out, a
+
+
+def liba_map_result(out):
+    """The output dict with the status unpacked and the lists cut to their lengths."""
+    N, nFix, nPt, nE = (int(v) for v in out['nLists'])
+    r = dict(out, status=int(out['status'][0]), num_OptKF=N, num_fixedKF=nFix, num_MPs=nPt, num_edges=nE)
+    r['optKF'], r['fixedKF'], r['localPoint'], r['ieLinked'] = out['optKF'][:N].copy(), out['fixedKF'][:nFix].copy(), out['localPoint'][:nPt].copy(), \
+        out['ieLinked'][:N].copy()
+    for n in ('kfPose7', 'kfCenter', 'kfVelocity', 'kfBias6'):
+        r[n] = out[n][:N].copy()
+    for n in ('optState21', 'optTcw12'):
+        if n in r:
+            r[n] = out[n][:N + nFix].copy()
+    for n in ('pointPos', 'pointBad', 'pointRefKF', 'normal', 'minDistance', 'maxDistance', 'optPoint'):
+        if n in r:
+            r[n] = out[n][:nPt].copy()
+    return r
 
 
 class _OrbVocabulary(C.Structure):

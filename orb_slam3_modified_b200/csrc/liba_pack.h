@@ -39,11 +39,12 @@ inline std::string check(const LocalInertialBAProblem& p) {
     return "";
 }
 
-inline Layout make_layout(const LocalInertialBAProblem& p) {
+// The layout of a problem of at most nKF keyframes, nO of them in the window, nI inertial edges, nL points and nE mono edges of which nFree
+// observe a window keyframe.  Every array of a problem within these bounds fits at the same offsets, so local_inertial_ba_map_batch lays
+// out the problems its walk kernel builds on the device from bounds the host reads off the map.
+inline Layout make_layout(size_t nKF, size_t nO, size_t nI, size_t nL, size_t nE, int nFree) {
     Layout L;
-    const size_t nKF = p.nKF, nO = p.nOpt, nI = p.nInertial, nL = p.nPoints, nE = p.nEdges, n = 15 * nO;
-    int nFree = 0;
-    for (int e = 0; e < p.nEdges; ++e) nFree += p.edgeKf[e] < p.nOpt;
+    const size_t n = 15 * nO;
     L.nFreeEdges = nFree;
     size_t o = 0;
     L.kfState = bump(o, nKF * 21 * 8); L.kfTcw = bump(o, nKF * 12 * 8); L.cam = bump(o, nKF * 4 * 4); L.extr = bump(o, 24 * 8);
@@ -66,6 +67,12 @@ inline Layout make_layout(const LocalInertialBAProblem& p) {
     L.outState = bump(o, nKF * 21 * 8); L.outTcw = bump(o, nKF * 12 * 8); L.outPts = bump(o, nL * 3 * 8); L.erase = bump(o, nE); L.chi2 = bump(o, nE * 8); L.stats = bump(o, 8 * 8); L.prof = bump(o, 8 * 8);
     L.outBytes = o;
     return L;
+}
+
+inline Layout make_layout(const LocalInertialBAProblem& p) {
+    int nFree = 0;
+    for (int e = 0; e < p.nEdges; ++e) nFree += p.edgeKf[e] < p.nOpt;
+    return make_layout(p.nKF, p.nOpt, p.nInertial, p.nPoints, p.nEdges, nFree);
 }
 
 // fills the input region (host memory); returns an error text when a (point, keyframe) pair is observed twice

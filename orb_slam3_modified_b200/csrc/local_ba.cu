@@ -20,7 +20,7 @@
 #include "device_utils.cuh"
 #include "frame_pose.cuh"
 #include "local_ba.h"
-#include "normal_depth.cuh"
+#include "map_walk.cuh"
 #include "staging.h"
 
 namespace lba_local {
@@ -28,6 +28,7 @@ namespace lba_local {
 using orbx::set_error;
 using orbx::csr_ok;
 using orbx::all_distinct;
+using orbx::segment;
 
 constexpr int WT = 512;
 constexpr unsigned char KF_SKIP = ORBM_KF_BAD | ORBM_KF_OTHER_MAP;   // isBad() || GetMap() != pCurrentMap
@@ -59,28 +60,6 @@ struct Map {
 
 // What the finish kernel reads of the solve: status (LBA_LOCAL_*), solved (0: nothing was optimised), the slot's results.
 struct Solve { int status, solved; lba::SlotOut r; };
-
-// the segment r of base [0..R] (ascending, base[0] = 0, base[R] > q) with base[r] <= q < base[r + 1]
-__device__ __forceinline__ int segment(const int* base, int R, int q) {
-    int lo = 0, hi = R;
-    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (base[mid] <= q) lo = mid; else hi = mid; }
-    return lo;
-}
-
-// Numbers the positions q in [0, Q) with flag(q) in order: emit(q, rank).  Returns the count.  All threads.
-template <class Flag, class Emit>
-__device__ int compact(int Q, int* sm, Flag flag, Emit emit) {
-    int carry = 0;
-    for (int b = 0; b < Q; b += WT) {
-        const int q = b + (int)threadIdx.x;
-        const bool f = q < Q && flag(q);
-        int tot;
-        const int r = orbx::block_scan_excl<WT>(f ? 1 : 0, sm, tot);
-        if (f) emit(q, carry + r);
-        carry += tot;
-    }
-    return carry;
-}
 
 // ascending bitonic sort of key / val [n2], n2 a power of two, in global memory.  All threads.
 __device__ void bitonic(unsigned long long* key, int* val, int n2) {
@@ -134,7 +113,7 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     };
     for (int q = tid; q < Qs; q += WT) { const int p = slotPt(q); if (p >= 0) atomicMin(&M.firstPt[p], q); }
     __syncthreads();
-    const int nL = compact(Qs, sm, [&](int q) { const int p = slotPt(q); return p >= 0 && M.firstPt[p] == q; },
+    const int nL = orbx::compact<WT>(Qs, sm, [&](int q) { const int p = slotPt(q); return p >= 0 && M.firstPt[p] == q; },
                            [&](int q, int r) { M.localPoint[r] = slotPt(q); });
     __syncthreads();
     // lFixedCameras: first appearance over (local point, observation) of the unmarked observers, kept when good and in the current map
@@ -146,7 +125,7 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
         if (M.kfRank[k] == -1 && !(M.kfFlags[k] & KF_SKIP)) atomicMin(&M.firstFix[k], q);
     }
     __syncthreads();
-    const int nFix = compact(Qo, sm, [&](int q) { const int k = M.obsKF[obsAt(q)]; return M.kfRank[k] == -1 && M.firstFix[k] == q; },
+    const int nFix = orbx::compact<WT>(Qo, sm, [&](int q) { const int k = M.obsKF[obsAt(q)]; return M.kfRank[k] == -1 && M.firstFix[k] == q; },
                              [&](int q, int r) { M.fixedKF[r] = M.obsKF[obsAt(q)]; });
     __syncthreads();
     const int numFixed = nFix + s_init;
@@ -191,7 +170,7 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     }
     __syncthreads();
     // edges in insertion order: local points in list order, observations in key order, observers good and in the current map
-    const int nE = compact(Qo, sm, [&](int q) { return !(M.kfFlags[M.obsKF[obsAt(q)]] & KF_SKIP); }, [&](int q, int e) {
+    const int nE = orbx::compact<WT>(Qo, sm, [&](int q) { return !(M.kfFlags[M.obsKF[obsAt(q)]] & KF_SKIP); }, [&](int q, int e) {
         const int r = segment(M.lpBase, nL, q);
         const int p = M.localPoint[r], o = M.obsStart[p] + q - M.lpBase[r], k = M.obsKF[o];
         M.bEPt[e] = M.ptVert[p]; M.bEPose[e] = M.kfVert[k];
@@ -268,41 +247,20 @@ __global__ void __launch_bounds__(WT) local_ba_finish_kernel(const Map* __restri
     // per local point: the outlier test and the erase loop (:1417-1460) in edge order -- the point's observations in key order, points
     // being independent -- then SetWorldPos and UpdateNormalAndDepth (:1474-1481)
     for (int i = tid; i < nL; i += WT) {
-        const int p = M.localPoint[i], o0 = M.obsStart[p], o1 = M.obsStart[p + 1];
-        int nObs = o1 - o0, ref = M.refKF[p];
-        bool bad = false;
-        for (int o = o0; o < o1; ++o) {
-            const int e = M.obsEdge[o];
-            if (e < 0) continue;
-            const double chi2 = V.solved ? V.r.chi2[e] : 0.0;
-            const uint8_t dpos = V.solved ? V.r.depthPos[e] : 1;
-            if (M.edgeChi2) { M.edgeChi2[o] = chi2; M.edgeDepthPos[o] = dpos; }
-            const bool erase = chi2 > 5.991 || !dpos;
-            M.obsFlag[o] = erase ? LBA_OBS_ERASED : LBA_OBS_KEPT;
-            if (!erase || bad) continue;               // EraseObservation of a bad point finds no observation
-            --nObs;
-            if (M.obsKF[o] == ref) {                   // mpRefKF = mObservations.begin()->first
-                ref = -1;
-                for (int j = o0; j < o1 && ref < 0; ++j)
-                    if (M.obsFlag[j] != LBA_OBS_ERASED) ref = M.obsKF[j];
-            }
-            if (nObs <= 2) bad = true;                 // SetBadFlag: the observations are cleared
-        }
+        const int p = M.localPoint[i];
         double X[3];
         pointOf(i, X);
         if (M.optPoint) for (int c = 0; c < 3; ++c) M.optPoint[3 * i + c] = X[c];
         float pos[3] = {(float)X[0], (float)X[1], (float)X[2]};
         for (int c = 0; c < 3; ++c) M.pointPos[3 * i + c] = pos[c];
-        M.pointBad[i] = bad; M.pointRefKF[i] = ref;
-        if (bad || o1 == o0) continue;                 // UpdateNormalAndDepth returns on a bad point or an empty mObservations
-        int o = o0;
-        auto next = [&](int& k, int& oct) {
-            while (o < o1 && M.obsFlag[o] == LBA_OBS_ERASED) ++o;
-            if (o == o1) return false;
-            k = M.obsKF[o]; oct = M.obsOctave[o]; ++o;
-            return true;
-        };
-        orbx::update_normal_and_depth(pos, M.Ow2, ref, M.scaleFactors, M.nlevels, next, M.normal + 3 * i, M.minDistance + i, M.maxDistance + i);
+        orbx::finish_point(M.obsKF, M.obsOctave, M.obsStart[p], M.obsStart[p + 1], M.obsFlag, M.refKF[p], [&](int o) -> uint8_t {
+            const int e = M.obsEdge[o];
+            if (e < 0) return LBA_OBS_NO_EDGE;
+            const double chi2 = V.solved ? V.r.chi2[e] : 0.0;
+            const uint8_t dpos = V.solved ? V.r.depthPos[e] : 1;
+            if (M.edgeChi2) { M.edgeChi2[o] = chi2; M.edgeDepthPos[o] = dpos; }
+            return chi2 > 5.991 || !dpos ? LBA_OBS_ERASED : LBA_OBS_KEPT;
+        }, pos, M.Ow2, M.scaleFactors, M.nlevels, M.pointBad + i, M.pointRefKF + i, M.normal + 3 * i, M.minDistance + i, M.maxDistance + i);
     }
 }
 

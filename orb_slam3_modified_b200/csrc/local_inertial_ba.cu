@@ -89,6 +89,12 @@ __global__ void __launch_bounds__(NT) local_inertial_ba_kernel(const Dev* __rest
     }
 }
 
+// One CTA per problem of the device table probs [count]; local_inertial_ba_map.cu launches it on problems its walk kernel built.
+cudaError_t launch_solver(const Dev* probs, int count, cudaStream_t st) {
+    local_inertial_ba_kernel<<<count, NT, 0, st>>>(probs);
+    return cudaGetLastError();
+}
+
 }  // namespace liba
 
 extern "C" int local_inertial_ba_batch(int count, const LocalInertialBAProblem* problems, const LocalInertialBAResult* results, int32_t* iterationsOut, int device) {
@@ -136,8 +142,7 @@ extern "C" int local_inertial_ba_batch(int count, const LocalInertialBAProblem* 
     const double msPack = ms_since(tStart);
     const auto tGpu = std::chrono::steady_clock::now();
     CK(S->upload(S->stream));
-    local_inertial_ba_kernel<<<count, NT, 0, S->stream>>>(S->dev<const Dev>(pDev));
-    CK(cudaGetLastError());
+    CK(launch_solver(S->dev<const Dev>(pDev), count, S->stream));
     CK(S->download(S->stream));
     const double msGpu = ms_since(tGpu);
     for (int i = 0; i < count; ++i) {
