@@ -1087,6 +1087,73 @@ int orbv_transform_batch_device(orbv_handle* h, int batch, const uint8_t* d_desc
                                 double* d_scratchWeight, int* d_scratchNode, int* d_wordId, double* d_wordValue, int* d_nWords, int* d_fvNode,
                                 int* d_fvFeature, int* d_nEntries, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * KeyFrameDatabase (src/KeyFrameDatabase.cc): the inverted file on the device, and phase 1 of DetectRelocalizationCandidates
+ * (Tracking::Relocalization) and DetectNBestCandidates (LoopClosing::NewDetectCommonRegions) -- the walk over the inverted-file lists
+ * of the query's words and the L1Scoring::score of the keyframes that share more than minCommonWords -- for a batch of queries.
+ * Phase 2 (accumulation over GetBestCovisibilityKeyFrames(10), the sort and the selection) stays with the caller (INTEGRATION.md §2).
+ * One handle serves maxDatabases databases (one per SLAM system) from one pool of maxKeyFrames keyframes of at most maxWords words.
+ * Scoring is L1Scoring, what ORBvoc.txt's header declares and ORB-SLAM3 uses; vocabularyWords = mpVoc->size() bounds the word ids.
+ * A keyframe is a caller key unique within its database, such as (uint64_t)KeyFrame*; a BowVector is its (id, value) pairs with
+ * ascending ids, as orbv_transform_batch returns them.  Host pointers throughout.
+ * THREADS: the staging buffers, the slot pool and the launch count belong to the handle, not to one database, so the handle serialises
+ * its calls: every orbv_db_* entry point holds the handle's mutex for the whole call, and threads of different SLAM systems may call
+ * one handle at once.  The caller keeps the reference's per-database mMutex around a detection and the replay of its record (the
+ * marks, counters and scores live in its KeyFrame objects; INTEGRATION.md §2).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct orbv_db_handle orbv_db_handle;
+/* ORB_ERR_ARG for a size < 1 or maxWords > 8192; ORB_ERR_CUDA without an sm_90 device. */
+int orbv_db_create(orbv_db_handle** out, int vocabularyWords, int maxDatabases, int maxKeyFrames, int maxWords, int device);
+void orbv_db_destroy(orbv_db_handle* h);
+/* add(pKF) for n keyframes, in array order: keyframe i goes to database dbIndex[i] with the BowVector wordId / wordValue
+ * [wordStart[i], wordStart[i + 1]).  One upload, one launch.  ORB_ERR_ARG before anything changes: a database index out of range, a
+ * key already in its database or added twice by the call (the reference would list that keyframe twice), more than maxWords words, a
+ * word id outside [0, vocabularyWords), ids that do not ascend, a wordStart that does not start at 0 or decreases, a null pointer.
+ * ORB_ERR_CAPACITY: fewer than n free slots.  A call that fails leaves the database and the free slots as they were. */
+int orbv_db_add_batch(orbv_db_handle* h, int n, const int32_t* dbIndex, const uint64_t* key, const int32_t* wordStart, const int32_t* wordId,
+                      const double* wordValue);
+/* erase(pKF) for n keyframes: a key not in its database is a no-op, as in the reference.  clearMap(pMap) is this call with the map's
+ * keyframes: the entries that remain keep their relative order either way.  No launch. */
+int orbv_db_erase_batch(orbv_db_handle* h, int n, const int32_t* dbIndex, const uint64_t* key);
+/* clear(): empties one database.  No launch. */
+int orbv_db_clear(orbv_db_handle* h, int dbIndex);
+/* The number of keyframes in a database (ORB_ERR_ARG for an index out of range). */
+int orbv_db_size(const orbv_db_handle* h, int dbIndex);
+enum { ORBV_DB_RELOC = 0, ORBV_DB_NBEST = 1 };
+/* One query.  kind ORBV_DB_RELOC: DetectRelocalizationCandidates(F, pMap) with F->mBowVec; ORBV_DB_NBEST: DetectNBestCandidates(pKF, ...)
+ * with pKF->mBowVec and the keys of pKF->GetConnectedKeyFrames() (keys not in the database are ignored).
+ * Outputs: lKFsSharingWords in the reference's order, the first min(nSharing, cap) entries: key, words = the mnRelocWords /
+ * mnPlaceRecognitionWords counter, scored = words > minCommonWords (the entry is in lScoreAndMatch), score = the float mRelocScore /
+ * mPlaceRecognitionScore of a scored entry (0 otherwise); entries past that are 0.  nSharing = |lKFsSharingWords|,
+ * maxCommonWords = the largest counter (0 when the list is empty; minCommonWords = (int)(maxCommonWords * 0.8f)). */
+typedef struct OrbvDbQuery {
+    int32_t dbIndex;
+    int32_t kind;                  /* ORBV_DB_RELOC or ORBV_DB_NBEST */
+    int32_t nWords;
+    const int32_t* wordId;         /* [nWords] ascending */
+    const double* wordValue;       /* [nWords] */
+    int32_t nConnected;            /* NBEST only */
+    const uint64_t* connected;     /* [nConnected] NBEST only */
+    int32_t cap;
+    uint64_t* key;                 /* [cap] out */
+    int32_t* words;                /* [cap] out */
+    uint8_t* scored;               /* [cap] out */
+    float* score;                  /* [cap] out */
+    int32_t* nSharing;             /* [1] out */
+    int32_t* maxCommonWords;       /* [1] out */
+} OrbvDbQuery;
+/* Phase 1 of every query, mixing kinds and databases: one upload through the handle's staging, three launches whatever nQueries
+ * (orbv_db_last_launch_count; 0 for nQueries == 0), one download.  Scores equal L1Scoring::score bit for bit: the common words' terms
+ * fabs(vi - wi) - fabs(vi) - fabs(wi) are added in ascending word order in double, then -score / 2.0 is rounded to float.
+ * PRECONDITIONS, as the reference's walk needs them: no keyframe of the database carries the query's mark (mnRelocQuery /
+ * mnPlaceRecognitionQuery == the query's mnId) at the call, and a keyframe's mBowVec does not change while it is in the database.
+ * ORB_ERR_ARG before any launch: nQueries outside [0, 2^24 - 1], a database index out of range, an unknown kind, a negative cap or nConnected, a word id outside
+ * [0, vocabularyWords), ids that do not ascend, more than maxWords words, a null pointer.  ORB_ERR_CAPACITY after the call: a query
+ * with nSharing > cap (its outputs hold the first cap entries, nSharing and maxCommonWords are exact). */
+int orbv_db_query_batch(orbv_db_handle* h, int nQueries, const OrbvDbQuery* q);
+/* Kernel launches of the handle's last add / erase / clear / query call. */
+int orbv_db_last_launch_count(const orbv_db_handle* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,6 +4,7 @@
 //   ORB_SLAM3::ORBextractor   reference include/ORBextractor.h:43-109
 //   ORB_SLAM3::ORBmatcher     reference include/ORBmatcher.h:36-103   (per-frame hot functions)
 //   ORB_SLAM3::Optimizer      reference include/Optimizer.h:46-102    (LocalBundleAdjustment numeric core)
+//   ORB_SLAM3::KeyFrameDatabase  reference include/KeyFrameDatabase.h  (the inverted file and phase 1 of both detections, over keys)
 #pragma once
 #include <cstdint>
 #include <stdexcept>
@@ -347,6 +348,47 @@ public:
     static void LocalInertialBABatch(int nMaps, const LocalInertialBAMap* maps, int device = 0) {
         orb_check(local_inertial_ba_map_batch(nMaps, maps, device), "local_inertial_ba_map_batch");
     }
+};
+
+// KeyFrameDatabase over caller keys (such as (uint64_t)KeyFrame*), the inverted file resident on the device; one object serves
+// maxDatabases databases, one per SLAM system.  add / erase / clear are the reference's members for one database; clearMap(pMap) is
+// erase of the map's keyframes.  QueryBatch runs phase 1 of DetectRelocalizationCandidates / DetectNBestCandidates for a batch of
+// queries; the caller replays the records onto its keyframes and keeps the reference's phase 2 (INTEGRATION.md §2).  The reference's
+// mMutex stays with the caller: Tracking and LoopClosing share one database.
+class KeyFrameDatabase {
+public:
+    struct BowVector { std::vector<int32_t> id; std::vector<double> value; };   // DBoW2::BowVector in map order
+    KeyFrameDatabase(int vocabularyWords, int maxDatabases, int maxKeyFrames, int maxWords, int device = 0) {
+        orb_check(orbv_db_create(&h_, vocabularyWords, maxDatabases, maxKeyFrames, maxWords, device), "orbv_db_create");
+    }
+    ~KeyFrameDatabase() { orbv_db_destroy(h_); }
+    KeyFrameDatabase(const KeyFrameDatabase&) = delete;
+    KeyFrameDatabase& operator=(const KeyFrameDatabase&) = delete;
+
+    void add(int db, uint64_t key, const BowVector& bow) { add(std::vector<int32_t>{db}, std::vector<uint64_t>{key}, std::vector<BowVector>{bow}); }
+    // add(pKF) for each keyframe, in order
+    void add(const std::vector<int32_t>& db, const std::vector<uint64_t>& keys, const std::vector<BowVector>& bows) {
+        std::vector<int32_t> start(1, 0), id;
+        std::vector<double> value;
+        for (const BowVector& b : bows) {
+            id.insert(id.end(), b.id.begin(), b.id.end());
+            value.insert(value.end(), b.value.begin(), b.value.end());
+            start.push_back((int32_t)id.size());
+        }
+        orb_check(orbv_db_add_batch(h_, (int)keys.size(), db.data(), keys.data(), start.data(), id.data(), value.data()), "orbv_db_add_batch");
+    }
+    void erase(int db, uint64_t key) { erase(std::vector<int32_t>{db}, std::vector<uint64_t>{key}); }
+    void erase(const std::vector<int32_t>& db, const std::vector<uint64_t>& keys) {
+        orb_check(orbv_db_erase_batch(h_, (int)keys.size(), db.data(), keys.data()), "orbv_db_erase_batch");
+    }
+    void clear(int db) { orb_check(orbv_db_clear(h_, db), "orbv_db_clear"); }
+    void QueryBatch(const std::vector<OrbvDbQuery>& queries) {
+        orb_check(orbv_db_query_batch(h_, (int)queries.size(), queries.data()), "orbv_db_query_batch");
+    }
+    orbv_db_handle* handle() { return h_; }
+
+private:
+    orbv_db_handle* h_ = nullptr;
 };
 
 }  // namespace ORB_SLAM3

@@ -137,6 +137,15 @@ SIGNATURES = {
     'orbv_create': (_i, [_out, _vp, _i]),
     'orbv_destroy': (None, [_vp]),
     'orbv_transform_batch': (_i, [_vp, _i, _vp, _vp, _i, _i] + [_vp] * 6),
+    # KeyFrameDatabase
+    'orbv_db_create': (_i, [_out, _i, _i, _i, _i, _i]),
+    'orbv_db_destroy': (None, [_vp]),
+    'orbv_db_add_batch': (_i, [_vp, _i] + [_vp] * 5),
+    'orbv_db_erase_batch': (_i, [_vp, _i, _vp, _vp]),
+    'orbv_db_clear': (_i, [_vp, _i]),
+    'orbv_db_size': (_i, [_vp, _i]),
+    'orbv_db_query_batch': (_i, [_vp, _i, _vp]),
+    'orbv_db_last_launch_count': (_i, [_vp]),
 }
 
 _lib = None
@@ -1734,6 +1743,7 @@ class ORBVocabulary:
 
     def __init__(self, L, child_start, children, desc, weight, word_id, weighting=0, norm=1, device=0):
         self._keep = [_c(child_start, np.int32), _c(children, np.int32), _c(desc, np.uint8), _c(weight, np.float64), _c(word_id, np.int32)]
+        self.n_words = int((self._keep[4] >= 0).sum())     # mpVoc->size()
         s = _OrbVocabulary(len(self._keep[4]), int(L), int(weighting), int(norm), *[a.ctypes.data for a in self._keep])
         self._h = C.c_void_p()
         rc = lib().orbv_create(C.byref(self._h), C.byref(s), device)
@@ -1767,3 +1777,105 @@ class ORBVocabulary:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbv_transform_batch')
         return [(wid[b, :nw[b]].copy(), wv[b, :nw[b]].copy(), fn[b, :ne[b]].copy(), ff[b, :ne[b]].copy()) for b in range(B)]
+
+
+#: OrbvDbQuery's kinds (ORBV_DB_*, include/orb_b200.h)
+DB_RELOC, DB_NBEST = 0, 1
+
+
+class OrbvDbQuery(C.Structure):
+    """One query of orbv_db_query_batch (include/orb_b200.h)."""
+    _fields_ = [('dbIndex', C.c_int32), ('kind', C.c_int32), ('nWords', C.c_int32), ('wordId', C.c_void_p), ('wordValue', C.c_void_p),
+                ('nConnected', C.c_int32), ('connected', C.c_void_p), ('cap', C.c_int32)] + \
+               [(n, C.c_void_p) for n in ('key', 'words', 'scored', 'score', 'nSharing', 'maxCommonWords')]
+
+
+def db_query_struct(q, cap):
+    """OrbvDbQuery over query dict `q` (db, kind, word_id, word_value, connected = keys or None) with fresh outputs of width `cap`:
+    (struct, out dict, arrays to keep alive)."""
+    wid, wv = _c(q['word_id'], np.int32), _c(q['word_value'], np.float64)
+    conn = _c(q['connected'] if q.get('connected') is not None else np.zeros(0), np.uint64)
+    out = dict(key=np.zeros(cap, np.uint64), words=np.zeros(cap, np.int32), scored=np.zeros(cap, np.uint8), score=np.zeros(cap, np.float32),
+               nSharing=np.zeros(1, np.int32), maxCommonWords=np.zeros(1, np.int32))
+    s = OrbvDbQuery(int(q['db']), int(q['kind']), len(wid), _ptr(wid), _ptr(wv), len(conn), _ptr(conn), cap,
+                    *[_ptr(out[n]) for n in ('key', 'words', 'scored', 'score', 'nSharing', 'maxCommonWords')])
+    return s, out, (wid, wv, conn)
+
+
+class KeyFrameDatabase:
+    """Mirror of ``ORB_SLAM3::KeyFrameDatabase`` over keys: the inverted file on the device (orbv_db_*), ``maxDatabases`` databases in one
+    handle.  ``voc`` is the vocabulary's word count (``mpVoc->size()``) or an :class:`ORBVocabulary`.  A BowVector is (word ids ascending,
+    values), as :meth:`ORBVocabulary.transform` returns it.  :meth:`query_batch` runs phase 1 of ``DetectRelocalizationCandidates`` /
+    ``DetectNBestCandidates``; phase 2 stays with the caller (INTEGRATION.md §2)."""
+
+    def __init__(self, voc, max_databases=1, max_keyframes=1024, max_words=2048, device=0):
+        words = voc.n_words if isinstance(voc, ORBVocabulary) else int(voc)
+        self.max_keyframes = int(max_keyframes)
+        self._h = C.c_void_p()
+        rc = lib().orbv_db_create(C.byref(self._h), words, int(max_databases), self.max_keyframes, int(max_words), device)
+        if rc != ORB_OK:
+            self._h = None
+            raise OrbError(rc, 'orbv_db_create')
+
+    def close(self):
+        if getattr(self, '_h', None):
+            lib().orbv_db_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, db, keys, bows):
+        """``add(pKF)`` for each keyframe in order: ``db`` an index or one per key, ``keys`` uint64, ``bows`` [(word ids, values)]."""
+        keys = _c(keys, np.uint64)
+        dbs = _c(np.broadcast_to(np.asarray(db, np.int32), keys.shape), np.int32)
+        start = np.zeros(len(keys) + 1, np.int32)
+        start[1:] = np.cumsum([len(b[0]) for b in bows]) if len(bows) else []
+        wid = _c(np.concatenate([np.asarray(b[0], np.int32) for b in bows]) if len(bows) else np.zeros(0), np.int32)
+        wv = _c(np.concatenate([np.asarray(b[1], np.float64) for b in bows]) if len(bows) else np.zeros(0), np.float64)
+        rc = lib().orbv_db_add_batch(self._h, len(keys), _ptr(dbs), _ptr(keys), _ptr(start), _ptr(wid), _ptr(wv))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbv_db_add_batch')
+
+    def erase(self, db, keys):
+        """``erase(pKF)`` for each key (absent keys are no-ops); ``clearMap(pMap)`` is this with the map's keyframes."""
+        keys = _c(keys, np.uint64)
+        dbs = _c(np.broadcast_to(np.asarray(db, np.int32), keys.shape), np.int32)
+        rc = lib().orbv_db_erase_batch(self._h, len(keys), _ptr(dbs), _ptr(keys))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbv_db_erase_batch')
+
+    def clear(self, db=0):
+        rc = lib().orbv_db_clear(self._h, int(db))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbv_db_clear')
+
+    def size(self, db=0):
+        n = lib().orbv_db_size(self._h, int(db))
+        if n < 0:
+            raise OrbError(n, 'orbv_db_size')
+        return n
+
+    def last_launch_count(self):
+        return lib().orbv_db_last_launch_count(self._h)
+
+    def query_batch(self, queries, cap=None):
+        """Phase 1 of every query in one call (orbv_db_query_batch).  Each query is a dict(db, kind = DB_RELOC or DB_NBEST, word_id,
+        word_value, connected = the keys of GetConnectedKeyFrames() for DB_NBEST).  Returns per query dict(key, words, scored, score) in
+        lKFsSharingWords order, nSharing and maxCommonWords.  ``cap`` defaults to max_keyframes (never exceeded)."""
+        cap = self.max_keyframes if cap is None else int(cap)
+        built = [db_query_struct(q, cap) for q in queries]
+        arr = (OrbvDbQuery * max(len(built), 1))(*[b[0] for b in built])
+        rc = lib().orbv_db_query_batch(self._h, len(built), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbv_db_query_batch')
+        res = []
+        for _, out, _ in built:
+            n = int(out['nSharing'][0])
+            r = {k: out[k][:n].copy() for k in ('key', 'words', 'scored', 'score')}
+            r.update(nSharing=n, maxCommonWords=int(out['maxCommonWords'][0]))
+            res.append(r)
+        return res
