@@ -1074,15 +1074,24 @@ typedef struct OrbVocabulary {
     const double* weight;         /* [nNodes]: m_nodes[n].weight (idf of a word; 0 = stopped) */
     const int32_t* wordId;        /* [nNodes]: m_nodes[n].word_id for leaves, -1 otherwise */
 } OrbVocabulary;
+/* ORB_ERR_ARG, before anything is uploaded: nNodes < 2, L < 1, weighting outside [0, 3], norm outside [0, 2], a null pointer, a root
+ * (node 0) without children, a childStart that does not start at 0 or decreases, a node with more than 2^20 children, a child index
+ * outside [1, nNodes), a node listed as a child more than once (so a table with a cycle is refused: with the root nobody's child and
+ * every other node at most one node's, the nodes the descent can reach form a tree), or a leaf with a negative wordId.  A leaf is a node
+ * without children; a stopped word is a leaf with weight 0. */
 int orbv_create(orbv_handle** out, const OrbVocabulary* voc, int device);
 void orbv_destroy(orbv_handle* h);
 /* transform() for `batch` frames; frame f has n[f] descriptors in desc [batch][cap][32].  Outputs in the iteration order of the reference's
  * std::map containers: BowVector as wordId / wordValue [batch][cap] (nWords[f] entries, ascending word id; values are DBoW2's doubles bit
  * for bit), FeatureVector as parallel arrays fvNode / fvFeature [batch][cap] (nEntries[f] entries: ascending node id, feature indices
- * ascending within a node).  levelsup = 4 in the reference.  Host pointers. */
+ * ascending within a node).  A feature whose leaf lies above depth L - levelsup is filed under node 0 (the reference leaves that node id
+ * unset).  levelsup = 4 in the reference.  Host pointers.  ORB_ERR_ARG before anything is staged: batch < 1, cap outside [1, 16384],
+ * levelsup < 0, n[f] outside [0, cap], or a null pointer. */
 int orbv_transform_batch(orbv_handle* h, int batch, const uint8_t* desc, const int32_t* n, int cap, int levelsup, int32_t* wordId, double* wordValue,
                          int32_t* nWords, int32_t* fvNode, int32_t* fvFeature, int32_t* nEntries);
-/* Device form: all pointers device pointers; d_scratch* are [batch][cap] work arrays owned by the caller; enqueues on `stream`. */
+/* Device form: all pointers device pointers; d_scratch* are [batch][cap] work arrays owned by the caller; enqueues on `stream`.
+ * ORB_ERR_ARG before any launch: batch < 1, cap outside [1, 16384], levelsup < 0, or a null pointer.  d_n is read on the device only,
+ * where a count above cap stands for cap and a negative one for 0. */
 int orbv_transform_batch_device(orbv_handle* h, int batch, const uint8_t* d_desc, const int* d_n, int cap, int levelsup, int* d_scratchWord,
                                 double* d_scratchWeight, int* d_scratchNode, int* d_wordId, double* d_wordValue, int* d_nWords, int* d_fvNode,
                                 int* d_fvFeature, int* d_nEntries, void* stream);

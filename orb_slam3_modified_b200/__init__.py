@@ -137,6 +137,7 @@ SIGNATURES = {
     'orbv_create': (_i, [_out, _vp, _i]),
     'orbv_destroy': (None, [_vp]),
     'orbv_transform_batch': (_i, [_vp, _i, _vp, _vp, _i, _i] + [_vp] * 6),
+    'orbv_transform_batch_device': (_i, [_vp, _i, _vp, _vp, _i, _i] + [_vp] * 10),
     # KeyFrameDatabase
     'orbv_db_create': (_i, [_out, _i, _i, _i, _i, _i]),
     'orbv_db_destroy': (None, [_vp]),
@@ -1777,6 +1778,27 @@ class ORBVocabulary:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbv_transform_batch')
         return [(wid[b, :nw[b]].copy(), wv[b, :nw[b]].copy(), fn[b, :ne[b]].copy(), ff[b, :ne[b]].copy()) for b in range(B)]
+
+    def transform_device(self, d_desc, d_n, levelsup, scratch, out, stream=0):
+        """Device form of :meth:`transform` (orbv_transform_batch_device) on torch CUDA tensors: d_desc [B, cap, 32] u8, d_n [B] i32;
+        ``scratch`` = (word i32, weight f64, node i32), each [B, cap]; ``out`` = (word_id [B, cap] i32, word_value [B, cap] f64,
+        n_words [B] i32, fv_node [B, cap] i32, fv_feature [B, cap] i32, n_entries [B] i32), rows laid out as :meth:`transform` returns
+        them.  Enqueues on ``stream`` and returns immediately."""
+        import torch
+        if len(scratch) != 3 or len(out) != 6:
+            raise ValueError('transform_device: scratch takes 3 tensors and out 6')
+        B, cap = d_desc.shape[0], d_desc.shape[1]
+        want = [(d_desc, torch.uint8, (B, cap, 32)), (d_n, torch.int32, (B,))] + \
+            [(t, dt, (B, cap)) for t, dt in zip(scratch, (torch.int32, torch.float64, torch.int32))] + \
+            [(t, dt, sh) for t, dt, sh in zip(out, (torch.int32, torch.float64, torch.int32, torch.int32, torch.int32, torch.int32),
+                                              ((B, cap), (B, cap), (B,), (B, cap), (B, cap), (B,)))]
+        for k, (t, dt, sh) in enumerate(want):
+            if not t.is_cuda or t.dtype != dt or tuple(t.shape) != sh or not t.is_contiguous():
+                raise ValueError('transform_device: operand %d must be a contiguous CUDA %s tensor of shape %s' % (k, dt, sh))
+        rc = lib().orbv_transform_batch_device(self._h, B, _ptr(d_desc), _ptr(d_n), cap, int(levelsup), *[_ptr(t) for t in scratch],
+                                               *[_ptr(t) for t in out], C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbv_transform_batch_device')
 
 
 #: OrbvDbQuery's kinds (ORBV_DB_*, include/orb_b200.h)

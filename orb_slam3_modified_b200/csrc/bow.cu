@@ -13,6 +13,7 @@
 #include <math.h>
 #include <string.h>
 #include <string>
+#include <vector>
 
 #include "../../include/orb_b200.h"
 #include "device_utils.cuh"
@@ -71,6 +72,7 @@ __global__ void __launch_bounds__(BD_NT) bow_descend_kernel(Voc V, int batch, in
 }
 
 constexpr int BA_NT = 512;
+constexpr int MAX_CAP = 16384;   // bow_assemble_kernel sorts a frame in shared memory: 12 * 16384 B = 192 KiB
 __device__ void bitonic_sort(unsigned long long* k, int n2) {   // n2: power of two, all threads of the CTA
     for (int size = 2; size <= n2; size <<= 1)
         for (int stride = size >> 1; stride > 0; stride >>= 1) {
@@ -164,7 +166,16 @@ int orbv_create(orbv_handle** out, const OrbVocabulary* voc, int device) {
     if (voc->childStart[0] != 0 || voc->childStart[1] <= 0) { set_error("orbv_create: node 0 must be the root and have children"); return ORB_ERR_ARG; }
     const int nChildren = voc->childStart[n];
     for (int i = 0; i < n; ++i) if (voc->childStart[i + 1] < voc->childStart[i]) { set_error("orbv_create: childStart must be non-decreasing"); return ORB_ERR_ARG; }
+    for (int i = 0; i < n; ++i)    // bow_descend_kernel packs a child's list position into 20 bits
+        if (voc->childStart[i + 1] - voc->childStart[i] > (1 << 20)) { set_error("orbv_create: a node has more than 2^20 children"); return ORB_ERR_ARG; }
     for (int c = 0; c < nChildren; ++c) if (voc->children[c] <= 0 || voc->children[c] >= n) { set_error("orbv_create: child index out of range"); return ORB_ERR_ARG; }
+    // The root is nobody's child (above) and every other node the child of at most one list entry, so the nodes reachable from the root
+    // form a tree and the descent reaches a leaf within nNodes steps.  A table with a cycle fails this test.
+    std::vector<uint8_t> listed(n, 0);
+    for (int c = 0; c < nChildren; ++c)
+        if (listed[voc->children[c]]++) { set_error("orbv_create: a node is listed as a child more than once"); return ORB_ERR_ARG; }
+    for (int i = 1; i < n; ++i)    // the kernels would drop a negative word id's features where DBoW2 files them under (unsigned)id
+        if (voc->childStart[i + 1] == voc->childStart[i] && voc->wordId[i] < 0) { set_error("orbv_create: a leaf has a negative wordId"); return ORB_ERR_ARG; }
     if (int rc = orbx::check_device(device)) return rc;
     CK(cudaSetDevice(device));
     orbv_handle* h = new orbv_handle();
@@ -191,7 +202,7 @@ void orbv_destroy(orbv_handle* h) { delete h; }
 
 int orbv_transform_batch_device(orbv_handle* h, int batch, const uint8_t* d_desc, const int* d_n, int cap, int levelsup, int* d_scratchWord, double* d_scratchWeight,
                                 int* d_scratchNode, int* d_wordId, double* d_wordValue, int* d_nWords, int* d_fvNode, int* d_fvFeature, int* d_nEntries, void* stream) {
-    if (!h || batch < 1 || cap < 1 || cap > 16384 || !d_desc || !d_n || !d_scratchWord || !d_scratchWeight || !d_scratchNode || !d_wordId || !d_wordValue || !d_nWords ||
+    if (!h || batch < 1 || cap < 1 || cap > MAX_CAP || !d_desc || !d_n || !d_scratchWord || !d_scratchWeight || !d_scratchNode || !d_wordId || !d_wordValue || !d_nWords ||
         !d_fvNode || !d_fvFeature || !d_nEntries || levelsup < 0) { set_error("orbv_transform_batch_device: bad argument (cap <= 16384)"); return ORB_ERR_ARG; }
     Vocabulary& v = h->v;
     CK(cudaSetDevice(v.device));
@@ -209,7 +220,10 @@ int orbv_transform_batch_device(orbv_handle* h, int batch, const uint8_t* d_desc
 
 int orbv_transform_batch(orbv_handle* h, int batch, const uint8_t* desc, const int32_t* n, int cap, int levelsup, int32_t* wordId, double* wordValue, int32_t* nWords,
                          int32_t* fvNode, int32_t* fvFeature, int32_t* nEntries) {
-    if (!h || batch < 1 || cap < 1 || !desc || !n || !wordId || !wordValue || !nWords || !fvNode || !fvFeature || !nEntries) { set_error("orbv_transform_batch: bad argument"); return ORB_ERR_ARG; }
+    if (!h || batch < 1 || cap < 1 || cap > MAX_CAP || !desc || !n || !wordId || !wordValue || !nWords || !fvNode || !fvFeature || !nEntries || levelsup < 0) {
+        set_error("orbv_transform_batch: bad argument (cap <= 16384)"); return ORB_ERR_ARG;
+    }
+    if (int rc = orbx::check_row_counts("orbv_transform_batch", n, batch, cap)) return rc;
     Vocabulary& v = h->v;
     CK(cudaSetDevice(v.device));
     const size_t B = batch, K = cap;
