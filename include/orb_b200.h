@@ -754,6 +754,10 @@ int orbm_bf_knn2(orbm_handle* h, const uint8_t* query, int Q, const uint8_t* tra
 /* ORBmatcher::DescriptorDistance (src/ORBmatcher.cc:2058-2074) for n descriptor pairs a[i], b[i]; n is unbounded.  Host pointers. */
 int orbm_descriptor_distance(orbm_handle* h, const uint8_t* a, const uint8_t* b, int n, int32_t* out);
 int orbm_last_launch_count(const orbm_handle* h);
+/* Thread-block-cluster size (CTAs per frame, 1..8) of the handle's last SearchByProjection or SearchForInitialization launch.  For
+ * SearchByProjection it is the largest size with batch x size <= 2 x SMs whose clusters are all resident at once, for the call's batch
+ * and shared-memory size; SearchForInitialization always uses 8.  A refused call leaves it unchanged (and orbm_last_launch_count() is 0). */
+int orbm_last_cluster_size(const orbm_handle* h);
 
 /* ------------------------------------------------------------------------------------------
  * Optimizer::LocalBundleAdjustment (reference include/Optimizer.h:71, src/Optimizer.cc:1116-1498): the numeric

@@ -107,6 +107,7 @@ SIGNATURES = {
     'orbm_bf_knn2': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp]),
     'orbm_descriptor_distance': (_i, [_vp, _vp, _vp, _i, _vp]),
     'orbm_last_launch_count': (_i, [_vp]),
+    'orbm_last_cluster_size': (_i, [_vp]),
     # Optimizer
     'lba_create': (_i, [_out, _i, _i, _i, _i]),
     'lba_create_batch': (_i, [_out, _i, _i, _i, _i, _i]),
@@ -1259,6 +1260,10 @@ class ORBmatcher:
 
     def last_launch_count(self):
         return lib().orbm_last_launch_count(self._h)
+
+    def last_cluster_size(self):
+        """CTAs per frame of the last SearchByProjection / SearchForInitialization launch (1..8)."""
+        return lib().orbm_last_cluster_size(self._h)
 
 
 # =============================================================================================

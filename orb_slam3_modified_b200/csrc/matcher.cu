@@ -193,9 +193,11 @@ __device__ __forceinline__ TopK<K> scan_candidates(const MatchParams& P, const F
         const int ny = nMaxCellY - nMinCellY + 1, nx = nMaxCellX - nMinCellX + 1;
         const uint8_t* gdesc = P.desc + (size_t)f * P.kcap * 32;
         const bool bCheckLevels = (minLevel > 0) || (maxLevel >= 0);
-        const unsigned nyMagic = 0xFFFFFFFFu / (unsigned)ny + 1u;          // c / ny by multiply-high (exact: c * ny < 2^32)
+        // c / ny by multiply-high (exact: c * ny < 2^32).  For ny = 1 (a window clipped to the first or last grid row) the magic
+        // wraps to 0, so the quotient is c itself.
+        const unsigned nyMagic = 0xFFFFFFFFu / (unsigned)ny + 1u;
         for (int c = lane; c < nx * ny; c += 32) {
-            const int cq = (int)__umulhi((unsigned)c, nyMagic);
+            const int cq = ny > 1 ? (int)__umulhi((unsigned)c, nyMagic) : c;
             const int ix = nMinCellX + cq, iy = nMinCellY + (c - cq * ny);
             const int cell = ix * GRID_ROWS + iy;
             const int a = S.cellStart[cell], b = S.cellStart[cell + 1];
@@ -1352,8 +1354,9 @@ struct Matcher {
         return ORB_OK;
     }
     // kUse / mUse: the largest keypoint / map-point count any frame of this call can have (the slab capacities when the
-    // counts live on the device): they size the kernel's shared memory.
+    // counts live on the device): they size the kernel's shared memory.  A refused call launches nothing and reports 0 launches.
     int run(MatchParams& P, int kUse, int mUse, cudaStream_t st) {
+        launches = 0;
         P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX);   // src/Frame.cc:342-343
         P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
         P.query = d_query; P.resultIdx = d_resultIdx; P.resultDist = d_resultDist; P.status = d_status;
@@ -1632,6 +1635,7 @@ int orbm_create(orbm_handle** out, int max_batch, int max_keypoints, int max_map
 
 void orbm_destroy(orbm_handle* h) { delete h; }
 int orbm_last_launch_count(const orbm_handle* h) { return h ? h->m.launches : ORB_ERR_ARG; }
+int orbm_last_cluster_size(const orbm_handle* h) { return h ? h->m.lastCluster : ORB_ERR_ARG; }
 #ifdef MF_PHASES
 // out[8]: match_frame_kernel's phase counters (mf_phase) since the last call, which zeroes them; returns the last call's cluster size.
 int orbm_match_phases(const orbm_handle* h, unsigned long long* out) {

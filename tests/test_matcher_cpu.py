@@ -42,21 +42,28 @@ def test_descriptor_distance_properties():
 
 
 def test_features_in_area_bruteforce():
-    kps, _ = S.extract(3)
+    """Frame::GetFeaturesInArea: the set equals a brute-force window test, and the ORDER equals the (cell x, cell y, index) order of
+    matcher_scenes.Cands -- the order breaks ties between equal Hamming distances in every search.  Frames: a seeded one, the
+    keypoints placed on cell ties, and the ones placed just outside undistortion-like bounds."""
+    frames = [(S.extract(3)[0], (0.0, 0.0, 640.0, 480.0), 200)] + [(S.special_scene(n, 0)['kps'], S.special_scene(n, 0)['bounds'], 1000) for n in ('ties', 'edges')]
     rng = np.random.default_rng(4)
-    b = (0.0, 0.0, 640.0, 480.0)
-    for _ in range(200):
-        x, y, r = rng.uniform(-20, 660), rng.uniform(-20, 500), rng.uniform(1, 60)
-        lo, hi = int(rng.integers(-1, 6)), int(rng.integers(-1, 8))
-        got = O.features_in_area(kps, b, x, y, r, lo, hi)
-        x32, y32, r32 = np.float32(x), np.float32(y), np.float32(r)
-        ok = (np.abs(kps['x'] - x32) < r32) & (np.abs(kps['y'] - y32) < r32)
-        if lo > 0 or hi >= 0:
-            ok &= kps['octave'] >= lo
-            if hi >= 0:
-                ok &= kps['octave'] <= hi
-        assert sorted(got.tolist()) == np.nonzero(ok)[0].tolist()
-        assert len(set(got.tolist())) == len(got)
+    for kps, b, nq in frames:
+        C = S.Cands(kps, b)
+        inside = 0
+        for _ in range(nq):
+            x, y, r = rng.uniform(b[0] - 20, b[2] + 20), rng.uniform(b[1] - 20, b[3] + 20), rng.uniform(1, 60)
+            lo, hi = int(rng.integers(-1, 6)), int(rng.integers(-1, 8))
+            got = O.features_in_area(kps, b, x, y, r, lo, hi)
+            x32, y32, r32 = np.float32(x), np.float32(y), np.float32(r)
+            ok = (np.abs(kps['x'] - x32) < r32) & (np.abs(kps['y'] - y32) < r32) & C.ingrid
+            if lo > 0 or hi >= 0:
+                ok &= kps['octave'] >= lo
+                if hi >= 0:
+                    ok &= kps['octave'] <= hi
+            assert sorted(got.tolist()) == np.nonzero(ok)[0].tolist()
+            assert got.tolist() == C.query(x, y, r, lo, hi), (x, y, r, lo, hi)
+            inside += int((~C.ingrid[got]).sum() == 0 and ((kps['x'][got] < b[0]) | (kps['y'][got] < b[1])).any())
+        assert b[0] == 0 or inside > 0        # keypoints left of / above the bounds that still fall into cell 0 are returned
 
 
 def test_last_frame_scene_matches_well():

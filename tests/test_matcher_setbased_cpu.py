@@ -11,35 +11,6 @@ import oracle_lib as O
 TH_HIGH, HISTO = 100, 30
 
 
-class Cands:
-    def __init__(self, kps, bounds):
-        self.k = kps
-        self.minX, self.minY, maxX, maxY = (np.float32(b) for b in bounds)
-        self.wi = np.float32(64) / (maxX - self.minX)
-        self.hi = np.float32(48) / (maxY - self.minY)
-        self.cx = np.round((kps['x'] - self.minX) * self.wi).astype(int)       # Frame::PosInGrid (round half away; positives here)
-        self.cy = np.round((kps['y'] - self.minY) * self.hi).astype(int)
-        self.order = np.lexsort((np.arange(len(kps)), self.cy, self.cx))
-        self.ingrid = (self.cx >= 0) & (self.cx < 64) & (self.cy >= 0) & (self.cy < 48)
-
-    def query(self, x, y, r, lo, hi):
-        x, y, r = np.float32(x), np.float32(y), np.float32(r)
-        x0 = max(0, int(np.floor((x - self.minX - r) * self.wi)))
-        x1 = min(63, int(np.ceil((x - self.minX + r) * self.wi)))
-        y0 = max(0, int(np.floor((y - self.minY - r) * self.hi)))
-        y1 = min(47, int(np.ceil((y - self.minY + r) * self.hi)))
-        if x0 >= 64 or x1 < 0 or y0 >= 48 or y1 < 0:
-            return []
-        k = self.k
-        ok = self.ingrid & (self.cx >= x0) & (self.cx <= x1) & (self.cy >= y0) & (self.cy <= y1)
-        if lo > 0 or hi >= 0:
-            ok &= k['octave'] >= lo
-            if hi >= 0:
-                ok &= k['octave'] <= hi
-        ok &= (np.abs(k['x'] - x) < r) & (np.abs(k['y'] - y) < r)
-        return [i for i in self.order if ok[i]]
-
-
 def _ham(a, b):
     return int(np.unpackbits(a ^ b).sum())
 
@@ -60,81 +31,95 @@ def _three_maxima(sizes):
     return ind
 
 
-def test_local_map_search_set_based():
-    for t in (6, 9):
-        s = S.local_map_scene(t)
-        kps, desc, sf, p = s['kps'], s['desc'], s['sf'], s['pts']
-        C = Cands(kps, s['bounds'])
-        th, nnratio = 3.0, np.float32(0.8)
-        match = np.full(len(kps), -1, np.int32); claimed = np.zeros(len(kps), np.uint8); n = 0
-        for i in range(len(p['projX'])):
-            if not p['inView'][i] or p['bad'][i]:
+def _local_map(s, th, nnratio=0.8):
+    kps, desc, sf, p = s['kps'], s['desc'], s['sf'], s['pts']
+    C = S.Cands(kps, s['bounds'])
+    nnratio = np.float32(nnratio)
+    match = np.full(len(kps), -1, np.int32); claimed = np.zeros(len(kps), np.uint8); n = 0
+    for i in range(len(p['projX'])):
+        if not p['inView'][i] or p['bad'][i]:
+            continue
+        lvl = int(p['level'][i])
+        r = np.float32(2.5 if p['viewCos'][i] > 0.998 else 4.0)
+        if th != 1.0:
+            r = r * np.float32(th)
+        best, best2, bl, bl2, bi = 256, 256, -1, -1, -1
+        for idx in C.query(p['projX'][i], p['projY'][i], r * sf[lvl], lvl - 1, lvl):
+            if match[idx] >= 0 and claimed[idx]:
                 continue
-            lvl = int(p['level'][i])
-            r = np.float32(2.5 if p['viewCos'][i] > 0.998 else 4.0) * np.float32(th)
-            best, best2, bl, bl2, bi = 256, 256, -1, -1, -1
-            for idx in C.query(p['projX'][i], p['projY'][i], r * sf[lvl], lvl - 1, lvl):
-                if match[idx] >= 0 and claimed[idx]:
-                    continue
-                d = _ham(p['descriptors'][i], desc[idx])
-                if d < best:
-                    best2, best, bl2, bl, bi = best, d, bl, int(kps['octave'][idx]), idx
-                elif d < best2:
-                    bl2, best2 = int(kps['octave'][idx]), d
-            if best <= TH_HIGH:
-                if bl == bl2 and best > nnratio * np.float32(best2):
-                    continue
-                match[bi] = i; claimed[bi] = p['hasObs'][i]; n += 1
-        m2 = np.full(len(kps), -1, np.int32); c2 = np.zeros(len(kps), np.uint8)
-        n2 = O.search_local_map(kps, desc, s['bounds'], sf, p, th, 0.8, False, 50.0, m2, c2)
-        assert n == n2 and np.array_equal(match, m2) and np.array_equal(claimed, c2)
+            d = _ham(p['descriptors'][i], desc[idx])
+            if d < best:
+                best2, best, bl2, bl, bi = best, d, bl, int(kps['octave'][idx]), idx
+            elif d < best2:
+                bl2, best2 = int(kps['octave'][idx]), d
+        if best <= TH_HIGH:
+            if bl == bl2 and best > nnratio * np.float32(best2):
+                continue
+            match[bi] = i; claimed[bi] = p['hasObs'][i]; n += 1
+    return n, match, claimed
 
 
-def test_last_frame_search_set_based():
-    for t in (5, 8):
-        s = S.last_frame_scene(t)
-        kps, desc, sf, L = s['kps'], s['desc'], s['sf'], s['last']
-        C = Cands(kps, s['bounds'])
-        # the oracle's own projection (the float evaluation order of Tcw * x is part of its contract): take (u, v) from a 1-keypoint probe
-        qw, qx, qy, qz, tx, ty, tz = (np.float32(v) for v in s['Tcw'])
-        fx, fy, cx, cy = (np.float32(v) for v in s['cam'])
-        th = np.float32(15.0)
-        match = np.full(len(kps), -1, np.int32); claimed = np.zeros(len(kps), np.uint8); n = 0
-        hist = [[] for _ in range(HISTO)]
-        for i in range(len(L['valid'])):
-            if not L['valid'][i]:
+def _last_frame(s, th, ori=True):
+    kps, desc, sf, L = s['kps'], s['desc'], s['sf'], s['last']
+    C = S.Cands(kps, s['bounds'])
+    qw, qx, qy, qz, tx, ty, tz = (np.float32(v) for v in s['Tcw'])
+    fx, fy, cx, cy = (np.float32(v) for v in s['cam'])
+    th = np.float32(th)
+    match = np.full(len(kps), -1, np.int32); claimed = np.zeros(len(kps), np.uint8); n = 0
+    hist = [[] for _ in range(HISTO)]
+    for i in range(len(L['valid'])):
+        if not L['valid'][i]:
+            continue
+        px, py, pz = (np.float32(v) for v in L['xyz'][i])
+        ux, uy, uz = qy * pz - qz * py, qz * px - qx * pz, qx * py - qy * px
+        ux, uy, uz = ux + ux, uy + uy, uz + uz
+        xc = (px + qw * ux) + (qy * uz - qz * uy) + tx
+        yc = (py + qw * uy) + (qz * ux - qx * uz) + ty
+        zc = (pz + qw * uz) + (qx * uy - qy * ux) + tz
+        if np.float32(1.0 / np.float64(zc)) < 0:
+            continue
+        u, v = fx * xc / zc + cx, fy * yc / zc + cy
+        if u < C.minX or u > np.float32(s['bounds'][2]) or v < C.minY or v > np.float32(s['bounds'][3]):
+            continue
+        oc = int(L['octave'][i])
+        best, bi = 256, -1
+        for idx in C.query(u, v, th * sf[oc], oc - 1, oc + 1):
+            if match[idx] >= 0 and claimed[idx]:
                 continue
-            px, py, pz = (np.float32(v) for v in L['xyz'][i])
-            ux, uy, uz = qy * pz - qz * py, qz * px - qx * pz, qx * py - qy * px
-            ux, uy, uz = ux + ux, uy + uy, uz + uz
-            xc = (px + qw * ux) + (qy * uz - qz * uy) + tx
-            yc = (py + qw * uy) + (qz * ux - qx * uz) + ty
-            zc = (pz + qw * uz) + (qx * uy - qy * ux) + tz
-            if np.float32(1.0 / np.float64(zc)) < 0:
-                continue
-            u, v = fx * xc / zc + cx, fy * yc / zc + cy
-            if u < C.minX or u > np.float32(s['bounds'][2]) or v < C.minY or v > np.float32(s['bounds'][3]):
-                continue
-            oc = int(L['octave'][i])
-            best, bi = 256, -1
-            for idx in C.query(u, v, th * sf[oc], oc - 1, oc + 1):
-                if match[idx] >= 0 and claimed[idx]:
-                    continue
-                d = _ham(L['descriptors'][i], desc[idx])
-                if d < best:
-                    best, bi = d, idx
-            if best <= TH_HIGH:
-                match[bi] = i; claimed[bi] = L['hasObs'][i]; n += 1
-                rot = np.float32(L['angle'][i]) - np.float32(kps['angle'][bi])
-                if rot < 0:
-                    rot = rot + np.float32(360)
-                b = int(np.floor(np.float64(rot * np.float32(1.0 / HISTO)) + 0.5))      # round(): half away from zero, rot >= 0
-                hist[0 if b == HISTO else b].append(bi)
+            d = _ham(L['descriptors'][i], desc[idx])
+            if d < best:
+                best, bi = d, idx
+        if best <= TH_HIGH:
+            match[bi] = i; claimed[bi] = L['hasObs'][i]; n += 1
+            rot = np.float32(L['angle'][i]) - np.float32(kps['angle'][bi])
+            if rot < 0:
+                rot = rot + np.float32(360)
+            b = int(np.floor(np.float64(rot * np.float32(1.0 / HISTO)) + 0.5))      # round(): half away from zero, rot >= 0
+            hist[0 if b == HISTO else b].append(bi)
+    if ori:
         keep = _three_maxima([len(h) for h in hist])
         for b in range(HISTO):
             if b not in keep:
                 for idx in hist[b]:
                     match[idx] = -1; claimed[idx] = 0; n -= 1
-        m2 = np.full(len(kps), -1, np.int32); c2 = np.zeros(len(kps), np.uint8)
-        n2 = O.search_last_frame(kps, desc, s['bounds'], sf, s['Tcw'], s['cam'], L, 15.0, True, m2, c2)
-        assert n == n2 and np.array_equal(match, m2) and np.array_equal(claimed, c2)
+    return n, match, claimed
+
+
+def test_local_map_search_set_based():
+    """Every scene of matcher_scenes: the seeded ones, the other geometries and bounds, and the placed ones."""
+    cases = [(S.local_map_scene(t), 3.0) for t in (6, 9)] + [(S.special_scene(name, 0), 1.0) for name in S.SPECIAL]
+    for k, (s, th) in enumerate(cases):
+        n, match, claimed = _local_map(s, th)
+        m2 = np.full(len(s['kps']), -1, np.int32); c2 = np.zeros(len(s['kps']), np.uint8)
+        n2 = O.search_local_map(s['kps'], s['desc'], s['bounds'], s['sf'], s['pts'], th, 0.8, False, 50.0, m2, c2)
+        assert n == n2 and np.array_equal(match, m2) and np.array_equal(claimed, c2), k
+
+
+def test_last_frame_search_set_based():
+    cases = [S.last_frame_scene(t) for t in (5, 8)] + [S.special_scene(name, 1) for name in S.SPECIAL]
+    for k, s in enumerate(cases):
+        # the restatement projects with the oracle's float evaluation order of Tcw * x, which is part of its contract
+        n, match, claimed = _last_frame(s, 15.0)
+        m2 = np.full(len(s['kps']), -1, np.int32); c2 = np.zeros(len(s['kps']), np.uint8)
+        n2 = O.search_last_frame(s['kps'], s['desc'], s['bounds'], s['sf'], s['Tcw'], s['cam'], s['last'], 15.0, True, m2, c2)
+        assert n == n2 and np.array_equal(match, m2) and np.array_equal(claimed, c2), k

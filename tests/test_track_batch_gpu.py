@@ -17,6 +17,11 @@ def orb():
     return m
 
 
+def torch_sms():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
 def _streams(B, seed, g):
     out = []
     for b in range(B):
@@ -75,8 +80,9 @@ def _compare(R, chain, streams, exact=True):
             assert np.abs(r2['pose7'][b] - lm['pose7']).max() < 1e-8 and np.abs(R['r1']['pose7'][b] - mm['pose7']).max() < 1e-8
 
 
-@pytest.mark.parametrize('B,far', [(1, False), (7, False), (7, True), (240, False)])
+@pytest.mark.parametrize('B,far', [(1, False), (7, False), (7, True), (37, False), (88, True), (240, False)])
 def test_equals_per_frame_chain_of_existing_entry_points(orb, B, far):
+    """B = 37, 88 and 240 run the local-map search with clusters of fewer than 8 CTAs (batch x size <= 2 x SMs)."""
     g = T.globals_()
     if far:
         g.update(bFarPoints=1, thFarPoints=7.0)
@@ -85,6 +91,7 @@ def test_equals_per_frame_chain_of_existing_entry_points(orb, B, far):
     m = orb.ORBmatcher(0.8, False, max_batch=B, max_keypoints=2048, max_mappoints=2048, device=0)
     R = _batched(m, streams, g, th)
     assert m.last_launch_count() == 5
+    assert B * m.last_cluster_size() <= 2 * torch_sms() and (B <= 33 or m.last_cluster_size() < 8), m.last_cluster_size()
     _compare(R, _chain(T.GpuChainBackend(orb, orb.ORBmatcher(0.8, False, max_batch=1, max_keypoints=2048, max_mappoints=2048)), streams, g, th), streams)
     assert (R['r2']['nmatches'] > 0).any() and (R['r1']['discarded'] > 0).any()
     if B > 1:   # the scene with one point held at two keypoints is among them
