@@ -131,7 +131,7 @@ int orbx_copy_candidates(orbx_handle* h, int frame, int level, int* xys, int cap
 int orbx_last_launch_count(const orbx_handle* h);
 /* Per-kernel device times of the pipeline (the reference's REGISTER_TIMES analogue, include/Settings.h:24): with profiling on,
  * CUDA events bracket each stage on the launching stream (the blur then runs in line instead of on its forked stream).
- * ms6 = pyramid, blur, FAST cells, quadtree+orientation, assemble, BRIEF of the last profiled call. */
+ * ms6 = pyramid, blur, FAST cells, quadtree, assemble, orientation + BRIEF of the last profiled call. */
 int orbx_set_profiling(orbx_handle* h, int on);
 int orbx_get_stage_ms(orbx_handle* h, float* ms6);
 

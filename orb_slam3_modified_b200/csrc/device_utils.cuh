@@ -88,7 +88,7 @@ template <int NT> __device__ __forceinline__ int block_scan_excl(int v, int* sm,
 // of the block must call; on return `out` is visible to all of them.
 template <int NT, class Count> __device__ __forceinline__ int block_prefix(int n, int* out, int* sm, Count count) {
     int carry = 0;
-    // An unsigned tile base: with a signed one the compiler unrolls this loop, and quadtree_orient_kernel spills more
+    // An unsigned tile base: with a signed one the compiler unrolls this loop
     for (unsigned b = 0; b < (unsigned)n; b += NT) {
         const int i = (int)(b + threadIdx.x);
         int tot;

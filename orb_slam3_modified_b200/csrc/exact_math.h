@@ -223,10 +223,9 @@ ORB_HD void sx_insertion_sort(T* first, T* last, Less less) {
     }
 }
 
-// One __introsort_loop iteration on [lo, hi): __move_median_to_first(first, first+1, mid, last-1) + __unguarded_partition(first+1, last,
-// pivot = *first); returns the cut.
+// __move_median_to_first(first, first+1, mid, last-1) on [lo, hi)
 template <class T, class Less>
-ORB_HD int sx_partition_step(T* a, int lo, int hi, Less less) {
+ORB_HD void sx_median_to_first(T* a, int lo, int hi, Less less) {
     T* first = a + lo;
     T* A = first + 1;
     T* B = first + (hi - lo) / 2;
@@ -240,12 +239,20 @@ ORB_HD int sx_partition_step(T* a, int lo, int hi, Less less) {
     else if (less(*B, *C)) med = C;
     else med = B;
     { T t = *first; *first = *med; *med = t; }
+}
+
+// One __introsort_loop iteration on [lo, hi): sx_median_to_first + __unguarded_partition(first+1, last, pivot = *first); returns the cut.
+template <class T, class Less>
+ORB_HD int sx_partition_step(T* a, int lo, int hi, Less less) {
+    sx_median_to_first(a, lo, hi, less);
+    T* first = a + lo;
+    const T pivot = *first;   // the loop below never writes *first: l > first, and r stops at first at the latest
     T* l = first + 1;
     T* r = a + hi;
     while (true) {
-        while (less(*l, *first)) ++l;
+        while (less(*l, pivot)) ++l;
         --r;
-        while (less(*first, *r)) --r;
+        while (less(pivot, *r)) --r;
         if (!(l < r)) break;
         T t = *l; *l = *r; *r = t;
         ++l;
@@ -293,7 +300,7 @@ ORB_HD void libstdcxx_sort(T* a, int n, Less less) {
 
 
 // ---------------------------------------------------------------------------
-// The same sort as a sequence of ROUNDS of independent tasks (what quadtree_orient_kernel runs with one thread per task):
+// The same sort as a sequence of ROUNDS of independent tasks (what quadtree_kernel runs with one lane per task):
 //   round r: every pending range longer than 16 does ONE partition step (or the heapsort fallback when its depth budget is spent) and
 //            hands its two parts to the next round; parts of <= 16 elements become leaves;
 //   finally every leaf is insertion-sorted on its own.

@@ -84,7 +84,7 @@ struct Extractor {
     cudaStream_t stream = nullptr, stream2 = nullptr;
     cudaEvent_t evWait = nullptr;      // blocking-sync event: batch calls sleep on it instead of spinning (device_utils.cuh)
     cudaEvent_t evFork = nullptr, evJoin = nullptr;
-    bool profiling = false; cudaEvent_t evStage[8] = {};   // pyramid | blur | fast | quadtree | assemble | describe
+    bool profiling = false; cudaEvent_t evStage[8] = {};   // pyramid | blur | fast | quadtree | assemble | orientation + BRIEF
     float stageMs[6] = {0, 0, 0, 0, 0, 0};
     size_t smemFast = 0, smemQt = 0, smemAs = 0;
     int launches = 0;
@@ -150,7 +150,7 @@ struct Extractor {
         P.nlevels = nlevels; P.iniTh = iniTh; P.minTh = minTh; P.rows = r; P.cols = c;
         cells.clear(); fastBlocks.clear(); xtab.clear(); ytab.clear();
         size_t planeOff = 0, listOff = 0, candOff = 0;
-        int selOff = 0, blurTiles = 0, maxNodes = 0, maxCells = 0;
+        int selOff = 0, blurTiles = 0, qtEnd = 0;
         maxKp = 0;
         smemFast = 0;
         for (int l = 0; l < nlevels; ++l) {
@@ -220,15 +220,16 @@ struct Extractor {
                 G.fastBoxW = (int)alignUp(bw, 16); G.fastBoxH = bh;
                 smemFast = std::max(smemFast, (size_t)fast_smem_layout(G.fastBoxW, G.fastBoxH, iwm, ihm).total);
             }
-            maxCells = std::max(maxCells, G.nCells);
             G.candOff = (uint32_t)candOff; G.candCap = (uint32_t)G.nCells * G.cellCap;
+            if (G.candCap >= (1u << 24)) { set_error("too many FAST cells per level for the quadtree's 24-bit candidate index"); return ORB_ERR_ARG; }
             candOff += alignUp(G.candCap, 64);
             G.nDesired = featPerLevel[l];
             G.nIni = (int)roundf((float)(G.maxBX - G.minBX) / (G.maxBY - G.minBY));
             if (G.nIni < 1) { set_error("aspect ratio < 0.5: reference divides by zero (ORBextractor.cc:559-561)"); return ORB_ERR_ASPECT; }
             G.hX = (float)(G.maxBX - G.minBX) / G.nIni;
-            const int nodes = std::max(G.nDesired + 3, 4 * G.nIni) + 4;
-            maxNodes = std::max(maxNodes, nodes);
+            G.qtNodes = std::max(G.nDesired + 3, 4 * G.nIni) + 4;
+            if (G.qtNodes > QT_MAX_NODES) { set_error("nfeatures too large for the quadtree kernel"); return ORB_ERR_ARG; }
+            qtEnd = std::max(qtEnd, qt_layout(G.qtNodes, G.nCells).cand);
             G.selCap = std::max(G.nDesired + 3, 4 * G.nIni);
             G.selOff = selOff; selOff += G.selCap;
             maxKp += G.selCap;
@@ -282,9 +283,8 @@ struct Extractor {
         P.candStride = alignUp(candOff, 64);
         P.selStride = (size_t)selOff;
         P.blurTilesTotal = blurTiles;
-        P.maxNodes = maxNodes;
-        P.maxCellsPerLevel = maxCells;
-        smemQt = (size_t)maxNodes * (2 * sizeof(QtNode) + 2 * 4 + 3 * 4 + 3 * 16 + sizeof(QtSort) + 8) + 16 + 4 * ((size_t)maxCells + 1);
+        smemQt = alignUp((size_t)qtEnd + 6 * QT_SMEM_CANDS, 128);   // one quadtree warp's slab
+        P.qtSlab = (int)smemQt;
         smemAs = 2 * P.selStride * sizeof(int);
         rows = r; cols = c;
         return ORB_OK;
@@ -335,16 +335,26 @@ struct Extractor {
         CK(cudaMemcpyToSymbol(c_pattern, h_pattern, sizeof(h_pattern)));
         CK(cudaMemcpyToSymbol(c_umax, umax, sizeof(umax)));
         maxSmemFast = 96 * 1024;   // a cell interior is at most 69 x 69 px, so a 2 x 2 block needs at most ~90 KB
-        maxSmemQt = smemQt + 16 * 1024; maxSmemAs = 2 * capSel * sizeof(int);
-        if (maxSmemQt > 200 * 1024) { set_error("nfeatures too large for the quadtree kernel's shared memory"); return ORB_ERR_ARG; }
+        maxSmemQt = smemQt + 4 * 1024; maxSmemAs = 2 * capSel * sizeof(int);   // per quadtree warp: room for other aspect ratios
+        if (maxSmemQt > prop.sharedMemPerBlockOptin) { set_error("nfeatures too large for the quadtree kernel's shared memory"); return ORB_ERR_ARG; }
         // process-wide monotonic maxima (device_utils.cuh): a smaller handle created later must not lower another handle's limit
-        if (ensure_dynamic_smem(fast_cells_kernel, maxSmemFast, device) || ensure_dynamic_smem(quadtree_orient_kernel, maxSmemQt, device) ||
+        if (ensure_dynamic_smem(fast_cells_kernel, maxSmemFast, device) ||
             ensure_dynamic_smem(assemble_kernel, std::max<size_t>(maxSmemAs, 1024), device)) return ORB_ERR_CUDA;
+        // quadtree warps per CTA: the most resident warps per SM by the occupancy calculator, the fewest warps per CTA among equals
+        qtWarps = 0;
+        for (int w = 1, best = 0; w <= QT_MAX_WARPS && w * maxSmemQt <= prop.sharedMemPerBlockOptin; w *= 2) {
+            int nb = 0;
+            if (ensure_dynamic_smem(quadtree_kernel, w * maxSmemQt, device)) return ORB_ERR_CUDA;
+            CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, quadtree_kernel, 32 * w, w * smemQt));
+            if (nb * w > best) { best = nb * w; qtWarps = w; }
+        }
+        if (!qtWarps) { set_error("the quadtree kernel does not fit on the device"); return ORB_ERR_CUDA; }
         maxKpAlloc = (int)capSel;
         rows = cols = 0;   // force set_size on first use
         return set_size(maxH, maxW);
     }
     size_t maxSmemFast = 0, maxSmemQt = 0, maxSmemAs = 0;
+    int qtWarps = 0;
     size_t capPyr = 0, capCells = 0, capCellCount = 0, capCellList = 0, capCand = 0, capSel = 0, capX = 0, capY = 0;
     int maxKpAlloc = 0;
 
@@ -445,14 +455,14 @@ struct Extractor {
         fast_cells_kernel<<<dim3(Q.nFastBlocks, batch), FAST_NT, smemFast, st>>>(Q, map0, d_maps);
         ++launches;
         if (profiling) CK(cudaEventRecord(evStage[3], st));
-        quadtree_orient_kernel<<<dim3(nlevels, batch), QT_NT, smemQt, st>>>(Q);
+        quadtree_kernel<<<dim3(nlevels, (batch + qtWarps - 1) / qtWarps), 32 * qtWarps, qtWarps * smemQt, st>>>(Q);
         ++launches;
         if (profiling) CK(cudaEventRecord(evStage[4], st));
         assemble_kernel<<<batch, AS_NT, smemAs, st>>>(Q);
         ++launches;
         if (profiling) CK(cudaEventRecord(evStage[5], st));
         if (!profiling) CK(cudaStreamWaitEvent(st, evJoin, 0));
-        describe_kernel<<<dim3((unsigned)((Q.selStride + DS_NT / 32 - 1) / (DS_NT / 32)), batch), DS_NT, 0, st>>>(Q);
+        orient_describe_kernel<<<dim3((unsigned)((Q.selStride + DS_NT / 32 - 1) / (DS_NT / 32)), batch), DS_NT, 0, st>>>(Q);
         ++launches;
         if (profiling) CK(cudaEventRecord(evStage[6], st));
         CK(cudaGetLastError());
@@ -702,6 +712,18 @@ int orbx_set_profiling(orbx_handle* h, int on) {
     h->e.profiling = on != 0;
     return ORB_OK;
 }
+
+#ifdef QT_PHASES
+// out[kMaxLevels * 9]: quadtree_kernel's phase counters per level (qt_phase) since the last call, which zeroes them.
+int orbx_qt_phases(unsigned long long* out) {
+    if (!out) return ORB_ERR_ARG;
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpyFromSymbol(out, orbx::qt_phase, sizeof(orbx::qt_phase)));
+    static const unsigned long long zero[kMaxLevels * 9] = {};
+    CK(cudaMemcpyToSymbol(orbx::qt_phase, zero, sizeof(zero)));
+    return ORB_OK;
+}
+#endif
 
 int orbx_get_stage_ms(orbx_handle* h, float* ms6) {
     if (!h || !ms6 || !h->e.evStage[6]) { set_error("orbx_get_stage_ms: no profiled call yet"); return ORB_ERR_ARG; }

@@ -452,32 +452,20 @@ __global__ void __launch_bounds__(256) pyr_resize_tma_kernel(ExtractParams P, in
 }
 
 // ------------------------------------------------------------------------------------------
-// K3: quadtree distribution + orientation.  One CTA per (level, frame).
+// K3: quadtree distribution.  One warp per (level, frame); the warps of a CTA share the level.
 // Reference: ORBextractor::DistributeOctTree src/ORBextractor.cc:555-779,
-// ExtractorNode::DivideNode :480-536, compareNodes :538-553, IC_Angle :76-103.
+// ExtractorNode::DivideNode :480-536, compareNodes :538-553.
 //
 // The std::list / push_front choreography of the reference is restated as a rebuild of the
 // whole node list per pass ("split a set of nodes in processing order, children blocks go to the
 // front in reverse processing order, unsplit nodes keep their relative order"); the only
 // sequential piece is the libstdc++ std::sort emulation that decides ties in the final phase.
+// A problem's list state and, when they fit, its candidates live in the warp's shared-memory slab
+// (qt_layout), so a pass costs warp scans and __syncwarp instead of CTA barriers; counts and best
+// keys are shared-memory atomics.  The orientation of the selected keypoints is computed
+// by orient_describe_kernel, one warp per keypoint across the batch.
 // ------------------------------------------------------------------------------------------
-constexpr int QT_NT = 256;
-
-struct QtNode { int16_t ulx, uly, brx, bry; };
-struct QtSort { int size; int ulx; int node; };
-
-struct QtShared {
-    QtNode* bnd[2];
-    int* cnt[2];
-    int* proc;        // per list node: processing index or -1
-    int* procNode;    // per processing index: list node
-    int* childCnt;    // 4 per processing index
-    int* childPos;    // 4 per processing index: new list position (or -1)
-    int* keepPos;     // per list node: new position when unsplit
-    int* scanA;       // scratch, 4*maxNodes
-    QtSort* v;        // expandable children in creation order
-    unsigned long long* best;
-};
+constexpr int QT_MAX_WARPS = 8;
 
 __device__ __forceinline__ int qt_child(const QtNode& n, int px, int py, int& midx, int& midy) {
     const int halfX = (int)ceilf((float)(n.brx - n.ulx) / 2);
@@ -486,298 +474,395 @@ __device__ __forceinline__ int qt_child(const QtNode& n, int px, int py, int& mi
     return (px < midx ? 0 : 1) + (py < midy ? 0 : 2);
 }
 
-
-// std::sort emulation by the whole CTA (see exact_math.h: rounds of independent tasks).  leaf: capacity n entries; qA / qB: n / 17 + 1 each.
-__device__ void cta_libstdcxx_sort(QtSort* a, int n, SxTask* leaf, SxTask* qA, SxTask* qB, int* cnt /* shared: nCur, nNext, nLeaf */) {
-    const auto less = [](const QtSort& x, const QtSort& y) { return x.size < y.size || (x.size == y.size && x.ulx < y.ulx); };
-    const int tid = threadIdx.x;
-    if (n < 2) return;
-    if (n <= 16) { if (tid == 0) sx_insertion_sort(a, a + n, less); __syncthreads(); return; }
-    if (tid == 0) {
-        int depth = 0;
-        for (int t = n; t > 1; t >>= 1) depth++;
-        qA[0] = SxTask{0, n, 2 * depth};
-        cnt[0] = 1; cnt[1] = 0; cnt[2] = 0;
-    }
-    __syncthreads();
-    SxTask *cur = qA, *nxt = qB;
-    for (;;) {
-        const int nc = cnt[0];
-        if (nc == 0) break;
-        for (int i = tid; i < nc; i += blockDim.x) {
-            const SxTask t = cur[i];
-            if (t.d == 0) { sx_heapsort(a + t.lo, t.hi - t.lo, less); continue; }
-            const int cut = sx_partition_step(a, t.lo, t.hi, less);
-            const SxTask right = {cut, t.hi, t.d - 1}, left = {t.lo, cut, t.d - 1};
-            if (right.hi - right.lo > 16) nxt[atomicAdd(&cnt[1], 1)] = right; else if (right.hi - right.lo > 1) leaf[atomicAdd(&cnt[2], 1)] = right;
-            if (left.hi - left.lo > 16) nxt[atomicAdd(&cnt[1], 1)] = left; else if (left.hi - left.lo > 1) leaf[atomicAdd(&cnt[2], 1)] = left;
-        }
-        __syncthreads();
-        if (tid == 0) { cnt[0] = cnt[1]; cnt[1] = 0; }
-        SxTask* sw = cur; cur = nxt; nxt = sw;
-        __syncthreads();
-    }
-    const int nl = cnt[2];
-    for (int i = tid; i < nl; i += blockDim.x) sx_insertion_sort(a + leaf[i].lo, a + leaf[i].hi, less);
-    __syncthreads();
+__device__ __forceinline__ unsigned lanemask_lt() { unsigned m; asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m)); return m; }
+__device__ __forceinline__ int warp_incl_scan(int v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+    return v;
 }
 
-__global__ void __launch_bounds__(QT_NT, 4) quadtree_orient_kernel(ExtractParams P) {
+// sx_partition_step by one warp.  The unguarded partition's k-th swap exchanges the k-th element from the left (from lo + 1) that is not
+// below the pivot with the k-th from the right (from hi - 1) that is not above it, as long as the first lies left of the second: ballots
+// list both kinds of stop in order (lpos / rpos, hi - lo entries each), the swaps run at once, and the cut is where the scan from the left
+// stops first after the last swap.
+template <class Less>
+__device__ int warp_partition_step(QtSort* a, int lo, int hi, int16_t* lpos, int16_t* rpos, int lane, Less less) {
+    if (lane == 0) sx_median_to_first(a, lo, hi, less);
+    __syncwarp();
+    const QtSort pivot = a[lo];
+    int nL = 0, nR = 0;
+    for (int b = lo + 1; b < hi; b += 32) {
+        const int p = b + lane;
+        const bool stop = p < hi && !less(a[p], pivot);
+        const unsigned m = __ballot_sync(0xffffffffu, stop);
+        if (stop) lpos[nL + __popc(m & lanemask_lt())] = (int16_t)p;
+        nL += __popc(m);
+    }
+    for (int b = hi - 1; b >= lo; b -= 32) {
+        const int p = b - lane;
+        const bool stop = p >= lo && !less(pivot, a[p]);
+        const unsigned m = __ballot_sync(0xffffffffu, stop);
+        if (stop) rpos[nR + __popc(m & lanemask_lt())] = (int16_t)p;
+        nR += __popc(m);
+    }
+    __syncwarp();
+    const int nk = min(nL, nR);
+    int K = 0;                            // swaps: lpos[k] < rpos[k] holds for a prefix of k
+    for (int b = 0; b < nk; b += 32) {
+        const unsigned m = __ballot_sync(0xffffffffu, b + lane < nk && lpos[b + lane] < rpos[b + lane]);
+        K += __popc(m);
+        if (m != 0xffffffffu) break;
+    }
+    for (int k = lane; k < K; k += 32) { const int pl = lpos[k], pr = rpos[k]; const QtSort x = a[pl]; a[pl] = a[pr]; a[pr] = x; }
+    const int rPrev = K > 0 ? rpos[K - 1] : hi;
+    const int cut = K < nL ? min((int)lpos[K], rPrev) : rPrev;
+    __syncwarp();
+    return cut;
+}
+
+// std::sort emulation by one warp (see exact_math.h: rounds of independent tasks); the warp runs the partition steps of a round one
+// after another (warp_partition_step).  leaf: n / 2 + 1 tasks; qA / qB: n / 17 + 1 each; lpos / rpos: n entries each.  The final insertion
+// sort of a leaf (of the whole range when n <= 16) moves an element only past strictly greater ones, so it is the stable sort of the leaf:
+// a half-warp per leaf places each element at its stable rank.
+__device__ void warp_libstdcxx_sort(QtSort* a, int n, SxTask* leaf, SxTask* qA, SxTask* qB, int16_t* lpos, int16_t* rpos, int lane) {
+    const auto less = [](const QtSort& x, const QtSort& y) { return x.size < y.size || (x.size == y.size && x.ulx < y.ulx); };
+    if (n < 2) return;
+    int nc = 1, nl = 0;
+    if (n <= 16) { nc = 0; nl = 1; if (lane == 0) leaf[0] = SxTask{0, n, 0}; }
+    int depth = 0;
+    for (int t = n; t > 1; t >>= 1) depth++;
+    if (lane == 0 && nc) qA[0] = SxTask{0, n, 2 * depth};
+    __syncwarp();
+    SxTask *cur = qA, *nxt = qB;
+    while (nc) {
+        int nn = 0;
+        for (int i = 0; i < nc; ++i) {
+            const SxTask t = cur[i];
+            if (t.d == 0) {                   // depth budget spent: heapsort on one lane
+                if (lane == 0) sx_heapsort(a + t.lo, t.hi - t.lo, less);
+                __syncwarp();
+                continue;
+            }
+            const int cut = warp_partition_step(a, t.lo, t.hi, lpos, rpos, lane, less);
+            const SxTask right = {cut, t.hi, t.d - 1}, left = {t.lo, cut, t.d - 1};
+            const int rs = right.hi - right.lo, ls = left.hi - left.lo;
+            if (lane == 0) {
+                if (rs > 16) nxt[nn] = right; else if (rs > 1) leaf[nl] = right;
+                if (ls > 16) nxt[nn + (rs > 16)] = left; else if (ls > 1) leaf[nl + (rs > 1 && rs <= 16)] = left;
+            }
+            nn += (rs > 16) + (ls > 16);
+            nl += (rs > 1 && rs <= 16) + (ls > 1 && ls <= 16);
+        }
+        __syncwarp();
+        SxTask* sw = cur; cur = nxt; nxt = sw;
+        nc = nn;
+    }
+    for (int b = 0; b < nl; b += 2) {
+        const int li = b + (lane >> 4), e = lane & 15;
+        int lo = 0, len = 0;
+        if (li < nl) { lo = leaf[li].lo; len = leaf[li].hi - lo; }
+        QtSort x = {0, 0, 0};
+        unsigned long long key = ~0ull;   // above every real key: (size, ulx) with size < 2^31, ulx >= 0
+        if (e < len) { x = a[lo + e]; key = ((unsigned long long)(unsigned)x.size << 16) | (uint16_t)x.ulx; }
+        int rank = 0;
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            const unsigned long long kk = __shfl_sync(0xffffffffu, key, k, 16);
+            rank += kk < key || (kk == key && k < e);
+        }
+        __syncwarp();
+        if (e < len) a[lo + rank] = x;
+        __syncwarp();
+    }
+}
+
+// Phase stamps of quadtree_kernel (build with -DQT_PHASES, read by tools/stage_times.py through orbx_qt_phases): lane 0 of every warp
+// adds its clock64() spans per level.  [l][0] gather, [1] roots, [2] split passes before the careful phase, [3] careful-phase sorts,
+// [4] careful passes without their sort, [5] best key per node + selection, [6] passes, [7] careful passes, [8] problems.
+#ifdef QT_PHASES
+__device__ unsigned long long qt_phase[kMaxLevels][9];
+#define QT_STAMP(t) long long t = 0; if (lane == 0) t = clock64()
+#define QT_ADD(k, v) if (lane == 0) atomicAdd(&qt_phase[l][k], (unsigned long long)(v))
+#define QT_ONLY(x) x
+#else
+#define QT_STAMP(t)
+#define QT_ADD(k, v)
+#define QT_ONLY(x)
+#endif
+
+__global__ void __launch_bounds__(QT_MAX_WARPS * 32) quadtree_kernel(ExtractParams P) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
-    const int l = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
+    const int l = blockIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int f = blockIdx.y * (blockDim.x >> 5) + w;
+    if (f >= P.batch) return;
+    QT_STAMP(t0);
     const LevelGeom& G = P.lv[l];
-    const int MN = P.maxNodes;
-    __shared__ int s_warp[33];
-    __shared__ int s_P;
-    __shared__ int s_sortCnt[3];
-
-    // carve shared memory
-    QtShared S;
-    uint8_t* p = smem_raw;
-    S.bnd[0] = (QtNode*)p; p += sizeof(QtNode) * MN;
-    S.bnd[1] = (QtNode*)p; p += sizeof(QtNode) * MN;
-    S.cnt[0] = (int*)p; p += 4 * MN;
-    S.cnt[1] = (int*)p; p += 4 * MN;
-    S.proc = (int*)p; p += 4 * MN;
-    S.procNode = (int*)p; p += 4 * MN;
-    S.keepPos = (int*)p; p += 4 * MN;
-    S.childCnt = (int*)p; p += 16 * MN;
-    S.childPos = (int*)p; p += 16 * MN;
-    S.scanA = (int*)p; p += 16 * MN;
-    S.v = (QtSort*)p; p += sizeof(QtSort) * MN;
-    p = (uint8_t*)(((uintptr_t)p + 7) & ~(uintptr_t)7);
-    S.best = (unsigned long long*)p; p += 8 * MN;
-    int* cellOff = (int*)p;   // maxCellsPerLevel + 1
-
-    uint32_t* cand = P.cand + (size_t)f * P.candStride + G.candOff;
-    uint16_t* nodeOf = P.nodeOf + (size_t)f * P.candStride + G.candOff;
+    const QtLayout L = qt_layout(G.qtNodes, G.nCells);
+    uint8_t* base = smem_raw + (size_t)w * P.qtSlab;
+    QtNode* bnd0 = (QtNode*)(base + L.bnd0); QtNode* bnd1 = (QtNode*)(base + L.bnd1);
+    int* cnt0 = (int*)(base + L.cnt0); int* cnt1 = (int*)(base + L.cnt1);
+    int* childCnt = (int*)(base + L.scratch);
+    QtSort* v = (QtSort*)(base + L.v);
+    int16_t* proc = (int16_t*)(base + L.proc);          // per list node: processing index or -1
+    int16_t* procNode = (int16_t*)(base + L.procNode);  // per processing index: list node
+    int16_t* keepPos = (int16_t*)(base + L.keepPos);    // per list node: new position when unsplit
+    int16_t* kExcl = (int16_t*)(base + L.kExcl);        // per processing index: children of the earlier ones
+    int16_t* childPos = (int16_t*)(base + L.childPos);  // 4 per processing index: new list position (or -1)
     SelKp* sel = P.sel + (size_t)f * P.selStride + G.selOff;
 
     // ---- gather the per-cell lists into candidate order (cell row-major, then y, x) ----
+    int* cellOff = childCnt;
     const int* cellCount = P.cellCount + (size_t)f * P.cellCountStride + G.cellBase;
-    for (int c = tid; c < G.nCells; c += QT_NT) cellOff[c] = cellCount[c];
-    __syncthreads();
-    const int n = block_prefix<QT_NT>(G.nCells, cellOff, s_warp, [&](int c) { return cellOff[c]; });
-    {
-        const uint32_t* lists = P.cellList + (size_t)f * P.cellListStride;
-        const int wid = tid >> 5, lane = tid & 31;
-        for (int c = wid; c < G.nCells; c += QT_NT / 32) {
-            const int cnt = cellCount[c], o = cellOff[c];
-            const uint32_t* src = lists + P.cells[G.cellBase + c].listOff;
-            for (int k = lane; k < cnt; k += 32) cand[o + k] = src[k];
+    int n = 0;
+    for (int c0 = 0; c0 < G.nCells; c0 += 32) {
+        const int c = c0 + lane;
+        const int k = c < G.nCells ? cellCount[c] : 0;
+        const int inc = warp_incl_scan(k, lane);
+        if (c < G.nCells) cellOff[c] = n + inc - k;
+        n += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    __syncwarp();
+    const int capS = (P.qtSlab - L.cand) / 6;
+    const bool inSmem = n <= capS;
+    uint32_t* cand = inSmem ? (uint32_t*)(base + L.cand) : P.cand + (size_t)f * P.candStride + G.candOff;
+    uint16_t* nodeOf = inSmem ? (uint16_t*)(base + L.cand + 4 * capS) : P.nodeOf + (size_t)f * P.candStride + G.candOff;
+    if (n > 0) {
+        // the lists of a level's cells are consecutive, cellCap apart; candidate i is in the last cell whose offset is <= i
+        const uint32_t* lists = P.cellList + (size_t)f * P.cellListStride + P.cells[G.cellBase].listOff;
+        int top = 1;
+        while (top * 2 < G.nCells) top *= 2;
+        for (int i0 = 0; i0 < n; i0 += 128) {
+            int c[4] = {0, 0, 0, 0};
+            for (int step = top; step; step >>= 1)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int t = c[j] + step;
+                    if (t < G.nCells && cellOff[t] <= i0 + 32 * j + lane) c[j] = t;
+                }
+            uint32_t x[4] = {0, 0, 0, 0};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = i0 + 32 * j + lane;
+                if (i < n) x[j] = lists[c[j] * G.cellCap + (i - cellOff[c[j]])];
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) if (i0 + 32 * j + lane < n) cand[i0 + 32 * j + lane] = x[j];
         }
     }
-    __syncthreads();
+    __syncwarp();
+    QT_STAMP(t1);
+    QT_ADD(0, t1 - t0);
 
-    int cur = 0;
     // ---- root nodes (:559-598) ----
-    for (int i = tid; i < G.nIni; i += QT_NT) {
+    for (int i = lane; i < G.nIni; i += 32) {
         QtNode nd;
         nd.ulx = (int16_t)(int)fmul(G.hX, (float)i); nd.uly = 0;
         nd.brx = (int16_t)(int)fmul(G.hX, (float)(i + 1)); nd.bry = (int16_t)(G.maxBY - G.minBY);
-        S.bnd[0][i] = nd; S.cnt[0][i] = 0;
+        bnd0[i] = nd; cnt0[i] = 0;
     }
-    __syncthreads();
-    for (int i = tid; i < n; i += QT_NT) {
-        const int r = (int)fdiv((float)cand_x(cand[i]), G.hX);
-        nodeOf[i] = (uint16_t)r;
-        atomicAdd(&S.cnt[0][r], 1);
+    __syncwarp();
+    for (int i0 = 0; i0 < n; i0 += 32) {
+        const int i = i0 + lane;
+        int r = -1;
+        if (i < n) { r = (int)fdiv((float)cand_x(cand[i]), G.hX); nodeOf[i] = (uint16_t)r; }
+        if (r >= 0) atomicAdd(&cnt0[r], 1);
     }
-    __syncthreads();
+    __syncwarp();
     // erase empty roots, keep order
-    for (int i = tid; i < G.nIni; i += QT_NT) S.scanA[i] = S.cnt[0][i] > 0;
-    __syncthreads();
-    int m = block_prefix<QT_NT>(G.nIni, S.scanA, s_warp, [&](int i) { return S.scanA[i]; });
-    for (int i = tid; i < G.nIni; i += QT_NT) {
-        S.keepPos[i] = S.cnt[0][i] > 0 ? S.scanA[i] : -1;
-        if (S.cnt[0][i] > 0) { S.bnd[1][S.scanA[i]] = S.bnd[0][i]; S.cnt[1][S.scanA[i]] = S.cnt[0][i]; }
+    int m = 0;
+    for (int i0 = 0; i0 < G.nIni; i0 += 32) {
+        const int i = i0 + lane;
+        const bool keep = i < G.nIni && cnt0[i] > 0;
+        const unsigned b = __ballot_sync(0xffffffffu, keep);
+        const int pos = m + __popc(b & lanemask_lt());
+        if (i < G.nIni) keepPos[i] = (int16_t)(keep ? pos : -1);
+        if (keep) { bnd1[pos] = bnd0[i]; cnt1[pos] = cnt0[i]; }
+        m += __popc(b);
     }
-    __syncthreads();
-    for (int i = tid; i < n; i += QT_NT) nodeOf[i] = (uint16_t)S.keepPos[nodeOf[i]];
-    cur = 1;
-    __syncthreads();
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) nodeOf[i] = (uint16_t)keepPos[nodeOf[i]];
+    __syncwarp();
+    QT_STAMP(t2);
+    QT_ADD(1, t2 - t1);
 
+    QtNode *bndC = bnd1, *bndN = bnd0;
+    int *cntC = cnt1, *cntN = cnt0;
     const int N = G.nDesired;
     bool finish = (n == 0);
     bool careful = false;
-    int q = 0;   // size of S.v
+    int q = 0;   // size of v
     while (!finish) {
+        QT_STAMP(tp);
+        QT_ONLY(long long tsort = 0;)
         const int prevSize = m;
-        QtNode* bndC = S.bnd[cur]; int* cntC = S.cnt[cur];
-        QtNode* bndN = S.bnd[cur ^ 1]; int* cntN = S.cnt[cur ^ 1];
         // --- A. processing order of the nodes to split ---
-        int P0;
+        int P0 = 0;
         if (!careful) {
-            for (int s = tid; s < m; s += QT_NT) S.scanA[s] = cntC[s] > 1;
-            __syncthreads();
-            P0 = block_prefix<QT_NT>(m, S.scanA, s_warp, [&](int s) { return S.scanA[s]; });
-            for (int s = tid; s < m; s += QT_NT) {
-                if (cntC[s] > 1) { S.proc[s] = S.scanA[s]; S.procNode[S.scanA[s]] = s; }
-                else S.proc[s] = -1;
+            for (int s0 = 0; s0 < m; s0 += 32) {
+                const int s = s0 + lane;
+                const bool split = s < m && cntC[s] > 1;
+                const unsigned b = __ballot_sync(0xffffffffu, split);
+                const int pi = P0 + __popc(b & lanemask_lt());
+                if (s < m) proc[s] = (int16_t)(split ? pi : -1);
+                if (split) procNode[pi] = (int16_t)s;
+                P0 += __popc(b);
             }
         } else {
             // std::sort(vPrev.begin(), vPrev.end(), compareNodes) (:705): the libstdc++ introsort, whose order among equal keys the result
-            // depends on, run as rounds of independent partition steps (one thread per pending range) + independent leaf insertion
+            // depends on, run as rounds of independent partition steps (a warp per partition step) + independent leaf insertion
             // sorts -- exact_math.h: libstdcxx_sort_rounds_host is the same sequence, checked against std::sort on the host
-            cta_libstdcxx_sort(S.v, q, reinterpret_cast<SxTask*>(S.scanA), reinterpret_cast<SxTask*>(S.scanA + 3 * MN),
-                               reinterpret_cast<SxTask*>(S.scanA + 3 * MN) + MN / 6, s_sortCnt);
-            for (int s = tid; s < m; s += QT_NT) S.proc[s] = -1;
-            __syncthreads();
+            SxTask* tasks = reinterpret_cast<SxTask*>(childCnt);   // childPos is dead until step E: the partition's stop lists
+            warp_libstdcxx_sort(v, q, tasks, tasks + q / 2 + 1, tasks + q / 2 + 1 + q / 17 + 1, childPos, childPos + G.qtNodes, lane);
+            QT_ONLY(if (lane == 0) tsort = clock64() - tp;)
+            for (int s = lane; s < m; s += 32) proc[s] = -1;
+            __syncwarp();
             P0 = q;
-            for (int j = tid; j < q; j += QT_NT) {   // processed from the back (:706)
+            for (int j = lane; j < q; j += 32) {   // processed from the back (:706)
                 const int pi = q - 1 - j;
-                S.proc[S.v[j].node] = pi; S.procNode[pi] = S.v[j].node;
+                proc[v[j].node] = (int16_t)pi; procNode[pi] = v[j].node;
             }
         }
-        for (int i = tid; i < 4 * P0; i += QT_NT) S.childCnt[i] = 0;
-        __syncthreads();
-        // --- C. distribute the keys of every split node to its four children (:512-526) ---
-        for (int i = tid; i < n; i += QT_NT) {
-            const int s = nodeOf[i], pi = S.proc[s];
-            if (pi >= 0) {
-                int mx, my;
-                const uint32_t c = cand[i];
-                const int ch = qt_child(bndC[s], cand_x(c), cand_y(c), mx, my);
-                atomicAdd(&S.childCnt[4 * pi + ch], 1);
+        for (int i = lane; i < 4 * P0; i += 32) childCnt[i] = 0;
+        __syncwarp();
+        // --- C. distribute the keys of every split node to its four children (:512-526); the child index goes to nodeOf's bits 12-13.
+        //        Four keys per lane and sweep, their loads issued before any of them is used ---
+        for (int i0 = 0; i0 < n; i0 += 128) {
+            int s[4], pi[4];
+            uint32_t c[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = i0 + 32 * j + lane;
+                s[j] = i < n ? nodeOf[i] : -1; c[j] = i < n ? cand[i] : 0;
             }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) pi[j] = s[j] >= 0 ? proc[s[j]] : -1;
+            QtNode nd[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) if (pi[j] >= 0) nd[j] = bndC[s[j]];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (pi[j] >= 0) {
+                    int mx, my;
+                    const int ch = qt_child(nd[j], cand_x(c[j]), cand_y(c[j]), mx, my);
+                    nodeOf[i0 + 32 * j + lane] = (uint16_t)(s[j] | ch << 12);
+                    atomicAdd(&childCnt[4 * pi[j] + ch], 1);
+                }
         }
-        __syncthreads();
-        // --- D. in the careful phase stop as soon as the list reaches N nodes (:755-756) ---
-        int Pn = P0;
-        for (int pi = tid; pi < P0; pi += QT_NT) {
-            const int* cc = S.childCnt + 4 * pi;
-            S.scanA[pi] = (cc[0] > 0) + (cc[1] > 0) + (cc[2] > 0) + (cc[3] > 0);
-        }
-        __syncthreads();
-        // exclusive scan of k -> scanA; keep k in childPos scratch? recompute instead
-        const int totalK = block_prefix<QT_NT>(P0, S.scanA, s_warp, [&](int pi) { return S.scanA[pi]; });
-        if (careful) {
-            if (tid == 0) s_P = P0;
-            __syncthreads();
-            for (int pi = tid; pi < P0; pi += QT_NT) {
-                const int* cc = S.childCnt + 4 * pi;
-                const int k = (cc[0] > 0) + (cc[1] > 0) + (cc[2] > 0) + (cc[3] > 0);
-                const int sizeAfter = prevSize + (S.scanA[pi] + k) - (pi + 1);
-                if (sizeAfter >= N) atomicMin(&s_P, pi + 1);
+        __syncwarp();
+        // --- D. children per processed node; in the careful phase stop as soon as the list reaches N nodes (:755-756) ---
+        int Pn = P0, totalChildren = 0;
+        for (int pi0 = 0; pi0 < P0; pi0 += 32) {
+            const int pi = pi0 + lane;
+            int k = 0;
+            if (pi < P0) { const int* cc = childCnt + 4 * pi; k = (cc[0] > 0) + (cc[1] > 0) + (cc[2] > 0) + (cc[3] > 0); }
+            const int inc = warp_incl_scan(k, lane);
+            if (pi < P0) kExcl[pi] = (int16_t)(totalChildren + inc - k);
+            if (careful) {
+                const unsigned hit = __ballot_sync(0xffffffffu, pi < P0 && prevSize + (totalChildren + inc) - (pi + 1) >= N);
+                if (hit) {
+                    const int h = __ffs(hit) - 1;
+                    Pn = pi0 + h + 1;
+                    totalChildren += __shfl_sync(0xffffffffu, inc, h);
+                    break;
+                }
             }
-            __syncthreads();
-            Pn = s_P;
-            for (int pi = Pn + tid; pi < P0; pi += QT_NT) S.proc[S.procNode[pi]] = -1;
-            __syncthreads();
+            totalChildren += __shfl_sync(0xffffffffu, inc, 31);
         }
-        // children of the first Pn processed nodes: inclusive prefix at Pn-1
-        int totalChildren;
-        if (Pn == P0) totalChildren = totalK;
-        else totalChildren = S.scanA[Pn];   // exclusive prefix at Pn == sum over pi < Pn
+        for (int pi = Pn + lane; pi < P0; pi += 32) proc[procNode[pi]] = -1;
+        __syncwarp();
         // --- E/G. positions of the children: blocks in reverse processing order, n4..n1 inside ---
-        for (int pi = tid; pi < Pn; pi += QT_NT) {
-            const int* cc = S.childCnt + 4 * pi;
+        for (int pi = lane; pi < Pn; pi += 32) {
+            const int* cc = childCnt + 4 * pi;
             const int k = (cc[0] > 0) + (cc[1] > 0) + (cc[2] > 0) + (cc[3] > 0);
-            const int blockStart = totalChildren - (S.scanA[pi] + k);
+            const int blockStart = totalChildren - (kExcl[pi] + k);
             int after = 0;
-            const QtNode pn = bndC[S.procNode[pi]];
+            const QtNode pn = bndC[procNode[pi]];
             int mx, my;
             qt_child(pn, 0, 0, mx, my);
             for (int ch = 3; ch >= 0; --ch) {
                 if (cc[ch] > 0) {
                     const int pos = blockStart + after;
                     ++after;
-                    S.childPos[4 * pi + ch] = pos;
+                    childPos[4 * pi + ch] = (int16_t)pos;
                     QtNode c;
                     c.ulx = (ch & 1) ? (int16_t)mx : pn.ulx; c.brx = (ch & 1) ? pn.brx : (int16_t)mx;
                     c.uly = (ch & 2) ? (int16_t)my : pn.uly; c.bry = (ch & 2) ? pn.bry : (int16_t)my;
                     bndN[pos] = c; cntN[pos] = cc[ch];
-                } else S.childPos[4 * pi + ch] = -1;
+                } else childPos[4 * pi + ch] = -1;
             }
         }
         // --- F. unsplit nodes keep their order behind the new blocks ---
-        for (int s = tid; s < m; s += QT_NT) S.keepPos[s] = S.proc[s] < 0;
-        __syncthreads();
-        const int nKeep = block_prefix<QT_NT>(m, S.keepPos, s_warp, [&](int s) { return S.keepPos[s]; });
-        for (int s = tid; s < m; s += QT_NT) {
-            if (S.proc[s] < 0) {
-                const int pos = totalChildren + S.keepPos[s];
-                S.keepPos[s] = pos;
+        int nKeep = 0;
+        for (int s0 = 0; s0 < m; s0 += 32) {
+            const int s = s0 + lane;
+            const bool keep = s < m && proc[s] < 0;
+            const unsigned b = __ballot_sync(0xffffffffu, keep);
+            if (keep) {
+                const int pos = totalChildren + nKeep + __popc(b & lanemask_lt());
+                keepPos[s] = (int16_t)pos;
                 bndN[pos] = bndC[s]; cntN[pos] = cntC[s];
             }
+            nKeep += __popc(b);
         }
+        __syncwarp();
         // --- new expandable list in creation order (processing order, n1..n4) (:634-668) ---
-        for (int i = tid; i < 4 * Pn; i += QT_NT) S.scanA[i] = S.childCnt[i] > 1;
-        __syncthreads();
-        const int qNew = block_prefix<QT_NT>(4 * Pn, S.scanA, s_warp, [&](int i) { return S.scanA[i]; });
-        for (int i = tid; i < 4 * Pn; i += QT_NT) {
-            if (S.childCnt[i] > 1) {
-                QtSort e; e.size = S.childCnt[i]; e.node = S.childPos[i]; e.ulx = bndN[e.node].ulx;
-                S.v[S.scanA[i]] = e;
+        int qNew = 0;
+        for (int i0 = 0; i0 < 4 * Pn; i0 += 32) {
+            const int i = i0 + lane;
+            const bool e = i < 4 * Pn && childCnt[i] > 1;
+            const unsigned b = __ballot_sync(0xffffffffu, e);
+            if (e) {
+                QtSort x; x.size = childCnt[i]; x.node = childPos[i]; x.ulx = bndN[x.node].ulx;
+                v[qNew + __popc(b & lanemask_lt())] = x;
             }
+            qNew += __popc(b);
         }
         // --- H. re-home the keys ---
-        for (int i = tid; i < n; i += QT_NT) {
-            const int s = nodeOf[i], pi = S.proc[s];
-            if (pi >= 0) {
-                int mx, my;
-                const uint32_t c = cand[i];
-                const int ch = qt_child(bndC[s], cand_x(c), cand_y(c), mx, my);
-                nodeOf[i] = (uint16_t)S.childPos[4 * pi + ch];
-            } else nodeOf[i] = (uint16_t)S.keepPos[s];
+        for (int i0 = 0; i0 < n; i0 += 128) {
+            int t[4], pi[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) t[j] = i0 + 32 * j + lane < n ? nodeOf[i0 + 32 * j + lane] : 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) pi[j] = proc[t[j] & 0xFFF];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) t[j] = pi[j] >= 0 ? childPos[4 * pi[j] + (t[j] >> 12)] : keepPos[t[j] & 0xFFF];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) if (i0 + 32 * j + lane < n) nodeOf[i0 + 32 * j + lane] = (uint16_t)t[j];
         }
-        __syncthreads();
+        __syncwarp();
+        QT_STAMP(te);
+        QT_ADD(3, tsort);
+        QT_ADD(careful ? 4 : 2, te - tp - tsort);
+        QT_ADD(6, 1);
+        QT_ADD(7, careful ? 1 : 0);
         m = totalChildren + nKeep;
         q = qNew;
-        cur ^= 1;
+        { QtNode* t = bndC; bndC = bndN; bndN = t; int* c = cntC; cntC = cntN; cntN = c; }
         // --- termination (:684-764) ---
         if (m >= N || m == prevSize) finish = true;
         else if (!careful && m + 3 * q > N) careful = true;
     }
+    QT_STAMP(t3);
 
-    // ---- best response per node, first maximum in candidate order (:767-783) ----
-    for (int s = tid; s < m; s += QT_NT) S.best[s] = 0ull;
-    __syncthreads();
-    for (int i = tid; i < n; i += QT_NT) {
-        const unsigned long long key = ((unsigned long long)cand_s(cand[i]) << 32) | (unsigned)(0xFFFFFFFFu - (unsigned)i);
-        atomicMax(&S.best[nodeOf[i]], key);
-    }
-    __syncthreads();
-    if (tid == 0) {
+    // ---- best response per node, first maximum in candidate order (:767-783): key = score << 24 | ~i (i < 2^24, checked on the host) ----
+    unsigned* best = reinterpret_cast<unsigned*>(childCnt);
+    for (int s = lane; s < m; s += 32) best[s] = 0u;
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) atomicMax(&best[nodeOf[i]], ((unsigned)cand_s(cand[i]) << 24) | (0xFFFFFFu - (unsigned)i));
+    __syncwarp();
+    if (lane == 0) {
         P.selCount[f * kMaxLevels + l] = m;
         if (m > G.selCap) atomicOr(&P.status[f], 1);
     }
     const int mOut = min(m, G.selCap);
-    // ---- orientation: one warp per keypoint, lane = row of the radius-15 disc (:76-103) ----
-    int pitch;
-    const uint8_t* img = plane_ptr(P, f, l, pitch);
-    const int wid = tid >> 5, lane = tid & 31;
-    for (int s = wid; s < mOut; s += QT_NT / 32) {
-        const unsigned idx = 0xFFFFFFFFu - (unsigned)(S.best[s] & 0xFFFFFFFFull);
-        const uint32_t c = cand[idx];
-        const int x = cand_x(c) + G.minBX, y = cand_y(c) + G.minBY;
-        // lane = column u of the radius-15 disc, rows walked together: every load instruction of the warp reads one contiguous 31-byte
-        // row segment (one or two sectors) instead of 31 different rows (ncu r2a: 28 % of the kernel's stall samples sat on the
-        // row-per-lane form of this loop, all long-scoreboard)
-        int m10 = 0, m01 = 0;
-        {
-            const int u = lane - HALF_PATCH;
-            const int au = u < 0 ? -u : u;
-            const uint8_t* centre = img + (size_t)y * pitch + x + (lane < 31 ? u : 0);
-            int colsum = 0;
-#pragma unroll
-            for (int v = -HALF_PATCH; v <= HALF_PATCH; ++v) {
-                const int px = (lane < 31 && au <= c_umax[v < 0 ? -v : v]) ? centre[v * pitch] : 0;
-                colsum += px; m01 += v * px;
-            }
-            m10 = u * colsum;
-        }
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            m10 += __shfl_xor_sync(0xffffffffu, m10, o);
-            m01 += __shfl_xor_sync(0xffffffffu, m01, o);
-        }
-        if (lane == 0) {
-            SelKp k; k.x = (int16_t)x; k.y = (int16_t)y; k.response = cand_s(c);
-            k.angle = fast_atan2_deg((float)m01, (float)m10);
-            sel[s] = k;
-        }
+    for (int s = lane; s < mOut; s += 32) {
+        const uint32_t c = cand[0xFFFFFFu - (best[s] & 0xFFFFFFu)];
+        SelKp k; k.x = (int16_t)(cand_x(c) + G.minBX); k.y = (int16_t)(cand_y(c) + G.minBY); k.response = cand_s(c);
+        sel[s] = k;
     }
+    QT_STAMP(t4);
+    QT_ADD(5, t4 - t3);
+    QT_ADD(8, 1);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -956,7 +1041,7 @@ __global__ void __launch_bounds__(AS_NT) assemble_kernel(ExtractParams P) {
             OrbKeyPoint o;
             o.x = (float)k.x; o.y = (float)k.y;
             if (l != 0) { o.x = fmul(o.x, P.lv[l].scale); o.y = fmul(o.y, P.lv[l].scale); }
-            o.size = P.lv[l].sizeScaled; o.angle = k.angle; o.response = (float)k.response;
+            o.size = P.lv[l].sizeScaled; o.angle = 0.f; o.response = (float)k.response;   // the angle: orient_describe_kernel
             o.octave = l; o.class_id = -1;
             out[at] = o;
         }
@@ -969,12 +1054,14 @@ __global__ void __launch_bounds__(AS_NT) assemble_kernel(ExtractParams P) {
 }
 
 // ------------------------------------------------------------------------------------------
-// K6: rotated BRIEF.  One warp per keypoint, lane = descriptor byte.
-// Reference: computeOrbDescriptor src/ORBextractor.cc:107-146 on the blurred plane.
+// K6: orientation + rotated BRIEF.  One warp per selected keypoint of the batch.
+// Reference: IC_Angle src/ORBextractor.cc:76-103 on the pyramid plane, then computeOrbDescriptor
+// :107-146 on the blurred plane with lane = descriptor byte.  The angle goes to the output slab,
+// where assemble_kernel left it unset.
 // ------------------------------------------------------------------------------------------
 constexpr int DS_NT = 256;
 
-__global__ void __launch_bounds__(DS_NT) describe_kernel(ExtractParams P) {
+__global__ void __launch_bounds__(DS_NT) orient_describe_kernel(ExtractParams P) {
     __shared__ char4 s_pat[8][32];   // [pair-in-byte][byte] -> conflict-free across lanes
     const int f = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
     for (int i = tid; i < 256; i += DS_NT) {
@@ -991,10 +1078,33 @@ __global__ void __launch_bounds__(DS_NT) describe_kernel(ExtractParams P) {
     const int at = P.dstIndex[(size_t)f * P.selStride + slot];
     if (at < 0) return;
     const SelKp k = P.sel[(size_t)f * P.selStride + slot];
+    int pitch;
+    // lane = column u of the radius-15 disc, rows walked together: every load instruction of the warp reads one contiguous 31-byte
+    // row segment (one or two sectors) instead of 31 different rows
+    int m10 = 0, m01 = 0;
+    {
+        const uint8_t* img = plane_ptr(P, f, l, pitch);
+        const int u = lane - HALF_PATCH;
+        const int au = u < 0 ? -u : u;
+        const uint8_t* centre = img + (size_t)k.y * pitch + k.x + (lane < 31 ? u : 0);
+        int colsum = 0;
+#pragma unroll
+        for (int v = -HALF_PATCH; v <= HALF_PATCH; ++v) {
+            const int px = (lane < 31 && au <= c_umax[v < 0 ? -v : v]) ? centre[v * pitch] : 0;
+            colsum += px; m01 += v * px;
+        }
+        m10 = u * colsum;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        m10 += __shfl_xor_sync(0xffffffffu, m10, o);
+        m01 += __shfl_xor_sync(0xffffffffu, m01, o);
+    }
+    const float angle = fast_atan2_deg((float)m01, (float)m10);
+    if (lane == 0) reinterpret_cast<OrbKeyPoint*>(P.outKp)[(size_t)f * P.outCap + at].angle = angle;
     const float factorPI = 0.01745329238474369049072265625f;   // (float)(CV_PI/180.f), :106
     float a, b;
-    sincosf_glibc(fmul(k.angle, factorPI), &b, &a);
-    int pitch;
+    sincosf_glibc(fmul(angle, factorPI), &b, &a);
     const uint8_t* img = blur_ptr(P, f, l, pitch);
     const uint8_t* c = img + (size_t)k.y * pitch + k.x;
     int val = 0;

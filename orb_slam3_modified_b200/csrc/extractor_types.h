@@ -21,6 +21,7 @@ struct LevelGeom {
     int nDesired;             // mnFeaturesPerLevel[level]
     int selOff, selCap;       // selected-keypoint slots of this level inside one frame
     int nIni; float hX;       // quadtree roots (:559-561)
+    int qtNodes;              // quadtree list capacity: max(nDesired + 3, 4 nIni) + 4
     float scale; float sizeScaled;    // mvScaleFactor[level], (float)(int)(31*scale)
     int area2x;               // level is an exact 2x decimation of the previous (cv::resize -> INTER_AREA)
     uint32_t xtabOff, ytabOff;        // resize coefficient tables (entries, not bytes)
@@ -64,12 +65,38 @@ __host__ __device__ inline FastSmem fast_smem_layout(int boxW, int boxH, int iw,
     return L;
 }
 
-// Selected keypoint before output assembly.
+// Selected keypoint before output assembly (its angle is computed by orient_describe_kernel).
 struct SelKp {
     int16_t x, y;             // level coordinates (border offset already added)
     int32_t response;
-    float angle;
 };
+
+// Quadtree list nodes and the shared-memory slab of one quadtree warp (one (level, frame) problem).  Host and device both use the
+// layout, so the launch size is exactly what the kernel addresses.  A node id shares nodeOf's 16 bits with a 2-bit child index
+// (bits 12-13), hence QT_MAX_NODES.
+constexpr int QT_MAX_NODES = 4096;
+constexpr int QT_SMEM_CANDS = 2048;   // candidates kept in shared memory at the level with the largest node state (more at the others)
+struct QtNode { int16_t ulx, uly, brx, bry; };
+struct QtSort { int size; int16_t ulx, node; };
+struct QtLayout { int bnd0, bnd1, cnt0, cnt1, scratch, v, proc, procNode, keepPos, kExcl, childPos, cand; };
+// scratch: 4 child counts per processed node; in turn also the sort's task lists, the cell offsets of the gather and the best keys
+__host__ __device__ inline QtLayout qt_layout(int mn, int nCells) {
+    QtLayout L;
+    int o = 0;
+    L.bnd0 = o; o += 8 * mn;
+    L.bnd1 = o; o += 8 * mn;
+    L.cnt0 = o; o += 4 * mn;
+    L.cnt1 = o; o += 4 * mn;
+    L.scratch = o; o += 16 * mn > 4 * (nCells + 1) ? 16 * mn : 4 * (nCells + 1);
+    L.v = o; o += 8 * mn;
+    L.proc = o; o += 2 * mn;
+    L.procNode = o; o += 2 * mn;
+    L.keepPos = o; o += 2 * mn;
+    L.kExcl = o; o += 2 * mn;
+    L.childPos = o; o += 8 * mn;
+    L.cand = (o + 15) & ~15;          // then uint32 cand[c], uint16 nodeOf[c] for c = (slab - cand) / 6
+    return L;
+}
 
 struct ExtractParams {
     int nlevels, batch;
@@ -95,7 +122,7 @@ struct ExtractParams {
     // outputs
     void* outKp; uint8_t* outDesc; int outCap; int* outN; int* outMono;
     int* status;                                    // [batch] sticky error flags
-    int maxNodes, maxCellsPerLevel;
+    int qtSlab;                                     // shared-memory bytes per quadtree warp
     int dbg;
 };
 
