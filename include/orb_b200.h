@@ -461,6 +461,48 @@ int orbm_search_by_bow(orbm_handle* h, const OrbmBowFrame* KF, const uint8_t* kf
  * match12 [KF1.N] = feature of KF2 whose map point goes to vpMatches12[idx1] (-1 = NULL).  KF1.N <= max_mappoints, KF2.N <= max_keypoints. */
 int orbm_search_by_bow_kf(orbm_handle* h, const OrbmBowFrame* KF1, const uint8_t* point1, const OrbmBowFrame* KF2, const uint8_t* point2, float nnratio,
                           int checkOrientation, int32_t* match12, int* nmatches);
+/* LoopClosing::DetectCommonRegionsFromBoW (src/LoopClosing.cc, v1.0) up to the Sim3Solver, for several place-recognition queries: per
+ * candidate pKFi of vpBowCand, in order,
+ *   1. NULL or isBad(): SKIPPED;
+ *   2. vpCovKFi = pKFi->GetBestCovisibilityKeyFrames(10), [pKFi] when empty, else [pKFi, cov1, ..., cov(n-1), cov0];
+ *   3. an entry of vpCovKFi in mpCurrentKF->GetConnectedKeyFrames(): ABORTED_NEAR (bAbortByNearKF);
+ *   4. otherwise RAN: ORBmatcher(0.9, true).SearchByBoW(mpCurrentKF, vpCovKFi[j], vvpMatchedMPs[j]) for every non-bad entry j;
+ *   5. the merge: for j, k ascending, a good point vvpMatchedMPs[j][k] not yet in spMatchedMPi is inserted, counted in numBoWMatches and
+ *      written to vpMatchedPoints[k] / vpKeyFrameMatchedMP[k] (a later j overwrites slot k only with a point not seen before).
+ * The caller keeps `if(numBoWMatches >= nBoWMatches)` and everything after it (Sim3Solver, SearchByProjection, OptimizeSim3).  The map is
+ * read once, at the call; candidates do not change anything another candidate's sweep reads, so a query may hold the loop candidates and
+ * the merge candidates of one keyframe.  Two launches whatever nQueries (the sweep: one CTA per (current keyframe, entry)
+ * pair; the merge: one CTA per RAN candidate), ONE upload through the handle's staging and ONE download; orbm_last_launch_count() is 2,
+ * or 0 when no candidate is RAN.  Host pointers.
+ * ORB_ERR_ARG before any launch, the outputs unchanged: a negative count, nKF < 1, a null pointer a query needs, an index out of range
+ * (cand in [-1, nKF) without 0, cov in [1, nKF), point in [-1, nPoints)), covStart not starting at 0 or decreasing, more than 10
+ * covisibles, nEntries outside [0, N], an unsorted or out-of-range FeatureVector, kf[0].N > max_mappoints or a candidate / covisible
+ * with N > max_keypoints.  ORB_ERR_CAPACITY: more than 2^31 - 1 features in the keyframes the call uploads. */
+enum { ORBM_CR_SKIPPED = 0, ORBM_CR_ABORTED_NEAR = 1, ORBM_CR_RAN = 2 };
+enum { ORBM_CR_MAX_COV = 11 };
+typedef struct OrbmCommonRegionsKF {
+    OrbmBowFrame frame;            /* N, mvKeysUn, mDescriptors and the FeatureVector as orbv_transform_batch writes it */
+    const int32_t* point;          /* [frame.N] GetMapPointMatches() as point-table indices, -1 = NULL */
+    int bad;                       /* isBad() */
+    int connected;                 /* in mpCurrentKF->GetConnectedKeyFrames() */
+} OrbmCommonRegionsKF;
+typedef struct OrbmCommonRegionsQuery {
+    int nKF;
+    const OrbmCommonRegionsKF* kf; /* [nKF] kf[0] = mpCurrentKF, then the candidates and their covisibles */
+    int nPoints;
+    const uint8_t* pointBad;       /* [nPoints] isBad(); each MapPoint* of the query once */
+    int nCand;
+    const int32_t* cand;           /* [nCand] vpBowCand as table indices (loop candidates, then merge candidates), -1 = NULL */
+    const int32_t* covStart;       /* [nCand + 1] */
+    const int32_t* cov;            /* [covStart[nCand]] each candidate's GetBestCovisibilityKeyFrames(10) */
+    uint8_t* status;               /* [nCand] out: ORBM_CR_* */
+    int32_t* covList;              /* [nCand][11] out: vpCovKFi as table indices, -1 padded (empty unless RAN) */
+    int32_t* nmatches;             /* [nCand][11] out: SearchByBoW's return per entry, -1 where skipped or absent */
+    int32_t* numBoWMatches;        /* [nCand] out: 0 unless RAN */
+    int32_t* matchedCov;           /* [nCand][kf[0].frame.N] out: j of vpKeyFrameMatchedMP[k], -1 = NULL */
+    int32_t* matchedPoint;         /* [nCand][kf[0].frame.N] out: point index of vpMatchedPoints[k], -1 = NULL */
+} OrbmCommonRegionsQuery;
+int orbm_common_regions_bow_batch(orbm_handle* h, int nQueries, const OrbmCommonRegionsQuery* queries);
 
 /* bool Tracking::TrackReferenceKeyFrame() (reference src/Tracking.cc:2723, monocular; the mono-inertial path runs the same body before
  * the IMU is initialised) after Frame::ComputeBoW, for `batch` streams in four launches whatever the batch size.  The caller computes the

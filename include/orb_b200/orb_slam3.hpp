@@ -224,6 +224,21 @@ public:
     void KeyFrameCullingBatch(const std::vector<OrbmCullingMap>& maps) {
         orb_check(orbm_keyframe_culling_batch(detail::matcher_handle(1, 1, device_), (int)maps.size(), maps.data()), "orbm_keyframe_culling_batch");
     }
+    // LoopClosing::DetectCommonRegionsFromBoW up to the Sim3Solver for several place-recognition queries in two launches
+    // (orbm_common_regions_bow_batch): every query's outputs receive each candidate's status, vpCovKFi, the SearchByBoW counts, numBoWMatches
+    // and the merged vpKeyFrameMatchedMP / vpMatchedPoints; the caller replays them and keeps the reference's text from
+    // `if(numBoWMatches >= nBoWMatches)` on (INTEGRATION.md §2).  The searches use the reference's ORBmatcher(0.9, true), whatever this
+    // object's settings.
+    void CommonRegionsBoWBatch(const std::vector<OrbmCommonRegionsQuery>& queries) {
+        int maxK = 1, maxM = 1;
+        for (const OrbmCommonRegionsQuery& q : queries)
+            for (int e = 0; q.kf && e < q.nKF; ++e) {
+                int& need = e == 0 ? maxM : maxK;
+                if (q.kf[e].frame.N > need) need = q.kf[e].frame.N;
+            }
+        orb_check(orbm_common_regions_bow_batch(detail::matcher_handle(maxK, maxM, device_), (int)queries.size(), queries.data()),
+                  "orbm_common_regions_bow_batch");
+    }
     // Tracking::UpdateLocalMap's UpdateLocalKeyFrames and UpdateLocalPoints for a batch of streams in one launch (orbm_update_local_map_batch).
     // `out` receives every stream's local keyframes, reference keyframe and local points, and the local map in the slabs of
     // OrbmLocalMapBatch; the caller replays the marks, mpReferenceKF and the NULLing of the voting frame's bad points (INTEGRATION.md §2).

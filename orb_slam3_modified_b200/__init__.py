@@ -92,6 +92,7 @@ SIGNATURES = {
     'orbm_search_for_initialization': (_i, [_vp, _vp, _vp, _vp, _i, _f, _i, _vp, _vp]),
     'orbm_search_by_bow': (_i, [_vp, _vp, _vp, _vp, _f, _i, _vp, _vp]),
     'orbm_search_by_bow_kf': (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _vp, _vp]),
+    'orbm_common_regions_bow_batch': (_i, [_vp, _i, _vp]),
     'orbm_fuse_search': (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
     'orbm_fuse_search_batch': (_i, [_vp, _i, _vp]),
     'orbm_fuse_search_sim3': (_i, [_vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
@@ -464,6 +465,47 @@ class _OrbmFusePoints(C.Structure):
 class _OrbmFuseItem(C.Structure):
     _fields_ = [('KF', _OrbmFrame), ('invLevelSigma2', C.c_void_p), ('logScaleFactor', C.c_float), ('Tcw7', C.c_float * 7), ('Ow', C.c_float * 3),
                 ('cam', C.c_float * 4), ('th', C.c_float), ('pts', _OrbmFusePoints), ('bestIdx', C.c_void_p), ('bestDist', C.c_void_p)]
+
+
+#: OrbmCommonRegionsQuery's candidate statuses (ORBM_CR_*) and the length of vpCovKFi's rows (include/orb_b200.h)
+CR_SKIPPED, CR_ABORTED_NEAR, CR_RAN = range(3)
+CR_MAX_COV = 11
+
+
+class OrbmCommonRegionsKF(C.Structure):
+    """One keyframe of an OrbmCommonRegionsQuery's table (include/orb_b200.h)."""
+    _fields_ = [('frame', _OrbmBowFrame), ('point', C.c_void_p), ('bad', C.c_int), ('connected', C.c_int)]
+
+
+class OrbmCommonRegionsQuery(C.Structure):
+    """One place-recognition query of orbm_common_regions_bow_batch (include/orb_b200.h)."""
+    _fields_ = [('nKF', C.c_int), ('kf', C.POINTER(OrbmCommonRegionsKF)), ('nPoints', C.c_int), ('pointBad', C.c_void_p), ('nCand', C.c_int)] + \
+               [(n, C.c_void_p) for n in ('cand', 'covStart', 'cov', 'status', 'covList', 'nmatches', 'numBoWMatches', 'matchedCov', 'matchedPoint')]
+
+
+def common_regions_struct(q):
+    """OrbmCommonRegionsQuery over query dict `q` with fresh outputs: (struct, out dict, objects to keep alive).  `q`: kfs = [dict(kps,
+    desc, fv=(nodes, features), point, bad, connected)] (entry 0 the current keyframe), pointBad [nPoints], cand [nCand] (-1 = NULL),
+    cov = one list of table indices per candidate (GetBestCovisibilityKeyFrames(10))."""
+    keep = []
+    table = (OrbmCommonRegionsKF * max(len(q['kfs']), 1))()
+    for e, kf in enumerate(q['kfs']):
+        a = [_c(kf['kps'], KP_DTYPE), _c(kf['desc'], np.uint8).reshape(-1, 32), _c(kf['fv'][0], np.int32), _c(kf['fv'][1], np.int32),
+             _c(kf['point'], np.int32)]
+        keep.append(a)
+        table[e] = OrbmCommonRegionsKF(_OrbmBowFrame(len(a[0]), a[0].ctypes.data, a[1].ctypes.data, len(a[2]), a[2].ctypes.data, a[3].ctypes.data),
+                                       a[4].ctypes.data, int(kf['bad']), int(kf['connected']))
+    pbad, cand = _c(q['pointBad'], np.uint8), _c(q['cand'], np.int32)
+    cov_start = np.zeros(len(cand) + 1, np.int32)
+    cov_start[1:] = np.cumsum([len(c) for c in q['cov']])
+    cov = np.array([e for c in q['cov'] for e in c], np.int32)
+    nC, N0 = len(cand), len(q['kfs'][0]['kps']) if q['kfs'] else 0
+    out = dict(status=np.zeros(nC, np.uint8), covList=np.zeros((nC, CR_MAX_COV), np.int32), nmatches=np.zeros((nC, CR_MAX_COV), np.int32),
+               numBoWMatches=np.zeros(nC, np.int32), matchedCov=np.zeros((nC, N0), np.int32), matchedPoint=np.zeros((nC, N0), np.int32))
+    keep += [table, pbad, cand, cov_start, cov]
+    s = OrbmCommonRegionsQuery(len(q['kfs']), C.cast(table, C.POINTER(OrbmCommonRegionsKF)), len(pbad), _ptr(pbad), nC, _ptr(cand), _ptr(cov_start),
+                               _ptr(cov), *[_ptr(out[n]) for n in ('status', 'covList', 'nmatches', 'numBoWMatches', 'matchedCov', 'matchedPoint')])
+    return s, out, keep
 
 
 #: OrbmCullingMap's statuses (ORBM_KFC_*, include/orb_b200.h), by code
@@ -1102,6 +1144,19 @@ class ORBmatcher:
         if rc != ORB_OK:
             raise OrbError(rc, 'orbm_search_by_bow_kf')
         return n.value, m12
+
+    def common_regions_bow_batch(self, queries):
+        """``LoopClosing::DetectCommonRegionsFromBoW`` up to the Sim3Solver for several place-recognition queries in two launches
+        (orbm_common_regions_bow_batch): per candidate its status (CR_*), vpCovKFi, SearchByBoW's count per entry, numBoWMatches and the merged
+        vpKeyFrameMatchedMP (as j) / vpMatchedPoints (as point index).  Each query is a dict as :func:`common_regions_struct` takes it.  The
+        searches use the reference's ``ORBmatcher(0.9, true)``, not this matcher's settings.  Returns one dict of arrays per query (the
+        header's output names)."""
+        built = [common_regions_struct(q) for q in queries]
+        arr = (OrbmCommonRegionsQuery * max(len(queries), 1))(*[b[0] for b in built])
+        rc = lib().orbm_common_regions_bow_batch(self._h, len(queries), arr)
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbm_common_regions_bow_batch')
+        return [b[1] for b in built]
 
     @staticmethod
     def _tri_frame(kf, keep):

@@ -695,6 +695,10 @@ struct BowMatchParams {
     // the batched TrackReferenceKeyFrame (orbm_track_reference_keyframe_batch*): streams not in `active` are skipped (null: all);
     // poseActive[f] = the stream is active and nmatches >= gate, nmatchesCopy[f] = nmatches (both null elsewhere)
     const uint8_t* active; uint8_t* poseActive; int* nmatchesCopy; int gate;
+    // orbm_common_regions_bow_batch: CTA f matches the table entries pairEntry[f] = (keyframe side, frame side), whose operands start at
+    // entryBase[entry] and whose counts nKF / nF / eKF / eF are indexed by entry; the outputs and scratch stay at f times the strides.
+    // Null elsewhere: the operands and counts are CTA f's own.
+    const int2* pairEntry; const int* entryBase;
 };
 constexpr int BM_NT = 256;
 __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
@@ -702,10 +706,13 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
     const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (Q.active && !Q.active[f]) { if (tid == 0 && Q.poseActive) Q.poseActive[f] = 0; return; }
     const size_t kb = (size_t)f * Q.kfStride, fb = (size_t)f * Q.fStride;
-    const int nKF = min(Q.nKF[f], Q.kfStride), nF = min(Q.nF[f], Q.fStride), eKF = min(Q.eKF[f], nKF), eF = min(Q.eF[f], nF);
-    const OrbKeyPoint *kpsKF = Q.kpsKF + kb, *kpsF = Q.kpsF + fb;
-    const uint8_t *descKF = Q.descKF + 32 * kb, *descF = Q.descF + 32 * fb, *kfPoint = Q.kfPoint + kb, *fPoint = Q.fPoint ? Q.fPoint + fb : nullptr;
-    const int *fvNodeKF = Q.fvNodeKF + kb, *fvFeatKF = Q.fvFeatKF + kb, *fvNodeF = Q.fvNodeF + fb, *fvFeatF = Q.fvFeatF + fb;
+    int cKF = f, cF = f;
+    size_t kIn = kb, fIn = fb;
+    if (Q.pairEntry) { const int2 pe = Q.pairEntry[f]; cKF = pe.x; cF = pe.y; kIn = (size_t)Q.entryBase[cKF]; fIn = (size_t)Q.entryBase[cF]; }
+    const int nKF = min(Q.nKF[cKF], Q.kfStride), nF = min(Q.nF[cF], Q.fStride), eKF = min(Q.eKF[cKF], nKF), eF = min(Q.eF[cF], nF);
+    const OrbKeyPoint *kpsKF = Q.kpsKF + kIn, *kpsF = Q.kpsF + fIn;
+    const uint8_t *descKF = Q.descKF + 32 * kIn, *descF = Q.descF + 32 * fIn, *kfPoint = Q.kfPoint + kIn, *fPoint = Q.fPoint ? Q.fPoint + fIn : nullptr;
+    const int *fvNodeKF = Q.fvNodeKF + kIn, *fvFeatKF = Q.fvFeatKF + kIn, *fvNodeF = Q.fvNodeF + fIn, *fvFeatF = Q.fvFeatF + fIn;
     int *match = Q.match + fb, *match12 = Q.match12 ? Q.match12 + kb : nullptr, *groupStart = Q.groupStart + (size_t)f * (Q.kfStride + 1);
     uint8_t* evBin = Q.evBin + fb;
     for (int i = tid; i < Q.fStride; i += BM_NT) { match[i] = -1; evBin[i] = 0; }
@@ -794,6 +801,73 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
         if (Q.nmatchesCopy) Q.nmatchesCopy[f] = n;
         if (Q.poseActive) Q.poseActive[f] = n >= Q.gate ? 1 : 0;
     }
+}
+
+// ---------------------------------------------------------------------------------------------
+// The merge of LoopClosing::DetectCommonRegionsFromBoW (step 5 of orbm_common_regions_bow_batch): one CTA per RAN candidate over the
+// matches of its sweep pairs.  Pair t of the candidate holds vpCovKFi[j] with j ascending in t, so the sequential walk "j, k ascending,
+// insert a point not yet in spMatchedMPi" keeps match (t, k) of point p iff t * N0 + k is the least position of p among the candidate's
+// matches.  Pass 1 takes that minimum per point with atomicMin into an open-addressing hash (capacity a power of two >= twice the match
+// bound, so every probe ends); pass 2 counts the kept matches and gives slot k the largest t among them (the last write of the walk);
+// pass 3 resolves slot k's pair into (j, point).  Nothing depends on thread order.
+// ---------------------------------------------------------------------------------------------
+struct CrMergeItem {
+    int pairBegin, nPairs, N0, hashCap;
+    const uint8_t* pointBad;                 // the query's point table
+    int *matchedCov, *matchedPoint, *numBoW; // outputs [N0], [N0], [1]
+    int *hashKey, *hashPos;                  // scratch [hashCap]
+};
+struct CrMergeParams {
+    const CrMergeItem* items;
+    const int* match12; int kfStride;        // the sweep's result: pair f's match12 at f * kfStride
+    const int2* pairEntry; const int* entryBase; const int* slotPoint; const int* pairJ;
+};
+constexpr int CRM_NT = 256;
+__device__ __forceinline__ unsigned cr_hash(int p) { unsigned x = (unsigned)p * 0x9E3779B1u; return x ^ (x >> 15); }
+__global__ void __launch_bounds__(CRM_NT) common_regions_merge_kernel(CrMergeParams P) {
+    __shared__ int s_n;
+    const CrMergeItem& C = P.items[blockIdx.x];
+    const int tid = threadIdx.x, N0 = C.N0, total = C.nPairs * N0;
+    const unsigned mask = (unsigned)C.hashCap - 1u;
+    // the good point pair t brings to current-keyframe feature k, or -1
+    auto pointAt = [&](int t, int k) -> int {
+        const int f = C.pairBegin + t;
+        const int i2 = P.match12[(size_t)f * P.kfStride + k];
+        if (i2 < 0) return -1;
+        const int p = P.slotPoint[P.entryBase[P.pairEntry[f].y] + i2];
+        return (p < 0 || C.pointBad[p]) ? -1 : p;
+    };
+    for (int i = tid; i < C.hashCap; i += CRM_NT) { C.hashKey[i] = -1; C.hashPos[i] = 0x7fffffff; }
+    for (int k = tid; k < N0; k += CRM_NT) C.matchedCov[k] = -1;
+    if (tid == 0) s_n = 0;
+    __syncthreads();
+    for (int i = tid; i < total; i += CRM_NT) {
+        const int p = pointAt(i / N0, i % N0);
+        if (p < 0) continue;
+        for (unsigned s = cr_hash(p) & mask;; s = (s + 1) & mask) {
+            const int prev = atomicCAS(&C.hashKey[s], -1, p);
+            if (prev == -1 || prev == p) { atomicMin(&C.hashPos[s], i); break; }
+        }
+    }
+    __syncthreads();
+    int n = 0;
+    for (int i = tid; i < total; i += CRM_NT) {
+        const int p = pointAt(i / N0, i % N0);
+        if (p < 0) continue;
+        unsigned s = cr_hash(p) & mask;
+        while (C.hashKey[s] != p) s = (s + 1) & mask;
+        if (C.hashPos[s] != i) continue;
+        ++n;
+        atomicMax(&C.matchedCov[i % N0], i / N0);
+    }
+    if (n) atomicAdd(&s_n, n);
+    __syncthreads();
+    for (int k = tid; k < N0; k += CRM_NT) {
+        const int t = C.matchedCov[k];
+        C.matchedPoint[k] = t >= 0 ? pointAt(t, k) : -1;
+        C.matchedCov[k] = t >= 0 ? P.pairJ[C.pairBegin + t] : -1;
+    }
+    if (tid == 0) *C.numBoW = s_n;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1895,6 +1969,176 @@ int orbm_search_by_bow_kf(orbm_handle* h, const OrbmBowFrame* KF1, const uint8_t
                           int checkOrientation, int32_t* match12, int* nmatches) {
     if (!point2 || !match12) { set_error("orbm_search_by_bow_kf: bad argument"); return ORB_ERR_ARG; }
     return search_by_bow_impl(h, KF1, point1, KF2, point2, nnratio, checkOrientation, nullptr, match12, nmatches);
+}
+
+// ORB_ERR_ARG with a message naming the query, or ORB_OK.
+static int check_common_regions_query(const Matcher& m, const OrbmCommonRegionsQuery& q, int qi) {
+    auto bad = [qi](const std::string& what) {
+        set_error("orbm_common_regions_bow_batch: query " + std::to_string(qi) + ": " + what); return ORB_ERR_ARG;
+    };
+    if (q.nKF < 1 || q.nPoints < 0 || q.nCand < 0) return bad("nKF < 1 or a negative count");
+    if (!q.kf) return bad("kf is null");
+    if (q.nPoints > 0 && !q.pointBad) return bad("pointBad is null");
+    if (q.nCand > 0 && (!q.cand || !q.covStart || !q.status || !q.covList || !q.nmatches || !q.numBoWMatches)) return bad("cand / covStart / an output is null");
+    if (q.nCand > 0 && q.kf[0].frame.N > 0 && (!q.matchedCov || !q.matchedPoint)) return bad("matchedCov / matchedPoint is null");
+    for (int e = 0; e < q.nKF; ++e) {
+        const OrbmCommonRegionsKF& K = q.kf[e];
+        const OrbmBowFrame& F = K.frame;
+        const std::string who = "kf " + std::to_string(e) + ": ";
+        if (F.N < 0 || F.nEntries < 0 || F.nEntries > F.N) return bad(who + "N < 0 or nEntries outside [0, N]");
+        if (F.N > (e == 0 ? m.mcap : m.kcap)) return bad(who + (e == 0 ? "N > max_mappoints" : "N > max_keypoints"));
+        if (F.N > 0 && (!F.keypoints || !F.descriptors || !K.point)) return bad(who + "keypoints / descriptors / point is null");
+        if (F.nEntries > 0 && (!F.fvNode || !F.fvFeature)) return bad(who + "fvNode / fvFeature is null");
+        if (!fv_ok(F.fvNode, F.fvFeature, F.nEntries, F.N)) return bad(who + "feature vector not sorted / out of range");
+        for (int i = 0; i < F.N; ++i) if (K.point[i] < -1 || K.point[i] >= q.nPoints) return bad(who + "point index out of range");
+    }
+    if (q.nCand > 0) {
+        if (!csr_ok(q.nCand, q.covStart)) return bad("covStart must start at 0 and not decrease");
+        if (q.covStart[q.nCand] > 0 && !q.cov) return bad("cov is null");
+        for (int c = 0; c < q.nCand; ++c) {
+            if (q.cand[c] < -1 || q.cand[c] == 0 || q.cand[c] >= q.nKF) return bad("cand outside [-1, nKF) or the current keyframe");
+            if (q.covStart[c + 1] - q.covStart[c] > ORBM_CR_MAX_COV - 1) return bad("more than 10 covisibles");
+        }
+        for (int i = 0; i < q.covStart[q.nCand]; ++i)
+            if (q.cov[i] < 1 || q.cov[i] >= q.nKF) return bad("cov outside [1, nKF)");
+    }
+    return ORB_OK;
+}
+
+int orbm_common_regions_bow_batch(orbm_handle* h, int nQueries, const OrbmCommonRegionsQuery* queries) {
+    if (!h || nQueries < 0 || (nQueries > 0 && !queries)) { set_error("orbm_common_regions_bow_batch: bad argument"); return ORB_ERR_ARG; }
+    Matcher& m = h->m;
+    for (int qi = 0; qi < nQueries; ++qi)
+        if (int rc = check_common_regions_query(m, queries[qi], qi)) return rc;
+    // Steps 1-4 on the host: each candidate's vpCovKFi and status, and the (current keyframe, entry) pairs of the RAN candidates.  Only the
+    // keyframes of those pairs are uploaded; `slot` numbers them in the call.
+    struct Ran { int q, c, pairBegin, nPairs; };
+    std::vector<Ran> ran;
+    std::vector<int2> pairEntry;                  // call slots
+    std::vector<int> pairJ, slotQ, slotE;         // pair -> j; slot -> (query, table entry)
+    std::vector<std::vector<int>> slotOf(nQueries);
+    long long nFeat = 0;
+    int maxN0 = 0, maxN = 0;
+    auto slot = [&](int qi, int e) {
+        int& s = slotOf[qi][e];
+        if (s < 0) { s = (int)slotQ.size(); slotQ.push_back(qi); slotE.push_back(e); nFeat += queries[qi].kf[e].frame.N; }
+        return s;
+    };
+    for (int qi = 0; qi < nQueries; ++qi) {
+        const OrbmCommonRegionsQuery& q = queries[qi];
+        slotOf[qi].assign(q.nKF, -1);
+        const int N0 = q.kf[0].frame.N;
+        for (int c = 0; c < q.nCand; ++c) {
+            int32_t* covList = q.covList + (size_t)c * ORBM_CR_MAX_COV;
+            int32_t* nm = q.nmatches + (size_t)c * ORBM_CR_MAX_COV;
+            for (int j = 0; j < ORBM_CR_MAX_COV; ++j) { covList[j] = -1; nm[j] = -1; }
+            q.numBoWMatches[c] = 0;
+            for (int k = 0; k < N0; ++k) { q.matchedCov[(size_t)c * N0 + k] = -1; q.matchedPoint[(size_t)c * N0 + k] = -1; }
+            const int cand = q.cand[c];
+            if (cand < 0 || q.kf[cand].bad) { q.status[c] = ORBM_CR_SKIPPED; continue; }
+            const int c0 = q.covStart[c], nc = q.covStart[c + 1] - c0;
+            int n = 0;
+            covList[n++] = cand;
+            for (int i = 1; i < nc; ++i) covList[n++] = q.cov[c0 + i];
+            if (nc > 0) covList[n++] = q.cov[c0];
+            bool near = false;
+            for (int j = 0; j < n; ++j) near = near || q.kf[covList[j]].connected;
+            if (near) { q.status[c] = ORBM_CR_ABORTED_NEAR; continue; }
+            q.status[c] = ORBM_CR_RAN;
+            Ran r{qi, c, (int)pairJ.size(), 0};
+            for (int j = 0; j < n; ++j) {
+                if (q.kf[covList[j]].bad) continue;
+                pairEntry.push_back(make_int2(slot(qi, 0), slot(qi, covList[j])));
+                pairJ.push_back(j);
+                maxN = std::max(maxN, q.kf[covList[j]].frame.N);
+                ++r.nPairs;
+            }
+            maxN0 = std::max(maxN0, N0);
+            ran.push_back(r);
+        }
+    }
+    m.launches = 0;
+    if (ran.empty()) return ORB_OK;
+    if (nFeat > 0x7fffffffLL) { set_error("orbm_common_regions_bow_batch: more than 2^31 - 1 features to upload"); return ORB_ERR_CAPACITY; }
+    CK(cudaSetDevice(m.device));
+    const size_t nSlots = slotQ.size(), nPairs = pairJ.size(), F = (size_t)std::max<long long>(nFeat, 1);
+    const size_t kfStride = (size_t)std::max(maxN0, 1), fStride = (size_t)std::max(maxN, 1);
+    Staging& S = m.staging;
+    S.begin();
+    const int pKps = S.in(nullptr, sizeof(OrbKeyPoint) * F), pDesc = S.in(nullptr, 32 * F), pFlag = S.in(nullptr, F), pNode = S.in(nullptr, 4 * F),
+              pFeat = S.in(nullptr, 4 * F), pPoint = S.in(nullptr, 4 * F), pBase = S.in(nullptr, 4 * nSlots), pN = S.in(nullptr, 4 * nSlots),
+              pE = S.in(nullptr, 4 * nSlots), pPair = S.in(pairEntry.data(), sizeof(int2) * nPairs), pJ = S.in(pairJ.data(), 4 * nPairs),
+              pItems = S.in(nullptr, sizeof(CrMergeItem) * ran.size()), pNm = S.out(nullptr, 4 * nPairs);
+    std::vector<int> pBad(nQueries, -1);
+    for (int qi = 0; qi < nQueries; ++qi)
+        if (queries[qi].nPoints > 0) pBad[qi] = S.in(queries[qi].pointBad, queries[qi].nPoints);
+    std::vector<int> pOut(ran.size()), pHash(ran.size());
+    std::vector<size_t> cap(ran.size());
+    for (size_t r = 0; r < ran.size(); ++r) {
+        const OrbmCommonRegionsQuery& q = queries[ran[r].q];
+        const size_t N0 = (size_t)q.kf[0].frame.N, c = (size_t)ran[r].c;
+        pOut[r] = S.out(q.matchedCov ? q.matchedCov + c * N0 : nullptr, 4 * N0);
+        S.out(q.matchedPoint ? q.matchedPoint + c * N0 : nullptr, 4 * N0);
+        S.out(q.numBoWMatches + c, 4);
+        size_t hc = 1;
+        while (hc < 2 * (size_t)ran[r].nPairs * N0) hc <<= 1;
+        cap[r] = hc;
+        pHash[r] = S.scratch(8 * hc);
+    }
+    const int pM12 = S.scratch(4 * nPairs * kfStride), pMatch = S.scratch(4 * nPairs * fStride), pGs = S.scratch(4 * nPairs * (kfStride + 1)),
+              pEv = S.scratch(nPairs * fStride);
+    if (int rc = S.reserve()) return rc;
+    OrbKeyPoint* kps = S.host<OrbKeyPoint>(pKps);
+    uint8_t *desc = S.host(pDesc), *flag = S.host(pFlag);
+    int *node = S.host<int>(pNode), *feat = S.host<int>(pFeat), *point = S.host<int>(pPoint), *base = S.host<int>(pBase), *cnt = S.host<int>(pN),
+        *ent = S.host<int>(pE);
+    size_t off = 0;
+    for (size_t s = 0; s < nSlots; ++s) {
+        const OrbmCommonRegionsQuery& q = queries[slotQ[s]];
+        const OrbmCommonRegionsKF& K = q.kf[slotE[s]];
+        const size_t N = (size_t)K.frame.N, E = (size_t)K.frame.nEntries;
+        base[s] = (int)off; cnt[s] = K.frame.N; ent[s] = K.frame.nEntries;
+        if (N) {
+            memcpy(kps + off, K.frame.keypoints, sizeof(OrbKeyPoint) * N);
+            memcpy(desc + 32 * off, K.frame.descriptors, 32 * N);
+            memcpy(point + off, K.point, 4 * N);
+        }
+        if (E) { memcpy(node + off, K.frame.fvNode, 4 * E); memcpy(feat + off, K.frame.fvFeature, 4 * E); }
+        for (size_t i = 0; i < N; ++i) flag[off + i] = K.point[i] < 0 ? 0 : q.pointBad[K.point[i]] ? 2 : 1;
+        off += N;
+    }
+    CrMergeItem* items = S.host<CrMergeItem>(pItems);
+    for (size_t r = 0; r < ran.size(); ++r) {
+        const OrbmCommonRegionsQuery& q = queries[ran[r].q];
+        CrMergeItem& it = items[r];
+        it.pairBegin = ran[r].pairBegin; it.nPairs = ran[r].nPairs; it.N0 = q.kf[0].frame.N; it.hashCap = (int)cap[r];
+        it.pointBad = pBad[ran[r].q] >= 0 ? S.dev(pBad[ran[r].q]) : nullptr;
+        it.matchedCov = S.dev<int>(pOut[r]); it.matchedPoint = S.dev<int>(pOut[r] + 1); it.numBoW = S.dev<int>(pOut[r] + 2);
+        it.hashKey = S.dev<int>(pHash[r]); it.hashPos = it.hashKey + cap[r];
+    }
+    BowMatchParams Q; memset(&Q, 0, sizeof(Q));
+    Q.nKF = Q.nF = S.dev<int>(pN); Q.eKF = Q.eF = S.dev<int>(pE); Q.kfStride = (int)kfStride; Q.fStride = (int)fStride;
+    Q.kpsKF = Q.kpsF = S.dev<OrbKeyPoint>(pKps); Q.descKF = Q.descF = S.dev(pDesc); Q.kfPoint = Q.fPoint = S.dev(pFlag);
+    Q.fvNodeKF = Q.fvNodeF = S.dev<int>(pNode); Q.fvFeatKF = Q.fvFeatF = S.dev<int>(pFeat);
+    Q.nnratio = 0.9f; Q.checkOri = 1; Q.strictLow = 1;          // ORBmatcher matcherBoW(0.9, true) (src/LoopClosing.cc)
+    Q.match12 = S.dev<int>(pM12); Q.match = S.dev<int>(pMatch); Q.nmatches = S.dev<int>(pNm); Q.groupStart = S.dev<int>(pGs); Q.evBin = S.dev(pEv);
+    Q.pairEntry = S.dev<int2>(pPair); Q.entryBase = S.dev<int>(pBase);
+    CrMergeParams P;
+    P.items = S.dev<CrMergeItem>(pItems); P.match12 = Q.match12; P.kfStride = (int)kfStride;
+    P.pairEntry = Q.pairEntry; P.entryBase = Q.entryBase; P.slotPoint = S.dev<int>(pPoint); P.pairJ = S.dev<int>(pJ);
+    cudaStream_t st = m.stream;
+    CK(S.upload(st));
+    bow_match_kernel<<<(unsigned)nPairs, BM_NT, 0, st>>>(Q);
+    CK(cudaGetLastError());
+    common_regions_merge_kernel<<<(unsigned)ran.size(), CRM_NT, 0, st>>>(P);
+    CK(cudaGetLastError());
+    m.launches = 2;
+    CK(S.download(st));
+    const int* nm = S.host<int>(pNm);
+    for (const Ran& r : ran)
+        for (int t = 0; t < r.nPairs; ++t)
+            queries[r.q].nmatches[(size_t)r.c * ORBM_CR_MAX_COV + pairJ[r.pairBegin + t]] = nm[r.pairBegin + t];
+    return ORB_OK;
 }
 
 // One search of fuse_search_kernel's table, host pointers.  invLevelSigma2 == nullptr: no chi-square gate.
