@@ -135,6 +135,36 @@ int orbx_last_launch_count(const orbx_handle* h);
 int orbx_set_profiling(orbx_handle* h, int on);
 int orbx_get_stage_ms(orbx_handle* h, float* ms6);
 
+/* Frame::UndistortKeyPoints (reference src/Frame.cc:747) and Frame::ComputeImageBounds (called at src/Frame.cc:793) for a pinhole camera
+ * with lens distortion (mK, mDistCoef).  A 4-coefficient calibration (k1 k2 p1 p2) passes k3 = 0, which OpenCV treats identically. */
+typedef struct OrbPinholeCamera {
+    float fx, fy, cx, cy;
+    float k1, k2, p1, p2, k3;
+} OrbPinholeCamera;
+/* mvKeysUn from mvKeys for `batch` frames: d_kps / d_kpsUn are [batch][cap] device slabs (as orbx_extract_batch_device writes them),
+ * d_n the [batch] counts.  Rows [0, n[f]) of frame f become copies of mvKeys[i] with pt replaced by cv::undistortPoints(pt, K, mDistCoef,
+ * cv::Mat(), K), bit for bit; size, angle, response, octave and class_id are kept.  With k1 == 0 (either sign) the rows are copied byte for
+ * byte, as the reference's `if(mDistCoef.at<float>(0)==0.0)` does whatever k2, p1, p2 and k3 are.  Rows past n[f], and every row of a frame
+ * with n[f] > cap (the extractor's overflow), are not touched.  d_kpsUn must not overlap d_kps: the stereo matcher and the last-frame search
+ * (OrbmLastFrame.octave) still read mvKeys.  Enqueues ONE launch on `stream` (none for batch == 0) and returns without synchronising.
+ * ORB_ERR_ARG before any launch: a null pointer, batch < 0, cap < 1, overlapping slabs, fx or fy zero, a non-finite camera member. */
+int orbx_undistort_keypoints_device(orbx_handle* h, const OrbPinholeCamera* cam, int batch, const OrbKeyPoint* d_kps, const int* d_n, int cap,
+                                    OrbKeyPoint* d_kpsUn, void* stream);
+/* The same for the frames of the handle's last orbx_extract / orbx_extract_batch call (its resident slabs, orbx_resident_slabs): mvKeysUn
+ * goes to a second [max_batch][orbx_max_keypoints] slab the handle owns (allocated on first use), whose device address *d_kpsUn receives
+ * when d_kpsUn is not NULL -- the `kps` to give the matchers' _resident forms.  It stays valid until the handle is destroyed and is
+ * rewritten by the next call.  When kpsUn is not NULL it receives that slab's [batch][cap] rows (cap must equal orbx_max_keypoints; rows
+ * at or past n[f] are unspecified).  Synchronises.  ORB_ERR_ARG before any launch: the errors of the device form, or a last call that was
+ * not a host-buffer extraction of at least `batch` frames. */
+int orbx_undistort_keypoints(orbx_handle* h, const OrbPinholeCamera* cam, int batch, OrbKeyPoint* kpsUn, int cap, const OrbKeyPoint** d_kpsUn);
+/* mnMinX, mnMaxX, mnMinY, mnMaxY of a cols x rows image into bounds4, computed on `device` with the same device function from the four
+ * undistorted corners (0, cols, 0, rows when k1 == 0).  ONE launch; host pointers.  ORB_ERR_ARG: the camera errors above, cols or rows < 1,
+ * a null pointer. */
+int orbx_image_bounds(const OrbPinholeCamera* cam, int cols, int rows, float* bounds4, int device);
+/* Launches of the calling thread's last orbx_undistort_keypoints[_device] or orbx_image_bounds call (0 after a refused call or an empty
+ * batch).  orbx_last_launch_count() keeps counting extraction launches only. */
+int orbx_undistort_last_launch_count(void);
+
 /* ------------------------------------------------------------------------------------------
  * ORBmatcher (reference include/ORBmatcher.h:36-103): the per-frame projection matchers, the Hamming
  * primitive and the brute-force kNN used by the reference.  All inputs are flat arrays: the host shim

@@ -105,6 +105,21 @@ struct FrameView {
         f.scaleFactors = mvScaleFactors.data(); f.nlevels = (int)mvScaleFactors.size();
         return f;
     }
+    // void Frame::UndistortKeyPoints() (src/Frame.cc:747): mvKeysUn from mvKeys, the keypoints `extractor` returned in its last call, on
+    // the GPU (the extractor's resident slab, no upload).  k1 == 0 copies mvKeys.
+    void UndistortKeyPoints(ORBextractor& extractor, const OrbPinholeCamera& cam, const std::vector<KeyPoint>& mvKeys) {
+        const int cap = orbx_max_keypoints(extractor.handle());
+        std::vector<KeyPoint> slab((size_t)cap);
+        orb_check(orbx_undistort_keypoints(extractor.handle(), &cam, 1, slab.data(), cap, nullptr), "orbx_undistort_keypoints");
+        mvKeysUn.assign(slab.begin(), slab.begin() + (std::ptrdiff_t)mvKeys.size());
+    }
+    // void Frame::ComputeImageBounds(const cv::Mat& imLeft) (called at src/Frame.cc:793): mnMinX, mnMaxX, mnMinY, mnMaxY from the
+    // undistorted image corners (0, cols, 0, rows when k1 == 0).
+    void ComputeImageBounds(const OrbPinholeCamera& cam, int cols, int rows, int device = 0) {
+        float b[4];
+        orb_check(orbx_image_bounds(&cam, cols, rows, b, device), "orbx_image_bounds");
+        mnMinX = b[0]; mnMaxX = b[1]; mnMinY = b[2]; mnMaxY = b[3];
+    }
 };
 
 namespace detail {

@@ -42,6 +42,35 @@ class OrbmNewPointsItem(C.Structure):
     _fields_ = [('in_', OrbmNewPointsIn), ('out', C.c_void_p), ('nNew', C.c_void_p), ('nmatches', C.c_void_p), ('ncreated', C.c_void_p)]
 
 
+class OrbPinholeCamera(C.Structure):
+    """Pinhole calibration with lens distortion (include/orb_b200.h): fx fy cx cy, then k1 k2 p1 p2 k3 (k3 = 0 for 4 coefficients)."""
+    _fields_ = [(n, C.c_float) for n in ('fx', 'fy', 'cx', 'cy', 'k1', 'k2', 'p1', 'p2', 'k3')]
+
+
+def pinhole_camera(K, D):
+    """OrbPinholeCamera from (fx, fy, cx, cy) and 4 or 5 distortion coefficients (k1, k2, p1, p2[, k3])."""
+    D = list(D)
+    if len(D) not in (4, 5):
+        raise ValueError('4 or 5 distortion coefficients expected (k1 k2 p1 p2 [k3])')
+    return OrbPinholeCamera(*[float(v) for v in K], *[float(v) for v in D + [0.0] * (5 - len(D))])
+
+
+def image_bounds(K, D, cols, rows, device=0):
+    """``Frame::ComputeImageBounds``: (mnMinX, mnMinY, mnMaxX, mnMaxY) -- the order the matchers' ``bounds`` take -- of a cols x rows
+    image from its four corners undistorted on the GPU.  With k1 == 0 they are (0, 0, cols, rows)."""
+    cam = pinhole_camera(K, D)
+    out = np.zeros(4, np.float32)
+    rc = lib().orbx_image_bounds(C.byref(cam), int(cols), int(rows), _ptr(out), device)
+    if rc != ORB_OK:
+        raise OrbError(rc, 'orbx_image_bounds')
+    return float(out[0]), float(out[2]), float(out[1]), float(out[3])
+
+
+def undistort_last_launch_count():
+    """Launches of this thread's last undistort_keypoints[_device] / image_bounds call."""
+    return lib().orbx_undistort_last_launch_count()
+
+
 _vp, _i, _f, _d, _sz, _out = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.POINTER(C.c_void_p)
 
 #: (restype, argtypes) of every liborb_b200.so function the package, its tests and its tools call, as include/orb_b200.h declares it.
@@ -69,6 +98,10 @@ SIGNATURES = {
     'orbx_last_launch_count': (_i, [_vp]),
     'orbx_set_profiling': (_i, [_vp, _i]),
     'orbx_get_stage_ms': (_i, [_vp, _vp]),
+    'orbx_undistort_keypoints_device': (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp]),
+    'orbx_undistort_keypoints': (_i, [_vp, _vp, _i, _vp, _i, _out]),
+    'orbx_image_bounds': (_i, [_vp, _i, _i, _vp, _i]),
+    'orbx_undistort_last_launch_count': (_i, []),
     # ORBmatcher
     'orbm_create': (_i, [_out, _i, _i, _i, _i]),
     'orbm_destroy': (None, [_vp]),
@@ -363,6 +396,30 @@ class ORBextractor:
 
     def last_launch_count(self):
         return lib().orbx_last_launch_count(self._h)
+
+    # --- Frame::UndistortKeyPoints (src/Frame.cc:747) ---
+    def undistort_keypoints_device(self, K, D, d_kps, d_n, d_kpsUn, stream=0):
+        """mvKeysUn for the slabs extract_batch_device wrote (torch CUDA tensors): d_kps / d_kpsUn [B, cap, 7] (28-byte rows, not
+        overlapping), d_n [B] i32; K = (fx, fy, cx, cy), D = 4 or 5 coefficients.  Rows past n[f] and overflowing frames are not touched;
+        k1 == 0 copies.  Enqueues one launch on ``stream`` and returns immediately."""
+        cam = pinhole_camera(K, D)
+        B, cap = d_kps.shape[:2]
+        rc = lib().orbx_undistort_keypoints_device(self._h, C.byref(cam), B, _ptr(d_kps), _ptr(d_n), cap, _ptr(d_kpsUn), C.c_void_p(stream))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbx_undistort_keypoints_device')
+
+    def undistort_keypoints(self, K, D, batch=1, host=True):
+        """mvKeysUn for the frames of the last extract / extract_batch call, into a slab the handle owns.  Returns (device address of
+        that [max_batch, max_keypoints] slab -- the ``kps`` of the matchers' resident forms --, and with ``host`` its [batch, cap]
+        KP_DTYPE rows; rows at or past n[f] are unspecified)."""
+        cam = pinhole_camera(K, D)
+        cap = self.max_keypoints
+        out = np.zeros((batch, cap), KP_DTYPE) if host else None
+        d = C.c_void_p()
+        rc = lib().orbx_undistort_keypoints(self._h, C.byref(cam), batch, _ptr(out), cap, C.byref(d))
+        if rc != ORB_OK:
+            raise OrbError(rc, 'orbx_undistort_keypoints')
+        return d.value, out
 
     STAGES = ('pyramid', 'blur', 'fast_cells', 'quadtree_orient', 'assemble', 'brief')
 

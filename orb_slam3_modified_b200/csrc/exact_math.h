@@ -30,6 +30,8 @@ ORB_HD float fsub(float a, float b) { return __fsub_rn(a, b); }
 ORB_HD float fdiv(float a, float b) { return __fdiv_rn(a, b); }
 ORB_HD float ffma(float a, float b, float c) { return __fmaf_rn(a, b, c); }
 ORB_HD double dmul(double a, double b) { return __dmul_rn(a, b); }
+ORB_HD double dadd(double a, double b) { return __dadd_rn(a, b); }
+ORB_HD double dsub(double a, double b) { return __dsub_rn(a, b); }
 ORB_HD double dfma(double a, double b, double c) { return __fma_rn(a, b, c); }
 ORB_HD int round_half_even(float v) { return __float2int_rn(v); }
 ORB_HD float d2f(double v) { return __double2float_rn(v); }
@@ -40,6 +42,8 @@ ORB_HD float fsub(float a, float b) { return a - b; }
 ORB_HD float fdiv(float a, float b) { return a / b; }
 ORB_HD float ffma(float a, float b, float c) { return fmaf(a, b, c); }
 ORB_HD double dmul(double a, double b) { return a * b; }
+ORB_HD double dadd(double a, double b) { return a + b; }
+ORB_HD double dsub(double a, double b) { return a - b; }
 ORB_HD double dfma(double a, double b, double c) { return fma(a, b, c); }
 ORB_HD int round_half_even(float v) { return (int)nearbyintf(v); }
 ORB_HD float d2f(double v) { return (float)v; }

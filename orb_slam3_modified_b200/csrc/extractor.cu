@@ -91,6 +91,7 @@ struct Extractor {
     int maxKp = 0;
     ExtractParams lastQ; bool hasLast = false;   // geometry + plane pointers of the last enqueued call (the pyramid the stereo matcher reads)
     int* d_stereoSad = nullptr; float *d_stereoU = nullptr, *d_stereoD = nullptr; int* h_stereoStatus = nullptr;
+    OrbKeyPoint* d_outKpUn = nullptr;   // mvKeysUn of the resident slab (orbx_undistort_keypoints), allocated on first use
     TmaMaps maps;            // per-level TMA descriptors of the internal pyramid planes (level 0: internal copy)
     CUtensorMap* d_maps = nullptr;   // device copy of `maps`
     TmaMaps pyrMaps;         // pyrMaps.lv[l]: level l-1 with the source box of level l's resize tiles (host copy: passed by value per launch)
@@ -101,7 +102,8 @@ struct Extractor {
     void release() {
         cudaSetDevice(device);
         void* ptrs[] = {d_pyr, d_blur, d_cells, d_fastBlocks, d_cellCount, d_cellList, d_cand, d_nodeOf, d_sel, d_selCount, d_dstIndex,
-                        d_status, d_xtab, d_ytab, d_img, d_outKp, d_outDesc, d_outN, d_outMono, d_maps, d_blurMaps, d_stereoSad, d_stereoU, d_stereoD};
+                        d_status, d_xtab, d_ytab, d_img, d_outKp, d_outDesc, d_outN, d_outMono, d_maps, d_blurMaps, d_stereoSad, d_stereoU, d_stereoD,
+                        d_outKpUn};
         for (void* p : ptrs) if (p) cudaFree(p);
         if (h_counts) cudaFreeHost(h_counts);
         if (h_stereoStatus) cudaFreeHost(h_stereoStatus);
@@ -477,6 +479,14 @@ using namespace orbx;
 
 struct orbx_handle { Extractor e; };
 
+namespace orbx {
+int handle_device(const orbx_handle* h) { return h->e.device; }
+extern thread_local int g_undistort_launches;
+int check_camera(const OrbPinholeCamera* cam, const char* where);
+int undistort_enqueue(const OrbPinholeCamera* cam, int batch, const OrbKeyPoint* kps, const int* n, int cap, OrbKeyPoint* out, cudaStream_t st,
+                      const char* where);
+}  // namespace orbx
+
 extern "C" {
 
 const char* orb_last_error(void) { return g_err.c_str(); }
@@ -706,6 +716,30 @@ int orbx_resident_slabs(const orbx_handle* h, const OrbKeyPoint** d_keypoints, c
 }
 
 int orbx_last_launch_count(const orbx_handle* h) { return h ? h->e.launches : ORB_ERR_ARG; }
+
+int orbx_undistort_keypoints(orbx_handle* h, const OrbPinholeCamera* cam, int batch, OrbKeyPoint* kpsUn, int cap, const OrbKeyPoint** d_kpsUn) {
+    g_undistort_launches = 0;
+    if (!h || batch < 0 || (kpsUn && cap != h->e.outCapInternal)) { set_error("orbx_undistort_keypoints: bad argument"); return ORB_ERR_ARG; }
+    if (int rc = check_camera(cam, "orbx_undistort_keypoints")) return rc;
+    Extractor& e = h->e;
+    if (batch > 0 && (!e.hasLast || e.lastQ.outKp != e.d_outKp || e.lastQ.batch < batch)) {
+        set_error("orbx_undistort_keypoints: the handle's last call was not orbx_extract[_batch] of at least `batch` frames");
+        return ORB_ERR_ARG;
+    }
+    CK(cudaSetDevice(e.device));
+    const size_t slab = sizeof(OrbKeyPoint) * (size_t)e.outCapInternal * e.maxBatch;
+    if (!e.d_outKpUn) {
+        CK(cudaMalloc(&e.d_outKpUn, slab));
+        CK(cudaMemset(e.d_outKpUn, 0, slab));
+    }
+    cudaStream_t st = e.stream;
+    int rc = undistort_enqueue(cam, batch, e.d_outKp, e.d_outN, e.outCapInternal, e.d_outKpUn, st, "orbx_undistort_keypoints");
+    if (rc) return rc;
+    if (kpsUn && batch > 0) CK(cudaMemcpyAsync(kpsUn, e.d_outKpUn, sizeof(OrbKeyPoint) * (size_t)e.outCapInternal * batch, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (d_kpsUn) *d_kpsUn = e.d_outKpUn;
+    return ORB_OK;
+}
 
 int orbx_set_profiling(orbx_handle* h, int on) {
     if (!h) return ORB_ERR_ARG;
