@@ -301,7 +301,8 @@ class Restatement:
         if op[0] == 'add':
             self.live += list(op[1])
         elif op[0] == 'erase':
-            self.live = [k for k in self.live if k not in op[1]]
+            gone = set(op[1])
+            self.live = [k for k in self.live if k not in gone]
         elif op[0] == 'clear':
             self.live = []
         elif op[0] == 'clearMap':
@@ -324,6 +325,38 @@ class Restatement:
         score = np.array([l1_score((q['word_id'], q['word_value']), self.sc.bows[k]) if s else 0 for k, s in zip(kf, scored)], np.float32)
         return dict(kf=kf, words=words, scored=scored, score=score, nSharing=len(rows), maxCommonWords=mx)
 
+    def phase1_np(self, q):
+        """phase1 over numpy arrays, for databases of thousands of keyframes: the live rows concatenated, each word's rank in the query
+        by a binary search, the counter and the first rank per keyframe by bincount / minimum.at, the list by a stable sort on the first
+        rank of the sharing keyframes in add order; a score is the common words' terms from intersect1d summed by add.accumulate (one
+        running double, in ascending word order).  The record also holds `rank`, each entry's first shared rank."""
+        qw, qv = np.asarray(q['word_id'], np.int64), np.asarray(q['word_value'], np.float64)
+        conn = set(q['connected']) if q['kind'] == NBEST else set()
+        live = [k for k in self.live if k not in conn]
+        lens = np.array([len(self.sc.bows[k][0]) for k in live], np.int64)
+        ids = np.concatenate([np.asarray(self.sc.bows[k][0], np.int64) for k in live]) if live else np.zeros(0, np.int64)
+        owner = np.repeat(np.arange(len(live)), lens)
+        pos = np.minimum(np.searchsorted(qw, ids), max(len(qw) - 1, 0))
+        hit = qw[pos] == ids if len(qw) else np.zeros(len(ids), bool)
+        cnt = np.bincount(owner[hit], minlength=len(live))
+        first = np.full(len(live), len(qw), np.int64)
+        np.minimum.at(first, owner[hit], pos[hit])
+        sel = np.flatnonzero(cnt > 0)
+        sel = sel[np.argsort(first[sel], kind='stable')]
+        mx = int(cnt.max()) if len(sel) else 0
+        mn = int(np.float32(mx) * np.float32(0.8))
+        words = cnt[sel].astype(np.int32)
+        scored = (words > mn).astype(np.uint8)
+        score = np.zeros(len(sel), np.float32)
+        for j in np.flatnonzero(scored):
+            b = self.sc.bows[live[sel[j]]]
+            _, iq, ib = np.intersect1d(qw, np.asarray(b[0], np.int64), assume_unique=True, return_indices=True)
+            vi, wi = qv[iq], np.asarray(b[1], np.float64)[ib]
+            s = np.add.accumulate(np.abs(vi - wi) - np.abs(vi) - np.abs(wi))[-1]
+            score[j] = np.float32(-s / 2.0)
+        return dict(kf=np.array([live[i] for i in sel], np.int32), words=words, scored=scored, score=score, nSharing=len(sel),
+                    maxCommonWords=mx, rank=first[sel])
+
     def phase2(self, q, rec, n_candidates=3):
         """Replays the record's marks and scores (as the host shim does), then the reference's phase 2."""
         kind, mark, sc_ = q['kind'], self.mark[q['kind']], self.score[q['kind']]
@@ -335,12 +368,13 @@ class Restatement:
         if not scored:
             return [] if kind == RELOC else ([], [])
         acc_list, best_acc = [], np.float32(0)
+        scored_now = set(rec['kf'][rec['scored'] > 0].tolist())
         for si, k in scored:
             best, acc, best_kf = si, si, k
             for k2 in self.sc.cov[k][:10]:
                 if mark[k2] != q['id']:
                     continue
-                if k2 not in set(rec['kf'][rec['scored'] > 0].tolist()):
+                if k2 not in scored_now:
                     self.stale_reads += 1
                 acc = np.float32(acc + sc_[k2])
                 if sc_[k2] > best:
