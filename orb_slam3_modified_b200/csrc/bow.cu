@@ -40,9 +40,8 @@ __global__ void __launch_bounds__(BD_NT) bow_descend_kernel(Voc V, int batch, in
     if (f >= batch) return;
     const int N = min(nFeat[f], cap);
     if (i >= N) return;                                       // whole half-warp leaves together (same i)
-    const uint4* fp = reinterpret_cast<const uint4*>(feats + ((size_t)f * cap + i) * 32);
-    const uint4 a0 = __ldg(fp), a1 = __ldg(fp + 1);
-    const uint32_t fd[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+    uint32_t fd[8];
+    orbx::load_desc(feats + ((size_t)f * cap + i) * 32, fd);
     const int nid_level = V.L - levelsup;
     int final_id = 0, nid = 0, level = 0;
     for (;;) {
@@ -51,9 +50,8 @@ __global__ void __launch_bounds__(BD_NT) bow_descend_kernel(Voc V, int batch, in
         unsigned best = 0xFFFFFFFFu;                          // distance << 20 | child rank: the first minimum wins (:1241-1246)
         for (int c = a + sl; c < b; c += 16) {
             const int id = V.children[c];
-            const uint4* dp = reinterpret_cast<const uint4*>(V.desc + (size_t)id * 32);
-            const uint4 d0 = __ldg(dp), d1 = __ldg(dp + 1);
-            const uint32_t dd[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+            uint32_t dd[8];
+            orbx::load_desc(V.desc + (size_t)id * 32, dd);
             best = min(best, ((unsigned)orbx::hamming256(fd, dd) << 20) | (unsigned)(c - a));
         }
 #pragma unroll

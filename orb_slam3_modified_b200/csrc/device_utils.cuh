@@ -122,6 +122,23 @@ __device__ __forceinline__ int hamming256(const uint32_t* a, const uint32_t* b) 
     return d;
 }
 
+// One 32-byte descriptor (16-byte aligned, not written by the kernel) as 8 words, through the read-only cache.
+__device__ __forceinline__ void load_desc(const uint8_t* p, uint32_t (&d)[8]) {
+    const uint4* q = reinterpret_cast<const uint4*>(p);
+    const uint4 a = __ldg(q), b = __ldg(q + 1);
+    d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
+}
+
+// std::lower_bound / std::upper_bound of key in the ascending a[lo, hi): the first index whose element is >= key / > key, or hi.
+__device__ __forceinline__ int lower_bound(const int* a, int lo, int hi, int key) {
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+__device__ __forceinline__ int upper_bound(const int* a, int lo, int hi, int key) {
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] <= key) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
 // MapPoint::ComputeDistinctiveDescriptors' choice (src/MapPoint.cc:329-403) among n <= 65535 rows, for one warp: lane l takes rows
 // l, l + 32, ...; row(j) gives the address of row j (32 bytes, 16-byte aligned, not written by the kernel).  Every lane returns the first
 // row with the least median distance to the others; the median (element (int)(0.5 (n - 1)) of the sorted row) is found by bisection on the
@@ -131,17 +148,15 @@ __device__ __forceinline__ int distinctive_best(int n, int lane, Row row) {
     const int k = (int)(0.5 * (double)(n - 1));
     unsigned bestKey = 0xFFFFFFFFu;
     for (int i = lane; i < n; i += 32) {
-        const uint4* pi = reinterpret_cast<const uint4*>(row(i));
-        const uint4 x0 = __ldg(pi), x1 = __ldg(pi + 1);
-        const uint32_t di[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+        uint32_t di[8];
+        load_desc(row(i), di);
         int lo = 0, hi = 256;                                    // smallest v with #{j : d(i, j) <= v} >= k + 1
         while (lo < hi) {
             const int mid = (lo + hi) >> 1;
             int cnt = 0;
             for (int j = 0; j < n; ++j) {
-                const uint4* pj = reinterpret_cast<const uint4*>(row(j));
-                const uint4 y0 = __ldg(pj), y1 = __ldg(pj + 1);
-                const uint32_t dj[8] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y, y1.z, y1.w};
+                uint32_t dj[8];
+                load_desc(row(j), dj);
                 cnt += (i == j ? 0 : hamming256(di, dj)) <= mid;
             }
             if (cnt >= k + 1) hi = mid; else lo = mid + 1;

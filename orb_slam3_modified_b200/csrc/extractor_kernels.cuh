@@ -1172,9 +1172,8 @@ __global__ void __launch_bounds__(ST_NT) stereo_matches_kernel(StereoParams Q) {
         const float minU = fsub(uL, maxD), maxU = fsub(uL, minD);
         unsigned best = 0xFFFFFFFFu;
         if (!(maxU < 0)) {
-            const uint4* pl = reinterpret_cast<const uint4*>(dl + (size_t)iL * 32);
-            const uint4 a0 = __ldg(pl), a1 = __ldg(pl + 1);
-            const uint32_t da[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            uint32_t da[8];
+            load_desc(dl + (size_t)iL * 32, da);
             for (int iR = lane; iR < Nr; iR += 32) {
                 const OrbKeyPoint kpR = kr[iR];
                 const float r = fmul(2.0f, Q.L.lv[min(max(kpR.octave, 0), Q.L.nlevels - 1)].scale);
@@ -1182,9 +1181,8 @@ __global__ void __launch_bounds__(ST_NT) stereo_matches_kernel(StereoParams Q) {
                 if (rowL < minr || rowL > maxr) continue;
                 if (kpR.octave < kpL.octave - 1 || kpR.octave > kpL.octave + 1) continue;
                 if (!(kpR.x >= minU && kpR.x <= maxU)) continue;
-                const uint4* pr = reinterpret_cast<const uint4*>(dr + (size_t)iR * 32);
-                const uint4 b0 = __ldg(pr), b1 = __ldg(pr + 1);
-                const uint32_t db[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+                uint32_t db[8];
+                load_desc(dr + (size_t)iR * 32, db);
                 const unsigned dist = (unsigned)hamming256(da, db);
                 if (dist < 100u) best = min(best, (dist << 16) | (unsigned)iR);      // bestDist starts at TH_HIGH, strict <
             }

@@ -20,6 +20,30 @@ __device__ __forceinline__ void set_pose_from_double(const double* T7, float* Tc
     Tcw7[4] = (float)T7[4]; Tcw7[5] = (float)T7[5]; Tcw7[6] = (float)T7[6];
 }
 
+// Sophus::SO3 rotation of a point (so3.hpp:358-367): uv = q.vec x p; uv += uv; (p + w uv) + q.vec x uv
+__device__ __forceinline__ void quat_rotate(const float* q, const float* p, float* o) {
+    using namespace orbx;
+    float ux = fsub(fmul(q[2], p[2]), fmul(q[3], p[1])), uy = fsub(fmul(q[3], p[0]), fmul(q[1], p[2])), uz = fsub(fmul(q[1], p[1]), fmul(q[2], p[0]));
+    ux = fadd(ux, ux); uy = fadd(uy, uy); uz = fadd(uz, uz);
+    const float cx = fsub(fmul(q[2], uz), fmul(q[3], uy)), cy = fsub(fmul(q[3], ux), fmul(q[1], uz)), cz = fsub(fmul(q[1], uy), fmul(q[2], ux));
+    o[0] = fadd(fadd(p[0], fmul(q[0], ux)), cx);
+    o[1] = fadd(fadd(p[1], fmul(q[0], uy)), cy);
+    o[2] = fadd(fadd(p[2], fmul(q[0], uz)), cz);
+}
+// SE3f::inverse: (conj q, -(conj q * t))
+__device__ __forceinline__ void se3_inverse(const float* T, float* I) {
+    I[0] = T[0]; I[1] = -T[1]; I[2] = -T[2]; I[3] = -T[3];
+    float r[3];
+    quat_rotate(I, T + 4, r);
+    I[4] = -r[0]; I[5] = -r[1]; I[6] = -r[2];
+}
+// Sophus' SE3 action on a point: T * p = q * p + t
+__device__ __forceinline__ void se3_transform(const float* T, const float* p, float* o) {
+    using namespace orbx;
+    quat_rotate(T, p, o);
+    o[0] = fadd(o[0], T[4]); o[1] = fadd(o[1], T[5]); o[2] = fadd(o[2], T[6]);
+}
+
 // Frame::UpdatePoseMatrices: mRcw = mTcw.rotationMatrix() (Eigen's QuaternionBase::toRotationMatrix, row-major), mtcw = mTcw.translation(),
 // mOw = mTcw.inverse().translation() = -(q^-1 * t) with Sophus' quaternion rotation (so3.hpp:358-367; oracle/ref_shim/ref_slam_types.cpp).
 __device__ __forceinline__ void update_pose_matrices(const float* T, float* R, float* t, float* Ow) {
@@ -33,13 +57,9 @@ __device__ __forceinline__ void update_pose_matrices(const float* T, float* R, f
     R[3] = fadd(txy, twz); R[4] = fsub(1.0f, fadd(txx, tzz)); R[5] = fsub(tyz, twx);
     R[6] = fsub(txz, twy); R[7] = fadd(tyz, twx); R[8] = fsub(1.0f, fadd(txx, tyy));
     t[0] = T[4]; t[1] = T[5]; t[2] = T[6];
-    const float ix = -qx, iy = -qy, iz = -qz, px = T[4], py = T[5], pz = T[6];
-    float ux = fsub(fmul(iy, pz), fmul(iz, py)), uy = fsub(fmul(iz, px), fmul(ix, pz)), uz = fsub(fmul(ix, py), fmul(iy, px));
-    ux = fadd(ux, ux); uy = fadd(uy, uy); uz = fadd(uz, uz);
-    const float cx = fsub(fmul(iy, uz), fmul(iz, uy)), cy = fsub(fmul(iz, ux), fmul(ix, uz)), cz = fsub(fmul(ix, uy), fmul(iy, ux));
-    Ow[0] = -fadd(fadd(px, fmul(qw, ux)), cx);
-    Ow[1] = -fadd(fadd(py, fmul(qw, uy)), cy);
-    Ow[2] = -fadd(fadd(pz, fmul(qw, uz)), cz);
+    float I[7];
+    se3_inverse(T, I);
+    Ow[0] = I[4]; Ow[1] = I[5]; Ow[2] = I[6];
 }
 
 // ---- Frame::SetImuPoseVelocity and GetImuRotation / GetImuPosition (src/Frame.cc) for the mono-inertial tracking call
@@ -48,16 +68,6 @@ __device__ __forceinline__ void update_pose_matrices(const float* T, float* R, f
 //      inverse, the SE3 product (quaternion product not renormalised) and Matrix3f * Matrix3f / Vector3f summed left to right.  Bit agreement
 //      with Eigen / Sophus is not claimed, as for set_pose_from_double. ----
 
-// Sophus::SO3 rotation of a point (so3.hpp:358-367): uv = q.vec x p; uv += uv; (p + w uv) + q.vec x uv
-__device__ __forceinline__ void quat_rotate(const float* q, const float* p, float* o) {
-    using namespace orbx;
-    float ux = fsub(fmul(q[2], p[2]), fmul(q[3], p[1])), uy = fsub(fmul(q[3], p[0]), fmul(q[1], p[2])), uz = fsub(fmul(q[1], p[1]), fmul(q[2], p[0]));
-    ux = fadd(ux, ux); uy = fadd(uy, uy); uz = fadd(uz, uz);
-    const float cx = fsub(fmul(q[2], uz), fmul(q[3], uy)), cy = fsub(fmul(q[3], ux), fmul(q[1], uz)), cz = fsub(fmul(q[1], uy), fmul(q[2], ux));
-    o[0] = fadd(fadd(p[0], fmul(q[0], ux)), cx);
-    o[1] = fadd(fadd(p[1], fmul(q[0], uy)), cy);
-    o[2] = fadd(fadd(p[2], fmul(q[0], uz)), cz);
-}
 // Sophus::SE3f(Matrix3f R, Vector3f t): Eigen's quaternion from a rotation matrix (R row-major); T = (w, x, y, z, t)
 __device__ __forceinline__ void se3_from_matrix(const float* R, const float* t, float* T) {
     using namespace orbx;
@@ -80,24 +90,15 @@ __device__ __forceinline__ void se3_from_matrix(const float* R, const float* t, 
     }
     T[4] = t[0]; T[5] = t[1]; T[6] = t[2];
 }
-// SE3f::inverse: (conj q, -(conj q * t))
-__device__ __forceinline__ void se3_inverse(const float* T, float* I) {
-    I[0] = T[0]; I[1] = -T[1]; I[2] = -T[2]; I[3] = -T[3];
-    float r[3];
-    quat_rotate(I, T + 4, r);
-    I[4] = -r[0]; I[5] = -r[1]; I[6] = -r[2];
-}
 // SE3f * SE3f: quaternion product, translation A.q * B.t + A.t
 __device__ __forceinline__ void se3_mul(const float* A, const float* B, float* C) {
     using namespace orbx;
     const float w = A[0], x = A[1], y = A[2], z = A[3];
-    float r[3];
-    quat_rotate(A, B + 4, r);
     C[0] = fsub(fsub(fsub(fmul(w, B[0]), fmul(x, B[1])), fmul(y, B[2])), fmul(z, B[3]));
     C[1] = fsub(fadd(fadd(fmul(w, B[1]), fmul(x, B[0])), fmul(y, B[3])), fmul(z, B[2]));
     C[2] = fsub(fadd(fadd(fmul(w, B[2]), fmul(y, B[0])), fmul(z, B[1])), fmul(x, B[3]));
     C[3] = fsub(fadd(fadd(fmul(w, B[3]), fmul(z, B[0])), fmul(x, B[2])), fmul(y, B[1]));
-    C[4] = fadd(r[0], A[4]); C[5] = fadd(r[1], A[5]); C[6] = fadd(r[2], A[6]);
+    se3_transform(A, B + 4, C + 4);
 }
 // Frame::SetImuPoseVelocity's pose part: mTcw = mImuCalib.mTcb * SE3f(Rwb, twb).inverse() (Tcb7 = (w, x, y, z, t)); then UpdatePoseMatrices
 // and what ImuCamPose(Frame*) reads back: GetImuRotation = mRwc * mTcb.rotationMatrix(), GetImuPosition = mRwc * mTcb.translation() + mOw

@@ -68,8 +68,7 @@ __global__ void __launch_bounds__(SH_NT) kfdb_share_kernel(Pool pool, const DbQu
         const int slot = Q.order[i];
         bool connected = false;
         if (Q.kind == ORBV_DB_NBEST) {
-            int lo = 0, hi = Q.nConn;
-            while (lo < hi) { const int mid = (lo + hi) >> 1; if (Q.conn[mid] < slot) lo = mid + 1; else hi = mid; }
+            const int lo = orbx::lower_bound(Q.conn, 0, Q.nConn, slot);
             connected = lo < Q.nConn && Q.conn[lo] == slot;
         }
         int count = 0;
@@ -79,8 +78,7 @@ __global__ void __launch_bounds__(SH_NT) kfdb_share_kernel(Pool pool, const DbQu
             const int* row = pool.word + (size_t)slot * pool.W;
             for (int k = lane; k < m; k += 32) {
                 const int w = row[k];
-                int lo = 0, hi = nW;
-                while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_qw[mid] < w) lo = mid + 1; else hi = mid; }
+                const int lo = orbx::lower_bound(s_qw, 0, nW, w);
                 if (lo < nW && s_qw[lo] == w) { ++count; first = min(first, (unsigned)lo); }
             }
             count = __reduce_add_sync(0xffffffffu, count);
@@ -157,8 +155,7 @@ __global__ void __launch_bounds__(SC_NT) kfdb_score_kernel(Pool pool, const DbQu
             bool hit = false;
             if (k < nr) {
                 const int w = row[k];
-                int lo = 0, hi = nW;
-                while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_qw[mid] < w) lo = mid + 1; else hi = mid; }
+                const int lo = orbx::lower_bound(s_qw, 0, nW, w);
                 if (lo < nW && s_qw[lo] == w) {
                     const double vi = s_qv[lo], wi = val[k];
                     term = __dsub_rn(__dsub_rn(fabs(__dsub_rn(vi, wi)), fabs(vi)), fabs(wi));   // fabs(vi-wi) - fabs(vi) - fabs(wi)

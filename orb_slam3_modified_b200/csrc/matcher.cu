@@ -115,6 +115,8 @@ __host__ __device__ inline size_t frame_smem_bytes(int Ks, int Ms, bool descInSm
     if (descInSmem) b += al16((size_t)32 * Ks);
     return b;
 }
+// The opt-in maximum of dynamic shared memory per CTA (227 KB on sm_90) less 2 KB for the frame kernels' static shared memory
+constexpr size_t FRAME_SMEM_LIMIT = 227 * 1024 - 2048;
 __device__ __forceinline__ FrameSmem carve_frame_smem(uint8_t* p, int Ks, int Ms, bool descInSmem) {
     FrameSmem S;
     S.cnt = (int*)p; p += al16(sizeof(int) * GRID_CELLS);
@@ -211,15 +213,14 @@ __device__ __forceinline__ TopK<K> scan_candidates(const MatchParams& P, const F
                 const float dx = fsub(S.kx[idx], u), dy = fsub(S.ky[idx], v);
                 if (!(fabsf(dx) < r && fabsf(dy) < r)) continue;
                 if (!usable(idx)) continue;
-                uint4 d0, d1;
+                uint32_t dd[8];
                 if (S.desc) {
                     const uint4* dp = reinterpret_cast<const uint4*>(S.desc + (size_t)idx * 8);
-                    d0 = dp[0]; d1 = dp[1];
+                    const uint4 d0 = dp[0], d1 = dp[1];
+                    dd[0] = d0.x; dd[1] = d0.y; dd[2] = d0.z; dd[3] = d0.w; dd[4] = d1.x; dd[5] = d1.y; dd[6] = d1.z; dd[7] = d1.w;
                 } else {
-                    const uint4* dp = reinterpret_cast<const uint4*>(gdesc + (size_t)idx * 32);
-                    d0 = __ldg(dp); d1 = __ldg(dp + 1);
+                    load_desc(gdesc + (size_t)idx * 32, dd);
                 }
-                const uint32_t dd[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
                 const int dist = hamming256(mpd, dd);
                 if (!usableDist(idx, dist)) continue;
                 t.insert(((unsigned long long)dist << 40) | ((unsigned long long)c << 20) | (unsigned)(e - a), idx);
@@ -230,10 +231,8 @@ __device__ __forceinline__ TopK<K> scan_candidates(const MatchParams& P, const F
     return t;
 }
 
-__device__ __forceinline__ void load_mp_desc(const MatchParams& P, int f, int i, uint32_t* mpd) {
-    const uint4* p = reinterpret_cast<const uint4*>(P.mpDesc + ((size_t)f * P.mcap + i) * 32);
-    const uint4 a = __ldg(p), b = __ldg(p + 1);
-    mpd[0] = a.x; mpd[1] = a.y; mpd[2] = a.z; mpd[3] = a.w; mpd[4] = b.x; mpd[5] = b.y; mpd[6] = b.z; mpd[7] = b.w;
+__device__ __forceinline__ void load_mp_desc(const MatchParams& P, int f, int i, uint32_t (&mpd)[8]) {
+    load_desc(P.mpDesc + ((size_t)f * P.mcap + i) * 32, mpd);
 }
 
 // Query of map point i: search centre, radius and level window; returns false when the reference `continue`s.
@@ -254,15 +253,9 @@ __device__ __forceinline__ bool make_query(const MatchParams& P, int f, int i, f
     }
     // last frame, mono (:1702-1741): x3Dc = Tcw * x3Dw with Sophus' quaternion form (so3.hpp:358-367)
     if (!P.valid[o]) return false;
-    const float* T = P.Tcw7 + (size_t)f * 7;
-    const float qw = T[0], qx = T[1], qy = T[2], qz = T[3];
-    const float px = P.xyz[3 * o], py = P.xyz[3 * o + 1], pz = P.xyz[3 * o + 2];
-    float ux = fsub(fmul(qy, pz), fmul(qz, py)), uy = fsub(fmul(qz, px), fmul(qx, pz)), uz = fsub(fmul(qx, py), fmul(qy, px));
-    ux = fadd(ux, ux); uy = fadd(uy, uy); uz = fadd(uz, uz);
-    const float cx_ = fsub(fmul(qy, uz), fmul(qz, uy)), cy_ = fsub(fmul(qz, ux), fmul(qx, uz)), cz_ = fsub(fmul(qx, uy), fmul(qy, ux));
-    const float xc = fadd(fadd(fadd(px, fmul(qw, ux)), cx_), T[4]);
-    const float yc = fadd(fadd(fadd(py, fmul(qw, uy)), cy_), T[5]);
-    const float zc = fadd(fadd(fadd(pz, fmul(qw, uz)), cz_), T[6]);
+    float xc3[3];
+    se3_transform(P.Tcw7 + (size_t)f * 7, P.xyz + 3 * o, xc3);
+    const float xc = xc3[0], yc = xc3[1], zc = xc3[2];
     const float invzc = (float)(1.0 / (double)zc);
     if (invzc < 0) return false;
     u = fadd(fdiv(fmul(P.cam[0], xc), zc), P.cam[2]);   // Pinhole::project, Pinhole.cpp:43-49
@@ -283,6 +276,30 @@ __device__ __forceinline__ int rot_bin(float lastAngle, float curAngle) {
     int bin = (int)roundf(fmul(rot, 1.0f / HISTO_LENGTH));
     if (bin == HISTO_LENGTH) bin = 0;
     return min(max(bin, 0), HISTO_LENGTH - 1);
+}
+
+// ComputeThreeMaxima (:2012-2053): the three fullest bins of the rotation histogram, -1 for the second and third when they hold less
+// than a tenth of the first
+__device__ __forceinline__ void three_maxima(const int* hist, int ind[3]) {
+    int ind1 = -1, ind2 = -1, ind3 = -1, max1 = 0, max2 = 0, max3 = 0;
+    for (int b = 0; b < HISTO_LENGTH; ++b) {
+        const int s = hist[b];
+        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = b; }
+        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = b; }
+        else if (s > max3) { max3 = s; ind3 = b; }
+    }
+    if ((float)max2 < fmul(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
+    else if ((float)max3 < fmul(0.1f, (float)max1)) { ind3 = -1; }
+    ind[0] = ind1; ind[1] = ind2; ind[2] = ind3;
+}
+// the matches of bin b survive the rotation filter
+__device__ __forceinline__ bool rot_kept(int b, const int ind[3]) { return b == ind[0] || b == ind[1] || b == ind[2]; }
+
+// The rotation events of SearchByBoW and SearchForTriangulation: match i's bin + 1 in evBin[i], counted in the histogram
+__device__ __forceinline__ void rot_event(int* hist, uint8_t* evBin, int i, float angle1, float angle2) {
+    const int b = rot_bin(angle1, angle2);
+    evBin[i] = (uint8_t)(b + 1);
+    atomicAdd(&hist[b], 1);
 }
 
 // Frame::AssignFeaturesToGrid + PosInGrid (src/Frame.cc:385-416, :725-735): counting sort of the keypoints into the 64x48 grid held in
@@ -510,25 +527,14 @@ __global__ void __launch_bounds__(MF_NT, 2) match_frame_kernel(MatchParams P) {
     if (nAcc) atomicAdd(&s_nAcc, nAcc);
     __syncthreads();
     if (hist) {
-        if (tid == 0) {
-            int ind1 = -1, ind2 = -1, ind3 = -1, max1 = 0, max2 = 0, max3 = 0;
-            for (int b = 0; b < HISTO_LENGTH; ++b) {
-                const int s = s_hist[b];
-                if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = b; }
-                else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = b; }
-                else if (s > max3) { max3 = s; ind3 = b; }
-            }
-            if ((float)max2 < fmul(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < fmul(0.1f, (float)max1)) { ind3 = -1; }
-            s_ind[0] = ind1; s_ind[1] = ind2; s_ind[2] = ind3;
-        }
+        if (tid == 0) three_maxima(s_hist, s_ind);
         __syncthreads();
         int removed = 0;
         for (int i = tid; i < M; i += MF_NT) {      // every event of a rejected bin clears its keypoint (:1868-1884)
             const unsigned ch = S.choice[i];
             if (ch == NONE16) continue;
             const int b = (S.mflags[i] >> 2) - 1;
-            if (b != s_ind[0] && b != s_ind[1] && b != s_ind[2]) { atomicOr(&removedBits[ch >> 5], 1u << (ch & 31)); ++removed; }
+            if (!rot_kept(b, s_ind)) { atomicOr(&removedBits[ch >> 5], 1u << (ch & 31)); ++removed; }
         }
         if (removed) atomicAdd(&s_nRemoved, removed);
         __syncthreads();
@@ -645,25 +651,13 @@ __global__ void __launch_bounds__(MF_NT) init_match_kernel(MatchParams P) {
         }
     }
     __syncthreads();
-    if (P.checkOri && tid == 0) {   // ComputeThreeMaxima (:2012-2053)
-        int ind1 = -1, ind2 = -1, ind3 = -1, max1 = 0, max2 = 0, max3 = 0;
-        for (int b = 0; b < HISTO_LENGTH; ++b) {
-            const int sz = s_hist[b];
-            if (sz > max1) { max3 = max2; max2 = max1; max1 = sz; ind3 = ind2; ind2 = ind1; ind1 = b; }
-            else if (sz > max2) { max3 = max2; max2 = sz; ind3 = ind2; ind2 = b; }
-            else if (sz > max3) { max3 = sz; ind3 = b; }
-        }
-        if ((float)max2 < fmul(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-        else if ((float)max3 < fmul(0.1f, (float)max1)) { ind3 = -1; }
-        s_ind[0] = ind1; s_ind[1] = ind2; s_ind[2] = ind3;
-    }
+    if (P.checkOri && tid == 0) three_maxima(s_hist, s_ind);
     __syncthreads();
     int n = 0;
     for (int i = tid; i < K1; i += MF_NT) {
         unsigned ch = S.choice[i];
         if (ch != NONE16 && P.checkOri) {                             // :733-754: events of rejected bins lose their match if they still hold one
-            const int b = (int)S.mflags[i] - 1;
-            if (b != s_ind[0] && b != s_ind[1] && b != s_ind[2]) ch = NONE16;
+            if (!rot_kept((int)S.mflags[i] - 1, s_ind)) ch = NONE16;
         }
         P.match[i] = ch == NONE16 ? -1 : (int)ch;
         float px = P.projX[i], py = P.projY[i];
@@ -731,27 +725,20 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
         const int node = fvNodeKF[a];
         int a1 = a;
         while (a1 < eKF && fvNodeKF[a1] == node) ++a1;
-        int lo = 0, hi = eF;                                     // lower_bound / upper_bound of `node` in the frame's vector
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (fvNodeF[mid] < node) lo = mid + 1; else hi = mid; }
-        const int b = lo;
-        hi = eF;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (fvNodeF[mid] <= node) lo = mid + 1; else hi = mid; }
-        const int b1 = lo;
+        const int b = lower_bound(fvNodeF, 0, eF, node), b1 = upper_bound(fvNodeF, b, eF, node);   // `node` in the frame's vector
         if (b1 == b) continue;
         for (int iKF = a; iKF < a1; ++iKF) {
             const int realIdxKF = fvFeatKF[iKF];
             if (kfPoint[realIdxKF] != 1) continue;               // no map point, or a bad one (:255-259)
-            const uint4* pk = reinterpret_cast<const uint4*>(descKF + (size_t)realIdxKF * 32);
-            const uint4 k0 = __ldg(pk), k1 = __ldg(pk + 1);
-            const uint32_t dk[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
+            uint32_t dk[8];
+            load_desc(descKF + (size_t)realIdxKF * 32, dk);
             Top2 t; t.init();
             for (int iF = b + lane; iF < b1; iF += 32) {
                 const int realIdxF = fvFeatF[iF];
                 if (match[realIdxF] >= 0) continue;              // already matched by an earlier keyframe feature of this node (:275-276)
                 if (fPoint && fPoint[realIdxF] != 1) continue;
-                const uint4* pf = reinterpret_cast<const uint4*>(descF + (size_t)realIdxF * 32);
-                const uint4 f0 = __ldg(pf), f1 = __ldg(pf + 1);
-                const uint32_t dfw[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
+                uint32_t dfw[8];
+                load_desc(descF + (size_t)realIdxF * 32, dfw);
                 t.insert(((unsigned long long)hamming256(dk, dfw) << 32) | (unsigned)(iF - b), realIdxF);
             }
             t.warp_merge();
@@ -760,11 +747,7 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
                 if (lane == 0) {
                     match[t.i[0]] = realIdxKF;
                     if (match12) match12[realIdxKF] = t.i[0];
-                    if (Q.checkOri) {
-                        const int bin = rot_bin(kpsKF[realIdxKF].angle, kpsF[t.i[0]].angle);
-                        evBin[t.i[0]] = (uint8_t)(bin + 1);
-                        atomicAdd(&s_hist[bin], 1);
-                    }
+                    if (Q.checkOri) rot_event(s_hist, evBin, t.i[0], kpsKF[realIdxKF].angle, kpsF[t.i[0]].angle);
                 }
                 ++acc;
             }
@@ -774,23 +757,12 @@ __global__ void __launch_bounds__(BM_NT) bow_match_kernel(BowMatchParams Q) {
     if (lane == 0 && acc) atomicAdd(&s_acc, acc);
     __syncthreads();
     if (Q.checkOri) {
-        if (tid == 0) {
-            int ind1 = -1, ind2 = -1, ind3 = -1, max1 = 0, max2 = 0, max3 = 0;
-            for (int bb = 0; bb < HISTO_LENGTH; ++bb) {
-                const int sz = s_hist[bb];
-                if (sz > max1) { max3 = max2; max2 = max1; max1 = sz; ind3 = ind2; ind2 = ind1; ind1 = bb; }
-                else if (sz > max2) { max3 = max2; max2 = sz; ind3 = ind2; ind2 = bb; }
-                else if (sz > max3) { max3 = sz; ind3 = bb; }
-            }
-            if ((float)max2 < fmul(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < fmul(0.1f, (float)max1)) { ind3 = -1; }
-            s_ind[0] = ind1; s_ind[1] = ind2; s_ind[2] = ind3;
-        }
+        if (tid == 0) three_maxima(s_hist, s_ind);
         __syncthreads();
         int rem = 0;
         for (int i = tid; i < nF; i += BM_NT) {
             const int bb = (int)evBin[i] - 1;
-            if (bb >= 0 && bb != s_ind[0] && bb != s_ind[1] && bb != s_ind[2]) { if (match12) match12[match[i]] = -1; match[i] = -1; ++rem; }
+            if (bb >= 0 && !rot_kept(bb, s_ind)) { if (match12) match12[match[i]] = -1; match[i] = -1; ++rem; }
         }
         if (rem) atomicAdd(&s_rem, rem);
         __syncthreads();
@@ -908,13 +880,10 @@ __global__ void __launch_bounds__(MF_NT) fuse_search_kernel(const FuseParams* __
             const float maxDist = fmul(1.2f, maxRaw), minDist = fmul(0.8f, Q.minD[i]);
             float dist3D;
             if (Q.mode == 0) {
-                const float qw = Q.Tcw[0], qx = Q.Tcw[1], qy = Q.Tcw[2], qz = Q.Tcw[3];
-                float ux = fsub(fmul(qy, pz), fmul(qz, py)), uy = fsub(fmul(qz, px), fmul(qx, pz)), uz = fsub(fmul(qx, py), fmul(qy, px));
-                ux = fadd(ux, ux); uy = fadd(uy, uy); uz = fadd(uz, uz);
-                const float cx_ = fsub(fmul(qy, uz), fmul(qz, uy)), cy_ = fsub(fmul(qz, ux), fmul(qx, uz)), cz_ = fsub(fmul(qx, uy), fmul(qy, ux));
-                const float xc = fadd(fadd(fadd(px, fmul(qw, ux)), cx_), Q.Tcw[4]);
-                const float yc = fadd(fadd(fadd(py, fmul(qw, uy)), cy_), Q.Tcw[5]);
-                const float zc = fadd(fadd(fadd(pz, fmul(qw, uz)), cz_), Q.Tcw[6]);
+                const float pw[3] = {px, py, pz};
+                float xc3[3];
+                se3_transform(Q.Tcw, pw, xc3);
+                const float xc = xc3[0], yc = xc3[1], zc = xc3[2];
                 go = !(zc < 0.0f);
                 u = fadd(fdiv(fmul(P.cam[0], xc), zc), P.cam[2]);
                 v = fadd(fdiv(fmul(P.cam[1], yc), zc), P.cam[3]);
@@ -941,9 +910,7 @@ __global__ void __launch_bounds__(MF_NT) fuse_search_kernel(const FuseParams* __
         }
         if (go) {      // warp-uniform: every lane computed the same query
             uint32_t mpd[8];
-            const uint4* dp = reinterpret_cast<const uint4*>(Q.mpDesc + (size_t)i * 32);
-            const uint4 a = __ldg(dp), b = __ldg(dp + 1);
-            mpd[0] = a.x; mpd[1] = a.y; mpd[2] = a.z; mpd[3] = a.w; mpd[4] = b.x; mpd[5] = b.y; mpd[6] = b.z; mpd[7] = b.w;
+            load_desc(Q.mpDesc + (size_t)i * 32, mpd);
             const float* isg = Q.invSigma2;
             const bool gate = Q.gate != 0;
             const TopK<1> t = scan_candidates<1>(P, S, 0, u, v, r, lvl - 1, lvl, mpd, [&](int idx) {
@@ -1000,17 +967,11 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams P) {
         const int idx1 = Q.fvFeat1[e1];
         if (Q.hasMP1[idx1]) continue;
         const int node = Q.fvNode1[e1];
-        int lo = 0, hi = R.E2;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (R.fvNode2[mid] < node) lo = mid + 1; else hi = mid; }
-        const int b = lo;
-        hi = R.E2;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (R.fvNode2[mid] <= node) lo = mid + 1; else hi = mid; }
-        const int b1 = lo;
+        const int b = lower_bound(R.fvNode2, 0, R.E2, node), b1 = upper_bound(R.fvNode2, b, R.E2, node);
         if (b1 == b) continue;
         const OrbKeyPoint kp1 = Q.kps1[idx1];
-        const uint4* p1 = reinterpret_cast<const uint4*>(Q.desc1 + (size_t)idx1 * 32);
-        const uint4 k0 = __ldg(p1), k1 = __ldg(p1 + 1);
-        const uint32_t d1[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
+        uint32_t d1[8];
+        load_desc(Q.desc1 + (size_t)idx1 * 32, d1);
         // epipolar line of kp1 in the second image, l = x1' F12 = [a b c]
         const float ea = fadd(__fmaf_rn(kp1.x, R.F12[0], fmul(kp1.y, R.F12[3])), R.F12[6]);
         const float eb = fadd(__fmaf_rn(kp1.x, R.F12[1], fmul(kp1.y, R.F12[4])), R.F12[7]);
@@ -1020,9 +981,8 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams P) {
         for (int i2 = b + lane; i2 < b1; i2 += 32) {
             const int idx2 = R.fvFeat2[i2];
             if (R.hasMP2[idx2]) continue;
-            const uint4* p2 = reinterpret_cast<const uint4*>(R.desc2 + (size_t)idx2 * 32);
-            const uint4 f0 = __ldg(p2), f1 = __ldg(p2 + 1);
-            const uint32_t d2[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
+            uint32_t d2[8];
+            load_desc(R.desc2 + (size_t)idx2 * 32, d2);
             const int dist = hamming256(d1, d2);
             if (dist > TH_LOW) continue;
             const OrbKeyPoint kp2 = R.kps2[idx2];
@@ -1044,11 +1004,7 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams P) {
             if (lane == 0) {
                 const int idx2 = R.fvFeat2[b + (int)(0xFFFFFFFFu - (unsigned)best)];
                 R.matches12[idx1] = idx2;
-                if (checkOri) {
-                    const int bin = rot_bin(kp1.angle, R.kps2[idx2].angle);
-                    R.evBin[idx1] = (uint8_t)(bin + 1);
-                    atomicAdd(&s_hist[bin], 1);
-                }
+                if (checkOri) rot_event(s_hist, R.evBin, idx1, kp1.angle, R.kps2[idx2].angle);
             }
             ++acc;
         }
@@ -1056,23 +1012,12 @@ __global__ void __launch_bounds__(TM_NT) tri_match_kernel(TriParams P) {
     if (lane == 0 && acc) atomicAdd(&s_acc, acc);
     __syncthreads();
     if (checkOri) {
-        if (tid == 0) {
-            int ind1 = -1, ind2 = -1, ind3 = -1, max1 = 0, max2 = 0, max3 = 0;
-            for (int bb = 0; bb < HISTO_LENGTH; ++bb) {
-                const int sz = s_hist[bb];
-                if (sz > max1) { max3 = max2; max2 = max1; max1 = sz; ind3 = ind2; ind2 = ind1; ind1 = bb; }
-                else if (sz > max2) { max3 = max2; max2 = sz; ind3 = ind2; ind2 = bb; }
-                else if (sz > max3) { max3 = sz; ind3 = bb; }
-            }
-            if ((float)max2 < fmul(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < fmul(0.1f, (float)max1)) { ind3 = -1; }
-            s_ind[0] = ind1; s_ind[1] = ind2; s_ind[2] = ind3;
-        }
+        if (tid == 0) three_maxima(s_hist, s_ind);
         __syncthreads();
         int rem = 0;
         for (int i = tid; i < Q.N1; i += TM_NT) {
             const int bb = (int)R.evBin[i] - 1;
-            if (bb >= 0 && bb != s_ind[0] && bb != s_ind[1] && bb != s_ind[2]) { R.matches12[i] = -1; ++rem; }
+            if (bb >= 0 && !rot_kept(bb, s_ind)) { R.matches12[i] = -1; ++rem; }
         }
         if (rem) atomicAdd(&s_rem, rem);
         __syncthreads();
@@ -1354,14 +1299,12 @@ __global__ void __launch_bounds__(BF_NT) bf_knn2_kernel(const uint8_t* __restric
                                                         int* __restrict__ idx, int* __restrict__ dist) {
     const int qi = blockIdx.x * (BF_NT / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (qi >= Q) return;
-    const uint4* qp = reinterpret_cast<const uint4*>(q + (size_t)qi * 32);
-    const uint4 a = __ldg(qp), b = __ldg(qp + 1);
-    const uint32_t qd[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint32_t qd[8];
+    load_desc(q + (size_t)qi * 32, qd);
     Top2 tt; tt.init();
     for (int j = lane; j < T; j += 32) {
-        const uint4* tp = reinterpret_cast<const uint4*>(t + (size_t)j * 32);
-        const uint4 c = __ldg(tp), d = __ldg(tp + 1);
-        const uint32_t td[8] = {c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w};
+        uint32_t td[8];
+        load_desc(t + (size_t)j * 32, td);
         tt.insert(((unsigned long long)hamming256(qd, td) << 32) | (unsigned)j, j);
     }
     tt.warp_merge();
@@ -1382,6 +1325,32 @@ __global__ void hamming_pairs_kernel(const uint8_t* __restrict__ a, const uint8_
     const uint32_t y[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
     out[i] = hamming256(x, y);
 }
+
+// Frame::AssignFeaturesToGrid's cell scale (src/Frame.cc:342-343) and the shared-memory layout of a frame of P.ks keypoints and P.ms
+// map points with `extra` bytes behind it: the descriptors are staged (P.descInSmem) when the whole then takes at most descLimit bytes.
+// Returns the dynamic shared memory, or 0 with `tooLarge` as the error when even without the descriptors it exceeds FRAME_SMEM_LIMIT.
+static size_t frame_layout(MatchParams& P, size_t extra, size_t descLimit, const char* tooLarge) {
+    P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX);
+    P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
+    P.descInSmem = frame_smem_bytes(P.ks, P.ms, true) + extra <= descLimit ? 1 : 0;
+    const size_t sm = frame_smem_bytes(P.ks, P.ms, P.descInSmem != 0) + extra;
+    if (sm > FRAME_SMEM_LIMIT) { set_error(tooLarge); return 0; }
+    return sm;
+}
+
+// The launch of match_frame_kernel / init_match_kernel: one cluster of MF_NT-thread CTAs per frame, `sm` bytes of dynamic shared memory.
+struct ClusterLaunch {
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute at[1];
+    ClusterLaunch(size_t sm, cudaStream_t st) {
+        cfg.blockDim = dim3(MF_NT); cfg.dynamicSmemBytes = sm; cfg.stream = st;
+        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        cfg.attrs = at; cfg.numAttrs = 1;
+    }
+    ClusterLaunch(const ClusterLaunch&) = delete;
+    // clusters of C CTAs for `frames` frames
+    const cudaLaunchConfig_t* shape(int frames, int C) { at[0].val.clusterDim.x = C; cfg.gridDim = dim3((unsigned)(frames * C)); return &cfg; }
+};
 
 struct Matcher {
     int device, maxBatch, kcap, mcap;
@@ -1431,22 +1400,15 @@ struct Matcher {
     // counts live on the device): they size the kernel's shared memory.  A refused call launches nothing and reports 0 launches.
     int run(MatchParams& P, int kUse, int mUse, cudaStream_t st) {
         launches = 0;
-        P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX);   // src/Frame.cc:342-343
-        P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
         P.query = d_query; P.resultIdx = d_resultIdx; P.resultDist = d_resultDist; P.status = d_status;
         P.ks = std::max(kUse, 1); P.ms = std::max(mUse, 1);
         if (P.ks > 65535 || P.ms > 65535) { set_error("more than 65535 keypoints or map points per frame"); return ORB_ERR_CAPACITY; }
-        const size_t limit = 227 * 1024 - 2048;              // opt-in maximum minus the kernel's static shared memory
-        P.descInSmem = frame_smem_bytes(P.ks, P.ms, true) <= 100 * 1024 ? 1 : 0;   // two CTAs per SM when the descriptors are staged
-        const size_t sm = frame_smem_bytes(P.ks, P.ms, P.descInSmem != 0);
-        if (sm > limit) { set_error("frame too large for the matcher's shared-memory grid (keypoints + map points)"); return ORB_ERR_CAPACITY; }
+        // the descriptors are staged only when two CTAs per SM still fit
+        const size_t sm = frame_layout(P, 0, 100 * 1024, "frame too large for the matcher's shared-memory grid (keypoints + map points)");
+        if (!sm) return ORB_ERR_CAPACITY;
         int rc = ensure_dynamic_smem(match_frame_kernel, sm, device);
         if (rc) return rc;
-        cudaLaunchConfig_t cfg = {};
-        cfg.blockDim = dim3(MF_NT); cfg.dynamicSmemBytes = sm; cfg.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
+        ClusterLaunch L(sm, st);
         // cluster size: the largest (up to 8) for which every frame's cluster is resident at once (pass 1 is spread over the
         // cluster; a second wave would double the call's time).  Asked from the occupancy calculator, which counts registers, shared
         // memory and the GPCs clusters cannot straddle; the answer depends only on (batch, shared memory), so it is kept.
@@ -1454,18 +1416,14 @@ struct Matcher {
             occC = 1;
             for (int cand = 8; cand > 1; --cand) {
                 if ((long)P.batch * cand > 2L * numSMs) continue;
-                at[0].val.clusterDim.x = cand;
-                cfg.gridDim = dim3((unsigned)(P.batch * cand));
                 int nClusters = 0;
-                if (cudaOccupancyMaxActiveClusters(&nClusters, match_frame_kernel, &cfg) == cudaSuccess && nClusters >= P.batch) { occC = cand; break; }
+                if (cudaOccupancyMaxActiveClusters(&nClusters, match_frame_kernel, L.shape(P.batch, cand)) == cudaSuccess && nClusters >= P.batch) { occC = cand; break; }
             }
             (void)cudaGetLastError();
             occBatch = P.batch; occSmem = sm;
         }
         const int C = occC;
-        at[0].val.clusterDim.x = C;
-        cfg.gridDim = dim3((unsigned)(P.batch * C));
-        CK(cudaLaunchKernelEx(&cfg, match_frame_kernel, P));
+        CK(cudaLaunchKernelEx(L.shape(P.batch, C), match_frame_kernel, P));
         launches = 1;
         lastCluster = C;
         return ORB_OK;
@@ -1514,25 +1472,17 @@ struct Matcher {
 
     // SearchForInitialization: F2 in shared memory (K2 keypoints), K1 keypoints of F1 as the queries
     int run_init(MatchParams& P, int K2, int K1, cudaStream_t st) {
-        P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX);
-        P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
         P.query = d_query; P.resultIdx = d_resultIdx; P.resultDist = d_resultDist; P.status = d_status;
         P.ks = std::max(K2, 1); P.ms = std::max(K1, 1);
         if (P.ks > 65535 || P.ms > 65535) { set_error("more than 65535 keypoints per frame"); return ORB_ERR_CAPACITY; }
-        const size_t limit = 227 * 1024 - 2048;
-        auto bytes = [&](bool d) { return frame_smem_bytes(P.ks, P.ms, d) + al16(sizeof(uint16_t) * (size_t)P.ks); };
-        P.descInSmem = bytes(true) <= limit ? 1 : 0;
-        const size_t sm = bytes(P.descInSmem != 0);
-        if (sm > limit) { set_error("frames too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
+        // vnMatches21 [K2] behind the frame
+        const size_t sm = frame_layout(P, al16(sizeof(uint16_t) * (size_t)P.ks), FRAME_SMEM_LIMIT, "frames too large for the matcher's shared-memory grid");
+        if (!sm) return ORB_ERR_CAPACITY;
         int rc = ensure_dynamic_smem(init_match_kernel, sm, device);
         if (rc) return rc;
-        cudaLaunchConfig_t cfg = {};
+        ClusterLaunch L(sm, st);
         const int C = 8;                                   // one pair of frames: pass 1 spread over a full cluster
-        cfg.gridDim = dim3(C); cfg.blockDim = dim3(MF_NT); cfg.dynamicSmemBytes = sm; cfg.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        CK(cudaLaunchKernelEx(&cfg, init_match_kernel, P));
+        CK(cudaLaunchKernelEx(L.shape(1, C), init_match_kernel, P));
         launches = 1;
         lastCluster = C;
         return ORB_OK;
@@ -2156,8 +2106,8 @@ static int fuse_search_run(Matcher& m, int n, const FuseJob* jobs) {
     CK(cudaSetDevice(m.device));
     for (int j = 0; j < n; ++j)
         for (int i = 0; i < jobs[j].pts->M; ++i) { jobs[j].bestIdx[i] = -1; jobs[j].bestDist[i] = 256; }
-    const size_t limit = 227 * 1024 - 2048;
     std::vector<int> act;
+    std::vector<MatchParams> frame;       // the keyframe part of each active job's MatchParams: bounds, grid scale, shared-memory layout
     size_t sm = 0;
     int nCta = 0;
     for (int j = 0; j < n; ++j) {
@@ -2165,10 +2115,14 @@ static int fuse_search_run(Matcher& m, int n, const FuseJob* jobs) {
         const int M = jobs[j].pts->M, K = KF->K;
         if (M == 0 || K == 0) continue;
         for (int k = 0; k < K; ++k) if (KF->keypoints[k].octave < 0 || KF->keypoints[k].octave >= KF->nlevels) { set_error("orbm_fuse_search: keypoint octave out of range"); return ORB_ERR_ARG; }
-        const size_t b = frame_smem_bytes(K, 1, frame_smem_bytes(K, 1, true) <= limit);
-        if (b > limit) { set_error("keyframe too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
+        MatchParams P = {};
+        P.minX = KF->minX; P.minY = KF->minY; P.maxX = KF->maxX; P.maxY = KF->maxY;
+        P.ks = K; P.ms = 1;
+        const size_t b = frame_layout(P, 0, FRAME_SMEM_LIMIT, "keyframe too large for the matcher's shared-memory grid");
+        if (!b) return ORB_ERR_CAPACITY;
         sm = std::max(sm, b);
         act.push_back(j);
+        frame.push_back(P);
         nCta += std::min(16, (M + 127) / 128);          // every CTA rebuilds its item's grid: a few CTAs per item, ~8 map points per warp
     }
     if (act.empty()) return ORB_OK;
@@ -2199,12 +2153,9 @@ static int fuse_search_run(Matcher& m, int n, const FuseJob* jobs) {
         FuseParams& Q = tab[a];
         memset(&Q, 0, sizeof(Q));
         MatchParams& P = Q.P;
+        P = frame[a];
         P.kps = S.dev<OrbKeyPoint>(p.kp); P.desc = S.dev(p.de); P.scaleFactors = S.dev<float>(p.sf); P.kcap = m.kcap; P.nlevels = KF->nlevels; P.batch = 1;
-        P.minX = KF->minX; P.minY = KF->minY; P.maxX = KF->maxX; P.maxY = KF->maxY;
-        P.gridWInv = (float)GRID_COLS / (P.maxX - P.minX); P.gridHInv = (float)GRID_ROWS / (P.maxY - P.minY);
         P.th = J.th; memcpy(P.cam, J.cam4, 16);
-        P.ks = KF->K; P.ms = 1;
-        P.descInSmem = frame_smem_bytes(P.ks, 1, true) <= limit ? 1 : 0;
         Q.K = KF->K; Q.M = J.pts->M; Q.state = S.dev(p.st); Q.mpDesc = S.dev(p.md); Q.xyz = S.dev<float>(p.xy); Q.normal = S.dev<float>(p.no);
         Q.minD = S.dev<float>(p.mi); Q.maxD = S.dev<float>(p.ma); Q.invSigma2 = S.dev<float>(p.is);
         if (J.mode == 0) { memcpy(Q.Tcw, J.Tcw7, 28); memcpy(Q.Ow, J.Ow3, 12); }
@@ -2841,7 +2792,7 @@ static int local_map_shape(const Matcher& m, const OrbmLocalMapBatch* in, const 
         set_error(std::string(who) + ": bad argument (sizes or null arrays)"); return ORB_ERR_ARG;
     }
     if (in->mcap > m.mcap) { set_error(std::string(who) + ": more local map points than max_mappoints"); return ORB_ERR_CAPACITY; }
-    if (frame_smem_bytes(in->kcap, in->mcap, false) > 227 * 1024 - 2048) { set_error(std::string(who) + ": frame too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
+    if (frame_smem_bytes(in->kcap, in->mcap, false) > FRAME_SMEM_LIMIT) { set_error(std::string(who) + ": frame too large for the matcher's shared-memory grid"); return ORB_ERR_CAPACITY; }
     return ORB_OK;
 }
 
