@@ -7,7 +7,8 @@
 //   4. local_ba_finish_kernel, one CTA per map: the outlier test, EraseObservation's cascade, SetPose, SetWorldPos, UpdateNormalAndDepth.
 // Every order the reference defines by list walks is rebuilt as a first-appearance order: a position space (the local keyframes' slots, or
 // the local points' observations, concatenated in list order) is scanned once with atomicMin for each item's first position, then one
-// ordered block scan over the positions numbers the items.
+// ordered block scan over the positions numbers the items.  The map table's check, staging, local-point walk and write-back of the local
+// points are map_walk.cuh's, shared with local_inertial_ba_map.cu.
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <stdint.h>
@@ -26,36 +27,29 @@
 namespace lba_local {
 
 using orbx::set_error;
-using orbx::csr_ok;
 using orbx::all_distinct;
 using orbx::segment;
 
 constexpr int WT = 512;
 constexpr unsigned char KF_SKIP = ORBM_KF_BAD | ORBM_KF_OTHER_MAP;   // isBad() || GetMap() != pCurrentMap
 
-// One map as the kernels see it: the caller's arrays, its outputs and its scratch in the staging buffer.
-struct Map {
-    int nKF, nCov, nPoints, nObs, nlevels, sortCap;
-    const unsigned long long* mnId; const uint8_t* kfFlags; const float *pose7, *Ow, *cam4;
-    const int *cov, *slotStart, *slotPoint;
-    const unsigned long long* pointId; const uint8_t* pointFlags; const float* pos; const int* refKF;
-    const int *obsStart, *obsKF, *obsOctave; const float* obsPt;
-    const float *invLevelSigma2, *scaleFactors;
+// One map as the kernels see it: the table (map_walk.cuh), and the caller's arrays, outputs and scratch only this function has.
+struct Map : orbx::MapTable {
+    int nCov, sortCap;
+    const unsigned long long* mnId; const uint8_t* kfFlags; const float* pose7; const int* cov;
+    const unsigned long long* pointId;
     // outputs
     int* sizes;                       // [8] walk verdict (0 built, 1 no fixed keyframe), nP, nL, nE, nF
-    int *counts, *nLists, *localKF, *fixedKF, *localPoint; uint8_t* obsFlag;
-    float *kfPose7, *kfCenter, *pointPos; uint8_t* pointBad; int* pointRefKF; float *normal, *minDistance, *maxDistance; double* lmStats;
-    double *optPose, *optPoint, *edgeChi2; uint8_t* edgeDepthPos;      // optional
+    int *counts, *nLists, *localKF, *fixedKF; double* lmStats;
+    double* optPose; uint8_t* edgeDepthPos;      // optional
     // the built problem (LbaProblem's layout)
     double* bPoses; uint8_t* bFixed; float* bCam; double* bPts; int *bEPt, *bEPose; double* bObs; float* bIsg;
     // scratch
     int *kfRank;                      // [nKF] local rank, -2 for the other entries of the covisible list (mnBALocalForKF), else -1
     int *kfVert, *ptVert;             // vertex of a keyframe / point, -1 none
-    int *firstFix, *firstPt;          // first position of a fixed-camera candidate / local point
-    int *obsEdge;                     // [nObs] edge of an observation, -1 none
-    int *locCand, *locBase, *lpBase;  // candidate of a local keyframe, slot base of the local keyframes, observation base of the local points
+    int *firstFix;                    // first position of a fixed-camera candidate
+    int *locCand, *locBase;           // candidate of a local keyframe, slot base of the local keyframes
     unsigned long long* key; int* val;   // [sortCap] sort buffers
-    float* Ow2;                       // [nKF][3] camera centres after SetPose
 };
 
 // What the finish kernel reads of the solve: status (LBA_LOCAL_*), solved (0: nothing was optimised), the slot's results.
@@ -85,8 +79,7 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     __syncthreads();
     // every output starts empty: lists -1, no edge, no estimate
     for (int k = tid; k < M.nKF; k += WT) { M.kfRank[k] = -1; M.kfVert[k] = -1; M.firstFix[k] = INT_MAX; M.localKF[k] = -1; M.fixedKF[k] = -1; }
-    for (int p = tid; p < M.nPoints; p += WT) { M.ptVert[p] = -1; M.firstPt[p] = INT_MAX; M.localPoint[p] = -1; }
-    for (int o = tid; o < M.nObs; o += WT) { M.obsEdge[o] = -1; M.obsFlag[o] = LBA_OBS_NO_EDGE; }
+    for (int p = tid; p < M.nPoints; p += WT) M.ptVert[p] = -1;
     __syncthreads();
     // lLocalKeyFrames: pKF, then the covisibles that are not bad and in the current map; every covisible is marked (mnBALocalForKF)
     if (tid == 0) {
@@ -104,29 +97,16 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     __syncthreads();
     const int nLocal = s_nLocal;
     // lLocalMapPoints: first appearance over the local keyframes' slots, bad and other-map points skipped
-    const int Qs = orbx::block_prefix<WT>(nLocal, M.locBase, sm, [&](int r) { const int c = M.locCand[r]; return M.slotStart[c + 1] - M.slotStart[c]; });
-    if (tid == 0) M.locBase[nLocal] = Qs;
-    auto slotPt = [&](int q) {
-        const int r = segment(M.locBase, nLocal, q);
-        const int p = M.slotPoint[M.slotStart[M.locCand[r]] + q - M.locBase[r]];
-        return p >= 0 && !(M.pointFlags[p] & KF_SKIP) ? p : -1;
-    };
-    for (int q = tid; q < Qs; q += WT) { const int p = slotPt(q); if (p >= 0) atomicMin(&M.firstPt[p], q); }
-    __syncthreads();
-    const int nL = orbx::compact<WT>(Qs, sm, [&](int q) { const int p = slotPt(q); return p >= 0 && M.firstPt[p] == q; },
-                           [&](int q, int r) { M.localPoint[r] = slotPt(q); });
-    __syncthreads();
+    int Qo;
+    const int nL = orbx::local_points<WT>(M, nLocal, [&](int r) { return M.locCand[r]; }, M.locBase, sm, KF_SKIP, Qo);
     // lFixedCameras: first appearance over (local point, observation) of the unmarked observers, kept when good and in the current map
-    const int Qo = orbx::block_prefix<WT>(nL, M.lpBase, sm, [&](int r) { const int p = M.localPoint[r]; return M.obsStart[p + 1] - M.obsStart[p]; });
-    if (tid == 0) M.lpBase[nL] = Qo;
-    auto obsAt = [&](int q) { const int r = segment(M.lpBase, nL, q); return M.obsStart[M.localPoint[r]] + q - M.lpBase[r]; };
     for (int q = tid; q < Qo; q += WT) {
-        const int k = M.obsKF[obsAt(q)];
+        const int k = M.obsKF[orbx::obs_at(M, nL, q)];
         if (M.kfRank[k] == -1 && !(M.kfFlags[k] & KF_SKIP)) atomicMin(&M.firstFix[k], q);
     }
     __syncthreads();
-    const int nFix = orbx::compact<WT>(Qo, sm, [&](int q) { const int k = M.obsKF[obsAt(q)]; return M.kfRank[k] == -1 && M.firstFix[k] == q; },
-                             [&](int q, int r) { M.fixedKF[r] = M.obsKF[obsAt(q)]; });
+    const int nFix = orbx::compact<WT>(Qo, sm, [&](int q) { const int k = M.obsKF[orbx::obs_at(M, nL, q)]; return M.kfRank[k] == -1 && M.firstFix[k] == q; },
+                             [&](int q, int r) { M.fixedKF[r] = M.obsKF[orbx::obs_at(M, nL, q)]; });
     __syncthreads();
     const int numFixed = nFix + s_init;
     if (numFixed == 0) {                              // :1178-1182: return before the optimiser is set up
@@ -170,7 +150,7 @@ __global__ void __launch_bounds__(WT) local_ba_walk_kernel(const Map* __restrict
     }
     __syncthreads();
     // edges in insertion order: local points in list order, observations in key order, observers good and in the current map
-    const int nE = orbx::compact<WT>(Qo, sm, [&](int q) { return !(M.kfFlags[M.obsKF[obsAt(q)]] & KF_SKIP); }, [&](int q, int e) {
+    const int nE = orbx::compact<WT>(Qo, sm, [&](int q) { return !(M.kfFlags[M.obsKF[orbx::obs_at(M, nL, q)]] & KF_SKIP); }, [&](int q, int e) {
         const int r = segment(M.lpBase, nL, q);
         const int p = M.localPoint[r], o = M.obsStart[p] + q - M.lpBase[r], k = M.obsKF[o];
         M.bEPt[e] = M.ptVert[p]; M.bEPose[e] = M.kfVert[k];
@@ -214,17 +194,8 @@ __global__ void __launch_bounds__(WT) local_ba_finish_kernel(const Map* __restri
         else for (int c = 0; c < 3; ++c) X[c] = (double)M.pos[3 * p + c];
     };
     // every output slot past the lists, and every slot of a map that did not run, holds zeros
-    for (int i = tid; i < M.nKF; i += WT) {
-        for (int c = 0; c < 7; ++c) M.kfPose7[7 * i + c] = 0.f;
-        for (int c = 0; c < 3; ++c) M.kfCenter[3 * i + c] = 0.f;
-        if (M.optPose) for (int c = 0; c < 7; ++c) M.optPose[7 * i + c] = 0.0;
-        for (int c = 0; c < 3; ++c) M.Ow2[3 * i + c] = M.Ow[3 * i + c];
-    }
-    for (int i = tid; i < M.nPoints; i += WT) {
-        for (int c = 0; c < 3; ++c) { M.pointPos[3 * i + c] = 0.f; M.normal[3 * i + c] = 0.f; }
-        M.pointBad[i] = 0; M.pointRefKF[i] = -1; M.minDistance[i] = M.maxDistance[i] = 0.f;
-        if (M.optPoint) for (int c = 0; c < 3; ++c) M.optPoint[3 * i + c] = 0.0;
-    }
+    orbx::clear_write_back<WT>(M);
+    if (M.optPose) for (int i = tid; i < M.nKF; i += WT) for (int c = 0; c < 7; ++c) M.optPose[7 * i + c] = 0.0;
     for (int o = tid; o < M.nObs; o += WT) {
         if (M.edgeChi2) M.edgeChi2[o] = 0.0;
         if (M.edgeDepthPos) M.edgeDepthPos[o] = 0;
@@ -246,22 +217,14 @@ __global__ void __launch_bounds__(WT) local_ba_finish_kernel(const Map* __restri
     __syncthreads();
     // per local point: the outlier test and the erase loop (:1417-1460) in edge order -- the point's observations in key order, points
     // being independent -- then SetWorldPos and UpdateNormalAndDepth (:1474-1481)
-    for (int i = tid; i < nL; i += WT) {
-        const int p = M.localPoint[i];
-        double X[3];
-        pointOf(i, X);
-        if (M.optPoint) for (int c = 0; c < 3; ++c) M.optPoint[3 * i + c] = X[c];
-        float pos[3] = {(float)X[0], (float)X[1], (float)X[2]};
-        for (int c = 0; c < 3; ++c) M.pointPos[3 * i + c] = pos[c];
-        orbx::finish_point(M.obsKF, M.obsOctave, M.obsStart[p], M.obsStart[p + 1], M.obsFlag, M.refKF[p], [&](int o) -> uint8_t {
-            const int e = M.obsEdge[o];
-            if (e < 0) return LBA_OBS_NO_EDGE;
-            const double chi2 = V.solved ? V.r.chi2[e] : 0.0;
-            const uint8_t dpos = V.solved ? V.r.depthPos[e] : 1;
-            if (M.edgeChi2) { M.edgeChi2[o] = chi2; M.edgeDepthPos[o] = dpos; }
-            return chi2 > 5.991 || !dpos ? LBA_OBS_ERASED : LBA_OBS_KEPT;
-        }, pos, M.Ow2, M.scaleFactors, M.nlevels, M.pointBad + i, M.pointRefKF + i, M.normal + 3 * i, M.minDistance + i, M.maxDistance + i);
-    }
+    orbx::write_back_points<WT>(M, nL, pointOf, [&](int o) -> uint8_t {
+        const int e = M.obsEdge[o];
+        if (e < 0) return LBA_OBS_NO_EDGE;
+        const double chi2 = V.solved ? V.r.chi2[e] : 0.0;
+        const uint8_t dpos = V.solved ? V.r.depthPos[e] : 1;
+        if (M.edgeChi2) { M.edgeChi2[o] = chi2; M.edgeDepthPos[o] = dpos; }
+        return chi2 > 5.991 || !dpos ? LBA_OBS_ERASED : LBA_OBS_KEPT;
+    });
 }
 
 // ORB_ERR_ARG with a message naming the map, or ORB_OK
@@ -284,31 +247,9 @@ int check_map(const LbaLocalMap& m, int j) {
         if (seen[m.cov[i]]) return bad("cov repeats a keyframe");
         seen[m.cov[i]] = 1;
     }
-    if (!csr_ok(m.nCov + 1, m.slotStart)) return bad("slotStart must start at 0 and not decrease");
-    const int nSlots = m.slotStart[m.nCov + 1];
-    if (nSlots > 0 && !m.slotPoint) return bad("slotPoint is null");
-    for (int s = 0; s < nSlots; ++s)
-        if (m.slotPoint[s] < -1 || m.slotPoint[s] >= m.nPoints) return bad("slotPoint out of range");
-    if (m.nPoints > 0) {
-        if (!all_distinct(m.pointId, m.nPoints)) return bad("point mnIds repeat");
-        if (!csr_ok(m.nPoints, m.obsStart)) return bad("obsStart must start at 0 and not decrease");
-        const int nObs = m.obsStart[m.nPoints];
-        if (nObs > 0 && (!m.obsKF || !m.obsIdx || !m.obsPt || !m.obsOctave || !m.obsFlag)) return bad("an observation array is null");
-        std::vector<int> stamp(m.nKF, -1);             // the last point each keyframe was seen observing
-        for (int p = 0; p < m.nPoints; ++p) {
-            bool refSeen = false;
-            for (int o = m.obsStart[p]; o < m.obsStart[p + 1]; ++o) {
-                if (m.obsKF[o] < 0 || m.obsKF[o] >= m.nKF) return bad("obsKF out of range");
-                if (m.obsIdx[o] < 0) return bad("obsIdx negative");
-                if (m.obsOctave[o] < 0 || m.obsOctave[o] >= m.nlevels) return bad("obsOctave outside [0, nlevels)");
-                if (stamp[m.obsKF[o]] == p) return bad("a keyframe observes a point twice");
-                stamp[m.obsKF[o]] = p;
-                refSeen |= m.obsKF[o] == m.refKF[p];
-            }
-            if (!(m.pointFlags[p] & ORBM_KF_BAD) && m.obsStart[p + 1] > m.obsStart[p] && !refSeen) return bad("a point's mpRefKF is not among its observers");
-        }
-    }
-    return ORB_OK;
+    if (int rc = orbx::check_slots(m, m.nCov + 1, bad)) return rc;
+    if (m.nPoints > 0 && !all_distinct(m.pointId, m.nPoints)) return bad("point mnIds repeat");
+    return orbx::check_observations(m, bad);
 }
 
 }  // namespace lba_local
@@ -327,35 +268,25 @@ extern "C" int lba_local_bundle_adjustment_batch(lba_handle* h, int nMaps, const
     const cudaStream_t st = lba::solver_stream(h);
     orbx::Staging& S = lba::solver_staging(h);
     S.begin();
-    struct Pieces { int mnId, flags, pose, Ow, cam, cov, slotStart, slotPoint, pid, pflags, pos, ref, obsStart, obsKF, obsPt, obsOct, isg, sf,
-                    sizes, counts, nLists, localKF, fixedKF, localPoint, obsFlag, kfPose, kfCenter, pointPos, pointBad, pointRef, normal, minD, maxD,
-                    lm, optPose, optPoint, chi2, dpos, bPoses, bFixed, bCam, bPts, bEPt, bEPose, bObs, bIsg, kfRank, kfVert, ptVert, firstFix,
-                    firstPt, obsEdge, locCand, locBase, lpBase, key, val, Ow2; int sortCap; };
-    std::vector<Pieces> pc(nMaps);
+    struct Pieces { orbx::MapTablePieces tab; int mnId, flags, pose, cov, pid, counts, nLists, localKF, fixedKF, lm, optPose, dpos, bPoses, bFixed,
+                    bCam, bPts, bEPt, bEPose, bObs, bIsg, kfRank, kfVert, ptVert, firstFix, locCand, locBase, key, val, sortCap; };
+    std::vector<Pieces> pc;
     const int sizesAll = S.out(nullptr, 32 * (size_t)nMaps);       // one piece, so that one small copy brings every map's sizes
     for (int j = 0; j < nMaps; ++j) {
         const LbaLocalMap& m = maps[j];
-        const size_t K = m.nKF, C = m.nCov, P = m.nPoints, NS = m.slotStart[m.nCov + 1], O = P ? m.obsStart[m.nPoints] : 0, L = m.nlevels;
-        Pieces& q = pc[j];
+        const size_t K = m.nKF, C = m.nCov, P = m.nPoints, O = P ? m.obsStart[m.nPoints] : 0;
+        pc.push_back({orbx::MapTablePieces(S, m, m.nCov + 1)});
+        Pieces& q = pc.back();
         q.sortCap = 1;
         while (q.sortCap < std::max<int>(m.nKF, m.nPoints)) q.sortCap <<= 1;
-        q.mnId = S.in(m.mnId, 8 * K); q.flags = S.in(m.kfFlags, K); q.pose = S.in(m.pose7, 28 * K); q.Ow = S.in(m.cameraCenter, 12 * K);
-        q.cam = S.in(m.cam4, 16 * K); q.cov = S.in(m.cov, 4 * C); q.slotStart = S.in(m.slotStart, 4 * (C + 2)); q.slotPoint = S.in(m.slotPoint, 4 * NS);
-        q.pid = S.in(m.pointId, 8 * P); q.pflags = S.in(m.pointFlags, P); q.pos = S.in(m.worldPos, 12 * P); q.ref = S.in(m.refKF, 4 * P);
-        q.obsStart = S.in(P ? m.obsStart : nullptr, P ? 4 * (P + 1) : 0); q.obsKF = S.in(m.obsKF, 4 * O); q.obsPt = S.in(m.obsPt, 8 * O);
-        q.obsOct = S.in(m.obsOctave, 4 * O); q.isg = S.in(m.invLevelSigma2, 4 * L); q.sf = S.in(m.scaleFactors, 4 * L);
-        q.sizes = j; q.counts = S.out(m.counts, 16); q.nLists = S.out(m.nLists, 12);
-        q.localKF = S.out(m.localKF, 4 * K); q.fixedKF = S.out(m.fixedKF, 4 * K); q.localPoint = S.out(m.localPoint, 4 * P); q.obsFlag = S.out(m.obsFlag, O);
-        q.kfPose = S.out(m.kfPose7, 28 * K); q.kfCenter = S.out(m.kfCenter, 12 * K); q.pointPos = S.out(m.pointPos, 12 * P);
-        q.pointBad = S.out(m.pointBad, P); q.pointRef = S.out(m.pointRefKF, 4 * P); q.normal = S.out(m.normal, 12 * P);
-        q.minD = S.out(m.minDistance, 4 * P); q.maxD = S.out(m.maxDistance, 4 * P); q.lm = S.out(m.lmStats, 40);
-        q.optPose = S.out(m.optPose, m.optPose ? 56 * K : 0); q.optPoint = S.out(m.optPoint, m.optPoint ? 24 * P : 0);
-        q.chi2 = S.out(m.edgeChi2, m.edgeChi2 ? 8 * O : 0); q.dpos = S.out(m.edgeDepthPositive, m.edgeChi2 ? O : 0);
+        q.mnId = S.in(m.mnId, 8 * K); q.flags = S.in(m.kfFlags, K); q.pose = S.in(m.pose7, 28 * K); q.cov = S.in(m.cov, 4 * C); q.pid = S.in(m.pointId, 8 * P);
+        q.counts = S.out(m.counts, 16); q.nLists = S.out(m.nLists, 12); q.localKF = S.out(m.localKF, 4 * K); q.fixedKF = S.out(m.fixedKF, 4 * K);
+        q.lm = S.out(m.lmStats, 40); q.optPose = S.out(m.optPose, m.optPose ? 56 * K : 0); q.dpos = S.out(m.edgeDepthPositive, m.edgeChi2 ? O : 0);
         q.bPoses = S.scratch(56 * K); q.bFixed = S.scratch(K); q.bCam = S.scratch(16 * K); q.bPts = S.scratch(24 * P);
         q.bEPt = S.scratch(4 * O); q.bEPose = S.scratch(4 * O); q.bObs = S.scratch(16 * O); q.bIsg = S.scratch(4 * O);
-        q.kfRank = S.scratch(4 * K); q.kfVert = S.scratch(4 * K); q.ptVert = S.scratch(4 * P); q.firstFix = S.scratch(4 * K); q.firstPt = S.scratch(4 * P);
-        q.obsEdge = S.scratch(4 * O); q.locCand = S.scratch(4 * (C + 1)); q.locBase = S.scratch(4 * (C + 2)); q.lpBase = S.scratch(4 * (P + 1));
-        q.key = S.scratch(8 * (size_t)q.sortCap); q.val = S.scratch(4 * (size_t)q.sortCap); q.Ow2 = S.scratch(12 * K);
+        q.kfRank = S.scratch(4 * K); q.kfVert = S.scratch(4 * K); q.ptVert = S.scratch(4 * P); q.firstFix = S.scratch(4 * K);
+        q.locCand = S.scratch(4 * (C + 1)); q.locBase = S.scratch(4 * (C + 2));
+        q.key = S.scratch(8 * (size_t)q.sortCap); q.val = S.scratch(4 * (size_t)q.sortCap);
     }
     const int tab = S.in(nullptr, sizeof(Map) * nMaps), fillTab = S.scratch(sizeof(lba::FillSrc) * nMaps), solveTab = S.scratch(sizeof(Solve) * nMaps);
     if (int rc = S.reserve()) return rc;
@@ -364,24 +295,17 @@ extern "C" int lba_local_bundle_adjustment_batch(lba_handle* h, int nMaps, const
         const LbaLocalMap& m = maps[j];
         const Pieces& q = pc[j];
         Map d;
-        d.nKF = m.nKF; d.nCov = m.nCov; d.nPoints = m.nPoints; d.nObs = m.nPoints ? m.obsStart[m.nPoints] : 0; d.nlevels = m.nlevels; d.sortCap = q.sortCap;
-        d.mnId = S.dev<unsigned long long>(q.mnId); d.kfFlags = S.dev(q.flags); d.pose7 = S.dev<float>(q.pose); d.Ow = S.dev<float>(q.Ow);
-        d.cam4 = S.dev<float>(q.cam); d.cov = S.dev<int>(q.cov); d.slotStart = S.dev<int>(q.slotStart); d.slotPoint = S.dev<int>(q.slotPoint);
-        d.pointId = S.dev<unsigned long long>(q.pid); d.pointFlags = S.dev(q.pflags); d.pos = S.dev<float>(q.pos); d.refKF = S.dev<int>(q.ref);
-        d.obsStart = S.dev<int>(q.obsStart); d.obsKF = S.dev<int>(q.obsKF); d.obsOctave = S.dev<int>(q.obsOct); d.obsPt = S.dev<float>(q.obsPt);
-        d.invLevelSigma2 = S.dev<float>(q.isg); d.scaleFactors = S.dev<float>(q.sf);
+        q.tab.bind(S, d);
+        d.nCov = m.nCov; d.sortCap = q.sortCap;
+        d.mnId = S.dev<unsigned long long>(q.mnId); d.kfFlags = S.dev(q.flags); d.pose7 = S.dev<float>(q.pose); d.cov = S.dev<int>(q.cov);
+        d.pointId = S.dev<unsigned long long>(q.pid);
         d.sizes = S.dev<int>(sizesAll) + 8 * j; d.counts = S.dev<int>(q.counts); d.nLists = S.dev<int>(q.nLists); d.localKF = S.dev<int>(q.localKF);
-        d.fixedKF = S.dev<int>(q.fixedKF); d.localPoint = S.dev<int>(q.localPoint); d.obsFlag = S.dev(q.obsFlag);
-        d.kfPose7 = S.dev<float>(q.kfPose); d.kfCenter = S.dev<float>(q.kfCenter); d.pointPos = S.dev<float>(q.pointPos); d.pointBad = S.dev(q.pointBad);
-        d.pointRefKF = S.dev<int>(q.pointRef); d.normal = S.dev<float>(q.normal); d.minDistance = S.dev<float>(q.minD); d.maxDistance = S.dev<float>(q.maxD);
-        d.lmStats = S.dev<double>(q.lm);
-        d.optPose = m.optPose ? S.dev<double>(q.optPose) : nullptr; d.optPoint = m.optPoint ? S.dev<double>(q.optPoint) : nullptr;
-        d.edgeChi2 = m.edgeChi2 ? S.dev<double>(q.chi2) : nullptr; d.edgeDepthPos = m.edgeChi2 ? S.dev(q.dpos) : nullptr;
+        d.fixedKF = S.dev<int>(q.fixedKF); d.lmStats = S.dev<double>(q.lm);
+        d.optPose = m.optPose ? S.dev<double>(q.optPose) : nullptr; d.edgeDepthPos = m.edgeChi2 ? S.dev(q.dpos) : nullptr;
         d.bPoses = S.dev<double>(q.bPoses); d.bFixed = S.dev(q.bFixed); d.bCam = S.dev<float>(q.bCam); d.bPts = S.dev<double>(q.bPts);
         d.bEPt = S.dev<int>(q.bEPt); d.bEPose = S.dev<int>(q.bEPose); d.bObs = S.dev<double>(q.bObs); d.bIsg = S.dev<float>(q.bIsg);
         d.kfRank = S.dev<int>(q.kfRank); d.kfVert = S.dev<int>(q.kfVert); d.ptVert = S.dev<int>(q.ptVert); d.firstFix = S.dev<int>(q.firstFix);
-        d.firstPt = S.dev<int>(q.firstPt); d.obsEdge = S.dev<int>(q.obsEdge); d.locCand = S.dev<int>(q.locCand); d.locBase = S.dev<int>(q.locBase);
-        d.lpBase = S.dev<int>(q.lpBase); d.key = S.dev<unsigned long long>(q.key); d.val = S.dev<int>(q.val); d.Ow2 = S.dev<float>(q.Ow2);
+        d.locCand = S.dev<int>(q.locCand); d.locBase = S.dev<int>(q.locBase); d.key = S.dev<unsigned long long>(q.key); d.val = S.dev<int>(q.val);
         T[j] = d;
     }
     CK(S.upload(st));

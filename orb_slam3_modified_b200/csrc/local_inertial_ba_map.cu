@@ -6,11 +6,11 @@
 //   2. local_inertial_ba_kernel (local_inertial_ba.cu), unchanged, on those entries;
 //   3. local_inertial_ba_map_finish_kernel, one CTA per map: the FAIL test, the write-back of the window, and per local point the erase
 //      cascade, SetWorldPos and UpdateNormalAndDepth.
-// The local points are a first-appearance order over the window's slots (map_walk.cuh, as local_ba.cu builds lLocalMapPoints).  The
-// rule that fills lFixedKeyFrames is sequential: each point's observers are marked as far as the first good one, so a point's effect
-// depends on every earlier point.  Only points with an observer outside the window and its predecessor can mark anything; the kernel
-// compacts those, then repeatedly finds the first one that still has an unmarked observer (one parallel probe per 512 candidates) and
-// lets one thread apply the rule to it.  Each such step marks at least one keyframe.
+// The map table's check, staging, local-point walk (a first-appearance order over the window's slots) and write-back of the local points
+// are map_walk.cuh's, shared with local_ba.cu.  The rule that fills lFixedKeyFrames is sequential: each point's observers are marked as
+// far as the first good one, so a point's effect depends on every earlier point.  Only points with an observer outside the window and its
+// predecessor can mark anything; the kernel compacts those, then repeatedly finds the first one that still has an unmarked observer (one
+// parallel probe per 512 candidates) and lets one thread apply the rule to it.  Each such step marks at least one keyframe.
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <stdint.h>
@@ -41,26 +41,19 @@ constexpr uint8_t MARK_LOCAL = 1, MARK_FIXED = 2;   // mnBALocalForKF / mnBAFixe
 
 thread_local int t_launches = 0;
 
-// One map as the kernels see it: the caller's arrays, its outputs and its scratch in the staging buffer, and its Dev entry.
-struct Map {
-    int nKF, nPoints, nObs, nlevels, Nd, bRecInit;
-    const uint8_t* kfFlags; const int* prevKF; const float *state21, *tcw12, *Ow, *cam4, *preint; const double* extr;
-    const int *slotStart, *slotPoint;
-    const uint8_t* pointFlags; const float *pos, *trackDepth; const int* refKF;
-    const int *obsStart, *obsKF, *obsOctave; const float* obsPt;
-    const float *invLevelSigma2, *scaleFactors;
+// One map as the kernels see it: the table (map_walk.cuh), the caller's arrays, outputs and scratch only this function has, and its Dev entry.
+struct Map : orbx::MapTable {
+    int Nd, bRecInit;
+    const uint8_t* kfFlags; const int* prevKF; const float *state21, *tcw12, *preint; const double* extr;
+    const float* trackDepth;
     // outputs
-    int *status, *nLists, *optKF, *fixedKF, *localPoint; uint8_t *ieLinked, *obsFlag;
-    float *kfPose7, *kfCenter, *kfVelocity, *kfBias6, *pointPos; uint8_t* pointBad; int* pointRefKF; float *normal, *minDistance, *maxDistance;
-    double* stats8; double *optState21, *optTcw12, *optPoint, *edgeChi2;   // the last four optional
+    int *status, *nLists, *optKF, *fixedKF; uint8_t* ieLinked;
+    float *kfVelocity, *kfBias6;
+    double* stats8; double *optState21, *optTcw12;   // optional, with optPoint and edgeChi2
     // scratch
     uint8_t* mark;                    // [nKF] MARK_LOCAL / MARK_FIXED, 0 unmarked
     int* kfIdx;                       // [nKF] problem keyframe, -1 none
-    int* firstPt;                     // [nPoints] first slot position of a local point
-    int* lpBase;                      // [nPoints + 1] observation base of the local points
     int* cand;                        // [nPoints] local points with an observer left unmarked by the window and its predecessor
-    int* obsEdge;                     // [nObs] mono edge of an observation, -1 none
-    float* Ow2;                       // [nKF][3] camera centres after SetPose
     liba::Dev* D;                     // the map's solver problem
 };
 
@@ -75,8 +68,6 @@ __global__ void __launch_bounds__(WT) local_inertial_ba_walk_kernel(const Map* _
     if (tid == 0) { M = maps[blockIdx.x]; D = *M.D; }
     __syncthreads();
     for (int k = tid; k < M.nKF; k += WT) { M.mark[k] = 0; M.kfIdx[k] = -1; M.optKF[k] = -1; M.fixedKF[k] = -1; M.ieLinked[k] = 0; }
-    for (int p = tid; p < M.nPoints; p += WT) { M.firstPt[p] = INT_MAX; M.localPoint[p] = -1; }
-    for (int o = tid; o < M.nObs; o += WT) { M.obsEdge[o] = -1; M.obsFlag[o] = LBA_OBS_NO_EDGE; }
     // vpOptimizableKFs (:2395-2410): pKF, then mPrevKF while it exists, Nd keyframes at most
     if (tid == 0) {
         int n = 0;
@@ -92,18 +83,8 @@ __global__ void __launch_bounds__(WT) local_inertial_ba_walk_kernel(const Map* _
     const int nWin = s_nWin;
     for (int i = tid; i < nWin; i += WT) M.mark[s_win[i]] = MARK_LOCAL;
     // lLocalMapPoints (:2413-2428): first appearance over the slots of the whole window (before the pop below), NULL and bad points skipped
-    const int Qs = orbx::block_prefix<WT>(nWin, s_winBase, sm, [&](int i) { const int k = s_win[i]; return M.slotStart[k + 1] - M.slotStart[k]; });
-    auto slotPt = [&](int q) {
-        const int i = orbx::segment(s_winBase, nWin, q), k = s_win[i];
-        const int p = M.slotPoint[M.slotStart[k] + q - s_winBase[i]];
-        return p >= 0 && !(M.pointFlags[p] & ORBM_KF_BAD) ? p : -1;
-    };
-    if (tid == 0) s_winBase[nWin] = Qs;
-    __syncthreads();
-    for (int q = tid; q < Qs; q += WT) { const int p = slotPt(q); if (p >= 0) atomicMin(&M.firstPt[p], q); }
-    __syncthreads();
-    const int nL = orbx::compact<WT>(Qs, sm, [&](int q) { const int p = slotPt(q); return p >= 0 && M.firstPt[p] == q; },
-                                     [&](int q, int r) { M.localPoint[r] = slotPt(q); });
+    int Qo;
+    const int nL = orbx::local_points<WT>(M, nWin, [&](int i) { return s_win[i]; }, s_winBase, sm, ORBM_KF_BAD, Qo);
     // lFixedKeyFrames' first entry (:2431-2442): the window's predecessor, or the window's last keyframe popped
     if (tid == 0) {
         const int back = s_win[nWin - 1], pred = M.prevKF[back];
@@ -181,12 +162,10 @@ __global__ void __launch_bounds__(WT) local_inertial_ba_walk_kernel(const Map* _
     for (int x = tid; x < nI * IMU_PREINT_FLOATS; x += WT)
         const_cast<float*>(D.preint)[x] = M.preint[(size_t)IMU_PREINT_FLOATS * s_ieSrc[x / IMU_PREINT_FLOATS] + x % IMU_PREINT_FLOATS];
     // mono edges (:2690-2763): local points in list order, observations in key order, observers marked, good and in the current map
-    const int Qo = orbx::block_prefix<WT>(nL, M.lpBase, sm, [&](int r) { const int p = M.localPoint[r]; return M.obsStart[p + 1] - M.obsStart[p]; });
-    if (tid == 0) M.lpBase[nL] = Qo;
-    __syncthreads();
-    auto obsAt = [&](int q) { const int r = orbx::segment(M.lpBase, nL, q); return M.obsStart[M.localPoint[r]] + q - M.lpBase[r]; };
-    const int nE = orbx::compact<WT>(Qo, sm, [&](int q) { const int k = M.obsKF[obsAt(q)]; return M.mark[k] && !(M.kfFlags[k] & (ORBM_KF_BAD | ORBM_KF_OTHER_MAP)); },
-                                     [&](int q, int e) {
+    const int nE = orbx::compact<WT>(Qo, sm, [&](int q) {
+        const int k = M.obsKF[orbx::obs_at(M, nL, q)];
+        return M.mark[k] && !(M.kfFlags[k] & (ORBM_KF_BAD | ORBM_KF_OTHER_MAP));
+    }, [&](int q, int e) {
         const int r = orbx::segment(M.lpBase, nL, q);
         const int o = M.obsStart[M.localPoint[r]] + q - M.lpBase[r];
         const_cast<int*>(D.ePt)[e] = r; const_cast<int*>(D.eKf)[e] = M.kfIdx[M.obsKF[o]];
@@ -254,19 +233,14 @@ __global__ void __launch_bounds__(WT) local_inertial_ba_map_finish_kernel(const 
     if (tid < 8) M.stats8[tid] = D.stats[tid];
     if (tid == 0) *M.status = failed ? LIBA_LOCAL_FAILED : LIBA_LOCAL_RAN;
     // every output slot past the lists, and every slot of a FAILED map, holds zeros
+    orbx::clear_write_back<WT>(M);
     for (int i = tid; i < M.nKF; i += WT) {
-        for (int c = 0; c < 7; ++c) M.kfPose7[7 * i + c] = 0.f;
-        for (int c = 0; c < 3; ++c) { M.kfCenter[3 * i + c] = 0.f; M.kfVelocity[3 * i + c] = 0.f; M.Ow2[3 * i + c] = M.Ow[3 * i + c]; }
+        for (int c = 0; c < 3; ++c) M.kfVelocity[3 * i + c] = 0.f;
         for (int c = 0; c < 6; ++c) M.kfBias6[6 * i + c] = 0.f;
         if (M.optState21) {
             for (int c = 0; c < 21; ++c) M.optState21[21 * i + c] = !failed && i < nK ? D.outState[21 * i + c] : 0.0;
             for (int c = 0; c < 12; ++c) M.optTcw12[12 * i + c] = !failed && i < nK ? D.outTcw[12 * i + c] : 0.0;
         }
-    }
-    for (int i = tid; i < M.nPoints; i += WT) {
-        for (int c = 0; c < 3; ++c) { M.pointPos[3 * i + c] = 0.f; M.normal[3 * i + c] = 0.f; }
-        M.pointBad[i] = 0; M.pointRefKF[i] = -1; M.minDistance[i] = M.maxDistance[i] = 0.f;
-        if (M.optPoint) for (int c = 0; c < 3; ++c) M.optPoint[3 * i + c] = 0.0;
     }
     for (int o = tid; o < M.nObs; o += WT) {
         const int e = M.obsEdge[o];
@@ -294,20 +268,10 @@ __global__ void __launch_bounds__(WT) local_inertial_ba_map_finish_kernel(const 
     __syncthreads();
     // per local point (:2848-2902, :2935-2950): the erase loop in vToErase order -- points in list order, each point's edges in key order,
     // points being independent -- then SetWorldPos and UpdateNormalAndDepth against the new camera centres
-    for (int i = tid; i < nL; i += WT) {
-        const int p = M.localPoint[i];
-        float pos[3];
-        for (int c = 0; c < 3; ++c) {
-            const double X = D.outPts[3 * i + c];
-            if (M.optPoint) M.optPoint[3 * i + c] = X;
-            pos[c] = (float)X;
-            M.pointPos[3 * i + c] = pos[c];
-        }
-        orbx::finish_point(M.obsKF, M.obsOctave, M.obsStart[p], M.obsStart[p + 1], M.obsFlag, M.refKF[p], [&](int o) -> uint8_t {
-            const int e = M.obsEdge[o];
-            return e < 0 ? LBA_OBS_NO_EDGE : D.erase[e] ? LBA_OBS_ERASED : LBA_OBS_KEPT;
-        }, pos, M.Ow2, M.scaleFactors, M.nlevels, M.pointBad + i, M.pointRefKF + i, M.normal + 3 * i, M.minDistance + i, M.maxDistance + i);
-    }
+    orbx::write_back_points<WT>(M, nL, [&](int i, double* X) { for (int c = 0; c < 3; ++c) X[c] = D.outPts[3 * i + c]; }, [&](int o) -> uint8_t {
+        const int e = M.obsEdge[o];
+        return e < 0 ? LBA_OBS_NO_EDGE : D.erase[e] ? LBA_OBS_ERASED : LBA_OBS_KEPT;
+    });
 }
 
 // ORB_ERR_ARG with a message naming the map, or ORB_OK; *nWin = the window's length before the pop (a bound on N)
@@ -342,30 +306,8 @@ int check_map(const LocalInertialBAMap& m, int j, int* nWin) {
     std::vector<int> sorted(chain);
     std::sort(sorted.begin(), sorted.end());
     if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return bad("the mPrevKF chain revisits a keyframe within Nd + 1 steps");
-    if (!orbx::csr_ok(m.nKF, m.slotStart)) return bad("slotStart must start at 0 and not decrease");
-    const int nSlots = m.slotStart[m.nKF];
-    if (nSlots > 0 && !m.slotPoint) return bad("slotPoint is null");
-    for (int s = 0; s < nSlots; ++s)
-        if (m.slotPoint[s] < -1 || m.slotPoint[s] >= m.nPoints) return bad("slotPoint out of range");
-    if (m.nPoints > 0) {
-        if (!orbx::csr_ok(m.nPoints, m.obsStart)) return bad("obsStart must start at 0 and not decrease");
-        const int nObs = m.obsStart[m.nPoints];
-        if (nObs > 0 && (!m.obsKF || !m.obsIdx || !m.obsPt || !m.obsOctave || !m.obsFlag)) return bad("an observation array is null");
-        std::vector<int> stamp(m.nKF, -1);             // the last point each keyframe was seen observing
-        for (int p = 0; p < m.nPoints; ++p) {
-            bool refSeen = false;
-            for (int o = m.obsStart[p]; o < m.obsStart[p + 1]; ++o) {
-                if (m.obsKF[o] < 0 || m.obsKF[o] >= m.nKF) return bad("obsKF out of range");
-                if (m.obsIdx[o] < 0) return bad("obsIdx negative");
-                if (m.obsOctave[o] < 0 || m.obsOctave[o] >= m.nlevels) return bad("obsOctave outside [0, nlevels)");
-                if (stamp[m.obsKF[o]] == p) return bad("a keyframe observes a point twice");
-                stamp[m.obsKF[o]] = p;
-                refSeen |= m.obsKF[o] == m.refKF[p];
-            }
-            if (!(m.pointFlags[p] & ORBM_KF_BAD) && m.obsStart[p + 1] > m.obsStart[p] && !refSeen) return bad("a point's mpRefKF is not among its observers");
-        }
-    }
-    return ORB_OK;
+    if (int rc = orbx::check_slots(m, m.nKF, bad)) return rc;
+    return orbx::check_observations(m, bad);
 }
 
 }  // namespace liba_map
@@ -384,32 +326,24 @@ extern "C" int local_inertial_ba_map_batch(int nMaps, const LocalInertialBAMap* 
     if (int rc = orbx::thread_staging(device, &S)) return rc;
     if (nMaps == 0) return ORB_OK;
     S->begin();
-    struct Pieces { int flags, prev, state, tcw, Ow, cam, preint, extr, slotStart, slotPoint, pflags, pos, td, ref, obsStart, obsKF, obsPt, obsOct, isg, sf,
-                    status, nLists, optKF, fixedKF, localPoint, ieLinked, obsFlag, kfPose, kfCenter, kfVel, kfBias, pointPos, pointBad, pointRef, normal,
-                    minD, maxD, stats, optState, optTcw, optPoint, chi2, mark, kfIdx, firstPt, lpBase, cand, obsEdge, Ow2, in, sc, out; liba::Layout lay; };
-    std::vector<Pieces> pc(nMaps);
+    struct Pieces { orbx::MapTablePieces tab; int flags, prev, state, tcw, preint, extr, td, status, nLists, optKF, fixedKF, ieLinked, kfVel, kfBias,
+                    stats, optState, optTcw, mark, kfIdx, cand, in, sc, out; liba::Layout lay; };
+    std::vector<Pieces> pc;
     for (int j = 0; j < nMaps; ++j) {
         const LocalInertialBAMap& m = maps[j];
-        const size_t K = m.nKF, P = m.nPoints, NS = m.slotStart[m.nKF], O = P ? m.obsStart[m.nPoints] : 0, L = m.nlevels;
+        const size_t K = m.nKF, P = m.nPoints, O = P ? m.obsStart[m.nPoints] : 0;
         bool preint = false;
         for (int k = 0; k < m.nKF; ++k) preint |= (m.kfFlags[k] & ORBM_KF_PREINT) != 0;
-        Pieces& q = pc[j];
+        pc.push_back({orbx::MapTablePieces(*S, m, m.nKF)});
+        Pieces& q = pc.back();
         q.flags = S->in(m.kfFlags, K); q.prev = S->in(m.prevKF, 4 * K); q.state = S->in(m.state21, 84 * K); q.tcw = S->in(m.tcw12, 48 * K);
-        q.Ow = S->in(m.cameraCenter, 12 * K); q.cam = S->in(m.cam4, 16 * K); q.preint = S->in(preint ? m.preint : nullptr, preint ? 4 * IMU_PREINT_FLOATS * K : 0);
-        q.extr = S->in(m.extrinsics24, 24 * 8); q.slotStart = S->in(m.slotStart, 4 * (K + 1)); q.slotPoint = S->in(m.slotPoint, 4 * NS);
-        q.pflags = S->in(m.pointFlags, P); q.pos = S->in(m.worldPos, 12 * P); q.td = S->in(m.trackDepth, 4 * P); q.ref = S->in(m.refKF, 4 * P);
-        q.obsStart = S->in(P ? m.obsStart : nullptr, P ? 4 * (P + 1) : 0); q.obsKF = S->in(m.obsKF, 4 * O); q.obsPt = S->in(m.obsPt, 8 * O);
-        q.obsOct = S->in(m.obsOctave, 4 * O); q.isg = S->in(m.invLevelSigma2, 4 * L); q.sf = S->in(m.scaleFactors, 4 * L);
+        q.preint = S->in(preint ? m.preint : nullptr, preint ? 4 * IMU_PREINT_FLOATS * K : 0); q.extr = S->in(m.extrinsics24, 24 * 8);
+        q.td = S->in(m.trackDepth, 4 * P);
         q.status = S->out(m.status, 4); q.nLists = S->out(m.nLists, 16); q.optKF = S->out(m.optKF, 4 * K); q.fixedKF = S->out(m.fixedKF, 4 * K);
-        q.localPoint = S->out(m.localPoint, 4 * P); q.ieLinked = S->out(m.ieLinked, K); q.obsFlag = S->out(m.obsFlag, O);
-        q.kfPose = S->out(m.kfPose7, 28 * K); q.kfCenter = S->out(m.kfCenter, 12 * K); q.kfVel = S->out(m.kfVelocity, 12 * K); q.kfBias = S->out(m.kfBias6, 24 * K);
-        q.pointPos = S->out(m.pointPos, 12 * P); q.pointBad = S->out(m.pointBad, P); q.pointRef = S->out(m.pointRefKF, 4 * P); q.normal = S->out(m.normal, 12 * P);
-        q.minD = S->out(m.minDistance, 4 * P); q.maxD = S->out(m.maxDistance, 4 * P); q.stats = S->out(m.stats8, 64);
+        q.ieLinked = S->out(m.ieLinked, K); q.kfVel = S->out(m.kfVelocity, 12 * K); q.kfBias = S->out(m.kfBias6, 24 * K); q.stats = S->out(m.stats8, 64);
         const bool dbg = m.optState21 != nullptr;
-        q.optState = S->out(m.optState21, dbg ? 168 * K : 0); q.optTcw = S->out(m.optTcw12, dbg ? 96 * K : 0); q.optPoint = S->out(m.optPoint, dbg ? 24 * P : 0);
-        q.chi2 = S->out(m.edgeChi2, dbg ? 8 * O : 0);
-        q.mark = S->scratch(K); q.kfIdx = S->scratch(4 * K); q.firstPt = S->scratch(4 * P); q.lpBase = S->scratch(4 * (P + 1)); q.cand = S->scratch(4 * P);
-        q.obsEdge = S->scratch(4 * O); q.Ow2 = S->scratch(12 * K);
+        q.optState = S->out(m.optState21, dbg ? 168 * K : 0); q.optTcw = S->out(m.optTcw12, dbg ? 96 * K : 0);
+        q.mark = S->scratch(K); q.kfIdx = S->scratch(4 * K); q.cand = S->scratch(4 * P);
         // the solver's regions, laid out from bounds: N <= nWin keyframes in the window and as many inertial edges, at most every table
         // keyframe, point and observation in the problem
         q.lay = liba::make_layout(K, nWin[j], nWin[j], P, O, (int)O);
@@ -426,24 +360,15 @@ extern "C" int local_inertial_ba_map_batch(int nMaps, const LocalInertialBAMap* 
         bound.iterations = m.bLarge ? 4 : 10; bound.bLarge = m.bLarge ? 1 : 0; bound.lambdaInit = m.bLarge ? 1e-2 : 1e0;
         liba::bind(hDev[j], bound, q.lay, S->dev(q.in), S->dev(q.sc), S->dev(q.out));
         Map d;
-        d.nKF = m.nKF; d.nPoints = m.nPoints; d.nObs = m.nPoints ? m.obsStart[m.nPoints] : 0; d.nlevels = m.nlevels;
+        q.tab.bind(*S, d);
         d.Nd = std::min(m.keyFramesInMap - 2, m.bLarge ? 25 : 10); d.bRecInit = m.bRecInit != 0;
         d.kfFlags = S->dev(q.flags); d.prevKF = S->dev<int>(q.prev); d.state21 = S->dev<float>(q.state); d.tcw12 = S->dev<float>(q.tcw);
-        d.Ow = S->dev<float>(q.Ow); d.cam4 = S->dev<float>(q.cam); d.preint = S->dev<float>(q.preint); d.extr = S->dev<double>(q.extr);
-        d.slotStart = S->dev<int>(q.slotStart); d.slotPoint = S->dev<int>(q.slotPoint);
-        d.pointFlags = S->dev(q.pflags); d.pos = S->dev<float>(q.pos); d.trackDepth = S->dev<float>(q.td); d.refKF = S->dev<int>(q.ref);
-        d.obsStart = S->dev<int>(q.obsStart); d.obsKF = S->dev<int>(q.obsKF); d.obsOctave = S->dev<int>(q.obsOct); d.obsPt = S->dev<float>(q.obsPt);
-        d.invLevelSigma2 = S->dev<float>(q.isg); d.scaleFactors = S->dev<float>(q.sf);
+        d.preint = S->dev<float>(q.preint); d.extr = S->dev<double>(q.extr); d.trackDepth = S->dev<float>(q.td);
         d.status = S->dev<int>(q.status); d.nLists = S->dev<int>(q.nLists); d.optKF = S->dev<int>(q.optKF); d.fixedKF = S->dev<int>(q.fixedKF);
-        d.localPoint = S->dev<int>(q.localPoint); d.ieLinked = S->dev(q.ieLinked); d.obsFlag = S->dev(q.obsFlag);
-        d.kfPose7 = S->dev<float>(q.kfPose); d.kfCenter = S->dev<float>(q.kfCenter); d.kfVelocity = S->dev<float>(q.kfVel); d.kfBias6 = S->dev<float>(q.kfBias);
-        d.pointPos = S->dev<float>(q.pointPos); d.pointBad = S->dev(q.pointBad); d.pointRefKF = S->dev<int>(q.pointRef); d.normal = S->dev<float>(q.normal);
-        d.minDistance = S->dev<float>(q.minD); d.maxDistance = S->dev<float>(q.maxD); d.stats8 = S->dev<double>(q.stats);
+        d.ieLinked = S->dev(q.ieLinked); d.kfVelocity = S->dev<float>(q.kfVel); d.kfBias6 = S->dev<float>(q.kfBias); d.stats8 = S->dev<double>(q.stats);
         const bool dbg = m.optState21 != nullptr;
         d.optState21 = dbg ? S->dev<double>(q.optState) : nullptr; d.optTcw12 = dbg ? S->dev<double>(q.optTcw) : nullptr;
-        d.optPoint = dbg ? S->dev<double>(q.optPoint) : nullptr; d.edgeChi2 = dbg ? S->dev<double>(q.chi2) : nullptr;
-        d.mark = S->dev(q.mark); d.kfIdx = S->dev<int>(q.kfIdx); d.firstPt = S->dev<int>(q.firstPt); d.lpBase = S->dev<int>(q.lpBase);
-        d.cand = S->dev<int>(q.cand); d.obsEdge = S->dev<int>(q.obsEdge); d.Ow2 = S->dev<float>(q.Ow2);
+        d.mark = S->dev(q.mark); d.kfIdx = S->dev<int>(q.kfIdx); d.cand = S->dev<int>(q.cand);
         d.D = S->dev<liba::Dev>(devTab) + j;
         T[j] = d;
     }
