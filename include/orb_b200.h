@@ -932,7 +932,8 @@ int lba_get_phase_ns(const lba_handle* h, int i, double* ns10);
  *   optional (may be NULL): optPose [nKF][7] / optPoint [nPoints][3], the solver's double estimates per local keyframe / point in list order;
  *     edgeChi2 / edgeDepthPositive [obsStart[nPoints]] per observation with an edge.
  * Errors: ORB_ERR_ARG for an index, octave or CSR offset out of range, a CSR that does not start at 0 or decreases, repeated keyframe /
- * point ids, a keyframe listed twice among a point's observations, or null arrays a map needs; ORB_ERR_CAPACITY when nMaps > max_batch or a map's built problem exceeds max_poses / max_points /
+ * point ids, a keyframe or point mnId of 2^64 - 1 (ORB-SLAM3 counts mnIds up from 0; the vertex sort pads with that value), a keyframe
+ * listed twice among a point's observations, or null arrays a map needs; ORB_ERR_CAPACITY when nMaps > max_batch or a map's built problem exceeds max_poses / max_points /
  * max_edges.  The message names the map.  Launches (lba_local_last_launches): walk, fill, structure, solver and finish whatever nMaps
  * when any map reaches the solver, else walk and finish.  One staging upload, one copy of the built sizes back, three small tables
  * (slot records, fill sources, solve results) to the device, one download. */

@@ -240,6 +240,9 @@ int check_map(const LbaLocalMap& m, int j) {
     if ((m.edgeChi2 == nullptr) != (m.edgeDepthPositive == nullptr)) return bad("edgeChi2 and edgeDepthPositive go together");
     if (m.kfFlags[0] & ORBM_KF_OTHER_MAP) return bad("pKF (entry 0) cannot be of another map");
     if (!all_distinct(m.mnId, m.nKF)) return bad("keyframe mnIds repeat");
+    // ~0ull pads the vertex sort's keys: an mnId equal to it could sort behind a padding entry and lose its vertex
+    for (int k = 0; k < m.nKF; ++k)
+        if (m.mnId[k] == ~0ull) return bad("a keyframe mnId is 2^64 - 1");
     std::vector<char> seen(m.nKF, 0);
     seen[0] = 1;
     for (int i = 0; i < m.nCov; ++i) {
@@ -249,6 +252,8 @@ int check_map(const LbaLocalMap& m, int j) {
     }
     if (int rc = orbx::check_slots(m, m.nCov + 1, bad)) return rc;
     if (m.nPoints > 0 && !all_distinct(m.pointId, m.nPoints)) return bad("point mnIds repeat");
+    for (int p = 0; p < m.nPoints; ++p)
+        if (m.pointId[p] == ~0ull) return bad("a point mnId is 2^64 - 1");
     return orbx::check_observations(m, bad);
 }
 
